@@ -1,10 +1,12 @@
-"""Flagship benchmark: fault-tolerant Llama-3-8B training throughput on B200.
+"""Flagship benchmark: fault-tolerant Llama-3 training throughput on H100.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
-Metric (BASELINE.json): whole-job tokens/s of Llama-3-8B bf16 training with the
+Metric: whole-job tokens/s of Llama-3 bf16 training (default ``llama3_1b``, 1.5 B parameters: its
+weights, gradients and fp32 AdamW state take 24 GB, so one replica group fits one 80 GB H100; the
+8B model's 128 GB of training state does not) with the
 per-step fault-tolerance protocol ON (Lighthouse quorum + cross-replica gradient
 reduction + commit decision + AdamW), N replica groups of one GPU each (HSDP with
 shard degree 1; weak scaling: per-GPU batch fixed), synthetic tokens, random-init
@@ -18,15 +20,18 @@ the held slices fused with the all-gather of the new bf16 weights under the next
             wall-clock, including per step the pinned-host -> device copy of tokens/targets
             and a device -> host read of the loss (pinned, read back one step late so the
             host never drains the GPU queue).
-`--impl reference` : the unmodified reference cannot be installed offline (its build
-            backend maturin + cargo/protoc are absent) -> prints {"unavailable": ...}.
+`--impl reference` : upstream torchft builds its native module with maturin + cargo/protoc;
+            without them it cannot be installed -> prints {"unavailable": ...}.
 `--impl nccl`      : same model/loop with the reference-EQUIVALENT structure: stock
             ProcessGroupNCCL re-created per quorum, all-reduce SUM then /N, host-synchronous
             should_commit RPC, full AdamW on every replica (reference manager.py:466-478,
             884-903, optim.py:52-55).
 The native arm also runs the nccl arm afterwards IN THE SAME PROCESS (the reference publishes
-no numbers, BASELINE.md) and reports `vs_baseline` = native / nccl-equivalent;
-`--no-baseline-arm` skips it.
+no numbers) and reports `vs_baseline` = native / nccl-equivalent; `--no-baseline-arm` skips it.
+`--dump-outputs DIR` : after the timed steps, rank 0 writes what the device-timed loop computed in
+            its last step as float32 .npy files: `loss.npy` and `weights_sample.npy` (the updated bf16
+            weights at a fixed, seeded set of positions in every parameter tensor). Inputs and weights
+            are seeded, so two builds can be compared output for output.
 """
 
 from __future__ import annotations
@@ -36,6 +41,7 @@ import json
 import os
 import statistics
 import sys
+import tempfile
 import threading
 import time
 from datetime import timedelta
@@ -110,6 +116,22 @@ class ClockSampler:
             except Exception:
                 pass
         return out
+
+
+def _sample_outputs(trainer, loss) -> dict:
+    """Host copies of the last step's loss and of the updated weights at seeded positions: up to 16384 elements of
+    every parameter tensor, in the trainer's fixed parameter order (16384 x 4 B x ~150 tensors of Llama-3 ~ 10 MB)."""
+    import numpy as np
+    import torch
+
+    gen = torch.Generator().manual_seed(0)
+    parts = []
+    for p in trainer.flat.params:
+        flat = p.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (16384,), generator=gen).sort().values if flat.numel() > 16384 else None
+        parts.append((flat if idx is None else flat[idx.to(flat.device)]).float().cpu())
+    return {"loss": np.asarray([float(loss.item())], dtype=np.float32),
+            "weights_sample": torch.cat(parts).numpy().astype(np.float32)}
 
 
 def run_arm(impl: str, args, rank: int, world: int, local: int, lh_addr: str) -> dict:
@@ -189,6 +211,7 @@ def run_arm(impl: str, args, rank: int, world: int, local: int, lh_addr: str) ->
     launches = _native.kernel_launches() - launches0
     dev_ms = ev0.elapsed_time(ev1) / args.steps
     loss_v = float(loss.item())
+    outputs = _sample_outputs(trainer, loss) if args.dump_outputs and rank == 0 else None
     committed = trainer.manager.current_step()
 
     # ---- phase B: end to end through the public API (H2D inputs + D2H loss every step) ----
@@ -212,6 +235,7 @@ def run_arm(impl: str, args, rank: int, world: int, local: int, lh_addr: str) ->
         "warmup": warmup, "cfg": cfg, "h2d": int(tok_cpu.numel() * 8 + tgt_cpu.numel() * 8),
         "zero1": bool(getattr(trainer, "zero1", False)),
         "state_gib": (trainer.zopt.state_bytes_held() / 2**30) if getattr(trainer, "zopt", None) is not None else None,
+        "outputs": outputs,
     }
     trainer.shutdown()
     barrier()  # every peer has unmapped our segments
@@ -230,21 +254,23 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "reference", "nccl"])
-    ap.add_argument("--model", default="llama3_8b")
+    ap.add_argument("--model", default="llama3_1b")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--batch", type=int, default=1, help="sequences per GPU per step")
     ap.add_argument("--bucket-mb", type=float, default=512.0)
     ap.add_argument("--quantize", action="store_true")
     ap.add_argument("--replication", type=int, default=2, help="FT-ZeRO-1: holders per slice of optimizer state")
     ap.add_argument("--shards", type=int, default=1,
-                    help="FSDP2 shard degree INSIDE a replica group (BASELINE config 2 headline: --gpus 8 --shards 2 = 4 groups x 2 "
-                         "shards); default 1 = every GPU is a replica group holding the full model (fits in 180 GB)")
+                    help="FSDP2 shard degree INSIDE a replica group (--gpus 8 --shards 2 = 4 groups x 2 shards); default 1 = "
+                         "every GPU is a replica group holding the full model")
     ap.add_argument("--ac", default=None, help="activation checkpointing: none|full (default: auto)")
     ap.add_argument("--no-baseline-arm", action="store_true",
                     help="native arm only: skip the in-process run of the reference-equivalent NCCL arm")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and a seeded sample of the updated weights as DIR/<name>.npy")
     ap.add_argument("--config", default="hsdp", choices=["hsdp", "diloco", "heal"],
-                    help="BASELINE.json config: hsdp (2, default: the flagship step), diloco (3: Llama-3-8B, outer step every "
-                         "100, fused fp8 outer all-reduce; launch under torchrun), heal (4: kill a replica group at step 50, "
+                    help="hsdp (default: the flagship step), diloco (Llama-3 DiLoCo, outer step every "
+                         "100, fused fp8 outer all-reduce; launch under torchrun), heal (kill a replica group at step 50, "
                          "rejoin at 80; launch WITHOUT torchrun, it spawns one process per GPU)")
     args, extra = ap.parse_known_args()
 
@@ -254,10 +280,10 @@ def main() -> None:
         script = {"diloco": "diloco_bench.py", "heal": "heal_bench.py"}[args.config]
         if args.config == "diloco":
             argv = ["--model", args.model, "--seq", str(args.seq), "--sync-every", "100", "--outer-steps", "1",
-                    "--out", "gpurun_out/bench_diloco.json"] + (["--quantize"] if args.quantize or "--no-quantize" not in extra else [])
+                    "--out", os.path.join(tempfile.gettempdir(), "bench_diloco.json")] + (["--quantize"] if args.quantize or "--no-quantize" not in extra else [])
         else:
             argv = ["--gpus", str(args.gpus), "--model", args.model, "--seq", str(args.seq), "--kill-at", "50", "--rejoin-at", "80",
-                    "--steps", "100", "--out", "gpurun_out/bench_heal.json"]
+                    "--steps", "100", "--out", os.path.join(tempfile.gettempdir(), "bench_heal.json")]
         argv += [x for x in extra if x != "--no-quantize"]
         sys.argv = [os.path.join(ROOT, "bench", script)] + argv
         runpy.run_path(sys.argv[0], run_name="__main__")
@@ -268,15 +294,16 @@ def main() -> None:
             return
         print(json.dumps({
             "impl": "reference",
-            "unavailable": "reference build backend (maturin) and its toolchain (cargo/rustc, protoc) are not "
-                           "installed and there is no network: `pip install --no-index ... /root/reference` fails "
-                           "with BackendUnavailable (see DESIGN.md)",
+            "unavailable": "upstream torchft's build backend (maturin) and its toolchain (cargo/rustc, protoc) are not "
+                           "installed, so it cannot be built here (see DESIGN.md)",
         }))
         return
 
     import torch
     import torch.distributed as dist
 
+    if args.dump_outputs and args.shards > 1:
+        ap.error("--dump-outputs needs --shards 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", str(rank)))
@@ -324,7 +351,7 @@ def main() -> None:
     if rank == 0:
         native = args.impl == "native"
         out = {
-            "metric": "tokens/sec (whole job, Llama-3-8B fault-tolerant training step, bf16)",
+            "metric": f"tokens/sec (whole job, {args.model} fault-tolerant training step, bf16)",
             "value": round(value, 1),
             "unit": "tokens/s",
             "n_gpus": world,
@@ -358,7 +385,8 @@ def main() -> None:
                 "commit": "device-side verdict kernel, host learns lazily (no stream sync, no RPC per step)" if res["zero1"]
                           else "host stream synchronize + should_commit RPC per step",
                 "quantized_allreduce": bool(args.quantize),
-                "l2_policy": "inputs larger than L2 (16 GB of weights + 16 GB of gradients stream through every step)",
+                "l2_policy": (f"inputs larger than L2 ({cfg.num_params() * 2 / 1e9:.0f} GB of weights + as many of gradients "
+                              "stream through every step)"),
                 "ft_protocol_per_step": "start_quorum(async, C++ control plane) + commit decision, in the timed region",
             },
             "e2e": {
@@ -394,6 +422,12 @@ def main() -> None:
                     "clocks": base["clocks"], "peak_mem_gib": round(base["peak_gib"], 1), "loss": round(base["loss"], 4),
                 }
         print(json.dumps(out), flush=True)
+        if args.dump_outputs:
+            import numpy as np
+
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, arr in res["outputs"].items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
 
     if world > 1:
         dist.barrier()  # every rank is done with the lighthouse before rank 0 stops it

@@ -86,7 +86,7 @@ def main() -> None:
     window_ms = sum(step_ms) / len(step_ms) * (a.sync_every - 1) + sum(sync_ms) / len(sync_ms)
     t = torch.tensor([window_ms, sum(step_ms) / len(step_ms), sum(sync_ms) / len(sync_ms)], dtype=torch.float64)
     # replicas run their inner steps unsynchronised, so at the sync the fast ones WAIT for the slowest (GPU clocks differ by a
-    # few % under the power cap: ~1 s after 100 steps of 390 ms). The slowest replica arrives last and waits for nobody:
+    # few % under a power cap, which adds up over the inner steps). The slowest replica arrives last and waits for nobody:
     # MIN over ranks of (sync step - own inner step) is the cost of the sync itself, MAX - MIN is straggler wait.
     own = torch.tensor([t[2] - t[1]], dtype=torch.float64)
     lo = own.clone()
@@ -102,7 +102,7 @@ def main() -> None:
                "straggler_wait_ms_fastest_replica": round(float(t[2] - t[1]) - float(lo[0]), 2), "outer_steps_committed": manager.current_step(),
                "pseudo_grad_bytes": nparam * 2, "flat_fast_path": not a.no_flat,
                "peak_mem_gib": round(torch.cuda.max_memory_allocated() / 2**30, 1),
-               "link_time_ms_at_770GBps": round((nparam * (1 if a.quantize else 2)) * 2 * (world - 1) / world / 770e6, 2)}
+               "link_time_ms_at_450GBps": round((nparam * (1 if a.quantize else 2)) * 2 * (world - 1) / world / 450e6, 2)}
         os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
         with open(a.out, "a") as f:
             f.write(json.dumps(res) + "\n")

@@ -4,12 +4,12 @@ Orchestrator (no torchrun): starts a Lighthouse, spawns one trainer process per 
 SIGKILLs replica `--victim` when the survivors reach step `--kill-at`, respawns it when
 they reach `--rejoin-at`, and collects per-step logs.
 
-    python bench/heal_bench.py --gpus 2 --model llama3_8b --kill-at 6 --rejoin-at 12 --steps 20
+    python bench/heal_bench.py --gpus 2 --model llama3_1b --kill-at 6 --rejoin-at 12 --steps 20
 
 Reports: steady step time before the kill, the stall caused by the drop (survivor's
 collective times out -> commit fails -> lighthouse drops the dead replica -> remap),
 steps lost, the heal transfer size / time / GB/s (NVLink P2P pull by a copy kernel,
-vs. 770 GB/s peer-copy roofline), and the step time of the step that carried the heal.
+vs. the 450 GB/s per-direction NVLink 4 rate of the H100 data sheet), and the step time of the step that carried the heal.
 """
 
 from __future__ import annotations
@@ -100,7 +100,7 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--role", default="orchestrator")
     ap.add_argument("--gpus", type=int, default=2)
-    ap.add_argument("--model", default="llama3_8b")
+    ap.add_argument("--model", default="llama3_1b")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--kill-at", type=int, default=6)
@@ -185,7 +185,7 @@ def main() -> None:
             "bytes": heals[0]["heal_bytes"] if heals else None,
             "copy_ms": round(heals[0]["heal_ms"], 2) if heals else None,
             "gbs": round(heals[0]["heal_bytes"] / heals[0]["heal_ms"] / 1e6, 1) if heals else None,
-            "frac_of_770_peer_copy": round(heals[0]["heal_bytes"] / heals[0]["heal_ms"] / 1e6 / 770, 3) if heals else None,
+            "frac_of_nvlink": round(heals[0]["heal_bytes"] / heals[0]["heal_ms"] / 1e6 / 450, 3) if heals else None,
             "victim_first_step_ms": round(vc[0]["ms"], 1) if vc else None,
             "survivor_step_ms_during_heal": round(first_full["ms"], 1) if first_full else None,
             "victim_restart_to_ready_s": next((round(e["setup_s"], 1) for e in read_log(logs[args.victim]) if e["event"] == "ready" and rejoin_t and e["t"] > rejoin_t), None),

@@ -1,11 +1,11 @@
-"""Per-kernel timing + roofline fractions for the hand-written sm_100a kernels (1 GPU).
+"""Per-kernel timing + roofline fractions for the hand-written sm_90a kernels (1 GPU).
 
-    python bench/kernel_micro.py --out gpurun_out/kernel_micro.json
+    python bench/kernel_micro.py --out kernel_micro.json
     ncu --set full --clock-control none --import-source on -k regex:adamw -c 2 -o gpurun_out/prof_adamw \
         python bench/kernel_micro.py --only adamw --iters 2
 
 CUDA-event timing, 3+ warm-ups, a >L2 buffer is rewritten between timed iterations;
-"frac" = algorithmic bytes / time / MEASURED_PEAKS.json hbm_gbs.
+"frac" = algorithmic bytes / time / the H100 SXM data-sheet HBM3 bandwidth (3 350 GB/s).
 """
 
 from __future__ import annotations
@@ -23,12 +23,7 @@ from torchft_b200.ops import _native, fused  # noqa: E402
 from torchft_b200 import quantization as Q  # noqa: E402
 
 
-def peaks() -> float:
-    try:
-        with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"])
-    except Exception:
-        return 6650.0
+HBM_GBS = 3350.0  # H100 SXM data sheet (HBM3); a power-limited card reaches less
 
 
 def timeit(fn, iters: int, flush: torch.Tensor) -> float:
@@ -56,7 +51,7 @@ def main() -> None:
     args = ap.parse_args()
     K = _native.load()
     dev = torch.device("cuda")
-    hbm = peaks()
+    hbm = HBM_GBS
     flush = torch.zeros(64 << 20, dtype=torch.float32, device=dev)  # 256 MB
     T, H, F, V = 8192, 4096, 14336, 128256
     res = {}
@@ -66,7 +61,7 @@ def main() -> None:
 
     def record(name, ms, nbytes):
         gbs = nbytes / ms / 1e6
-        res[name] = {"ms": round(ms, 4), "algo_gb": round(nbytes / 1e9, 3), "gbs": round(gbs, 1), "frac_of_measured_hbm": round(gbs / hbm, 3)}
+        res[name] = {"ms": round(ms, 4), "algo_gb": round(nbytes / 1e9, 3), "gbs": round(gbs, 1), "frac_of_hbm_datasheet": round(gbs / hbm, 3)}
         print(name, res[name], flush=True)
 
     sp = lambda: _native.stream_ptr()  # noqa: E731
@@ -83,7 +78,7 @@ def main() -> None:
         dw = torch.empty_like(w)
         record("rmsnorm_bwd", timeit(lambda: K.rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), rstd.data_ptr(), dx.data_ptr(), part.data_ptr(), dw.data_ptr(), False, T, H, sp()), args.iters, flush), 3 * x.numel() * 2)
         if args.only == "rmsnorm_sweep":  # CTA shape x prefetch x CTAs/SM (the default is set in model_ops.cu)
-            part = torch.empty(148 * 8, H, device=dev)
+            part = torch.empty(K.NUM_SMS * 8, H, device=dev)
             for tpb in (128, 256, 512):
                 for pf in (0, 1):
                     for cps in (2, 3, 4, 6, 8):
@@ -121,7 +116,7 @@ def main() -> None:
         m = torch.zeros(n, device=dev)
         v = torch.zeros(n, device=dev)
         record("adamw", timeit(lambda: K.adamw(p.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), g.data_ptr(), n, 1e-3, 0.9, 0.95, 1e-8, 0.1, 0.1, 0.05, 1.0, 0, sp()), args.iters, flush), n * 28)
-        for cap in (148, 296, 592, 1184, 2368):  # CTA-cap sweep (default = 4 CTAs/SM)
+        for cap in (K.NUM_SMS * c for c in (1, 2, 4, 8, 16)):  # CTA-cap sweep (default = 16 CTAs/SM)
             record(f"adamw_cap{cap}", timeit(lambda: K.adamw(p.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), g.data_ptr(), n, 1e-3, 0.9, 0.95, 1e-8, 0.1, 0.1, 0.05, 1.0, 0, sp(), cap), args.iters, flush), n * 28)
         del p, g, master, m, v
     if want("q8"):
@@ -137,9 +132,9 @@ def main() -> None:
         n = 1 << 30
         a = torch.empty(n, dtype=torch.uint8, device=dev)
         b = torch.empty(n, dtype=torch.uint8, device=dev)
-        for blocks in (32, 64, 148):
+        for blocks in (32, 64, K.NUM_SMS):
             record(f"heal_copy_local_b{blocks}", timeit(lambda: device_copy([(a.data_ptr(), b.data_ptr(), n)], blocks=blocks, bulk=False), args.iters, flush), 2 * n)
-        for blocks in (148, 296, 444):  # TMA variant: 64 KiB smem per CTA -> up to 3 CTAs per SM, 32 threads each
+        for blocks in (K.NUM_SMS, 2 * K.NUM_SMS, 3 * K.NUM_SMS):  # TMA variant: 64 KiB smem per CTA -> up to 3 CTAs per SM, 32 threads each
             record(f"heal_copy_bulk_tma_b{blocks}", timeit(lambda: device_copy([(a.data_ptr(), b.data_ptr(), n)], blocks=blocks, bulk=True), args.iters, flush), 2 * n)
         del a, b
     if want("diloco_outer"):
@@ -161,12 +156,12 @@ def main() -> None:
         g = torch.zeros(n, device=dev, dtype=torch.bfloat16)
         master, m, v = (torch.zeros(n, device=dev) for _ in range(3))
         gate = torch.ones(2, dtype=torch.int32, device=dev)
-        for cap in (296, 1184, 2368):
+        for cap in (K.NUM_SMS * c for c in (2, 8, 16)):
             record(f"zero1_update_w1_cap{cap}", timeit(lambda: c.zero1_update_("z1_param", 0, g.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), n, (1e-3, 0.9, 0.95, 1e-8, 0.1), gate, 1, 0, cap), args.iters, flush), n * 28)
     if args.out:
         os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
         with open(args.out, "w") as f:
-            json.dump({"hbm_gbs_measured": hbm, "kernels": res}, f, indent=1)
+            json.dump({"hbm_gbs_datasheet": hbm, "kernels": res}, f, indent=1)
 
 
 if __name__ == "__main__":

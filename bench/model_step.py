@@ -1,9 +1,9 @@
 """Single-GPU training-step timing/memory probe for the Llama configs (no FT plumbing).
 
-    python bench/model_step.py --model llama3_8b --seq 8192 --batch 1 --steps 5
+    python bench/model_step.py --model llama3_1b --seq 8192 --batch 1 --steps 5
 
-Used to size the flagship benchmark (does 8B + AdamW state + activations fit in
-180 GB, what does a step cost, where does the time go).
+Used to size the flagship benchmark (do the model's weights + AdamW state + activations fit in
+the 80 GB of an H100, what does a step cost, where does the time go).
 """
 
 from __future__ import annotations
@@ -67,7 +67,7 @@ def run(args, ac: str) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="llama3_8b")
+    ap.add_argument("--model", default="llama3_1b")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--batch", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)

@@ -6,7 +6,7 @@
 Each rank reads its GPU's NVLink data counters (NVML field NVLINK_THROUGHPUT_DATA_TX/RX summed over links, KiB; fallback:
 ``nvidia-smi nvlink -gt d``) before and after ``--iters`` launches of one kernel, device-times the launches (CUDA events,
 MAX over ranks), and reports per launch: counted TX/RX bytes (mean over ranks), the algorithmic bytes the kernel should
-move per rank, their ratio, and the achieved fraction of the 770 GB/s per-direction peer-copy reference. A kernel that
+move per rank, their ratio, and the achieved fraction of the 450 GB/s per-direction NVLink 4 rate of the H100 data sheet. A kernel that
 moved more than its algorithmic bytes (protocol overhead, N x traffic) shows a ratio above 1.
 """
 
@@ -28,7 +28,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from torchft_b200.checkpointing.p2p_transport import device_copy  # noqa: E402
 from torchft_b200.parallel.symm_mem import SymmetricComm  # noqa: E402
 
-LINK_GBS = 770.0
+LINK_GBS = 450.0
 
 
 class Counters:
@@ -133,9 +133,9 @@ def main() -> None:
         "zero1_reduce_scatter": (lambda: comm.zero1_reduce_scatter_("z1_grad", 0, nelem, 1.0 / W, True, k, 128),
                                  ((W - 1) + (k - 1)) / W * S, ((W - 1) + (k - 1)) / W * S),
         "zero1_update_allgather": (lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(),
-                                                              nelem, hp, gate, k, 0, 2368), (W - k) / W * S, (W - k) / W * S),
+                                                              nelem, hp, gate, k, 0, comm._K.NUM_SMS * 16), (W - k) / W * S, (W - k) / W * S),
         "heal_copy_pull_lsu": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=128, bulk=False), S, S),
-        "heal_copy_pull_bulk_tma": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=296, bulk=True), S, S),
+        "heal_copy_pull_bulk_tma": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=comm._K.MAX_BLOCKS, bulk=True), S, S),
     }
     if qb:
         q_total = n32 * (1 + 4.0 / 512)  # fp8 payload + one fp32 scale per 512 elements
@@ -175,7 +175,7 @@ def main() -> None:
                 "algorithmic_rx_mb_per_rank": round(alg_rx / 1e6, 2),
                 "counted_over_algorithmic": round(max(tx, rx) / max(alg_rx, alg_tx), 3) if alg_rx else None,
                 "achieved_gbs_per_direction": round(max(alg_rx, alg_tx) / float(mx[0]) / 1e6, 1),
-                "frac_of_770": round(max(alg_rx, alg_tx) / float(mx[0]) / 1e6 / LINK_GBS, 3),
+                "frac_of_link": round(max(alg_rx, alg_tx) / float(mx[0]) / 1e6 / LINK_GBS, 3),
             }
         except Exception as ex:  # keep the sweep going; the failure is part of the report
             res["ops"][name] = {"error": repr(ex)[:200]}

@@ -1,6 +1,6 @@
-"""Can the HBM-bound AdamW update hide under tensor-core GEMMs on one B200?
+"""Can the HBM-bound AdamW update hide under tensor-core GEMMs on one H100?
 
-Times, per "layer" (4 forward-shaped bf16 GEMMs of a Llama-3-8B block at 8192 tokens, ~2.4 ms,
+Times, per "layer" (4 forward-shaped bf16 GEMMs of a Llama-3-8B block at 8192 tokens,
 and the AdamW update of that layer's 218 M parameters, 6.1 GB of traffic):
   serial      GEMMs then AdamW on one stream
   overlapped  AdamW on a second stream (optionally narrowed to fewer CTAs / lower priority)
@@ -76,13 +76,13 @@ def main() -> None:
 
     res["gemm_only_ms"] = timed(only_gemm)
     res["adam_only_ms"] = timed(only_adam)
-    for b in (148, 296, 592):
+    for b in (K.NUM_SMS, 2 * K.NUM_SMS, 4 * K.NUM_SMS):
         res[f"adam_only_b{b}_ms"] = timed(lambda: only_adam(b))
     res["serial_ms"] = timed(serial)
 
     for prio_name, prio in (("lo", 0), ("hi", -1)):
         side = torch.cuda.Stream(priority=prio)
-        for blocks in (0, 592, 296, 148, 74):
+        for blocks in (0, 4 * K.NUM_SMS, 2 * K.NUM_SMS, K.NUM_SMS, K.NUM_SMS // 2):
             def overlapped() -> None:
                 # layer i's GEMMs wait only for layer i's update, later updates run underneath
                 side.wait_stream(main_s)

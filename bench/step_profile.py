@@ -1,4 +1,4 @@
-"""Where does a Llama-3-8B training step go? torch.profiler kernel table for ONE step (1 GPU),
+"""Where does a Llama-3 training step go? torch.profiler kernel table for ONE step (1 GPU),
 plus an SDPA backend shoot-out at the model's attention shape.
 
     python bench/step_profile.py --out gpurun_out/step_profile.txt
@@ -63,7 +63,7 @@ def attn_shootout(S=8192, Hq=32, Hkv=8, D=128, out=None):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="llama3_8b")
+    ap.add_argument("--model", default="llama3_1b")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--out", default="gpurun_out/step_profile.txt")
     args = ap.parse_args()

@@ -58,7 +58,7 @@ def intersect(a, b):
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--impl", default="native", choices=["native", "nccl"])
-    ap.add_argument("--model", default="llama3_8b")
+    ap.add_argument("--model", default="llama3_1b")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=4)

@@ -1,6 +1,6 @@
 """FT-ZeRO-1 kernel micro-benchmark: reduce-scatter (+buddy push) and gated AdamW + weight all-gather.
 
-Multi-GPU (device-timed, max over ranks, bus bytes per rank vs the 770 GB/s peer-copy reference):
+Multi-GPU (device-timed, max over ranks, bus bytes per rank vs the H100 data-sheet NVLink 4 rate, 450 GB/s per direction):
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port 29517 bench/zero1_bench.py --mb 436 --out gpurun_out/zero1_bench_nN.json
@@ -34,6 +34,7 @@ HP = (3e-4, 0.9, 0.95, 1e-8, 0.1)
 
 
 def run_rank(comm, nelem, k, rs_blocks, upd_blocks, iters, warmup, sync, reduce_max):
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
     dev = comm.device
     grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
     grad.normal_()
@@ -70,7 +71,7 @@ def main() -> None:
     ap.add_argument("--mb", type=float, default=436.0, help="unit size in MB of bf16 gradients (one Llama-3-8B block = 436 MB)")
     ap.add_argument("--replication", type=int, default=2)
     ap.add_argument("--rs-blocks", type=int, default=128)
-    ap.add_argument("--upd-blocks", type=int, default=2368)
+    ap.add_argument("--upd-blocks", type=int, default=0, help="grid cap of the update kernel (0: 16 per SM, the trainer default)")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--virtual", type=int, default=0, help="emulate this many ranks on ONE GPU (presignalled; for ncu)")
@@ -110,17 +111,17 @@ def main() -> None:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    res = {"world": world, "unit_mb": round(S / 2**20, 1), "replication": min(a.replication, world), "rs_blocks": a.rs_blocks, "upd_blocks": a.upd_blocks,
+    res = {"world": world, "unit_mb": round(S / 2**20, 1), "replication": min(a.replication, world), "rs_blocks": a.rs_blocks, "upd_blocks": a.upd_blocks or comm._K.NUM_SMS * 16,
            "mode": comm._mode, "nvls": bool(comm._mc)}
     t = run_rank(comm, nelem, a.replication, a.rs_blocks, a.upd_blocks, a.iters, a.warmup, sync, reduce_max)
     k = min(a.replication, world)
-    link = 770.0  # GB/s per direction per GPU (B200_PROFILING.md)
-    hbm = 6571.0
+    link = 450.0  # GB/s per direction per GPU: H100 SXM data sheet (NVLink 4, 900 GB/s bidirectional)
+    hbm = 3350.0  # GB/s: H100 SXM data sheet (HBM3)
     if "reduce_scatter" in t:
         inb = (world - 1) / world * S
         res["reduce_scatter"] = {"ms": round(t["reduce_scatter"], 3), "nvlink_in_gb": round(inb / 1e9, 3),
                                  "in_gbps": round(inb / t["reduce_scatter"] / 1e6, 1),
-                                 "frac_of_770": round(inb / t["reduce_scatter"] / 1e6 / link, 3)}
+                                 "frac_of_link": round(inb / t["reduce_scatter"] / 1e6 / link, 3)}
     outb = max(0, world - k) / world * S  # holders compute their own copy: the primary pushes to W - k ranks
     hbm_b = 28.0 * nelem * k / world
     floor_ms = max(outb / (link * 1e6), hbm_b / (hbm * 1e6)) if world > 1 else hbm_b / (hbm * 1e6)

@@ -1,4 +1,4 @@
-"""Sphinx configuration: `sphinx-build -b html docs/source docs/_build` (reference: /root/reference/docs/source/conf.py).
+"""Sphinx configuration: `sphinx-build -b html docs/source docs/_build` (reference: upstream docs/source/conf.py).
 
 The narrative pages are the Markdown files one directory up (included through MyST when it is installed); the API
 reference is generated with autodoc, one page per public module like the reference's docs/source/*.rst.

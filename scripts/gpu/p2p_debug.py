@@ -25,8 +25,8 @@ for staging, n in ((4 << 20, 300_001), (4 << 20, 20_000), (64 << 20, 300_001)):
         comms[2].recv_(ra, 0, s2)
     torch.cuda.synchronize()
     c0 = comms[0]
-    pad0 = comms[0].segment("core")[: c0._K.SIGNAL_PAD_BYTES].view(torch.int64).view(4, 296, 8)
-    pad2 = comms[2].segment("core")[: c0._K.SIGNAL_PAD_BYTES].view(torch.int64).view(4, 296, 8)
+    pad0 = comms[0].segment("core")[: c0._K.SIGNAL_PAD_BYTES].view(torch.int64).view(4, c0._K.MAX_BLOCKS, 8)
+    pad2 = comms[2].segment("core")[: c0._K.SIGNAL_PAD_BYTES].view(torch.int64).view(4, c0._K.MAX_BLOCKS, 8)
     print("staging", staging, "n", n, "mailbox", c0._mailbox_bytes, "took %.2fs" % (time.time() - t0), "match", bool(torch.equal(a, ra)),
           "first_bad", int((a != ra).nonzero()[0]) if not torch.equal(a, ra) else -1)
     print("  errs", [str(c.errored()) for c in comms])

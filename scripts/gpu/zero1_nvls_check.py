@@ -84,12 +84,12 @@ def main() -> None:
         comm.zero1_reduce_scatter_("z1_grad", 0, nelem, 1.0 / world, True, k, 128)
         sync()
         reduced = grad.clone()
-        comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), nelem, HP, gate, k, 0, 2368)
+        comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), nelem, HP, gate, k, 0, comm._K.NUM_SMS * 16)
         sync()
         weights = param.clone()
         times = {}
         for name, fn in (("reduce_scatter_ms", lambda: comm.zero1_reduce_scatter_("z1_grad", 0, nelem, 1.0 / world, True, k, 128)),
-                         ("update_ms", lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), nelem, HP, gate, k, 0, 2368))):
+                         ("update_ms", lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), nelem, HP, gate, k, 0, comm._K.NUM_SMS * 16))):
             for _ in range(2):
                 fn()
             sync()

@@ -1,4 +1,4 @@
-"""Reduce .ncu-rep files to the metrics the B200 profiling recipe asks for (CSV per report, one row per kernel launch).
+"""Reduce .ncu-rep files to the metrics the profiling recipe asks for (CSV per report, one row per kernel launch).
 
     python scripts/ncu_summarize.py gpurun_out/ncu/*.ncu-rep --out profiles/
 """

@@ -1,5 +1,5 @@
 """Build hook: the native modules are compiled in-tree by ``torchft_b200/_build.py`` (nvcc for
-sm_100a + g++ for the control plane) before setuptools collects the package, so an sdist/wheel or
+sm_90a + g++ for the control plane) before setuptools collects the package, so an sdist/wheel or
 ``pip install -e .`` carries ``_K*.so`` / ``_C*.so`` and the lighthouse binary."""
 
 import importlib.util

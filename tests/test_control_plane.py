@@ -1,7 +1,7 @@
 """Spec tests for the C++ control plane.
 
 The scenario tables re-create the reference's Rust unit tests
-(/root/reference/src/lighthouse.rs:627-1111, src/manager.rs:656-1218) against
+(upstream src/lighthouse.rs:627-1111, src/manager.rs:656-1218) against
 our implementation through the pybind11 module: pure decision functions first,
 then real servers on loopback (port 0) driven by real clients.
 """

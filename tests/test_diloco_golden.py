@@ -2,11 +2,11 @@
 
 Re-runs the reference's deterministic mocked-update scenario (constant gradient 2, inner lr 1,
 outer lr 2, two 1x1 fragments, sync_every 6, with/without sync delay, alpha in {0, .5, 1};
-/root/reference/torchft/diloco_regression_test.py) on OUR DiLoCo + Manager + Lighthouse + Gloo and
+upstream torchft/diloco_regression_test.py) on OUR DiLoCo + Manager + Lighthouse + Gloo and
 compares the complete per-step parameter history and the global-parameter history with the JSON
-histories the reference checked in (`test_fixtures/*.json` -- data, not code). Matching them pins
+histories upstream torchft checked in (its `test_fixtures/*.json`, stored here as
+`tests/golden/diloco/mocked_updates_<index>.json` -- data, not code). Matching them pins
 down the fragment schedule, pseudo-gradient sign, restore/merge order and alpha mixing exactly.
-Skipped when the reference tree is not mounted (e.g. on the GPU box).
 """
 
 import copy
@@ -27,10 +27,8 @@ from torchft_b200.local_sgd import DiLoCo
 from torchft_b200.manager import Manager
 from torchft_b200.process_group import ProcessGroupGloo
 
-FIXTURES = "/root/reference/test_fixtures"
+FIXTURES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "diloco")
 CASES = [(0, 0.0), (0, 0.5), (0, 1.0), (1, 0.0), (1, 0.5), (1, 1.0)]  # fixture index = position
-
-pytestmark = pytest.mark.skipif(not os.path.isdir(FIXTURES), reason="reference fixtures not mounted")
 
 
 class MockLinear(nn.Module):
@@ -102,8 +100,8 @@ def _replica(rid: int, lh_addr: str, delay: int, alpha: float, barrier: threadin
 @pytest.mark.parametrize("index", range(len(CASES)))
 def test_diloco_matches_reference_history(index):
     delay, alpha = CASES[index]
-    path = os.path.join(FIXTURES, f"torchft.diloco_regression_test.DiLoCoMockedUpdateTest.test_diloco_mocked_updates_{index}.json")
-    expected = json.load(open(path))
+    with open(os.path.join(FIXTURES, f"mocked_updates_{index}.json")) as f:
+        expected = json.load(f)
     lh = LighthouseServer(bind="[::]:0", min_replicas=2)
     barrier = threading.Barrier(2)
     try:

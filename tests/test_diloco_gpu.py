@@ -1,4 +1,4 @@
-"""DiLoCo on the B200 data plane: the flat fast path (one fused delta all-reduce + one fused outer-step kernel per sync)
+"""DiLoCo on the native data plane: the flat fast path (one fused delta all-reduce + one fused outer-step kernel per sync)
 must train exactly like the generic per-parameter path (reference semantics, local_sgd.py:339-384,445-475)."""
 
 from __future__ import annotations

@@ -304,8 +304,10 @@ def test_slurm_runner_resubmits_only_dead_replica_groups(tmp_path):
         first = log.read_text().splitlines()[1]
         assert "--job-name=tft_1" in first and "REPLICA_GROUP_ID=1,NUM_REPLICA_GROUPS=3,TORCHFT_LIGHTHOUSE=http://lh:1" in first
         assert "--master_port=29601 train.py" in first
-        # replica group 1 dies (leaves the queue): only that one comes back
-        state.write_text("".join(l + "\n" for l in state.read_text().splitlines() if not l.startswith("tft_1 ")))
+        # replica group 1 dies (leaves the queue): only that one comes back. The queue is replaced atomically: a poll
+        # between a truncate and the rewrite would see an empty queue and resubmit every group.
+        (tmp_path / "queue.new").write_text("".join(l + "\n" for l in state.read_text().splitlines() if not l.startswith("tft_1 ")))
+        os.replace(tmp_path / "queue.new", state)
         deadline = time.time() + 20
         while len(log.read_text().splitlines()) < 4 and time.time() < deadline:
             time.sleep(0.05)

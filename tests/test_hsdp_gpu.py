@@ -1,6 +1,6 @@
 """HSDPTrainer (FSDP2 inside a replica group x fault-tolerant all-reduce across groups) on one GPU: 1 group x 1 shard
 still runs FSDP2's all-gather / reduce-scatter / all-reduce-hook machinery against the fused model ops.
-Reference wiring: /root/reference/torchft/fsdp_test.py:57-72."""
+Reference wiring: upstream torchft/fsdp_test.py:57-72."""
 import os
 import subprocess
 import sys

@@ -1,4 +1,4 @@
-"""Numerics of the hand-written sm_100a kernels vs plain PyTorch fp32 references."""
+"""Numerics of the hand-written sm_90a kernels vs plain PyTorch fp32 references."""
 
 
 import pytest

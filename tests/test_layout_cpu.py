@@ -81,7 +81,7 @@ def test_allreduce_plan_is_well_formed(world):
             assert 8 <= blocks <= comm._max_blocks
         assert algo >= prev_algo, "once two-shot wins it keeps winning for larger messages"
         prev_algo = algo
-    # measured cross-overs: two-shot from 256 KB at 8 replicas, one-shot up to 2 MB at 2
+    # the plan's cross-overs: two-shot from 256 KB at 8 replicas, one-shot up to 2 MB at 2
     assert SymmetricComm._plan(comm, 4 << 20)[0] == 1
     assert SymmetricComm._plan(comm, 64 << 10)[0] == 0
     assert SymmetricComm._default_nvls_min(2) > (1 << 40) and SymmetricComm._default_nvls_min(4) > (1 << 40)

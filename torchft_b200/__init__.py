@@ -1,9 +1,9 @@
-"""torchft_b200 -- per-step fault-tolerant training, built for 8xB200 / NVLink 5 / NVSwitch.
+"""torchft_b200 -- per-step fault-tolerant training, built for 8xH100 / NVLink 4 / NVSwitch.
 
 Same capabilities and API surface as meta-pytorch/torchft (Lighthouse quorum
 server, Manager, reconfigurable process groups, fault-tolerant DDP/HSDP,
 LocalSGD/DiLoCo, live checkpoint recovery), with the control plane in C++ and
-the data plane as hand-written sm_100a kernels over NVLink peer memory.
+the data plane as hand-written sm_90a kernels over NVLink peer memory.
 """
 
 import logging as _logging

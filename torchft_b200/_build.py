@@ -2,13 +2,12 @@
 
 Two shared objects land next to this file so they travel with the source tree:
 
-* ``_K``  - CUDA data-plane kernels, ``nvcc -gencode arch=compute_100a,code=sm_100a``
-            (sm_100a only; pybind11; no torch headers => seconds to build).
+* ``_K``  - CUDA data-plane kernels for H100, ``nvcc -gencode arch=compute_90a,code=sm_90a``
+            (sm_90a only; pybind11; no torch headers => seconds to build).
 * ``_C``  - C++17 control plane (Lighthouse, ManagerServer, clients; pybind11).
 
-The reference builds its native module with maturin/cargo
-(/root/reference/pyproject.toml:1-3,39-44); neither exists here, and our native
-code is C++/CUDA anyway.
+Upstream torchft builds its native module with maturin/cargo
+(pyproject.toml:1-3,39-44); our native code is C++/CUDA, so plain g++ and nvcc do.
 """
 
 from __future__ import annotations
@@ -30,13 +29,12 @@ EXT = sysconfig.get_config_var("EXT_SUFFIX")
 
 NVCC = os.environ.get("TFT_NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 # Use the system g++ (dynamic libstdc++, same one nvcc uses as host compiler and
-# ABI-compatible with torch). The image exports CXX=/opt/gcc/bin/g++, a toolchain
-# that links libstdc++ STATICALLY -- two C++ runtimes in one process (ours +
-# torch's) corrupt each other, so $CXX is deliberately ignored; override with
-# TFT_CXX only.
+# ABI-compatible with torch). $CXX may name a toolchain that links libstdc++
+# STATICALLY -- two C++ runtimes in one process (ours + torch's) corrupt each
+# other, so $CXX is deliberately ignored; override with TFT_CXX only.
 CXX = os.environ.get("TFT_CXX") or ("/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++") or "g++")
 
-GENCODE = ["-gencode", "arch=compute_100a,code=sm_100a"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _includes() -> List[str]:
@@ -66,7 +64,7 @@ def _run(cmd: List[str]) -> None:
 
 
 def build_kernels(force: bool = False, verbose: bool = False) -> Path:
-    """Compile torchft_b200/_K*.so for sm_100a."""
+    """Compile torchft_b200/_K*.so for sm_90a."""
 
     kdir = CSRC / "kernels"
     cus = sorted(kdir.glob("*.cu"))

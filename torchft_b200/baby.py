@@ -3,7 +3,7 @@
 Why: a wedged NCCL/Gloo collective can only be reliably cancelled by killing the
 process that issued it. Hosting the real group in a child lets the trainer kill
 and respawn it on ``configure``/``abort`` without losing its own CUDA context or
-model state (reference: /root/reference/torchft/process_group.py:1356-2118; costs
+model state (reference: upstream torchft/process_group.py:1356-2118; costs
 documented there -- ~1 GB extra CUDA context per child, no comm/compute overlap --
 apply equally). ``ProcessGroupB200`` does not need this: its kernels are abortable.
 

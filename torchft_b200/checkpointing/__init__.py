@@ -1,6 +1,6 @@
 """Live checkpoint transports used to heal recovering replicas.
 
-* :class:`P2PTransport` -- B200-native default on a single NVSwitch domain:
+* :class:`P2PTransport` -- native default on a single NVSwitch domain:
   the healer pulls tensors GPU->GPU over NVLink from inside a copy kernel.
 * :class:`HTTPTransport` -- TCP fallback / CPU path (reference default).
 * :class:`PGTransport` -- over the fault-tolerant process group's send/recv.

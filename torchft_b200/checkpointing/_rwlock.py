@@ -1,7 +1,7 @@
 """Timed readers-writer lock built on one condition variable.
 
 Parity with the reference's ``RWLock``
-(/root/reference/torchft/checkpointing/_rwlock.py:46-136): every acquire takes
+(upstream torchft/checkpointing/_rwlock.py:46-136): every acquire takes
 at most ``timeout`` seconds and raises ``TimeoutError`` otherwise. Unlike the
 two-mutex construction used there, the write side here may be released from a
 different thread than the one that acquired it (the Manager takes it on the

@@ -2,7 +2,7 @@
 
 Uses ``torch.distributed._serialization``'s zero-copy streaming format when the
 installed torch has it and plain ``torch.save``/``torch.load`` otherwise
-(reference: /root/reference/torchft/checkpointing/_serialization.py:8-39).
+(reference: upstream torchft/checkpointing/_serialization.py:8-39).
 Checkpoints come from a trusted peer of the same job, hence ``weights_only=False``.
 """
 

@@ -1,7 +1,7 @@
 """HTTP live-checkpoint transport (TCP fallback / CPU path).
 
 Behavioural parity with the reference's default heal transport
-(/root/reference/torchft/checkpointing/http_transport.py:38-298): the source
+(upstream torchft/checkpointing/http_transport.py:38-298): the source
 stages its state_dict to host memory on a side stream, serves it from a
 threaded HTTP server while the checkpoint is "allowed", rejects requests for a
 different step with HTTP 400, and blocks new requests again in

@@ -1,8 +1,8 @@
-"""NVLink peer-to-peer live-recovery transport (B200-native default on one node).
+"""NVLink peer-to-peer live-recovery transport (native default on one node).
 
 The reference heals a rejoining replica by copying the source's state_dict
 GPU -> CPU, serving it over HTTP/TCP, and copying CPU -> GPU on the receiver
-(/root/reference/torchft/checkpointing/http_transport.py:219-284), or by one
+(upstream torchft/checkpointing/http_transport.py:219-284), or by one
 NCCL send/recv per tensor (pg_transport.py:214-303). Here the bytes never leave
 HBM/NVLink and no collective is involved:
 
@@ -18,7 +18,7 @@ HBM/NVLink and no collective is involved:
 3. The source keeps training state immutable until ``disallow_checkpoint``,
    which waits for in-flight pulls (reader lock) exactly like the HTTP transport.
 
-Roofline: bytes / 770 GB/s (one NVLink direction); the source's SMs are not used.
+Roofline: bytes / 450 GB/s (one NVLink 4 direction, H100 SXM data sheet); the source's SMs are not used.
 """
 
 from __future__ import annotations
@@ -78,7 +78,7 @@ def device_copy(entries: Sequence[Tuple[int, int, int]], stream: Optional[torch.
     with torch.cuda.stream(s):
         if bulk and chunk_bytes % 16 == 0:
             # 64 KiB of shared memory per CTA -> 3 CTAs per SM; enough CTAs to put > 2 MB (NVLink) / > 8 MB (HBM) in flight
-            K.heal_copy_bulk(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(max(blocks, 296), chunk0)), int(s.cuda_stream))
+            K.heal_copy_bulk(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(max(blocks, K.MAX_BLOCKS), chunk0)), int(s.cuda_stream))
         else:
             K.heal_copy(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(blocks, chunk0)), int(s.cuda_stream))
         table.record_stream(s)

@@ -1,6 +1,6 @@
 """Live-checkpoint transport over the fault-tolerant process group's send/recv.
 
-Parity target: /root/reference/torchft/checkpointing/pg_transport.py:32-305.
+Parity target: upstream torchft/checkpointing/pg_transport.py:32-305.
 Protocol (one pair of messages for the header, then one per tensor):
 
     tag 1: int64 length of the pickled header

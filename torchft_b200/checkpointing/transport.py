@@ -1,7 +1,7 @@
 """Abstract live-checkpoint transport used to heal a recovering replica.
 
 Same contract as the reference's ``CheckpointTransport``
-(/root/reference/torchft/checkpointing/transport.py:14-68): the up-to-date
+(upstream torchft/checkpointing/transport.py:14-68): the up-to-date
 replica calls :meth:`send_checkpoint` for the ranks assigned to it by the
 quorum, the healing replica calls :meth:`recv_checkpoint` with the source's
 :meth:`metadata` string, and the source stops serving in

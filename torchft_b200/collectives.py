@@ -1,8 +1,8 @@
 """Quantised (fp8) collectives over ANY reconfigurable process group.
 
-API parity with /root/reference/torchft/collectives.py (``allreduce_quantized``,
+API parity with upstream torchft/collectives.py (``allreduce_quantized``,
 ``reduce_scatter_quantized``, ``get_padded_sizes``, ``allocate_reduce_scatter_output``).
-This is the *generic* path (used when the group is NCCL/Gloo-backed): our sm_100a
+This is the *generic* path (used when the group is NCCL/Gloo-backed): our sm_90a
 quantise / reduce / dequantise kernels around the group's ``alltoall_base`` and
 ``allgather``. On :class:`ProcessGroupB200` the whole pipeline is a single fused
 kernel instead -- these functions detect that and delegate.

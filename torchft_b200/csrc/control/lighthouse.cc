@@ -119,8 +119,7 @@ uint32_t Lighthouse::handle_rpc(uint32_t method, const std::string& req, TimePoi
   // quorum. Without the join timeout (which the periodic tick serves) a quorum needs every member of the previous quorum
   // (fast path) or every healthy replica among the participants, so fewer participants than both cannot decide anything.
   // quorum_compute sorts and formats over all replicas: running it for each of N simultaneous joiners made forming a
-  // quorum O(N^2 log N) under the global lock (512 replica groups: 340 ms; with the counting pre-check below: see
-  // profiles/control_plane_bench_r2.json).
+  // quorum O(N^2 log N) under the global lock; the counting pre-check below skips it for joiners that cannot decide.
   bool may_decide = true;
   {
     const size_t np = state_.participants.size();

@@ -1,4 +1,4 @@
-// Fault-tolerant all-reduce over NVLink peer memory (sm_100a).
+// Fault-tolerant all-reduce over NVLink peer memory (sm_90a).
 //
 // Replaces the reference's `pg.allreduce([t], SUM)` + eager `t /= N`
 // (torchft/manager.py:466-478) with ONE kernel that
@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_twoshot_kernel(ARArgs a) {
     }
     const size_t lo = rank * slice + blockIdx.x * chunk;
     const size_t hi = min(min(lo + chunk, (size_t)(rank + 1) * slice), nvec);
-    // vectors in flight per thread: peer loads have ~2.5 us latency, so keep U*W >= 16 outstanding
+    // vectors in flight per thread: peer loads have microseconds of latency, so keep U*W >= 16 outstanding
     constexpr int U = (W >= 8) ? 2 : (W >= 3 ? 4 : 8);
     for (size_t base = lo; base < hi; base += (size_t)blockDim.x * U) {
       Vec16 in[U][W];
@@ -317,7 +317,7 @@ void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const vo
     // Degenerate quorum: out = scale * in (or zeros).
     const void* src = user_in ? user_in : (const char*)pt.data[0] + off;
     void* dst = user_out ? user_out : (char*)pt.data[0] + off;
-    const int g = (int)std::min<size_t>(1184, (nelem + 4095) / 4096 + 1);
+    const int g = (int)std::min<size_t>(kNumSMs * 8, (nelem + 4095) / 4096 + 1);
     switch (dtype) {
       case kF32:
         scale_copy_kernel<float><<<g, 512, 0, stream>>>((float*)dst, (const float*)src, nelem,

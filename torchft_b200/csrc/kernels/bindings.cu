@@ -156,9 +156,10 @@ bool can_access_peer(int dev, int peer) {
 void bind_vmm(py::module_& m);  // vmm.cu
 
 PYBIND11_MODULE(_K, m) {
-  m.doc() = "torchft_b200 data-plane kernels (sm_100a): P2P all-reduce, q8 all-reduce, heal copy, model ops";
+  m.doc() = "torchft_b200 data-plane kernels (sm_90a): P2P all-reduce, q8 all-reduce, heal copy, model ops";
   m.attr("MAX_RANKS") = kMaxRanks;
   m.attr("MAX_BLOCKS") = kMaxBlocks;
+  m.attr("NUM_SMS") = kNumSMs;
   m.attr("SIGNAL_CHANNELS") = kSignalChannels;
   m.attr("SIGNAL_PAD_BYTES") = sizeof(SignalPad);
   m.attr("Q8_GROUP") = 512;

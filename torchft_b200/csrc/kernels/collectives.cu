@@ -1,10 +1,10 @@
-// The rest of the c10d collective surface as peer-memory kernels (sm_100a): all-gather, broadcast,
+// The rest of the c10d collective surface as peer-memory kernels (sm_90a): all-gather, broadcast,
 // all-to-all (one "push exchange" kernel), reduce-scatter, and point-to-point send / recv.
 //
 // The reference forwards every one of these to a stock backend that is re-created per quorum
-// (/root/reference/torchft/process_group.py:510-629); its heal-over-process-group transport is built
-// on send/recv (/root/reference/torchft/checkpointing/pg_transport.py:214-303) and its quantised
-// reduce-scatter on alltoall (/root/reference/torchft/collectives.py:159-294). Here each is ONE launch
+// (upstream torchft/process_group.py:510-629); its heal-over-process-group transport is built
+// on send/recv (upstream torchft/checkpointing/pg_transport.py:214-303) and its quantised
+// reduce-scatter on alltoall (upstream torchft/collectives.py:159-294). Here each is ONE launch
 // that moves exactly the algorithmic bytes over NVLink with P2P stores/loads issued by the kernel:
 //
 //   push exchange   rank r stores what it owes peer p straight into p's staging slot r, one barrier,

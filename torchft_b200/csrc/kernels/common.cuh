@@ -1,4 +1,4 @@
-// Shared device helpers for the torchft_b200 data-plane kernels (sm_100a only).
+// Shared device helpers for the torchft_b200 data-plane kernels (sm_90a only).
 //
 // Everything here is header-only and free of torch/ATen dependencies: the
 // Python side hands us raw device pointers + CUDA stream handles, so this
@@ -14,8 +14,9 @@
 
 namespace tft {
 
-constexpr int kMaxRanks = 8;          // one NVSwitch domain (HGX B200)
-constexpr int kMaxBlocks = 296;       // 2 CTAs / SM * 148 SMs upper bound for comm grids
+constexpr int kMaxRanks = 8;          // one NVSwitch domain (HGX H100)
+constexpr int kNumSMs = 132;          // H100 SXM; sizes the grid caps of the bandwidth-bound kernels
+constexpr int kMaxBlocks = 2 * kNumSMs;  // 2 CTAs / SM upper bound for comm grids
 constexpr int kSignalChannels = 4;    // independent flag arrays (allreduce / q8 / heal / user)
 
 // dtype codes shared with Python (torchft_b200/ops/_dtypes.py)
@@ -59,8 +60,8 @@ struct PeerTable {
   SignalPad* pads[kMaxRanks];     // peer signal pads
   int rank;
   int world;
-  // Spin budget per wait, BY VALUE: run5 showed every waiter reading it (and the error word)
-  // from the host-mapped status block cost ~2 us per CTA, serialised over PCIe.
+  // Spin budget per wait, BY VALUE: every waiter reading it (and the error word) from the
+  // host-mapped status block would cost a PCIe round trip per CTA, serialised over PCIe.
   uint64_t timeout_ns;
 };
 
@@ -123,7 +124,7 @@ __device__ __forceinline__ void st_relaxed_sys(uint64_t* p, uint64_t v) {
 __device__ __forceinline__ bool wait_flag(const uint64_t* flag, uint64_t expected,
                                           StatusBlock* st, int peer, uint64_t budget_ns) {
   // Hot path touches ONLY the flag (local HBM/L2). The host-mapped status block (abort /
-  // latched error) is consulted every 256 polls (~10 us), the clock every 1024.
+  // latched error) is consulted every 256 polls, the clock every 1024.
   if (ld_relaxed_sys(flag) >= expected) return true;
   uint64_t t0 = 0;
   uint32_t spins = 0;

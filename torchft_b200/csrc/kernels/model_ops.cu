@@ -1,4 +1,4 @@
-// Fused bandwidth-bound model ops for the Llama training step (sm_100a):
+// Fused bandwidth-bound model ops for the Llama training step (sm_90a):
 // RMSNorm fwd/bwd, SwiGLU fwd/bwd, RoPE, softmax-cross-entropy fwd+bwd,
 // flat AdamW with fp32 master weights and a device-side commit gate.
 //
@@ -25,12 +25,10 @@ using P8 = Pack<bf16>;
 // kept PACKED in registers. The row-wide sum costs ONE __syncthreads (warp partials in a double-buffered smem line, every
 // thread adds the <= 16 partials itself), and with PF the next row's loads are issued before the current row's reduction so
 // a CTA always has a full row of 16 B loads in flight. Small CTAs (128 threads x 4 vectors) with 4 per SM keep ~64 KB per
-// SM in flight, which is what HBM3e needs (B200_PROFILING.md: ~40 KB/SM by Little's law); one 512-thread CTA with one
-// vector per thread and three barriers per row (round 1) reached 62 % (fwd) / 43 % (bwd) of the measured copy bandwidth.
+// SM in flight, more than HBM bandwidth times latency per SM (Little's law) asks for.
 constexpr int kRmsMaxVec = 4;
-// {forward, backward}: CTA threads, prefetch, CTAs per SM at 128 threads. Defaults from the B200 sweep at 8192 x 4096
-// (profiles/rmsnorm_sweep_r2.json): forward 128 x 4 vectors, 6 CTAs/SM = 0.77 of the measured copy bandwidth (was 0.61);
-// backward 256 x 2 vectors, 296 CTAs = 0.59 including the column-sum launch (was 0.43).
+// {forward, backward}: CTA threads, prefetch, CTAs per SM at 128 threads (rmsnorm_tune() overrides; bench/kernel_micro.py
+// sweeps them): forward 128 x 4 vectors at 6 CTAs/SM, backward 256 x 2 vectors at 4 CTAs/SM.
 static int g_rms_tpb[2] = {128, 256}, g_rms_pf[2] = {1, 1}, g_rms_cps[2] = {6, 4};
 
 template <int TPB>
@@ -213,8 +211,8 @@ __global__ void __launch_bounds__(TPB) rmsnorm_bwd_kernel(
 }
 
 // dw[h] (+)= sum_b partial[b][h]: a CTA owns 32 columns; its 32 warps stride over the partial rows (a warp load is one
-// 128 B line, up to 8 independent loads in flight per lane), then the 32 per-warp sums meet in shared memory. ncu of the
-// first version (8 warps, 4 loads in flight, 37 dependent rounds): 11.4 us for 4.9 MB -- a quarter of the whole backward.
+// 128 B line, up to 8 independent loads in flight per lane), then the 32 per-warp sums meet in shared memory. Fewer warps
+// with fewer loads in flight leave the column sum latency-bound: dozens of dependent rounds per CTA.
 __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ partial, int nb, int H,
                                                       bf16* __restrict__ dw, int accumulate) {
   __shared__ float acc[32][33];
@@ -291,8 +289,8 @@ __global__ void __launch_bounds__(512) swiglu_bwd_kernel(const bf16* __restrict_
 // in/out row strides in elements so q/k can be read straight out of the packed
 // qkv projection and written contiguous.
 // A thread keeps its vector-in-head index for the whole kernel and walks (token, head) "slots" two at a time (both 16 B
-// loads issued before either is used); all index math is 32-bit (round 1 did three 64-bit divisions per vector and had one
-// load in flight per thread: 60 % of the measured copy bandwidth).
+// loads issued before either is used); all index math is 32-bit (64-bit divisions per vector and a single load in flight
+// per thread leave the kernel latency-bound).
 __global__ void __launch_bounds__(256) rope_kernel(const bf16* __restrict__ in, bf16* __restrict__ out,
                                                    const float2* __restrict__ cs, unsigned nslots, unsigned S,
                                                    unsigned heads, unsigned D, size_t in_stride, size_t out_stride,
@@ -531,7 +529,7 @@ __global__ void __launch_bounds__(512, 2) adamw_kernel(AdamArgs a) {
 // DiLoCo outer step, fused: averaged pseudo-gradient -> Nesterov/momentum SGD on the last global weights ->
 // new global weights saved to the backup -> live weights = lerp(new global, local, alpha). The reference runs these
 // as four passes over the fragment (set grads, outer_optimizer.step(), save_parameters, _merge_parameters:
-// /root/reference/torchft/local_sgd.py:339-384,445-475); here every element is read and written once.
+// upstream torchft/local_sgd.py:339-384,445-475); here every element is read and written once.
 template <typename T>
 __global__ void __launch_bounds__(512, 2) diloco_outer_kernel(T* __restrict__ param, T* __restrict__ original,
                                                                const T* __restrict__ grad, float* __restrict__ mom,
@@ -632,9 +630,9 @@ __global__ void __launch_bounds__(512) heal_copy_kernel(const CopyEntry* __restr
     const size_t len = end - start;
     if ((((uintptr_t)s | (uintptr_t)d) & 15) == 0) {
       const size_t nv = len / 16;
-      // 8 x 16 B loads in flight per thread: a peer (NVLink) read has ~2-3 us latency, so
-      // one outstanding load per thread caps a 64-CTA copy at ~240 GB/s (run4); 8 per
-      // thread puts > 4 MB in flight and reaches link bandwidth.
+      // 8 x 16 B loads in flight per thread: a peer (NVLink) read has microseconds of latency,
+      // so one outstanding load per thread caps a 64-CTA copy far below link bandwidth; 8 per
+      // thread puts > 4 MB in flight, more than link bandwidth times peer latency.
       constexpr int U = 8;
       size_t v = threadIdx.x;
       for (; v + (size_t)(U - 1) * blockDim.x < nv; v += (size_t)U * blockDim.x) {
@@ -791,7 +789,7 @@ __global__ void __launch_bounds__(32) heal_copy_bulk_kernel(const CopyEntry* __r
 }
 
 // ------------------------------- launchers ----------------------------------
-static int grid_for(size_t work_items, int threads, int cap = 148 * 8) {
+static int grid_for(size_t work_items, int threads, int cap = kNumSMs * 8) {
   size_t g = (work_items + threads - 1) / threads;
   if (g < 1) g = 1;
   if (g > (size_t)cap) g = cap;
@@ -809,7 +807,7 @@ static void rms_shape(int nvec, int bwd, int& tpb, int& nv) {
   nv = kRmsMaxVec;
 }
 static int rms_grid(int rows, int bwd, int tpb) {
-  const int cap = 148 * std::max(1, g_rms_cps[bwd] * 128 / tpb);
+  const int cap = kNumSMs * std::max(1, g_rms_cps[bwd] * 128 / tpb);
   return rows < cap ? rows : cap;
 }
 
@@ -884,7 +882,7 @@ void rope_launch(const void* in, void* out, const void* cs, size_t T, int S, int
   if (T == 0) return;
   const unsigned vph = D / 8, per = 256 / vph, threads = per * vph;  // whole (token, head) slots per CTA pass
   const unsigned nslots = (unsigned)(T * heads);
-  const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), 148 * 8);
+  const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), kNumSMs * 8);
   rope_kernel<<<grid, threads, 0, s>>>((const bf16*)in, (bf16*)out, (const float2*)cs, nslots, (unsigned)S,
                                        (unsigned)heads, (unsigned)D, in_stride, out_stride, sign);
   TFT_CUDA_CHECK(cudaGetLastError());
@@ -920,7 +918,7 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
   a.dir = dir;
   const unsigned vph = D / 8, per = 256 / vph, threads = per * vph;
   const unsigned nslots = (unsigned)(T * heads);
-  const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), 148 * 8);
+  const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), kNumSMs * 8);
   rope_qkv_kernel<<<grid, threads, 0, s>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
@@ -938,16 +936,15 @@ void adamw_launch(void* p, float* master, float* m, float* v, const void* g, siz
                   float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale,
                   const int* gate, int max_blocks, cudaStream_t s) {
   AdamArgs a{(bf16*)p, master, m, v, (const bf16*)g, n, lr, b1, b2, eps, wd, bc1, bc2, gscale, gate};
-  // CTA-cap sweep at 1 Gi params (profiles/kernel_micro_adamw_caps.json): 148 -> 0.83, 592 -> 0.82,
-  // 1184 -> 0.89, 2368 -> 0.92 of measured HBM bandwidth: many short CTAs keep both resident slots of
-  // every SM refilled. max_blocks > 0 overrides.
-  adamw_kernel<<<grid_for(n / 8 + 1, 512, max_blocks > 0 ? max_blocks : 148 * 16), 512, 0, s>>>(a);
+  // Many short CTAs (16 per SM) keep both resident slots of every SM refilled; a CTA-cap sweep
+  // (bench/kernel_micro.py) reached the most HBM bandwidth at the largest cap. max_blocks > 0 overrides.
+  adamw_kernel<<<grid_for(n / 8 + 1, 512, max_blocks > 0 ? max_blocks : kNumSMs * 16), 512, 0, s>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
 void diloco_outer_launch(void* param, void* original, const void* grad, float* mom, size_t n, int dtype, float lr,
                          float mu, int nesterov, float alpha, const int* gate, cudaStream_t s) {
-  const int grid = grid_for(n / 4 + 1, 512, 148 * 16);
+  const int grid = grid_for(n / 4 + 1, 512, kNumSMs * 16);
   switch (dtype) {
     case kF32:
       diloco_outer_kernel<float><<<grid, 512, 0, s>>>((float*)param, (float*)original, (const float*)grad, mom, n, lr, mu,
@@ -967,7 +964,7 @@ void diloco_outer_launch(void* param, void* original, const void* grad, float* m
 }
 
 void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s) {
-  sumsq_kernel<<<grid_for(n / 8 + 1, 512, 148 * 4), 512, 0, s>>>((const bf16*)g, n, out);
+  sumsq_kernel<<<grid_for(n / 8 + 1, 512, kNumSMs * 4), 512, 0, s>>>((const bf16*)g, n, out);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -1,5 +1,5 @@
 // Group-wise FP8 (e4m3) quantisation kernels and the fused quantised
-// all-reduce over NVLink peer memory (sm_100a).
+// all-reduce over NVLink peer memory (sm_90a).
 //
 // Parity target: torchft/quantization.py (5 Triton kernels) +
 // torchft/collectives.py:297-415 (quantize -> alltoall -> reduce -> allgather
@@ -181,7 +181,7 @@ __global__ void __launch_bounds__(512) q8_dequantize_kernel(const char* qbuf, si
   const int lane = threadIdx.x & 31;
   const size_t warps = (size_t)gridDim.x * (blockDim.x >> 5);
   // a warp takes kU groups per pass and issues all their loads before the first use (one 16 B load in flight per lane
-  // measured 69 % of the copy bandwidth in round 1)
+  // leaves the pass latency-bound)
   constexpr int kU = 4;
   for (size_t g0 = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); g0 < ngroups;
        g0 += warps * kU) {
@@ -458,7 +458,7 @@ static int q8_grid(size_t ngroups, int max_blocks) {
 void q8_quantize_launch(const void* a, const void* b, size_t nelem, int dtype, int world,
                         void* qbuf, cudaStream_t stream) {
   const size_t ng = q8_ngroups(nelem, world);
-  const int grid = q8_grid(ng, 1184);
+  const int grid = q8_grid(ng, kNumSMs * 8);
   switch (dtype) {
     case kF32:
       q8_quantize_kernel<float><<<grid, 512, 0, stream>>>((const float*)a, (const float*)b, nelem,
@@ -480,7 +480,7 @@ void q8_quantize_launch(const void* a, const void* b, size_t nelem, int dtype, i
 void q8_dequantize_launch(const void* qbuf, size_t nelem, int dtype, int world, void* out,
                           cudaStream_t stream) {
   const size_t ng = q8_ngroups(nelem, world);
-  const int grid = q8_grid(ng, 1184);
+  const int grid = q8_grid(ng, kNumSMs * 8);
   switch (dtype) {
     case kF32:
       q8_dequantize_kernel<float><<<grid, 512, 0, stream>>>((const char*)qbuf, ng, (float*)out, nelem);
@@ -500,7 +500,7 @@ void q8_dequantize_launch(const void* qbuf, size_t nelem, int dtype, int world, 
 void q8_quantize_raw_launch(const void* a, const void* b, size_t nelem, size_t ngroups, int dtype, void* qbuf,
                             cudaStream_t stream) {
   if (ngroups == 0) return;
-  const int grid = q8_grid(ngroups, 1184);
+  const int grid = q8_grid(ngroups, kNumSMs * 8);
   switch (dtype) {
     case kF32:
       q8_quantize_kernel<float><<<grid, 512, 0, stream>>>((const float*)a, (const float*)b, nelem, ngroups, (char*)qbuf);
@@ -520,7 +520,7 @@ void q8_quantize_raw_launch(const void* a, const void* b, size_t nelem, size_t n
 void q8_dequantize_raw_launch(const void* qbuf, size_t ngroups, void* out, size_t nelem, int dtype,
                               cudaStream_t stream) {
   if (ngroups == 0 || nelem == 0) return;
-  const int grid = q8_grid(ngroups, 1184);
+  const int grid = q8_grid(ngroups, kNumSMs * 8);
   switch (dtype) {
     case kF32: q8_dequantize_kernel<float><<<grid, 512, 0, stream>>>((const char*)qbuf, ngroups, (float*)out, nelem); break;
     case kBF16:
@@ -535,7 +535,7 @@ void q8_dequantize_raw_launch(const void* qbuf, size_t ngroups, void* out, size_
 void q8_reduce_raw_launch(const void* const* srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo,
                           size_t g_hi, float post_scale, void* dst, cudaStream_t stream) {
   if (g_hi <= g_lo) return;
-  const int grid = q8_grid(g_hi - g_lo, 1184);
+  const int grid = q8_grid(g_hi - g_lo, kNumSMs * 8);
   q8_reduce_kernel<<<grid, 512, 0, stream>>>((const char* const*)srcs_dev, nsrc, first, ngroups, g_lo, g_hi,
                                              post_scale, (char*)dst);
   TFT_CUDA_CHECK(cudaGetLastError());
@@ -545,7 +545,7 @@ void q8_reduce_launch(const void* const* srcs_dev, int world, int rank, size_t n
                       float post_scale, void* dst, cudaStream_t stream) {
   const size_t ng = q8_ngroups(nelem, world);
   const size_t slice = ng / world;
-  const int grid = q8_grid(slice, 1184);
+  const int grid = q8_grid(slice, kNumSMs * 8);
   q8_reduce_kernel<<<grid, 512, 0, stream>>>((const char* const*)srcs_dev, world, rank, ng,
                                              rank * slice, (rank + 1) * slice, post_scale,
                                              (char*)dst);

@@ -1,8 +1,8 @@
-// FT-ZeRO-1: the partitioned optimizer update fused into the cross-replica collectives (sm_100a).
+// FT-ZeRO-1: the partitioned optimizer update fused into the cross-replica collectives (sm_90a).
 //
 // The reference all-reduces every gradient, divides by N on the host side and then runs the FULL
 // optimizer on every replica, gated by a host-synchronous should_commit
-// (/root/reference/torchft/manager.py:466-478, /root/reference/torchft/optim.py:52-55). Here the
+// (upstream torchft/manager.py:466-478, upstream torchft/optim.py:52-55). Here the
 // replicated dimension also partitions the optimizer:
 //
 //   backward :  per unit (transformer block), on the comm stream, overlapped with backward:
@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
 
 // ---------------------------------------------------------------------------
 // Commit verdict on the device (replaces current-stream synchronize + should_commit RPC for
-// replica groups of one rank, /root/reference/torchft/manager.py:884-903).
+// replica groups of one rank, upstream torchft/manager.py:884-903).
 // ---------------------------------------------------------------------------
 struct CommitArgs {
   PeerTable pt;        // pads only
@@ -348,7 +348,7 @@ void launch_upd(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
 }
 
 void check_grid(int blocks, int threads, const char* who) {
-  if (blocks < 1 || blocks > 148 * 32) throw std::runtime_error(std::string(who) + ": bad grid");
+  if (blocks < 1 || blocks > kNumSMs * 32) throw std::runtime_error(std::string(who) + ": bad grid");
   if (threads < 32 || threads > 512 || (threads & 31)) throw std::runtime_error(std::string(who) + ": bad block size");
 }
 

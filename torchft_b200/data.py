@@ -1,4 +1,4 @@
-"""Data sharding across replica groups (reference: /root/reference/torchft/data.py:24-77).
+"""Data sharding across replica groups (reference: upstream torchft/data.py:24-77).
 
 Fault tolerance keeps the WORLD elastic, so the dataset is sharded over the
 *maximum* grid ``num_replica_groups x num_replicas``; when a replica group is down

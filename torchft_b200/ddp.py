@@ -1,9 +1,9 @@
 """Fault-tolerant data parallelism across replica groups.
 
 * :class:`DistributedDataParallel` / :class:`PureDistributedDataParallel` -- API
-  parity with /root/reference/torchft/ddp.py:31-104 (torch DDP bucket hook /
+  parity with upstream torchft/ddp.py:31-104 (torch DDP bucket hook /
   per-parameter hooks feeding ``Manager.allreduce``).
-* :class:`FlatDistributedDataParallel` -- the B200-native path: all gradients live
+* :class:`FlatDistributedDataParallel` -- the native path: all gradients live
   in ONE flat bf16 buffer inside NVLink-symmetric memory; backward fills it
   front-to-back and each bucket is all-reduced IN PLACE by the fused P2P kernel
   on the process group's comm stream the moment its last gradient lands, so the

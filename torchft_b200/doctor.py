@@ -1,7 +1,7 @@
 """``python -m torchft_b200.doctor [--lighthouse http://host:29510]`` — is this box ready for the native data plane?
 
 Prints one line per check (OK / WARN / FAIL) and exits non-zero when something REQUIRED for the requested mode is
-missing: native extensions built and importable, CUDA devices and their compute capability (sm_100 expected), peer
+missing: native extensions built and importable, CUDA devices and their compute capability (sm_90 expected), peer
 access between every GPU pair (the peer-memory collectives need it), NVSwitch multicast support (NVLS kernels, VMM
 mode), shared-memory / file-descriptor limits that the fd-passing path needs, and — optionally — whether a Lighthouse
 answers. Every probe is independent and never raises.
@@ -66,8 +66,8 @@ def run(lighthouse: str = "", require_gpu: bool = False) -> List[Check]:
         def devices() -> Tuple[str, str]:
             caps = {torch.cuda.get_device_capability(i) for i in range(ngpu)}
             names = {torch.cuda.get_device_name(i) for i in range(ngpu)}
-            ok = caps == {(10, 0)}
-            return ("OK" if ok else "FAIL"), f"{ngpu} x {', '.join(sorted(names))}, compute capability {sorted(caps)} (kernels are built for sm_100a only)"
+            ok = caps == {(9, 0)}
+            return ("OK" if ok else "FAIL"), f"{ngpu} x {', '.join(sorted(names))}, compute capability {sorted(caps)} (kernels are built for sm_90a only)"
 
         def peers() -> Tuple[str, str]:
             bad = [(i, j) for i in range(ngpu) for j in range(ngpu) if i != j and not torch.cuda.can_device_access_peer(i, j)]

@@ -1,6 +1,6 @@
 """Job launch helpers: one torchrun role per replica group.
 
-Parity with the reference's torchx component ``hsdp`` (/root/reference/torchft/torchx.py:17-89):
+Parity with the reference's torchx component ``hsdp`` (upstream torchft/torchx.py:17-89):
 each replica group is launched as its own ``torchrun`` with ``--master_port=29600+id`` and the
 environment ``REPLICA_GROUP_ID`` / ``NUM_REPLICA_GROUPS`` / ``TORCHFT_LIGHTHOUSE``; process
 restarts are delegated to torchelastic's ``--max_restarts``. torchx is not available in this

@@ -1,6 +1,6 @@
 """Communication-efficient fault-tolerant algorithms: LocalSGD and (Streaming) DiLoCo.
 
-Semantics follow /root/reference/torchft/local_sgd.py (context managers driven by
+Semantics follow upstream torchft/local_sgd.py (context managers driven by
 inner-optimizer step hooks; quorum at the start of every sync window; on any
 failure the window is discarded and parameters reset to the last global copy;
 DiLoCo needs a synchronous quorum; fragments sync round-robin, prepared
@@ -8,7 +8,7 @@ DiLoCo needs a synchronous quorum; fragments sync round-robin, prepared
 mixes local and global weights; the backup copy and the outer optimizer travel
 with live heals).
 
-What is different (B200-first):
+What is different (native):
 
 * every fragment keeps its pseudo-gradients in ONE flat buffer; parameters see
   views of it, so "bucketization" is a slicing decision, not a pack/unpack copy
@@ -218,7 +218,7 @@ class _StreamingDiLoCoFragment:
             self.original_parameters[name] = t
         # persistent pseudo-gradient buffers in NVLink-symmetric memory (zero-copy / in-switch all-reduce)
         self._symm_flat: Dict[Tuple[torch.dtype, torch.device], torch.Tensor] = {}
-        # B200 fast path (see _try_flat_mode): the fragment is ONE flat buffer end to end
+        # Native fast path (see _try_flat_mode): the fragment is ONE flat buffer end to end
         self._flat_param: Optional[torch.Tensor] = None
         self._flat_orig: Optional[torch.Tensor] = None
         self._flat_grad: Optional[torch.Tensor] = None

@@ -1,7 +1,7 @@
 """Per-rank fault-tolerance state machine.
 
 One ``Manager`` per training process. A training step is three calls (semantics of
-/root/reference/torchft/manager.py:148-1053, SURVEY.md 3.2 and 7.4):
+upstream torchft/manager.py:148-1053, SURVEY.md 3.2 and 7.4):
 
 1. ``start_quorum()``  -- async by default (overlaps the forward pass): intra-group barrier + Lighthouse
    quorum through the C++ ``ManagerServer``; when the quorum id changed the process group is
@@ -13,7 +13,7 @@ One ``Manager`` per training process. A training step is three calls (semantics 
 
    * ``should_commit()`` -- the reference's host-synchronous form: drain the stream, AND over the ranks
      of the group through the ManagerServer, return a bool.
-   * ``commit_on_device(committer)`` -- B200-native form for replica groups of ONE rank: the verdict is
+   * ``commit_on_device(committer)`` -- native form for replica groups of ONE rank: the verdict is
      computed by a kernel (``zero1_commit_kernel``: AND of "no latched error, enough participants" over
      the quorum through the NVLink signal pads), lands in a device gate word that the fused optimizer
      kernels test, and the host learns it LAZILY -- on the quorum thread at the next ``start_quorum``,

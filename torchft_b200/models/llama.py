@@ -1,8 +1,8 @@
 """Llama-3 family decoder for the fault-tolerant training benchmarks.
 
 The reference ships no model: its flagship config (BASELINE.json, "Llama-3 8B
-fault-tolerant HSDP bf16") borrows torchtitan's. This is our own B200-first
-implementation, laid out for one-GPU-per-replica training in 180 GB of HBM3e:
+fault-tolerant HSDP bf16") borrows torchtitan's. This is our own implementation,
+laid out for one-GPU-per-replica training in the 80 GB of an H100:
 
 * every parameter is a view into ONE flat bf16 buffer and every gradient a view
   into ONE flat bf16 gradient buffer that can live in NVLink-symmetric memory,
@@ -10,7 +10,7 @@ implementation, laid out for one-GPU-per-replica training in 180 GB of HBM3e:
   and AdamW is a single launch over the whole model;
 * q/k/v and gate/up projections are fused GEMMs (cuBLAS);
 * RMSNorm, RoPE(+qkv split), SwiGLU, softmax-cross-entropy and AdamW are
-  hand-written sm_100a kernels (``torchft_b200/csrc/kernels/model_ops.cu``);
+  hand-written sm_90a kernels (``torchft_b200/csrc/kernels/model_ops.cu``);
 * normalised activations and the SwiGLU product are recomputed in backward
   instead of stored (see ``ops.fused.norm_linear`` / ``swiglu_linear``);
 * attention is the SDPA library kernel (flash / cuDNN), causal, GQA.

@@ -1,4 +1,4 @@
-"""Loader for the sm_100a data-plane extension ``torchft_b200._K``.
+"""Loader for the sm_90a data-plane extension ``torchft_b200._K``.
 
 The extension is built in-tree by ``torchft_b200._build`` (see
 ``__graft_entry__.build``). On a box with a GPU a missing extension is a hard
@@ -80,7 +80,7 @@ def load() -> Any:
             except Exception as e:  # pragma: no cover - build toolchain missing
                 _err = e
                 raise ImportError(
-                    "torchft_b200._K (sm_100a kernels) is not built and could not be built: "
+                    "torchft_b200._K (sm_90a kernels) is not built and could not be built: "
                     f"{first!r} / {e!r}. Run `python -m torchft_b200._build`."
                 ) from e
         _K = _Counting(mod)

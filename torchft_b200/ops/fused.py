@@ -1,4 +1,4 @@
-"""Autograd wrappers over the hand-written sm_100a model kernels.
+"""Autograd wrappers over the hand-written sm_90a model kernels.
 
 RMSNorm / SwiGLU / RoPE / chunked linear-cross-entropy / flat AdamW. All take
 bf16 CUDA tensors, reduce in fp32 and make one pass over HBM per direction.

@@ -6,7 +6,7 @@ Two sinks, both opt-in through the environment:
 * ``TORCHFT_USE_OTEL=true`` -- ship records through OpenTelemetry (OTLP + console),
   with per-logger resource attributes from the JSON file named by
   ``TORCHFT_OTEL_RESOURCE_ATTRIBUTES_JSON`` (same switches as the reference,
-  /root/reference/torchft/otel.py:44-103). Needs the ``opentelemetry`` SDK; a clear
+  upstream torchft/otel.py:44-103). Needs the ``opentelemetry`` SDK; a clear
   error is raised if it is requested but missing.
 * ``TORCHFT_B200_EVENTS_JSONL=/path/file.jsonl`` -- dependency-free JSON-lines sink
   (one object per quorum / commit / error event with job_id, replica_id, rank,

@@ -1,7 +1,7 @@
 """Fault-tolerant HSDP trainer: FSDP2 shards INSIDE a replica group, torchft_b200 ACROSS groups.
 
 BASELINE.json config 2 ("4 replica groups x 2-GPU FSDP shards"), wired the way the reference composes it
-(/root/reference/torchft/fsdp_test.py:57-72, README.md:62-69): ``fully_shard`` over the group's own mesh,
+(upstream torchft/fsdp_test.py:57-72, README.md:62-69): ``fully_shard`` over the group's own mesh,
 ``set_all_reduce_hook`` so every reduce-scattered gradient shard is averaged across replica groups through a
 ``ManagedProcessGroup`` (-> ``Manager.allreduce`` -> the fused NVLink all-reduce kernel on ``ProcessGroupB200``, with
 the 1/num_participants scale and the zero contribution of healing groups inside the kernel), one Manager per rank,

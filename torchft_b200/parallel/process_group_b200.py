@@ -1,12 +1,12 @@
-"""``ProcessGroupB200`` -- the B200-native fault-tolerant process group.
+"""``ProcessGroupB200`` -- the native fault-tolerant process group.
 
 Where the reference re-creates an NCCL communicator per quorum
-(/root/reference/torchft/process_group.py:435-471,848-873) and funnels every
+(upstream torchft/process_group.py:435-471,848-873) and funnels every
 gradient byte through NCCL (manager.py:466-468), this group
 
 * keeps CUDA context, streams, symmetric segments and signal pads alive across
   quorums and only *remaps peer handles* in ``configure`` (sub-millisecond);
-* runs every collective as ONE hand-written sm_100a kernel over NVLink peer memory (P2P loads +
+* runs every collective as ONE hand-written sm_90a kernel over NVLink peer memory (P2P loads +
   stores, epoch-tagged flags, bounded abortable spins) on a dedicated comm stream: all-reduce
   (one-/two-shot, NVLS) with the 1/N scale, dtype handling and the non-participant zero
   contribution fused; all-gather, broadcast and all-to-all (equal or per-peer splits) as a push exchange
@@ -117,7 +117,7 @@ class ProcessGroupB200(ProcessGroup):
                  device: Optional[torch.device] = None) -> None:
         super().__init__(0, 1)
         if not torch.cuda.is_available():
-            raise RuntimeError("ProcessGroupB200 needs a CUDA device (sm_100a); use ProcessGroupGloo on CPU")
+            raise RuntimeError("ProcessGroupB200 needs a CUDA device (sm_90a); use ProcessGroupGloo on CPU")
         self._timeout = timeout
         self._device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         self._comm = SymmetricComm(self._device, staging_bytes=staging_bytes, timeout=timeout)

@@ -1,6 +1,6 @@
 """NVLink peer-memory manager + collectives for one replica-group rank.
 
-This is the B200-native replacement for "destroy and re-create the NCCL
+This is the native replacement for "destroy and re-create the NCCL
 communicator on every quorum change" (reference:
 torchft/process_group.py:435-471,848-873). The CUDA context, streams, local
 segments and the signal pad survive reconfiguration; ``configure()`` only
@@ -41,7 +41,7 @@ _CH_Q8 = 1
 _CH_HEAL = 2
 _CH_USER = 3
 
-_ALIGN = 2 << 20  # segment sizes rounded to 2 MiB (TLB page granularity on Blackwell)
+_ALIGN = 2 << 20  # segment sizes rounded to 2 MiB (the VMM allocation granularity on H100)
 
 
 class _CAI:
@@ -111,7 +111,7 @@ class SymmetricComm:
         self._recv_seq: Dict[int, int] = {}
         self._pad_bytes = (self._K.SIGNAL_PAD_BYTES + 65535) // 65536 * 65536
         self._max_blocks = max(1, min(int(os.environ.get("TORCHFT_B200_AR_BLOCKS", "64")), self._K.MAX_BLOCKS))
-        self._q8_max_blocks = 148  # phases A/C of the fp8 kernel are local HBM passes: use the whole chip
+        self._q8_max_blocks = self._K.NUM_SMS  # phases A/C of the fp8 kernel are local HBM passes: use the whole chip
         self._threads = int(os.environ.get("TORCHFT_B200_AR_THREADS", "512"))
         self._oneshot_max = int(os.environ.get("TORCHFT_B200_ONESHOT_KB", "256")) << 10
         # "vmm": cuMemCreate-backed segments (survive exporter death, NVLS-capable); "ipc": cudaMalloc + cudaIpc
@@ -398,7 +398,7 @@ class SymmetricComm:
     def _plan(self, nbytes: int) -> Tuple[int, int]:
         """(algo, blocks): identical on every rank for a given message size.
 
-        Table from ``bench/comm_tune.py`` on B200 (profiles/comm_tune_*.json). One-shot (each
+        Thresholds from a ``bench/comm_tune.py`` sweep on an earlier NVLink generation; not re-measured on H100. One-shot (each
         rank reads the whole message from every peer; two flag exchanges, no write-back hop)
         wins while (world-1) x bytes still fits the latency budget; it likes MANY small CTAs
         (16 KB each, <= 64 KB because results stay in registers across the closing barrier).
@@ -419,8 +419,7 @@ class SymmetricComm:
     @staticmethod
     def _default_nvls_min(world: int) -> int:
         """In-switch reduction moves ~(1 + 1/N)·S per link direction, the P2P two-shot 2(N-1)/N·S: equal at
-        N=4 (measured: no gain), 1.5x worse at N=2 (measured 2.71 vs 1.67 ms per GiB), 1.3x better at N=8
-        (measured 2.28 vs 2.98 ms per GiB, ahead from 256 KB; profiles/comm_bench_vmm_nvls_8gpu.json)."""
+        N=4, 1.5x worse at N=2, 1.3x better at N=8, so NVLS is used from 5 ranks (and from 256 KB) up."""
         return (256 << 10) if world >= 5 else (1 << 62)
 
     def _next_flag(self) -> int:
@@ -524,13 +523,13 @@ class SymmetricComm:
                 if name.endswith("_q8") and seg.nbytes >= need and name in self._tables:
                     table = self._tables[name]
                     ngroups = self._K.q8_ngroups(n, self._world)
-                    big = max(1, min(148 * 16, ngroups // 16 + 1))
+                    big = max(1, min(self._K.NUM_SMS * 16, ngroups // 16 + 1))
                     if contribute:
                         K.q8_quantize_raw(a.data_ptr(), b.data_ptr() if b is not None else 0, n, ngroups, dt, seg.ptr, sp)
                     else:
                         K.memset_async(seg.ptr, 0, q_bytes, sp)  # zero scales: this replica adds nothing
                     self._handshake(2, True, _CH_Q8, sp)
-                    K.q8_slice_reduce(table, self._z1_ok(2), 0, q_bytes, n, scale, max(1, min(148 * 8, ngroups // self._world // 16 + 1)), sp)
+                    K.q8_slice_reduce(table, self._z1_ok(2), 0, q_bytes, n, scale, max(1, min(self._K.NUM_SMS * 8, ngroups // self._world // 16 + 1)), sp)
                     self._handshake(2, True, _CH_Q8, sp)
                     K.q8_gather_dequant(table, self._z1_ok(2), q_bytes, n, dt, out.data_ptr(), big, sp)
                     self.launches += 3
@@ -775,7 +774,7 @@ class SymmetricComm:
                 # healing / spare replica: its gradients count as zeros (reference manager.py:441-442)
                 self._K.memset_async(self._segments[segment].ptr + off, 0, nelem * 2, sp)
             self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
-            blocks = max(1, min(blocks, 148 * 32, (nelem // 8 + 511) // 512))
+            blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_reduce(self._tables[segment], self._z1_ok(0), self._mc_base(segment, nelem * 2), off, nelem, scale,
                                  replication, blocks, self._threads, sp)
             self.launches += 1
@@ -812,7 +811,7 @@ class SymmetricComm:
                 raise RuntimeError("SymmetricComm is not configured")
             lr, b1, b2, eps, wd = hyper
             sp = _native.stream_ptr(stream)
-            blocks = max(1, min(blocks, 148 * 32, (nelem // 8 + 511) // 512))
+            blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp)
             self.launches += 1

@@ -14,11 +14,11 @@ Two pipelines over the same model code (``models/llama.py``):
 
 ``backend="nccl"`` -- the reference-equivalent arm: stock ``ProcessGroupNCCL`` re-created per quorum,
 per-bucket all-reduce SUM then ``/N``, host-synchronous ``should_commit`` RPC, full AdamW on every
-replica (/root/reference/torchft/manager.py:466-478,884-903, /root/reference/torchft/optim.py:52-55).
+replica (upstream torchft/manager.py:466-478,884-903, upstream torchft/optim.py:52-55).
 ``backend="b200"`` with ``zero1=False`` runs that same classic structure on the native all-reduce kernels.
 
 This is the HSDP configuration of BASELINE.json with shard degree 1: every GPU is one replica group holding
-the full bf16 model (180 GB of HBM3e), and the replicated dimension is both the fault-tolerance dimension
+the full bf16 model and its training state (on an 80 GB H100: up to ~3 B parameters), and the replicated dimension is both the fault-tolerance dimension
 (README.md:37-42 of the reference) and -- new here -- the dimension the optimizer is partitioned over.
 """
 

@@ -1,8 +1,8 @@
 """FT-ZeRO-1: optimizer state partitioned across REPLICA GROUPS, without giving up fault tolerance.
 
 The reference keeps the full optimizer on every replica and all-reduces every gradient
-(/root/reference/torchft/manager.py:466-478, /root/reference/torchft/optim.py:52-55). Here the
-cross-replica collective and the optimizer are one pipeline of three hand-written sm_100a kernels
+(upstream torchft/manager.py:466-478, upstream torchft/optim.py:52-55). Here the
+cross-replica collective and the optimizer are one pipeline of three hand-written sm_90a kernels
 (``csrc/kernels/zero1.cu``):
 
 * backward:  ``reduce_scatter`` per unit (one transformer block = one unit), overlapped with backward;
@@ -186,7 +186,7 @@ class Zero1Optimizer:
         # the big kernels are sync-free, so their grids are free parameters: the reduce-scatter is NVLink-latency bound
         # and shares the SMs with backward; the update is HBM-bound and likes many short CTAs (cf. the AdamW cap sweep)
         self._rs_blocks = int(os.environ.get("TORCHFT_B200_Z1_RS_BLOCKS", 128))
-        self._upd_blocks = int(os.environ.get("TORCHFT_B200_Z1_UPD_BLOCKS", blocks or 2368))
+        self._upd_blocks = int(os.environ.get("TORCHFT_B200_Z1_UPD_BLOCKS", blocks or self._K.NUM_SMS * 16))
         self.param = pg.alloc_symmetric("z1_param", numel * 2).view(torch.bfloat16)
         self.grad = pg.alloc_symmetric("z1_grad", numel * 2).view(torch.bfloat16)
         self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)

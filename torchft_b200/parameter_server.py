@@ -1,6 +1,6 @@
 """Prototype parameter server on reconfigurable process groups.
 
-Parity: /root/reference/torchft/parameter_server.py:30-194. A client GETs
+Parity: upstream torchft/parameter_server.py:30-194. A client GETs
 ``/new_session`` and receives ``{"session_id", "store_addr"}``; both sides then
 configure a fresh 2-rank group (server = rank 0, client = rank 1) under that
 store prefix and the server runs :meth:`forward` for the session. The Lighthouse

@@ -3,13 +3,13 @@
 Every class here is a ``torch.distributed.ProcessGroup`` whose membership can
 change at runtime through :meth:`ProcessGroup.configure` (one call per quorum
 change) and whose failures surface as a *latched error* (:meth:`errored`)
-instead of a crashed process. API parity: /root/reference/torchft/process_group.py.
+instead of a crashed process. API parity: upstream torchft/process_group.py.
 
 =========================  =====================================================
-``ProcessGroupB200``       B200-native: collectives are hand-written sm_100a
+``ProcessGroupB200``       native: collectives are hand-written sm_90a
                            kernels over NVLink peer memory; ``configure`` remaps
-                           peer handles (~0.2 ms) instead of re-creating a
-                           communicator (~0.8 s); no NCCL on the hot path.
+                           peer handles instead of re-creating a
+                           communicator; no NCCL on the hot path.
 ``ProcessGroupNCCL``       reference-equivalent baseline: stock c10d NCCL
                            destroyed/re-created per quorum, user-space timeouts
                            + ``abort`` (reference :780-891).
@@ -23,7 +23,7 @@ wrappers                   ``ErrorSwallowingProcessGroupWrapper``,
 =========================  =====================================================
 
 Intel XPU twins (``ProcessGroupXCCL``) are intentionally absent: this framework
-targets sm_100a only.
+targets sm_90a only.
 """
 
 from __future__ import annotations
@@ -525,8 +525,8 @@ class ProcessGroupNCCL(ProcessGroupWrapper):
 class ProcessGroupXCCL(ProcessGroupWrapper):
     """Reconfigurable XCCL group for Intel XPUs (reference: process_group.py:894-1002).
 
-    API-parity component only: this package's compute and collective kernels are sm_100a CUDA and nothing here is
-    exercised on a B200. The wrapper follows the reference's shape -- per-quorum communicator over the prefixed store,
+    API-parity component only: this package's compute and collective kernels are sm_90a CUDA and nothing here is
+    exercised on an H100. The wrapper follows the reference's shape -- per-quorum communicator over the prefixed store,
     user-space timeouts that call ``abort`` -- and needs a torch build with XCCL (``torch.distributed.is_xccl_available()``);
     ``configure`` raises a clear error otherwise.
     """
@@ -545,7 +545,7 @@ class ProcessGroupXCCL(ProcessGroupWrapper):
 
     def _create_pg(self, store: Store, rank: int, world_size: int) -> BaseProcessGroup:
         if not self.available():
-            raise RuntimeError("ProcessGroupXCCL needs a PyTorch build with XCCL and an Intel XPU; on NVIDIA B200 use "
+            raise RuntimeError("ProcessGroupXCCL needs a PyTorch build with XCCL and an Intel XPU; on NVIDIA H100 use "
                                "ProcessGroupB200 (native NVLink kernels) or ProcessGroupNCCL")
         from torch.distributed import ProcessGroupXCCL as _XCCL  # type: ignore[attr-defined]
 

@@ -1,4 +1,4 @@
-"""FP8 (e4m3) quantisation primitives -- sm_100a CUDA kernels, not Triton.
+"""FP8 (e4m3) quantisation primitives -- sm_90a CUDA kernels, not Triton.
 
 API parity with the reference's ``torchft/quantization.py`` (three host
 functions around five Triton kernels): :func:`fused_quantize_into_fp8`,

@@ -20,7 +20,7 @@ __all__ = ["hsdp", "hsdp_spec"]
 def hsdp(*script_args: str, replicas: int = 2, workers_per_replica: int = 1, max_restarts: int = 10,
          script: str = "train_ddp.py", env: Optional[Dict[str, str]] = None, image: str = "",
          h: Optional[str] = None, cpu: int = 2, gpu: int = 0, memMB: int = 1024) -> Any:
-    """Build a ``torchx.specs.AppDef`` for fault-tolerant HSDP on B200 nodes.
+    """Build a ``torchx.specs.AppDef`` for fault-tolerant HSDP on H100 nodes.
 
     Args mirror the reference component; ``h`` is a torchx named resource, otherwise
     ``cpu/gpu/memMB`` are used. Raises ``ImportError`` when torchx is not installed.

@@ -1,4 +1,4 @@
-"""Small device helpers (reference: torchft/utils.py:17-67). CUDA only -- this framework targets B200."""
+"""Small device helpers (reference: torchft/utils.py:17-67). CUDA only -- this framework targets H100."""
 
 from __future__ import annotations
 
