@@ -10,6 +10,12 @@ Single GPU, for ncu / compute-sanitizer (ranks emulated in-process, flags pre-si
 
     ncu --set full -k regex:zero1 ... python bench/zero1_bench.py --virtual 8 --mb 64 --iters 2
 
+``--virtual W --compact`` times the update with flat state and with paged state (compact optimizer state: 64 Ki-element
+pages in a pool behind a page table, once in slot order and once in a random slot order) in the same process,
+alternating the three ``--repeats`` times; it
+reports the median and the spread of each. The peer stores hit local HBM there, so this compares the state addressing,
+not NVLink.
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -66,6 +72,63 @@ def run_rank(comm, nelem, k, rs_blocks, upd_blocks, iters, warmup, sync, reduce_
     return out
 
 
+def compact_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats, shift=16):
+    """Gated AdamW + weight push of one unit on flat state vs the same values in page pools, timed alternately: pages in
+    slot order (what a re-shard into an empty pool produces) and in a random slot order (a pool that has been through
+    many re-shards). All three must agree bit for bit."""
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
+    dev = comm.device
+    grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
+    grad.normal_()
+    gate = torch.ones(2, dtype=torch.int32, device=dev)
+    npages = (nelem + (1 << shift) - 1) >> shift
+    flat = [torch.randn(nelem, device=dev), torch.zeros(nelem, device=dev), torch.zeros(nelem, device=dev)]
+    layouts = {}
+    for name, table in (("ordered", torch.arange(npages, device=dev)), ("random", torch.randperm(npages, device=dev))):
+        idx = (table.long()[:, None] * (1 << shift) + torch.arange(1 << shift, device=dev)).view(-1)[:nelem]
+        pool = [torch.zeros(npages << shift, device=dev) for _ in flat]
+        for p, x in zip(pool, flat):
+            p[idx] = x
+        layouts[name] = (table.int(), idx, pool)
+
+    def upd_flat():
+        comm.zero1_update_("z1_param", 0, grad.data_ptr(), flat[0].data_ptr(), flat[1].data_ptr(), flat[2].data_ptr(), nelem,
+                           HP, gate, k, 0, upd_blocks)
+
+    def upd_paged(layout):
+        table, _, pool = layouts[layout]
+        return lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), pool[0].data_ptr(), pool[1].data_ptr(),
+                                          pool[2].data_ptr(), nelem, HP, gate, k, 0, upd_blocks, None, table.data_ptr(), 0,
+                                          shift)
+
+    arms = (("flat", upd_flat), ("paged_ordered", upd_paged("ordered")), ("paged_random", upd_paged("random")))
+    for _, fn in arms:
+        fn()
+    torch.cuda.synchronize()
+    same = all(torch.equal(p[idx], x) for _, idx, pool in layouts.values() for p, x in zip(pool, flat))
+    times = {name: [] for name, _ in arms}
+    for _ in range(repeats):
+        for name, fn in arms:
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    out = {"paged_equals_flat": same, "timing": "local HBM (virtual ranks), not NVLink"}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        out[f"adamw_allgather_{name}_ms"] = {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4),
+                                             "max": round(ts[-1], 4)}
+    for name in ("paged_ordered", "paged_random"):
+        out[f"{name}_over_flat"] = round(out[f"adamw_allgather_{name}_ms"]["median"] / out["adamw_allgather_flat_ms"]["median"], 4)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--mb", type=float, default=436.0, help="unit size in MB of bf16 gradients (one Llama-3-8B block = 436 MB)")
@@ -75,6 +138,8 @@ def main() -> None:
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--virtual", type=int, default=0, help="emulate this many ranks on ONE GPU (presignalled; for ncu)")
+    ap.add_argument("--compact", action="store_true", help="--virtual: A/B the update on flat vs paged optimizer state")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact: alternations of the flat and the paged timing")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -84,6 +149,15 @@ def main() -> None:
         torch.cuda.set_device(0)
         comms = SymmetricComm.virtual_world(a.virtual, {"z1_grad": S, "z1_param": S}, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
+        if a.compact:
+            res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
+            res["gpu"] = torch.cuda.get_device_name(0)
+            print("ZERO1_BENCH " + json.dumps(res), flush=True)
+            if a.out:
+                os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+                with open(a.out, "w") as f:
+                    json.dump(res, f, indent=1)
+            return
         for c in comms[:1]:  # rank 0's kernels are representative; every rank does the same work
             res.update(run_rank(c, nelem, a.replication, a.rs_blocks, a.upd_blocks, a.iters, a.warmup, torch.cuda.synchronize, lambda x: x))
         print("ZERO1_BENCH " + json.dumps(res), flush=True)

@@ -26,7 +26,9 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
 // zero1.cu -------------------------------------------------------------------
 // FT-ZeRO-1: one-CTA handshake (flag exchange with every peer, result mirrored to a device word), sync-free
 // reduce-scatter body (+ buddy push), device-side commit verdict, sync-free gated AdamW fused with the all-gather of the
-// new bf16 weights. mc_base != nullptr selects the NVLS (multimem) data path.
+// new bf16 weights. mc_base != nullptr selects the NVLS (multimem) data path. A non-null `table` selects paged
+// optimizer state: master/m/v are pools of 2^page_shift-element pages, element soff + i of the unit lives in page
+// table[(soff + i) >> page_shift]; a null table keeps flat addressing (state indexed like the unit).
 void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
                             int barrier_mode, cudaStream_t stream);
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
@@ -35,7 +37,8 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
                          int host_ok, int exchange, cudaStream_t stream);
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
-                         int replication, int mode, int blocks, int threads, cudaStream_t stream);
+                         int replication, int mode, int blocks, int threads, cudaStream_t stream,
+                         const int* table = nullptr, size_t soff = 0, int page_shift = 0);
 
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);

@@ -248,13 +248,15 @@ PYBIND11_MODULE(_K, m) {
       "zero1_update",
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,
          uintptr_t v, size_t nelem, float lr, float b1, float b2, float eps, float wd, int replication, int mode,
-         int blocks, int threads, uintptr_t stream) {
+         int blocks, int threads, uintptr_t stream, uintptr_t table, size_t soff, int page_shift) {
         zero1_update_launch(pt.pt, P<void>(mc_base), P<const int>(gate), poff, P<void>(grad), P<float>(master), P<float>(mm),
-                            P<float>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream));
+                            P<float>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream),
+                            P<const int>(table), soff, page_shift);
       },
       py::arg("pt"), py::arg("mc_base"), py::arg("gate"), py::arg("poff"), py::arg("grad"), py::arg("master"),
       py::arg("m"), py::arg("v"), py::arg("nelem"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"),
-      py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("blocks"), py::arg("threads"), py::arg("stream"));
+      py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("blocks"), py::arg("threads"), py::arg("stream"),
+      py::arg("table") = 0, py::arg("soff") = 0, py::arg("page_shift") = 0);
 
   m.def(
       "push_exchange",

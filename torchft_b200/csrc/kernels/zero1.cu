@@ -244,9 +244,15 @@ struct UpdArgs {
   float lr, b1, b2, eps, wd;
   int replication;
   int mode;            // 0 = gated update + push, 1 = refresh (re-broadcast bf16(master) of the primary slice, ungated)
+  // paged state (PAGED = true): master/m/v are page pools; element e of the flat vector (e = soff + local index)
+  // lives at pool[table[e >> page_shift] << page_shift | (e & (page - 1))]. A page is a multiple of 8 elements, so
+  // the two 16-byte vectors of one 8-element group never straddle a page.
+  const int* table;
+  size_t soff;
+  int page_shift;
 };
 
-template <int W, bool NVLS>
+template <int W, bool NVLS, bool PAGED>
 __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   if (a.mode == 0 && a.gate[0] == 0) return;  // uniform over the grid AND (unanimous verdict) over the quorum
   const int rank = a.pt.rank;
@@ -270,14 +276,26 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   for (int j = 0; j < (a.mode == 0 ? k : 1); ++j) {
     const int s = (rank - j + W) % W;  // j = 0: primary slice, j > 0: slices this rank backs up
     const size_t lo = g.lo(s), hi = g.hi(s);
+    // paged: the slot of the NEXT iteration's page is loaded one iteration ahead, so the state loads never wait for a
+    // dependent table load (a grid-stride step is larger than a page: every iteration is a different page)
+    const size_t pmask = (size_t(1) << a.page_shift) - 1;
+    int slot = 0;
+    if constexpr (PAGED) {
+      if (lo + tid < hi) slot = __ldg(a.table + ((a.soff + (lo + tid) * 8) >> a.page_shift));
+    }
     for (size_t v = lo + tid; v < hi; v += nthreads) {
+      size_t si = v * 8;  // index of the 8-element group in the state arrays
+      if constexpr (PAGED) {
+        si = ((size_t)slot << a.page_shift) | ((a.soff + v * 8) & pmask);
+        if (v + nthreads < hi) slot = __ldg(a.table + ((a.soff + (v + nthreads) * 8) >> a.page_shift));
+      }
       float w[8];
-      const Vec16 w0 = ld_stream(a.master + v * 8), w1 = ld_stream(a.master + v * 8 + 4);
+      const Vec16 w0 = ld_stream(a.master + si), w1 = ld_stream(a.master + si + 4);
       if (a.mode == 0) {
         // all 7 x 16 B loads in flight before any use
         const Vec16 gv = ld_stream(a.grad + v * 8);
-        const Vec16 m0 = ld_stream(a.m + v * 8), m1 = ld_stream(a.m + v * 8 + 4);
-        const Vec16 v0 = ld_stream(a.v + v * 8), v1 = ld_stream(a.v + v * 8 + 4);
+        const Vec16 m0 = ld_stream(a.m + si), m1 = ld_stream(a.m + si + 4);
+        const Vec16 v0 = ld_stream(a.v + si), v1 = ld_stream(a.v + si + 4);
         float gr[8], m[8], vv[8];
         P8::unpack(gv, gr);
         Pack<float>::unpack(w0, w);
@@ -293,12 +311,12 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
           const float denom = sqrtf(vv[i]) * inv_bc2_sqrt + a.eps;
           w[i] = w[i] * decay - step_size * __fdividef(m[i], denom);
         }
-        st_stream(a.master + v * 8, Pack<float>::pack(w));
-        st_stream(a.master + v * 8 + 4, Pack<float>::pack(w + 4));
-        st_stream(a.m + v * 8, Pack<float>::pack(m));
-        st_stream(a.m + v * 8 + 4, Pack<float>::pack(m + 4));
-        st_stream(a.v + v * 8, Pack<float>::pack(vv));
-        st_stream(a.v + v * 8 + 4, Pack<float>::pack(vv + 4));
+        st_stream(a.master + si, Pack<float>::pack(w));
+        st_stream(a.master + si + 4, Pack<float>::pack(w + 4));
+        st_stream(a.m + si, Pack<float>::pack(m));
+        st_stream(a.m + si + 4, Pack<float>::pack(m + 4));
+        st_stream(a.v + si, Pack<float>::pack(vv));
+        st_stream(a.v + si + 4, Pack<float>::pack(vv + 4));
       } else {
         Pack<float>::unpack(w0, w);
         Pack<float>::unpack(w1, w + 4);
@@ -332,17 +350,17 @@ void launch_rs(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
   }
 }
 
-template <bool NVLS>
+template <bool NVLS, bool PAGED>
 void launch_upd(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
   switch (a.pt.world) {
-    case 1: zero1_update_kernel<1, false><<<blocks, threads, 0, s>>>(a); break;
-    case 2: zero1_update_kernel<2, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_update_kernel<3, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_update_kernel<4, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_update_kernel<5, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_update_kernel<6, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_update_kernel<7, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_update_kernel<8, NVLS><<<blocks, threads, 0, s>>>(a); break;
+    case 1: zero1_update_kernel<1, false, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 2: zero1_update_kernel<2, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 3: zero1_update_kernel<3, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 4: zero1_update_kernel<4, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 5: zero1_update_kernel<5, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 6: zero1_update_kernel<6, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 7: zero1_update_kernel<7, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
+    case 8: zero1_update_kernel<8, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
     default: throw std::runtime_error("zero1_update: world size must be in [1, 8]");
   }
 }
@@ -383,15 +401,24 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
 
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
-                         int replication, int mode, int blocks, int threads, cudaStream_t stream) {
+                         int replication, int mode, int blocks, int threads, cudaStream_t stream, const int* table,
+                         size_t soff, int page_shift) {
   check_grid(blocks, threads, "zero1_update");
   if ((poff & 15) || (nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
+  if (table != nullptr && (page_shift < 3 || page_shift > 30 || (soff & 7)))
+    throw std::runtime_error("zero1_update: pages must be 2^3 .. 2^30 elements and the unit 8-element aligned");
   UpdArgs a{pt, reinterpret_cast<char*>(mc_base), gate, poff, reinterpret_cast<const bf16*>(grad), master, m, v,
-            nelem, lr, b1, b2, eps, wd, replication, mode};
-  if (mc_base != nullptr)
-    launch_upd<true>(a, blocks, threads, stream);
-  else
-    launch_upd<false>(a, blocks, threads, stream);
+            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift};
+  if (table != nullptr) {
+    if (mc_base != nullptr)
+      launch_upd<true, true>(a, blocks, threads, stream);
+    else
+      launch_upd<false, true>(a, blocks, threads, stream);
+  } else if (mc_base != nullptr) {
+    launch_upd<true, false>(a, blocks, threads, stream);
+  } else {
+    launch_upd<false, false>(a, blocks, threads, stream);
+  }
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

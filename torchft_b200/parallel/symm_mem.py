@@ -130,6 +130,7 @@ class SymmetricComm:
         self.launches = 0  # native kernel launches issued (bench reports this)
         self._ptrs: Dict[str, List[int]] = {}  # segment -> mapped base pointer per quorum rank
         self._z1_ok_buf: Optional[torch.Tensor] = None
+        self._aliased = False  # a virtual rank whose user segments are rank 0's (virtual_world(alias=True)): it frees none
         self._commit_seq = 0
         self._hostname = socket.gethostname()
 
@@ -300,7 +301,7 @@ class SymmetricComm:
     @staticmethod
     def virtual_world(world: int, segments: Dict[str, int], device: Optional[torch.device] = None,
                       presignal: bool = True, timeout: timedelta = timedelta(seconds=10),
-                      staging_bytes: int = 8 << 20) -> "List[SymmetricComm]":
+                      staging_bytes: int = 8 << 20, alias: bool = False) -> "List[SymmetricComm]":
         """``world`` ranks of ONE quorum inside this process, all on ``device`` (testing / self-check harness).
 
         Every rank gets its own segments and signal pad; the peer tables point at each other directly (no IPC).
@@ -310,30 +311,67 @@ class SymmetricComm:
         process, one kernel at a time, which is what profilers (ncu serialises launches), compute-sanitizer and
         the one-GPU test tier need. With ``presignal=False`` the ranks synchronise for real and must be launched
         concurrently on different streams.
+
+        ``alias=True`` (pre-signalled only) allocates ``segments`` on rank 0 alone and points every peer entry at rank 0's
+        segment: one GPU then holds a model whose W-rank quorum would not fit W times. The FT-ZeRO-1 kernels stay correct
+        on such aliases, since each thread reads all sources of its 16-byte vector before it writes that vector and every
+        push stores bits identical to the ones already there; what the aliased peers compute is not meaningful.
         """
+        if alias and not presignal:
+            raise ValueError("aliased virtual ranks share one buffer and cannot signal each other")
         comms = [SymmetricComm(device, staging_bytes=staging_bytes, timeout=timeout) for _ in range(world)]
-        for c in comms:
+        for r, c in enumerate(comms):
             c._mode = "ipc"
             # all ranks share ONE GPU: with real signalling every CTA of every rank must be resident at once
             c._max_blocks = c._q8_max_blocks = max(2, 112 // world)
             c._ensure_core()
-            for name, nbytes in segments.items():
-                c._alloc_segment(name, nbytes)
-        names = list(comms[0]._segments)
-        ptrs = {n: [c._segments[n].ptr for c in comms] for n in names}
-        for r, c in enumerate(comms):
-            pads = None
-            if presignal:
+            c._aliased = alias and r > 0
+        for name, nbytes in segments.items():
+            SymmetricComm._virtual_segment(comms, name, nbytes)
+        if presignal:
+            for c in comms:
                 # own pad: every slot reads "arrived" (>= any flag) and "verdict ok" (odd) forever; the flags this rank
                 # publishes go to a private sink instead of the peers' pads, so nothing ever un-signals a slot
                 pad = c._segments["core"].tensor[: c._K.SIGNAL_PAD_BYTES].view(torch.int64)
                 pad.fill_((1 << 62) | 1)
                 c._sink = torch.zeros(c._K.SIGNAL_PAD_BYTES, dtype=torch.uint8, device=c.device)
-                pads = [c._segments["core"].ptr if t == r else c._sink.data_ptr() for t in range(world)]
-            c._install({n: list(v) for n, v in ptrs.items()}, r, world, epoch=1, floor=0, pads=pads)
-            c._configured = True
+            SymmetricComm.virtual_quorum(comms)
+        else:
+            ptrs = {n: [c._segments[n].ptr for c in comms] for n in comms[0]._segments}
+            for r, c in enumerate(comms):
+                c._install({n: list(v) for n, v in ptrs.items()}, r, world, epoch=1, floor=0)
+                c._configured = True
         torch.cuda.synchronize(comms[0].device)
         return comms
+
+    @staticmethod
+    def _virtual_segment(comms: "List[SymmetricComm]", name: str, nbytes: int) -> None:
+        for c in comms:
+            if c._aliased:
+                c._segments[name] = comms[0]._segments[name]
+            else:
+                c._alloc_segment(name, nbytes)
+
+    @staticmethod
+    def virtual_alloc(comms: "List[SymmetricComm]", name: str, nbytes: int) -> torch.Tensor:
+        """Add segment ``name`` to a pre-signalled virtual world after it was built (on rank 0 only when the peers are
+        aliases) and re-point every rank's peer tables; returns rank 0's uint8 view."""
+        SymmetricComm._virtual_segment(comms, name, nbytes)
+        SymmetricComm.virtual_quorum(comms)
+        return comms[0]._segments[name].tensor[:nbytes]
+
+    @staticmethod
+    def virtual_quorum(comms: "List[SymmetricComm]", members: Optional[List[int]] = None, epoch: int = 1) -> None:
+        """Make the pre-signalled virtual ranks ``members`` (indices into ``comms``, default all) one quorum, in that
+        rank order: the in-process analogue of ``configure`` after a membership change."""
+        members = list(range(len(comms))) if members is None else list(members)
+        world = len(members)
+        ptrs = {n: [comms[m]._segments[n].ptr for m in members] for n in comms[members[0]]._segments}
+        for rank, m in enumerate(members):
+            c = comms[m]
+            pads = [c._segments["core"].ptr if t == rank else c._sink.data_ptr() for t in range(world)]
+            c._install({n: list(v) for n, v in ptrs.items()}, rank, world, epoch=epoch, floor=0, pads=pads)
+            c._configured = True
 
     def segment(self, name: str) -> torch.Tensor:
         """uint8 view of this rank's segment ``name``."""
@@ -802,10 +840,14 @@ class SymmetricComm:
 
     def zero1_update_(self, segment: str, poff: int, grad: int, master: int, m: int, v: int, nelem: int,
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,
-                      blocks: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+                      blocks: int, stream: Optional[torch.cuda.Stream] = None, table: int = 0, state_off: int = 0,
+                      page_shift: int = 0) -> None:
         """Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights into
         ``segment`` on the ranks that do not hold it (``mode`` 1: ungated re-broadcast of bf16(master) to everybody, no
-        state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed."""
+        state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed.
+
+        ``table`` (device pointer to int32 page slots, 0 = flat state) selects paged state: ``master``/``m``/``v`` are
+        then page pools and element ``state_off + i`` of the unit lives in pool page ``table[(state_off + i) >> page_shift]``."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -813,7 +855,8 @@ class SymmetricComm:
             sp = _native.stream_ptr(stream)
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
-                                 m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp)
+                                 m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp,
+                                 table, state_off, page_shift)
             self.launches += 1
             pushes = self._world > 1 and (mode == 1 or self._world > replication)
             if pushes:
@@ -880,6 +923,8 @@ class SymmetricComm:
             assert not self._configured, "shutdown() first"
             torch.cuda.synchronize(self.device)
             for seg in self._segments.values():
+                if self._aliased and seg.name != "core":
+                    continue  # rank 0 of the virtual world owns it
                 seg.tensor = torch.empty(0, dtype=torch.uint8)
                 try:
                     if self._mode == "vmm":

@@ -51,6 +51,8 @@ class FaultTolerantTrainer:
         zero1: partition the optimizer over the replicas and commit on the device (default for ``b200``;
             env ``TORCHFT_B200_ZERO1=0`` turns it off)
         replication: holders per slice of optimizer state (``k`` of FT-ZeRO-1)
+        compact_state: FT-ZeRO-1: store only the held slices of the optimizer state, in page pools sized for every
+            quorum of ``min_replica_size`` to 8 replicas (``None``: env ``TORCHFT_B200_Z1_COMPACT=1`` turns it on)
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -62,7 +64,8 @@ class FaultTolerantTrainer:
                  timeout: timedelta = timedelta(seconds=60), device: Optional[torch.device] = None,
                  activation_checkpoint: Optional[str] = None, init_sync: bool = False,
                  use_async_quorum: bool = True, overlap_optimizer: Optional[bool] = None,
-                 optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2) -> None:
+                 optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2,
+                 compact_state: Optional[bool] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -99,7 +102,8 @@ class FaultTolerantTrainer:
 
             # the optimizer owns the five symmetric flat buffers; FlatParams adopts two of them. Units (= gradient
             # buckets = update launches) are the forward stages, known once the parameters have offsets.
-            self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None)
+            self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
+                                       compact=compact_state, min_world=min_replica_size)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:

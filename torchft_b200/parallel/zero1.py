@@ -40,7 +40,10 @@ logger = logging.getLogger(__name__)
 
 Range = Tuple[int, int]
 
-__all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls"]
+__all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
+           "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges"]
+
+PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -152,25 +155,121 @@ def plan_pulls(need: Sequence[Range], holdings: Dict[int, Sequence[Range]], me: 
     return pulls, left
 
 
+# --------------------------------------------------------------------------- compact (paged) state
+def page_ranges(rs: Sequence[Range], shift: int) -> List[Range]:
+    """Page indices (as merged half-open ranges) that element ranges ``rs`` touch, for pages of ``2**shift`` elements."""
+    return merge_ranges([(lo >> shift, ((hi - 1) >> shift) + 1) for lo, hi in rs if hi > lo])
+
+
+def backed_ranges(rs: Sequence[Range], pages: Sequence[Range], shift: int) -> List[Range]:
+    """The parts of element ranges ``rs`` that lie in ``pages`` (page-index ranges of ``2**shift`` elements)."""
+    return intersect_ranges(rs, [(lo << shift, hi << shift) for lo, hi in pages])
+
+
+def reshard_page_steps(old_pages: Sequence[Range], new_pages: Sequence[Range], source_pages: Sequence[Range]
+                       ) -> Tuple[List[Range], List[Range], List[Range]]:
+    """The page sets of one rank's compact re-shard, in the order it applies them: ``(free_first, allocate,
+    free_last)``. ``free_first`` are the old pages that are neither kept nor read by a peer, ``allocate`` the new pages
+    it did not have, and ``free_last`` the old pages kept only for peers, which go once every peer has pulled."""
+    free_first = subtract_ranges(old_pages, merge_ranges(list(new_pages) + list(source_pages)))
+    allocate = subtract_ranges(new_pages, old_pages)
+    free_last = intersect_ranges(subtract_ranges(source_pages, new_pages), old_pages)
+    return free_first, allocate, free_last
+
+
+def plan_reshard(layout: ShardLayout, peers: Dict[int, Tuple[int, Sequence[Range]]], world: int
+                 ) -> Tuple[int, Dict[int, Tuple[List[Range], List[Tuple[int, int, int]], List[Range]]]]:
+    """Every rank's re-shard for a new quorum, from what each rank published (``peers[r] = (t, holdings)``): the
+    update count ``tmax`` the quorum agrees on and ``{rank: (need, pulls, lost)}``. Only holdings at ``tmax`` count;
+    a rank that missed an update holds nothing. This is what each rank of :class:`Zero1Optimizer` plans for itself, so
+    any rank can tell which of its ranges its peers are about to read."""
+    tmax = max(int(t) for t, _ in peers.values())
+    valid = {r: list(h) for r, (t, h) in peers.items() if int(t) == tmax}
+    plans = {}
+    for r in range(world):
+        need = subtract_ranges(layout.held(r, world), valid.get(r, []))
+        pulls, lost = plan_pulls(need, {q: h for q, h in valid.items() if q != r}, r)
+        plans[r] = (need, pulls, lost)
+    return tmax, plans
+
+
+def reshard_pages(layout: ShardLayout, plans: Dict[int, Tuple[List[Range], List[Tuple[int, int, int]], List[Range]]],
+                  old_pages: Dict[int, Sequence[Range]], world: int, shift: int) -> Dict[int, Tuple[List[Range], List[Range], int]]:
+    """Per rank ``(new_pages, source_pages, peak)`` of a compact re-shard: the pages it holds afterwards, the pages of
+    its old state that peers pull from, and the most pages it has allocated at once when it frees every page that is
+    neither kept nor a source before it allocates, and frees the sources only after every peer has pulled."""
+    sources: Dict[int, List[Range]] = {r: [] for r in range(world)}
+    for _, pulls, _ in plans.values():
+        for src, lo, hi in pulls:
+            sources[src].append((lo, hi))
+    out = {}
+    for r in range(world):
+        new = page_ranges(layout.held(r, world), shift)
+        src = page_ranges(sources[r], shift)
+        out[r] = (new, src, total(merge_ranges(new + intersect_ranges(old_pages.get(r, []), src))))
+    return out
+
+
+def pool_pages(layout: ShardLayout, min_world: int, page: int = 1 << PAGE_SHIFT, max_world: int = 8) -> int:
+    """Pages per state array that let every rank hold its slices at every world in ``[min_world, max_world]`` and ride
+    through every single-member loss or join between those worlds (the re-shard peak), for steady-state holders
+    that are all up to date."""
+    shift = page.bit_length() - 1
+    assert page == 1 << shift and page % 8 == 0, "a page is a power of two and a multiple of 8 elements"
+    if not 1 <= min_world <= max_world:
+        raise ValueError(f"min_world must be in [1, {max_world}]")
+
+    def held_pages(world: int) -> List[List[Range]]:
+        return [page_ranges(layout.held(r, world), shift) for r in range(world)]
+
+    best = max(total(p) for w in range(min_world, max_world + 1) for p in held_pages(w))
+    for w in range(min_world, max_world + 1):
+        old = [layout.held(r, w) for r in range(w)]
+        old_pg = held_pages(w)
+        transitions = []
+        if w - 1 >= min_world:  # member ``d`` is lost
+            transitions += [[(1, old[r], old_pg[r]) for r in range(w) if r != d] for d in range(w)]
+        if w + 1 <= max_world:  # a member with no state joins at quorum rank ``j``
+            transitions += [[(1, old[r], old_pg[r]) for r in range(j)] + [(0, [], [])] + [(1, old[r], old_pg[r]) for r in range(j, w)]
+                            for j in range(w + 1)]
+        for members in transitions:
+            nw = len(members)
+            _, plans = plan_reshard(layout, {r: (t, h) for r, (t, h, _) in enumerate(members)}, nw)
+            pages = reshard_pages(layout, plans, {r: pg for r, (_, _, pg) in enumerate(members)}, nw, shift)
+            best = max(best, max(pk for _, _, pk in pages.values()))
+    return best
+
+
 # --------------------------------------------------------------------------- the optimizer
 class Zero1Optimizer:
     """AdamW with fp32 master/m/v partitioned over the replicas of the current quorum (see module doc).
 
     All five flat buffers live in NVLink-symmetric segments of the process group: ``param`` and ``grad``
     (bf16; written/read by peers every step) and ``master``/``m``/``v`` (fp32; read by peers only when
-    ownership moves). The state arrays are full-size and addressed by GLOBAL element index -- only the
+    ownership moves). By default the state arrays are full-size and addressed by GLOBAL element index -- only the
     held ranges are kept up to date -- which makes re-sharding a plain ranged copy.
+
+    With ``compact=True`` the state arrays are pools of fixed-size pages instead, and a page table maps each page of
+    the flat vector that this rank holds to a pool slot: a rank stores only about ``k/W`` of the state. The pool is
+    sized for every world in ``[min_world, 8]`` including the re-shard peaks between them (:func:`pool_pages`); a quorum
+    below ``min_world`` or a plan that does not fit raises instead of dropping state. A compact re-shard completes
+    inside ``configure`` (it frees and reuses pages, so it synchronises with its peers before it returns).
 
     Args:
         pg: a ``ProcessGroupB200`` (symmetric segments must be allocated before its first ``configure``)
         numel: elements of the flat parameter vector (multiple of 8)
         units: element ranges in FORWARD order that tile ``[0, numel)`` (one per transformer block)
         replication: holders per slice (``k``); ``min(k, world)`` is used
+        compact: paged state (``None``: env ``TORCHFT_B200_Z1_COMPACT=1`` turns it on)
+        min_world: compact: the smallest quorum the pool must hold the state for
+        state_pages: compact: pool size in pages, overriding :func:`pool_pages`
+        page_shift: compact: pages of ``2**page_shift`` elements
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
                  betas: Tuple[float, float] = (0.9, 0.95), eps: float = 1e-8, weight_decay: float = 0.1,
-                 replication: int = 2, blocks: Optional[int] = None) -> None:
+                 replication: int = 2, blocks: Optional[int] = None, compact: Optional[bool] = None, min_world: int = 1,
+                 state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT) -> None:
         from torchft_b200.ops import _native
 
         assert numel % 8 == 0
@@ -187,15 +286,30 @@ class Zero1Optimizer:
         # and shares the SMs with backward; the update is HBM-bound and likes many short CTAs (cf. the AdamW cap sweep)
         self._rs_blocks = int(os.environ.get("TORCHFT_B200_Z1_RS_BLOCKS", 128))
         self._upd_blocks = int(os.environ.get("TORCHFT_B200_Z1_UPD_BLOCKS", blocks or self._K.NUM_SMS * 16))
+        if compact is None:
+            compact = os.environ.get("TORCHFT_B200_Z1_COMPACT", "0") == "1"
+        self.compact = bool(compact)
+        self.min_world = int(min_world)
         self.param = pg.alloc_symmetric("z1_param", numel * 2).view(torch.bfloat16)
         self.grad = pg.alloc_symmetric("z1_grad", numel * 2).view(torch.bfloat16)
-        self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
-        self.m = pg.alloc_symmetric("z1_m", numel * 4).view(torch.float32)
-        self.v = pg.alloc_symmetric("z1_v", numel * 4).view(torch.float32)
+        if not self.compact:
+            self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
+            self.m = pg.alloc_symmetric("z1_m", numel * 4).view(torch.float32)
+            self.v = pg.alloc_symmetric("z1_v", numel * 4).view(torch.float32)
+        else:
+            if not 1 <= self.min_world <= 8:
+                raise ValueError("min_world must be in [1, 8]")
+            self._page_shift = int(page_shift)
+            self._page = 1 << self._page_shift
+            if self._page < 8:
+                raise ValueError("a page holds at least 8 elements")
+            self._state_pages = state_pages
+            self.capacity = 0  # pool pages per state array, fixed by set_units (they decide the re-shard peak)
         # gate[0]: verdict of the last commit, gate[1]: applied updates (AdamW's t), both written on the device
         self.gate = torch.zeros(2, dtype=torch.int32, device=self.device)
         self.t = 0                       # host mirror of gate[1] (advanced when a verdict is resolved)
-        self._holdings: List[Range] = [(0, numel)]  # identical seed on every replica => everything valid at t = 0
+        # identical seed on every replica => everything valid at t = 0 (compact: seeded on the pages held at the first quorum)
+        self._holdings: List[Range] = [] if self.compact else [(0, numel)]
         self._lock = threading.Lock()
         self._reshard_stream = torch.cuda.Stream(device=self.device)
         self._reshard_event: Optional[torch.cuda.Event] = None
@@ -213,12 +327,39 @@ class Zero1Optimizer:
         """Fix the unit ranges (forward order, tiling ``[0, numel)``); call before the first quorum."""
         assert all(lo % 8 == 0 and hi % 8 == 0 for lo, hi in units)
         assert merge_ranges(units) == [(0, self.numel)] and total(units) == self.numel, "units must tile the flat buffer exactly"
+        if self.compact and self.capacity:
+            raise RuntimeError("compact state: the units are fixed once the page pools are allocated")
         self.layout = ShardLayout(tuple((int(a), int(b)) for a, b in units), self._replication)
+        if self.compact:
+            self._alloc_pools()
+
+    def _alloc_pools(self) -> None:
+        import numpy as np
+
+        cap = self._state_pages
+        if cap is None:
+            cap = pool_pages(self.layout, self.min_world, self._page)
+        self.capacity = int(cap)
+        n = self.capacity * self._page
+        if n >= self.numel:
+            logger.warning("zero1: compact state pools of %d pages are not smaller than full-size state (min_world=%d "
+                           "means a rank may have to hold everything): no memory is saved", self.capacity, self.min_world)
+        self.master = self.pg.alloc_symmetric("z1_master", n * 4).view(torch.float32)[:n]
+        self.m = self.pg.alloc_symmetric("z1_m", n * 4).view(torch.float32)[:n]
+        self.v = self.pg.alloc_symmetric("z1_v", n * 4).view(torch.float32)[:n]
+        npages = (self.numel + self._page - 1) >> self._page_shift
+        self._table_host = np.full(npages, -1, dtype=np.int32)  # page of the flat vector -> pool slot (-1: not held)
+        self._table = torch.full((npages,), -1, dtype=torch.int32, device=self.device)
+        self._free: List[int] = list(range(self.capacity - 1, -1, -1))  # pop() hands out the lowest slot
 
     # ------------------------------------------------------------------ init / heal
     @torch.no_grad()
     def seed_master(self) -> None:
-        """Call once after the bf16 weights were initialised (same seed on every replica)."""
+        """Call once after the bf16 weights were initialised (same seed on every replica). Compact state is seeded
+        from the weights at the first quorum, when the rank's slices are known."""
+        if self.compact:
+            self._seed(self._holdings)
+            return
         self.master.copy_(self.param)
         self.m.zero_()
         self.v.zero_()
@@ -249,11 +390,19 @@ class Zero1Optimizer:
                 # quorum (segments allocated later only become symmetric at the NEXT quorum change)
                 raise RuntimeError(f"FT-ZeRO-1 segments {missing} are not mapped on every replica of this quorum")
             me = {"t": self.t, "hold": self._holdings}
+            if self.compact:
+                if world < self.min_world:
+                    raise RuntimeError(f"zero1: a quorum of {world} is below min_world={self.min_world}; the compact "
+                                       f"state pools ({self.capacity} pages) are not sized for it")
+                me["pages"] = self._page_runs()
             store.set(f"z1/{rank}", json.dumps(me))
             peers: Dict[int, Dict[str, Any]] = {rank: me}
             for r in range(world):
                 if r != rank:
                     peers[r] = json.loads(bytes(store.get(f"z1/{r}")).decode())
+            if self.compact:
+                self._reshard_compact(store, rank, world, peers)
+                return
             tmax = max(int(p["t"]) for p in peers.values())
             if self.t < tmax:
                 self._holdings = []  # we missed an update: nothing we hold is current
@@ -290,6 +439,125 @@ class Zero1Optimizer:
             for src, lo, hi in pulls:
                 entries.append((ptrs[src] + lo * 4, local.data_ptr() + lo * 4, (hi - lo) * 4))
         device_copy(entries, torch.cuda.current_stream(), chunk_bytes=1 << 20)
+
+    # ------------------------------------------------------------------ compact (paged) state
+    def _page_runs(self) -> List[Tuple[int, int, int]]:
+        """The page table as ``(page, slot, count)`` runs of consecutive pages in consecutive slots."""
+        runs: List[List[int]] = []
+        for pg in map(int, (self._table_host >= 0).nonzero()[0]):
+            slot = int(self._table_host[pg])
+            if runs and runs[-1][0] + runs[-1][2] == pg and runs[-1][1] + runs[-1][2] == slot:
+                runs[-1][2] += 1
+            else:
+                runs.append([pg, slot, 1])
+        return [tuple(r) for r in runs]
+
+    def _pieces(self, table: Any, lo: int, hi: int) -> List[Tuple[int, int, int]]:
+        """``[lo, hi)`` cut at page boundaries as ``(elem_lo, elem_hi, pool_index)``, pieces in consecutive slots merged."""
+        out: List[Tuple[int, int, int]] = []
+        sh, mask = self._page_shift, self._page - 1
+        e = lo
+        while e < hi:
+            end = min(hi, ((e >> sh) + 1) << sh)
+            slot = int(table[e >> sh])
+            assert slot >= 0, f"zero1: element {e} is not mapped to a pool page"
+            at = (slot << sh) | (e & mask)
+            if out and out[-1][1] == e and out[-1][2] + (e - out[-1][0]) == at:
+                out[-1] = (out[-1][0], end, out[-1][2])
+            else:
+                out.append((e, end, at))
+            e = end
+        return out
+
+    def _free_pages(self, pages: Sequence[Range]) -> None:
+        for plo, phi in pages:
+            for pg in range(plo, phi):
+                slot = int(self._table_host[pg])
+                if slot >= 0:
+                    self._free.append(slot)
+                    self._table_host[pg] = -1
+        self._free.sort(reverse=True)
+
+    def _alloc_pages(self, pages: Sequence[Range]) -> None:
+        for plo, phi in pages:
+            for pg in range(plo, phi):
+                if self._table_host[pg] < 0:
+                    self._table_host[pg] = self._free.pop()
+
+    @torch.no_grad()
+    def _seed(self, ranges: Sequence[Range]) -> None:
+        """``master = float(param)``, ``m = v = 0`` on ``ranges`` (current stream)."""
+        for lo, hi in ranges:
+            for a, b, at in self._pieces(self._table_host, lo, hi):
+                self.master[at:at + b - a].copy_(self.param[a:b])
+                self.m[at:at + b - a].zero_()
+                self.v[at:at + b - a].zero_()
+
+    def _reshard_compact(self, store: Any, rank: int, world: int, peers: Dict[int, Dict[str, Any]]) -> None:
+        """Move to this quorum's slices inside the page pools. Every rank derives every peer's plan from the published
+        ``{t, hold, pages}``, so it knows which of its old pages are sources: it frees the pages that are neither kept
+        nor a source, allocates its new pages, pulls (one copy launch), waits for its pulls, meets its peers at a store
+        barrier, and only then frees the pages it kept for them."""
+        import numpy as np
+
+        from torchft_b200.checkpointing.p2p_transport import device_copy
+
+        sh = self._page_shift
+        info = {r: (int(p["t"]), [tuple(x) for x in p["hold"]]) for r, p in peers.items()}
+        old = {r: merge_ranges([(pg, pg + n) for pg, _, n in p["pages"]]) for r, p in peers.items()}
+        tmax, plans = plan_reshard(self.layout, info, world)
+        pages = reshard_pages(self.layout, plans, old, world, sh)
+        peak = max(pk for _, _, pk in pages.values())
+        if peak > self.capacity:
+            # every rank sees the same plans and raises alike, before anything is freed
+            raise RuntimeError(f"zero1: re-sharding to a quorum of {world} needs {peak} state pages on one rank, the "
+                               f"pools hold {self.capacity} (raise min_world's range or state_pages)")
+        need, pulls, lost = plans[rank]
+        new_pages, src_pages, _ = pages[rank]
+        mine_old = old[rank]
+        free_first, allocate, free_last = reshard_page_steps(mine_old, new_pages, src_pages)
+        s = self._reshard_stream
+        s.wait_stream(self._commit_stream)  # no update of the old quorum may still touch a page that is about to move
+        self._free_pages(free_first)
+        # from here on a failure (a peer dying before the barrier) leaves this rank at its old t: it must not claim
+        # ranges whose pages it gave back, or a later quorum would pull (or keep) state that is no longer there
+        kept = subtract_ranges(mine_old, free_first)
+        self._holdings = backed_ranges(self._holdings, kept, sh)
+        self._alloc_pages(allocate)
+        with torch.cuda.stream(s):
+            self._table.copy_(torch.from_numpy(self._table_host))
+            if pulls:
+                ptabs = {}
+                for src in {p[0] for p in pulls}:
+                    t = np.full(len(self._table_host), -1, dtype=np.int64)
+                    for pg, slot, n in peers[src]["pages"]:
+                        t[pg:pg + n] = np.arange(slot, slot + n)
+                    ptabs[src] = t
+                entries: List[Tuple[int, int, int]] = []
+                for name, local in (("z1_master", self.master), ("z1_m", self.m), ("z1_v", self.v)):
+                    ptrs = self.comm.peer_pointers(name)
+                    for src, lo, hi in pulls:
+                        for a, b, at in self._pieces(ptabs[src], lo, hi):
+                            for c, d, mine in self._pieces(self._table_host, a, b):
+                                entries.append((ptrs[src] + (at + c - a) * 4, local.data_ptr() + mine * 4, (d - c) * 4))
+                device_copy(entries, s, chunk_bytes=1 << 20)
+            self._seed(lost)  # nobody holds these: re-seed from the replicated bf16 weights
+        s.synchronize()
+        self.comm._store_barrier(store, "z1/pulled", world)  # every peer has finished reading our source pages
+        self._free_pages(free_last)
+        with torch.cuda.stream(s):
+            self._table.copy_(torch.from_numpy(self._table_host))
+            if self.t != tmax:
+                self.gate[1:2].fill_(tmax)
+            self._reshard_event = s.record_event()
+        if lost and tmax > 0:  # at t = 0 every replica has the same seed: a slice nobody holds yet is not lost
+            self.lost_elements += total(lost)
+            logger.warning("zero1: %d state elements had no surviving holder and were re-seeded from the weights "
+                           "(moments reset)", total(lost))
+        self.pulled_bytes += 12 * total([(lo, hi) for _, lo, hi in pulls])
+        self.t = tmax
+        self._holdings = self.layout.held(rank, world)
+        self._refresh_pending = world > 1
 
     # ------------------------------------------------------------------ per-step pipeline
     def unit_of(self, lo: int, hi: int) -> int:
@@ -344,6 +612,11 @@ class Zero1Optimizer:
         self._refresh_pending = False
         for i, (lo, hi) in enumerate(self.layout.units):
             for mode in modes:
+                if self.compact:
+                    self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr(),
+                                            self.m.data_ptr(), self.v.data_ptr(), hi - lo, hp, self.gate, k, mode,
+                                            self._upd_blocks, stream, self._table.data_ptr(), lo, self._page_shift)
+                    continue
                 self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr() + lo * 4,
                                         self.m.data_ptr() + lo * 4, self.v.data_ptr() + lo * 4, hi - lo, hp,
                                         self.gate, k, mode, self._upd_blocks, stream)
@@ -362,6 +635,22 @@ class Zero1Optimizer:
     # ------------------------------------------------------------------ introspection
     def state_bytes_held(self) -> int:
         return 12 * total(self.layout.held(self.comm.rank, max(self.comm.world, 1)))
+
+    def state_bytes_allocated(self) -> int:
+        """Device bytes of the fp32 master/m/v arrays (compact: the page pools)."""
+        return 12 * (self.capacity * self._page if self.compact else self.numel)
+
+    def held_state(self) -> Dict[Range, Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
+        """Copies of (master, m, v) over each range this rank holds, keyed by ``(lo, hi)`` (for inspection and tests)."""
+        out = {}
+        torch.cuda.synchronize(self.device)
+        for lo, hi in self._holdings:
+            if not self.compact:
+                out[(lo, hi)] = (self.master[lo:hi].clone(), self.m[lo:hi].clone(), self.v[lo:hi].clone())
+                continue
+            idx = torch.cat([torch.arange(at, at + b - a, device=self.device) for a, b, at in self._pieces(self._table_host, lo, hi)])
+            out[(lo, hi)] = (self.master[idx], self.m[idx], self.v[idx])
+        return out
 
     def zero_grad(self, set_to_none: bool = False) -> None:  # gradients are overwritten by the wgrad GEMMs
         pass
