@@ -16,6 +16,11 @@ alternating the three ``--repeats`` times; it
 reports the median and the spread of each. The peer stores hit local HBM there, so this compares the state addressing,
 not NVLink.
 
+``--virtual W --clip`` times reduce-scatter + commit + update of one unit (rank 0's launches) without and with global
+gradient-norm clipping, alternating the two ``--repeats`` times, and reports the median and the spread of each with the
+card's name and power limit. Clipping adds squares to the reduce, per-rank partial loads to the commit and one multiply
+per element to the update; the peer loads hit local HBM there, so NVLink costs are not part of the comparison.
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -129,6 +134,70 @@ def compact_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats, shift=16):
     return out
 
 
+def gpu_info() -> dict:
+    """Card name and power limit: part of every absolute number this script prints."""
+    import subprocess
+
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit"], info["max_sm_clock"] = [x.strip() for x in out.split(",")[:2]]
+    except Exception as e:  # noqa: BLE001 - the timing stands without it, but say why it is missing
+        info["power_limit"] = f"unavailable ({e})"
+    return info
+
+
+def clip_ab(comm, nelem, k, rs_blocks, upd_blocks, iters, warmup, repeats, max_norm=1.0):
+    """Reduce-scatter + commit + update of one unit without clipping and with it, timed alternately."""
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
+    dev = comm.device
+    grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
+    grad.normal_()
+    state = [torch.randn(nelem, device=dev), torch.zeros(nelem, device=dev), torch.zeros(nelem, device=dev)]
+    gate = torch.zeros(2, dtype=torch.int32, device=dev)
+    clip = torch.zeros(2, dtype=torch.float32, device=dev)
+    gn = comm.segment("z1_gnorm").data_ptr()
+    # only this rank reduces, and only its k holders' copies of slice 0 are non-zero: 1/k keeps the repeated reduce at a
+    # fixed point (1/W would decay the gradient to zero, and with it the norm and the clipping)
+    scale = 1.0 / min(k, comm.world)
+
+    def step(on):
+        def fn():
+            comm.zero1_reduce_scatter_("z1_grad", 0, nelem, scale, True, k, rs_blocks, gnorm=gn if on else 0)
+            if on:
+                comm.zero1_commit_(gate, True, True, gnorm="z1_gnorm", nunits=1, max_norm=max_norm, norm=clip)
+            else:
+                comm.zero1_commit_(gate, True, True)
+            comm.zero1_update_("z1_param", 0, grad.data_ptr(), state[0].data_ptr(), state[1].data_ptr(), state[2].data_ptr(),
+                               nelem, HP, gate, k, 0, upd_blocks, coef=clip.data_ptr() + 4 if on else 0)
+        return fn
+
+    arms = (("off", step(False)), ("clip", step(True)))
+    times = {name: [] for name, _ in arms}
+    for _ in range(repeats):
+        for name, fn in arms:
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    assert comm.errored() is None
+    out = {"timing": "local HBM (virtual ranks), not NVLink", "max_norm": max_norm, "last_norm": float(clip[0]),
+           "last_coef": float(clip[1])}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        out[f"rs_commit_update_{name}_ms"] = {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4),
+                                              "max": round(ts[-1], 4)}
+    out["clip_over_off"] = round(out["rs_commit_update_clip_ms"]["median"] / out["rs_commit_update_off_ms"]["median"], 4)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--mb", type=float, default=436.0, help="unit size in MB of bf16 gradients (one Llama-3-8B block = 436 MB)")
@@ -139,7 +208,8 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--virtual", type=int, default=0, help="emulate this many ranks on ONE GPU (presignalled; for ncu)")
     ap.add_argument("--compact", action="store_true", help="--virtual: A/B the update on flat vs paged optimizer state")
-    ap.add_argument("--repeats", type=int, default=5, help="--compact: alternations of the flat and the paged timing")
+    ap.add_argument("--clip", action="store_true", help="--virtual: A/B one unit's pipeline without and with gradient clipping")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip: alternations of the two arms")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -147,11 +217,15 @@ def main() -> None:
 
     if a.virtual:
         torch.cuda.set_device(0)
-        comms = SymmetricComm.virtual_world(a.virtual, {"z1_grad": S, "z1_param": S}, presignal=True)
+        segments = {"z1_grad": S, "z1_param": S, **({"z1_gnorm": 8} if a.clip else {})}
+        comms = SymmetricComm.virtual_world(a.virtual, segments, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
-        if a.compact:
-            res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
-            res["gpu"] = torch.cuda.get_device_name(0)
+        if a.compact or a.clip:
+            if a.compact:
+                res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
+            else:
+                res.update(clip_ab(comms[0], nelem, a.replication, a.rs_blocks, a.upd_blocks, a.iters, a.warmup, a.repeats))
+            res.update(gpu_info())
             print("ZERO1_BENCH " + json.dumps(res), flush=True)
             if a.out:
                 os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)

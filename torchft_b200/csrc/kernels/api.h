@@ -29,16 +29,22 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
 // new bf16 weights. mc_base != nullptr selects the NVLS (multimem) data path. A non-null `table` selects paged
 // optimizer state: master/m/v are pools of 2^page_shift-element pages, element soff + i of the unit lives in page
 // table[(soff + i) >> page_shift]; a null table keeps flat addressing (state indexed like the unit).
+// Gradient clipping (all null by default = off): the reduce writes the unit's fp64 sum of squares of its slice to `gn`
+// (per-CTA scratch `cta_sq` of >= blocks doubles and a zeroed `ticket`); at world 1 it scales in place. The commit sums
+// `gn[0..world-1][0..nunits-1]`, writes {norm, coef} to `norm`, posts the norm to the host ring and vetoes a non-finite
+// norm. The update multiplies the gradient by `*coef`.
 void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
                             int barrier_mode, cudaStream_t stream);
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
-                         int replication, int blocks, int threads, cudaStream_t stream);
+                         int replication, int blocks, int threads, cudaStream_t stream, double* gn = nullptr,
+                         double* cta_sq = nullptr, unsigned* ticket = nullptr);
 void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64_t flag, uint32_t seq, int channel,
-                         int host_ok, int exchange, cudaStream_t stream);
+                         int host_ok, int exchange, cudaStream_t stream, const double* const* gn = nullptr,
+                         int nunits = 0, float max_norm = 0.f, float* norm = nullptr);
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream,
-                         const int* table = nullptr, size_t soff = 0, int page_shift = 0);
+                         const int* table = nullptr, size_t soff = 0, int page_shift = 0, const float* coef = nullptr);
 
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);

@@ -53,6 +53,8 @@ class Status {
     const uint32_t v = host_->verdict[seq & (kVerdictRing - 1)];
     return (v >> 1) == (seq & 0x7fffffffu) ? (int)(v & 1u) : -1;
   }
+  // Global gradient norm the clipping commit kernel posted for `seq` (valid once verdict(seq) is not -1).
+  float grad_norm(uint32_t seq) const { return host_->gnorm[seq & (kVerdictRing - 1)]; }
   void set_timeout_ms(double ms) { host_->timeout_ns = (uint64_t)(ms * 1e6); }
   double timeout_ms() const { return (double)host_->timeout_ns / 1e6; }
   StatusBlock* dev() const { return dev_; }
@@ -172,6 +174,7 @@ PYBIND11_MODULE(_K, m) {
       .def("error", &Status::error)
       .def("clear", &Status::clear)
       .def("verdict", &Status::verdict)
+      .def("grad_norm", &Status::grad_norm)
       .def("set_timeout_ms", &Status::set_timeout_ms)
       .def("timeout_ms", &Status::timeout_ms);
 
@@ -230,33 +233,45 @@ PYBIND11_MODULE(_K, m) {
   m.def(
       "zero1_reduce",
       [](const PeerTableH& pt, uintptr_t ok, uintptr_t mc_base, size_t off, size_t nelem, float scale, int replication,
-         int blocks, int threads, uintptr_t stream) {
-        zero1_reduce_launch(pt.pt, P<const int>(ok), P<void>(mc_base), off, nelem, scale, replication, blocks, threads, S(stream));
+         int blocks, int threads, uintptr_t stream, uintptr_t gn, uintptr_t cta_sq, uintptr_t ticket) {
+        zero1_reduce_launch(pt.pt, P<const int>(ok), P<void>(mc_base), off, nelem, scale, replication, blocks, threads, S(stream),
+                            P<double>(gn), P<double>(cta_sq), P<unsigned>(ticket));
       },
       py::arg("pt"), py::arg("ok"), py::arg("mc_base"), py::arg("off"), py::arg("nelem"), py::arg("scale"),
-      py::arg("replication"), py::arg("blocks"), py::arg("threads"), py::arg("stream"));
+      py::arg("replication"), py::arg("blocks"), py::arg("threads"), py::arg("stream"), py::arg("gn") = 0,
+      py::arg("cta_sq") = 0, py::arg("ticket") = 0);
   m.def(
       "zero1_commit",
       [](const PeerTableH& pt, const Status& st, uintptr_t gate, uint64_t flag, uint32_t seq, int channel,
-         bool host_ok, bool exchange, uintptr_t stream) {
+         bool host_ok, bool exchange, uintptr_t stream, const std::vector<uintptr_t>& gnorm, int nunits, float max_norm,
+         uintptr_t norm) {
+        if (gnorm.empty()) {
+          zero1_commit_launch(pt.pt, st.dev(), P<int>(gate), flag, seq, channel, host_ok ? 1 : 0, exchange ? 1 : 0,
+                              S(stream));
+          return;
+        }
+        if ((int)gnorm.size() != pt.pt.world) throw std::runtime_error("zero1_commit: need one z1_gnorm pointer per rank");
+        const double* gn[kMaxRanks] = {};
+        for (size_t r = 0; r < gnorm.size(); ++r) gn[r] = P<const double>(gnorm[r]);
         zero1_commit_launch(pt.pt, st.dev(), P<int>(gate), flag, seq, channel, host_ok ? 1 : 0, exchange ? 1 : 0,
-                            S(stream));
+                            S(stream), gn, nunits, max_norm, P<float>(norm));
       },
       py::arg("pt"), py::arg("status"), py::arg("gate"), py::arg("flag"), py::arg("seq"), py::arg("channel"),
-      py::arg("host_ok"), py::arg("exchange"), py::arg("stream"));
+      py::arg("host_ok"), py::arg("exchange"), py::arg("stream"), py::arg("gnorm") = std::vector<uintptr_t>{},
+      py::arg("nunits") = 0, py::arg("max_norm") = 0.f, py::arg("norm") = 0);
   m.def(
       "zero1_update",
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,
          uintptr_t v, size_t nelem, float lr, float b1, float b2, float eps, float wd, int replication, int mode,
-         int blocks, int threads, uintptr_t stream, uintptr_t table, size_t soff, int page_shift) {
+         int blocks, int threads, uintptr_t stream, uintptr_t table, size_t soff, int page_shift, uintptr_t coef) {
         zero1_update_launch(pt.pt, P<void>(mc_base), P<const int>(gate), poff, P<void>(grad), P<float>(master), P<float>(mm),
                             P<float>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream),
-                            P<const int>(table), soff, page_shift);
+                            P<const int>(table), soff, page_shift, P<const float>(coef));
       },
       py::arg("pt"), py::arg("mc_base"), py::arg("gate"), py::arg("poff"), py::arg("grad"), py::arg("master"),
       py::arg("m"), py::arg("v"), py::arg("nelem"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"),
       py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("blocks"), py::arg("threads"), py::arg("stream"),
-      py::arg("table") = 0, py::arg("soff") = 0, py::arg("page_shift") = 0);
+      py::arg("table") = 0, py::arg("soff") = 0, py::arg("page_shift") = 0, py::arg("coef") = 0);
 
   m.def(
       "push_exchange",

@@ -39,6 +39,9 @@ struct StatusBlock {
   // device -> host: commit verdicts of the device-side commit kernel (zero1.cu). Slot seq % ring
   // holds (seq << 1) | verdict, so the host can tell a stale slot from the one it is waiting for.
   volatile uint32_t verdict[64];
+  // device -> host: global gradient norm of commit seq (slot seq % ring), written before the verdict of the same slot
+  // when the commit kernel clips (zero1.cu); read once that verdict is there
+  volatile float gnorm[64];
 };
 constexpr uint32_t kVerdictRing = 64;
 
@@ -79,6 +82,11 @@ __device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) {
 __device__ __forceinline__ uint64_t ld_relaxed_sys(const uint64_t* p) {
   uint64_t v;
   asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ double ld_relaxed_sys_f64(const double* p) {
+  double v;
+  asm volatile("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
   return v;
 }
 __device__ __forceinline__ uint64_t globaltimer_ns() {

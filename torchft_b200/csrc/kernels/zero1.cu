@@ -25,6 +25,11 @@
 //                                      multimem.st per 16 B) -- the all-gather is the epilogue of the update
 //                 handshake            "my weight pushes have landed" (skipped when every rank holds everything)
 //
+// Gradient clipping (opt-in, CLIP template flag / non-null pointers): the reduce kernel also sums the squares of the
+// bf16 values it stores (one fp64 partial per unit and rank, combined over CTAs without float atomics), the commit
+// kernel adds every rank's partials in rank order into the global norm and the clip coefficient -- vetoing the step on
+// every rank when the norm is not finite -- and the update kernel scales the gradient by that coefficient.
+//
 // The two big kernels contain NO inter-rank synchronisation at all: any grid size, no co-residency requirement, no
 // SM held by a spinning CTA while peers are skewed, profilable stand-alone. Ordering comes from the one-CTA handshake
 // kernels around them (bounded, abortable spins; epoch-tagged flags; error latched in the status block and mirrored
@@ -99,9 +104,59 @@ struct RSArgs {
   size_t nelem;       // elements in the unit (multiple of 8)
   float scale;
   int replication;    // k
+  // CLIP: this rank's fp64 slot of the unit in its z1_gnorm segment, one fp64 per CTA of scratch and the last-CTA-done
+  // ticket (zero between launches: the last CTA resets it)
+  double* gn;
+  double* cta_sq;
+  unsigned* ticket;
 };
 
-template <int W, bool NVLS>
+__device__ __forceinline__ float sumsq8(const Vec16& v) {
+  float f[8];
+  P8::unpack(v, f);
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) s = fmaf(f[i], f[i], s);
+  return s;
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// The unit's slice sum of squares: per-thread fp32 sums -> fp64 per CTA (fixed warp order) -> the CTA that arrives last
+// adds all CTA partials in a fixed order and writes the unit's partial. No float atomics: the bits depend only on the
+// data and the grid, never on timing. A bf16 value above ~1.8e19 squares to inf in fp32 and so makes the norm inf, like
+// torch's fp32 norm of a bf16 tensor.
+__device__ __forceinline__ void finish_unit_sumsq(const RSArgs& a, float sq) {
+  __shared__ double warp_sq[32];
+  __shared__ int last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const double s = warp_sum_f64((double)sq);
+  if (lane == 0) warp_sq[warp] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) b += warp_sq[w];
+    a.cta_sq[blockIdx.x] = b;
+    __threadfence();
+    last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last || warp != 0) return;
+  __threadfence();
+  double t = 0.0;
+  for (unsigned b = lane; b < gridDim.x; b += 32) t += __ldcg(a.cta_sq + b);
+  t = warp_sum_f64(t);
+  if (lane == 0) {
+    *a.gn = t;
+    *a.ticket = 0;
+  }
+}
+
+template <int W, bool NVLS, bool CLIP>
 __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
   if (*a.ok == 0) return;
   const int rank = a.pt.rank;
@@ -116,8 +171,10 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
   const char* mcbase = a.mc + a.off;
   const int k = min(a.replication, W);
   const size_t lo = g.lo(rank), hi = g.hi(rank);
-  constexpr int U = NVLS ? 8 : ((W >= 8) ? 2 : (W >= 3 ? 4 : 8));
+  // CLIP at W = 7: three vectors per thread in flight instead of four, so the extra accumulator does not spill
+  constexpr int U = NVLS ? 8 : ((W >= 8) ? 2 : ((CLIP && W == 7) ? 3 : (W >= 3 ? 4 : 8)));
   const size_t stride = (size_t)gridDim.x * blockDim.x * U;
+  float sq = 0.f;  // CLIP: squares of the bf16 values this thread stores
   for (size_t base = lo + (size_t)blockIdx.x * blockDim.x * U; base < hi; base += stride) {
     if constexpr (NVLS) {
       Vec16 r[U];
@@ -135,6 +192,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
 #pragma unroll
           for (int i = 0; i < 8; ++i) f[i] *= a.scale;
           const Vec16 out = P8::pack(f);
+          if constexpr (CLIP) sq += sumsq8(out);
 #pragma unroll
           for (int j = 0; j < W; ++j)
             if (j < k) st_stream(dst[j] + v * 8, out);
@@ -165,6 +223,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
 #pragma unroll
           for (int i = 0; i < 8; ++i) acc[i] *= a.scale;
           const Vec16 out = P8::pack(acc);
+          if constexpr (CLIP) sq += sumsq8(out);
 #pragma unroll
           for (int j = 0; j < W; ++j)
             if (j < k) st_stream(dst[j] + v * 8, out);
@@ -172,6 +231,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
       }
     }
   }
+  if constexpr (CLIP) finish_unit_sumsq(a, sq);
 }
 
 // ---------------------------------------------------------------------------
@@ -187,12 +247,42 @@ struct CommitArgs {
   int channel;
   int host_ok;         // host-side part of the verdict (enough participants, no host-latched error)
   int exchange;        // 1 = AND the verdict over the quorum through the signal pads
+  // gradient clipping (gn[rank] != nullptr): every rank's z1_gnorm segment (nunits fp64 partials each), the clip
+  // threshold, and the device pair norm[0] = global L2 norm, norm[1] = clip coefficient
+  const double* gn[kMaxRanks];
+  int nunits;
+  float max_norm;
+  float* norm;
 };
 
+// One rank's per-unit partials summed in unit order, 16 loads in flight at a time.
+__device__ __forceinline__ double rank_sumsq(const double* p, int n) {
+  double s = 0.0;
+  for (int u0 = 0; u0 < n; u0 += 16) {
+    double x[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) x[i] = (u0 + i < n) ? ld_relaxed_sys_f64(p + u0 + i) : 0.0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (u0 + i < n) s += x[i];
+  }
+  return s;
+}
+
+// Why one buffer of partials is enough: a peer overwrites its partials only in the reduce kernel of its next step, and
+// that kernel sits behind the reduce-scatter handshake every rank must reach. This rank reaches its next handshake only
+// after this commit kernel (Zero1Optimizer orders the comm stream behind its last commit), so the partials read here
+// cannot change under the loads. At W = 1 or without the exchange the same ordering protects this rank's own partials.
 __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
   const int t = threadIdx.x;
   const int W = a.pt.world, rank = a.pt.rank;
   const int local_ok = (a.host_ok && a.st->error == kOk && !a.st->abort) ? 1 : 0;
+  const bool clip = a.gn[rank] != nullptr;
+  __shared__ double rank_sq[kMaxRanks];  // a peer whose arrival was not acquired contributes 0 (the verdict is 0 anyway)
+  if (clip) {
+    if (t < kMaxRanks) rank_sq[t] = (t == rank) ? rank_sumsq(a.gn[rank], a.nunits) : 0.0;
+    __syncwarp();
+  }
   int ok = local_ok;
   if (a.exchange && W > 1) {
     const uint64_t f = a.flag + 1;
@@ -214,13 +304,31 @@ __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
         fence_acq_rel_sys();
         const uint64_t v = ld_relaxed_sys(&a.pt.pads[rank]->sig[a.channel][1][t]);
         ok = (v >= f * 2 && (v & 1ull)) ? local_ok : 0;  // stale (older) verdicts compare smaller
+        // the peer's reduce kernels (and so its partials) precede its arrival flag: read them over NVLink now
+        if (clip) rank_sq[t] = rank_sumsq(a.gn[t], a.nunits);
       } else {
         ok = 0;
       }
     }
     ok = __all_sync(0xffffffffu, ok);
   }
+  if (clip) __syncwarp();  // rank_sq[] written by the other lanes is visible to lane 0
   if (t == 0) {
+    if (clip) {
+      // ranks in rank order 0..W-1 in fp64: every rank of the quorum adds the same numbers in the same order, so norm
+      // and coefficient are bit-identical everywhere. coef = min(1, max_norm / (norm + 1e-6)) with torch's clip_grad_norm_
+      // rounding: torch evaluates float / tensor as reciprocal(tensor) * float, each step IEEE fp32 (max_norm = inf
+      // gives exactly 1).
+      double sq = 0.0;
+      for (int r = 0; r < W; ++r) sq += rank_sq[r];
+      const float norm = (float)sqrt(sq);
+      const float coef = fminf(1.f, __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), a.max_norm));
+      if ((__float_as_uint(norm) & 0x7f800000u) == 0x7f800000u) ok = 0;  // inf / nan: vetoed on every rank alike
+      a.norm[0] = norm;
+      a.norm[1] = coef;
+      a.st->gnorm[a.seq & (kVerdictRing - 1)] = norm;
+      __threadfence_system();  // the norm slot is complete before the host can see this seq's verdict
+    }
     a.gate[0] = ok;
     if (ok) a.gate[1] += 1;
     a.st->verdict[a.seq & (kVerdictRing - 1)] = (a.seq << 1) | (uint32_t)ok;
@@ -250,14 +358,19 @@ struct UpdArgs {
   const int* table;
   size_t soff;
   int page_shift;
+  const float* coef;   // CLIP: the clip coefficient the commit kernel wrote; the gradient is scaled by it (mode 0)
 };
 
-template <int W, bool NVLS, bool PAGED>
+template <int W, bool NVLS, bool PAGED, bool CLIP>
 __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   if (a.mode == 0 && a.gate[0] == 0) return;  // uniform over the grid AND (unanimous verdict) over the quorum
   const int rank = a.pt.rank;
   const Geo g(a.nelem, W);
   const int k = min(a.replication, W);
+  float cf = 1.f;
+  if constexpr (CLIP) {
+    if (a.mode == 0) cf = __ldg(a.coef);
+  }
   const float tf = (float)a.gate[1];
   const float bc1 = 1.f - powf(a.b1, tf), bc2 = 1.f - powf(a.b2, tf);
   const float step_size = a.lr / bc1;
@@ -298,6 +411,10 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
         const Vec16 v0 = ld_stream(a.v + si), v1 = ld_stream(a.v + si + 4);
         float gr[8], m[8], vv[8];
         P8::unpack(gv, gr);
+        if constexpr (CLIP) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) gr[i] *= cf;
+        }
         Pack<float>::unpack(w0, w);
         Pack<float>::unpack(w1, w + 4);
         Pack<float>::unpack(m0, m);
@@ -336,33 +453,48 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   }
 }
 
-template <bool NVLS>
+template <bool NVLS, bool CLIP>
 void launch_rs(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
   switch (a.pt.world) {
-    case 2: zero1_reduce_kernel<2, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_reduce_kernel<3, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_reduce_kernel<4, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_reduce_kernel<5, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_reduce_kernel<6, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_reduce_kernel<7, NVLS><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_reduce_kernel<8, NVLS><<<blocks, threads, 0, s>>>(a); break;
+    case 1:
+      // one rank: only the clipping path launches it (scale in place + the unit's sum of squares); never multicast
+      if constexpr (CLIP && !NVLS) {
+        zero1_reduce_kernel<1, false, true><<<blocks, threads, 0, s>>>(a);
+        break;
+      }
+      throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
+    case 2: zero1_reduce_kernel<2, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 3: zero1_reduce_kernel<3, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 4: zero1_reduce_kernel<4, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 5: zero1_reduce_kernel<5, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 6: zero1_reduce_kernel<6, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 7: zero1_reduce_kernel<7, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 8: zero1_reduce_kernel<8, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
     default: throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
+  }
+}
+
+template <bool NVLS, bool PAGED, bool CLIP>
+void launch_upd_w(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
+  switch (a.pt.world) {
+    case 1: zero1_update_kernel<1, false, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 2: zero1_update_kernel<2, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 3: zero1_update_kernel<3, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 4: zero1_update_kernel<4, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 5: zero1_update_kernel<5, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 6: zero1_update_kernel<6, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 7: zero1_update_kernel<7, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 8: zero1_update_kernel<8, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    default: throw std::runtime_error("zero1_update: world size must be in [1, 8]");
   }
 }
 
 template <bool NVLS, bool PAGED>
 void launch_upd(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
-  switch (a.pt.world) {
-    case 1: zero1_update_kernel<1, false, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 2: zero1_update_kernel<2, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_update_kernel<3, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_update_kernel<4, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_update_kernel<5, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_update_kernel<6, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_update_kernel<7, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_update_kernel<8, NVLS, PAGED><<<blocks, threads, 0, s>>>(a); break;
-    default: throw std::runtime_error("zero1_update: world size must be in [1, 8]");
-  }
+  if (a.coef != nullptr)
+    launch_upd_w<NVLS, PAGED, true>(a, blocks, threads, s);
+  else
+    launch_upd_w<NVLS, PAGED, false>(a, blocks, threads, s);
 }
 
 void check_grid(int blocks, int threads, const char* who) {
@@ -380,21 +512,42 @@ void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, u
 }
 
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
-                         int replication, int blocks, int threads, cudaStream_t stream) {
+                         int replication, int blocks, int threads, cudaStream_t stream, double* gn, double* cta_sq,
+                         unsigned* ticket) {
   check_grid(blocks, threads, "zero1_reduce");
   if ((off & 15) || (nelem & 7)) throw std::runtime_error("zero1_reduce: unit must be 16 B aligned and a multiple of 8 elements");
   if (replication < 1) throw std::runtime_error("zero1_reduce: replication must be >= 1");
-  RSArgs a{pt, ok, reinterpret_cast<char*>(mc_base), off, nelem, scale, replication};
-  if (mc_base != nullptr)
-    launch_rs<true>(a, blocks, threads, stream);
-  else
-    launch_rs<false>(a, blocks, threads, stream);
+  if (gn != nullptr && (cta_sq == nullptr || ticket == nullptr))
+    throw std::runtime_error("zero1_reduce: the gradient norm needs the per-CTA scratch and the ticket");
+  RSArgs a{pt, ok, reinterpret_cast<char*>(mc_base), off, nelem, scale, replication, gn, cta_sq, ticket};
+  if (gn != nullptr) {
+    if (mc_base != nullptr)
+      launch_rs<true, true>(a, blocks, threads, stream);
+    else
+      launch_rs<false, true>(a, blocks, threads, stream);
+  } else if (mc_base != nullptr) {
+    launch_rs<true, false>(a, blocks, threads, stream);
+  } else {
+    launch_rs<false, false>(a, blocks, threads, stream);
+  }
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
 void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64_t flag, uint32_t seq, int channel,
-                         int host_ok, int exchange, cudaStream_t stream) {
-  CommitArgs a{pt, st, gate, flag, seq, channel, host_ok, exchange};
+                         int host_ok, int exchange, cudaStream_t stream, const double* const* gn, int nunits,
+                         float max_norm, float* norm) {
+  CommitArgs a{pt, st, gate, flag, seq, channel, host_ok, exchange, {}, 0, 0.f, nullptr};
+  if (gn != nullptr) {
+    if (norm == nullptr || nunits < 1) throw std::runtime_error("zero1_commit: the gradient norm needs units and an output pair");
+    if (!(max_norm > 0.f)) throw std::runtime_error("zero1_commit: max_norm must be > 0");
+    for (int r = 0; r < pt.world; ++r) {
+      if (gn[r] == nullptr) throw std::runtime_error("zero1_commit: one z1_gnorm pointer per rank");
+      a.gn[r] = gn[r];
+    }
+    a.nunits = nunits;
+    a.max_norm = max_norm;
+    a.norm = norm;
+  }
   zero1_commit_kernel<<<1, 32, 0, stream>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
@@ -402,13 +555,13 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream, const int* table,
-                         size_t soff, int page_shift) {
+                         size_t soff, int page_shift, const float* coef) {
   check_grid(blocks, threads, "zero1_update");
   if ((poff & 15) || (nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
   if (table != nullptr && (page_shift < 3 || page_shift > 30 || (soff & 7)))
     throw std::runtime_error("zero1_update: pages must be 2^3 .. 2^30 elements and the unit 8-element aligned");
   UpdArgs a{pt, reinterpret_cast<char*>(mc_base), gate, poff, reinterpret_cast<const bf16*>(grad), master, m, v,
-            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift};
+            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift, coef};
   if (table != nullptr) {
     if (mc_base != nullptr)
       launch_upd<true, true>(a, blocks, threads, stream);

@@ -130,6 +130,7 @@ class SymmetricComm:
         self.launches = 0  # native kernel launches issued (bench reports this)
         self._ptrs: Dict[str, List[int]] = {}  # segment -> mapped base pointer per quorum rank
         self._z1_ok_buf: Optional[torch.Tensor] = None
+        self._z1_norm_scratch: Optional[torch.Tensor] = None
         self._aliased = False  # a virtual rank whose user segments are rank 0's (virtual_world(alias=True)): it frees none
         self._commit_seq = 0
         self._hostname = socket.gethostname()
@@ -789,10 +790,20 @@ class SymmetricComm:
         return mc[1] if (mc is not None and self._world > 1 and nbytes >= self._nvls_min) else 0
 
     def _z1_ok(self, slot: int) -> int:
-        """Device word the handshake kernels write their outcome to (slot 0: comm stream, slot 1: optimizer stream)."""
+        """Device word the handshake kernels write their outcome to (slot 0: comm stream, slot 1: optimizer stream;
+        slot 2 is never written and stays 1, for a kernel with no handshake in front of it)."""
         if self._z1_ok_buf is None:
             self._z1_ok_buf = torch.ones(4, dtype=torch.int32, device=self.device)
         return self._z1_ok_buf.data_ptr() + 4 * slot
+
+    def _z1_norm_scratch_ptrs(self) -> Tuple[int, int]:
+        """Per-CTA fp64 partials and the last-CTA-done ticket of the reduce kernel's sum of squares (one launch at a
+        time per rank: the launches of a rank are ordered on its comm stream)."""
+        n = self._K.NUM_SMS * 32  # the grid cap of the reduce kernel
+        if self._z1_norm_scratch is None:
+            self._z1_norm_scratch = torch.zeros(n + 1, dtype=torch.float64, device=self.device)
+        p = self._z1_norm_scratch.data_ptr()
+        return p, p + 8 * n
 
     def _handshake(self, slot: int, release: bool, channel: int, sp: int) -> None:
         self._K.zero1_handshake(self._tables["core"], self._status, self._z1_ok(slot), self._next_flag(), channel, release,
@@ -800,10 +811,15 @@ class SymmetricComm:
         self.launches += 1
 
     def zero1_reduce_scatter_(self, segment: str, off: int, nelem: int, scale: float, contribute: bool,
-                              replication: int, blocks: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+                              replication: int, blocks: int, stream: Optional[torch.cuda.Stream] = None,
+                              gnorm: int = 0) -> None:
         """Reduce-scatter ``nelem`` bf16 elements at byte offset ``off`` of ``segment`` in place: afterwards rank r
         (and its ``replication - 1`` successors) hold the scaled sum of slice r. Three launches on ``stream``:
-        handshake ("my unit is ready") -> sync-free reduce kernel (any grid) -> handshake ("my pushes landed")."""
+        handshake ("my unit is ready") -> sync-free reduce kernel (any grid) -> handshake ("my pushes landed").
+
+        ``gnorm`` (device address of one fp64, 0 = off): the kernel also writes there the sum of squares of the bf16
+        values of slice r it produced (this rank's partial of the global gradient norm). At world 1 that is the one
+        reduce launch: it scales the unit in place, with no handshake."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -811,25 +827,48 @@ class SymmetricComm:
             if not contribute:
                 # healing / spare replica: its gradients count as zeros (reference manager.py:441-442)
                 self._K.memset_async(self._segments[segment].ptr + off, 0, nelem * 2, sp)
-            self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
+            if gnorm:
+                scratch, ticket = self._z1_norm_scratch_ptrs()
+                one = self._world == 1
+                if not one:
+                    self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
+                self._K.zero1_reduce(self._tables[segment], self._z1_ok(2 if one else 0), self._mc_base(segment, nelem * 2),
+                                     off, nelem, scale, replication, blocks, self._threads, sp, gnorm, scratch, ticket)
+                self.launches += 1
+                if not one:
+                    self._handshake(0, True, _CH_ALLREDUCE, sp)
+                return
+            self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
             self._K.zero1_reduce(self._tables[segment], self._z1_ok(0), self._mc_base(segment, nelem * 2), off, nelem, scale,
                                  replication, blocks, self._threads, sp)
             self.launches += 1
             self._handshake(0, True, _CH_ALLREDUCE, sp)
 
     def zero1_commit_(self, gate: torch.Tensor, host_ok: bool, exchange: bool,
-                      stream: Optional[torch.cuda.Stream] = None) -> int:
+                      stream: Optional[torch.cuda.Stream] = None, gnorm: Optional[str] = None, nunits: int = 0,
+                      max_norm: float = float("inf"), norm: Optional[torch.Tensor] = None) -> int:
         """Device-side commit verdict (AND over the quorum when ``exchange``): writes ``gate[0]`` (verdict),
         increments ``gate[1]`` on success and posts the verdict to the host-mapped ring. Returns the sequence
-        number to pass to :meth:`verdict`."""
+        number to pass to :meth:`verdict`.
+
+        ``gnorm`` (name of a segment of ``nunits`` fp64 partials per rank, written by :meth:`zero1_reduce_scatter_`)
+        adds gradient clipping: the kernel sums every rank's partials in rank order (its own only at world 1 or without
+        ``exchange``), writes ``norm[0]`` = the global L2 norm and ``norm[1]`` = ``min(1, max_norm / (norm + 1e-6))``
+        (fp32 tensor of two), posts the norm for :meth:`grad_norm` and vetoes the step when the norm is not finite."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
             self._commit_seq = (self._commit_seq + 1) & 0x3fffffff
             seq = self._commit_seq
-            self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
-                                 bool(host_ok), bool(exchange), _native.stream_ptr(stream))
+            if gnorm is not None:
+                assert norm is not None and norm.dtype == torch.float32 and norm.numel() >= 2
+                self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
+                                     bool(host_ok), bool(exchange), _native.stream_ptr(stream), self._ptrs[gnorm],
+                                     int(nunits), float(max_norm), norm.data_ptr())
+            else:
+                self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
+                                     bool(host_ok), bool(exchange), _native.stream_ptr(stream))
             self.launches += 1
             return seq
 
@@ -838,16 +877,23 @@ class SymmetricComm:
         v = self._status.verdict(seq)
         return None if v < 0 else bool(v)
 
+    def grad_norm(self, seq: int) -> Optional[float]:
+        """Global gradient norm of clipping commit ``seq`` if the kernel has run, else ``None`` (never blocks)."""
+        if self.verdict(seq) is None:
+            return None
+        return float(self._status.grad_norm(seq))
+
     def zero1_update_(self, segment: str, poff: int, grad: int, master: int, m: int, v: int, nelem: int,
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,
                       blocks: int, stream: Optional[torch.cuda.Stream] = None, table: int = 0, state_off: int = 0,
-                      page_shift: int = 0) -> None:
+                      page_shift: int = 0, coef: int = 0) -> None:
         """Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights into
         ``segment`` on the ranks that do not hold it (``mode`` 1: ungated re-broadcast of bf16(master) to everybody, no
         state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed.
 
         ``table`` (device pointer to int32 page slots, 0 = flat state) selects paged state: ``master``/``m``/``v`` are
-        then page pools and element ``state_off + i`` of the unit lives in pool page ``table[(state_off + i) >> page_shift]``."""
+        then page pools and element ``state_off + i`` of the unit lives in pool page ``table[(state_off + i) >> page_shift]``.
+        ``coef`` (device address of an fp32, 0 = none): the gradient is multiplied by it (the clip coefficient)."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -856,7 +902,7 @@ class SymmetricComm:
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp,
-                                 table, state_off, page_shift)
+                                 table, state_off, page_shift, coef)
             self.launches += 1
             pushes = self._world > 1 and (mode == 1 or self._world > replication)
             if pushes:

@@ -53,6 +53,9 @@ class FaultTolerantTrainer:
         replication: holders per slice of optimizer state (``k`` of FT-ZeRO-1)
         compact_state: FT-ZeRO-1: store only the held slices of the optimizer state, in page pools sized for every
             quorum of ``min_replica_size`` to 8 replicas (``None``: env ``TORCHFT_B200_Z1_COMPACT=1`` turns it on)
+        max_grad_norm: FT-ZeRO-1: clip the global L2 norm of the reduced gradient to this, on the device; a step with a
+            non-finite norm is skipped on every replica (``inf``: only that). ``None``: env
+            ``TORCHFT_B200_Z1_MAX_GRAD_NORM``, unset = no clipping. Not available on the classic all-reduce pipeline.
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -65,7 +68,7 @@ class FaultTolerantTrainer:
                  activation_checkpoint: Optional[str] = None, init_sync: bool = False,
                  use_async_quorum: bool = True, overlap_optimizer: Optional[bool] = None,
                  optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2,
-                 compact_state: Optional[bool] = None) -> None:
+                 compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -78,6 +81,8 @@ class FaultTolerantTrainer:
         if zero1 and backend != "b200":
             raise ValueError("zero1 needs the b200 backend")
         self.zero1 = bool(zero1)
+        if max_grad_norm is not None and not self.zero1:
+            raise ValueError("max_grad_norm needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
 
         # the replica group's own store (group world size 1 => this process hosts it)
         self._store = TCPStore("127.0.0.1", 0, is_master=True, wait_for_workers=False)
@@ -103,7 +108,7 @@ class FaultTolerantTrainer:
             # the optimizer owns the five symmetric flat buffers; FlatParams adopts two of them. Units (= gradient
             # buckets = update launches) are the forward stages, known once the parameters have offsets.
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
-                                       compact=compact_state, min_world=min_replica_size)
+                                       compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:
@@ -291,6 +296,11 @@ class FaultTolerantTrainer:
         self._loss_host.copy_(loss.detach().float().reshape(1), non_blocking=True)
         self._loss_event.record()
         return prev
+
+    def last_grad_norm(self) -> Optional[float]:
+        """Global gradient norm of the most recently resolved step (FT-ZeRO-1 with clipping; ``None`` otherwise). Steps
+        resolve lazily, so after step ``n`` this is usually the norm of step ``n - 1``."""
+        return self.zopt.last_grad_norm if self.zopt is not None else None
 
     def last_loss(self) -> Optional[float]:
         """Loss of the most recent :meth:`step_async` (waits for it)."""

@@ -29,6 +29,7 @@ from __future__ import annotations
 
 import json
 import logging
+import math
 import os
 import threading
 from dataclasses import dataclass
@@ -41,9 +42,26 @@ logger = logging.getLogger(__name__)
 Range = Tuple[int, int]
 
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
-           "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges"]
+           "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges",
+           "clip_threshold"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
+GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
+
+
+def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
+    """The clipping threshold :class:`Zero1Optimizer` uses: ``max_grad_norm``, or env ``TORCHFT_B200_Z1_MAX_GRAD_NORM``
+    when it is ``None`` (unset or empty: no clipping). ``inf`` computes the norm and vetoes non-finite steps but never
+    scales; zero, negative and NaN thresholds raise ``ValueError``."""
+    if max_grad_norm is None:
+        env = os.environ.get("TORCHFT_B200_Z1_MAX_GRAD_NORM", "").strip()
+        if not env:
+            return None
+        max_grad_norm = float(env)
+    max_grad_norm = float(max_grad_norm)
+    if not max_grad_norm > 0:
+        raise ValueError(f"max_grad_norm must be > 0 (inf: compute the norm without scaling), got {max_grad_norm}")
+    return max_grad_norm
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -255,6 +273,13 @@ class Zero1Optimizer:
     below ``min_world`` or a plan that does not fit raises instead of dropping state. A compact re-shard completes
     inside ``configure`` (it frees and reuses pages, so it synchronises with its peers before it returns).
 
+    With ``max_grad_norm`` the global L2 norm of the reduced bf16 gradient is computed on the device inside the same
+    three kernels (no extra launch, no host sync): the reduce-scatter sums the squares of the slice it produces, the
+    commit kernel adds every rank's partials in rank order -- so every replica gets the same bits -- and the update
+    scales the gradient by ``min(1, max_grad_norm / (norm + 1e-6))``. A step whose norm is not finite is vetoed on
+    every replica (counted in ``nonfinite_steps``): no state changes and ``t`` does not advance. ``grad_norm`` is the
+    device scalar of the last commit, ``last_grad_norm`` the host value of the last resolved step.
+
     Args:
         pg: a ``ProcessGroupB200`` (symmetric segments must be allocated before its first ``configure``)
         numel: elements of the flat parameter vector (multiple of 8)
@@ -264,14 +289,18 @@ class Zero1Optimizer:
         min_world: compact: the smallest quorum the pool must hold the state for
         state_pages: compact: pool size in pages, overriding :func:`pool_pages`
         page_shift: compact: pages of ``2**page_shift`` elements
+        max_grad_norm: clip the global gradient norm to this (``inf``: only veto non-finite steps; ``None``: env
+            ``TORCHFT_B200_Z1_MAX_GRAD_NORM``, unset = no clipping)
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
                  betas: Tuple[float, float] = (0.9, 0.95), eps: float = 1e-8, weight_decay: float = 0.1,
                  replication: int = 2, blocks: Optional[int] = None, compact: Optional[bool] = None, min_world: int = 1,
-                 state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT) -> None:
+                 state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT,
+                 max_grad_norm: Optional[float] = None) -> None:
         from torchft_b200.ops import _native
 
+        self.max_grad_norm = clip_threshold(max_grad_norm)
         assert numel % 8 == 0
         self._K = _native.load()
         self.pg = pg
@@ -292,6 +321,16 @@ class Zero1Optimizer:
         self.min_world = int(min_world)
         self.param = pg.alloc_symmetric("z1_param", numel * 2).view(torch.bfloat16)
         self.grad = pg.alloc_symmetric("z1_grad", numel * 2).view(torch.bfloat16)
+        self.grad_norm: Optional[torch.Tensor] = None  # clipping: device fp32 norm of the last commit
+        self.last_grad_norm: Optional[float] = None    # clipping: host norm of the last resolved step
+        self.nonfinite_steps = 0                       # clipping: steps vetoed because the norm was inf / nan
+        if self.max_grad_norm is not None:
+            # symmetric segments are zero-filled at allocation, so the FlatParams.ALIGN padding of z1_grad, which no
+            # wgrad GEMM writes, adds nothing to the norm. One fp64 partial per unit; peers read them in the commit.
+            self._gnorm = pg.alloc_symmetric("z1_gnorm", GNORM_UNITS * 8).view(torch.float64)[:GNORM_UNITS]
+            self._clip = torch.zeros(2, dtype=torch.float32, device=self.device)  # [norm, coef] of the last commit
+            self.grad_norm = self._clip[0]
+            self._resolved_norm: Optional[float] = None
         if not self.compact:
             self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
             self.m = pg.alloc_symmetric("z1_m", numel * 4).view(torch.float32)
@@ -327,6 +366,8 @@ class Zero1Optimizer:
         """Fix the unit ranges (forward order, tiling ``[0, numel)``); call before the first quorum."""
         assert all(lo % 8 == 0 and hi % 8 == 0 for lo, hi in units)
         assert merge_ranges(units) == [(0, self.numel)] and total(units) == self.numel, "units must tile the flat buffer exactly"
+        if self.max_grad_norm is not None and len(units) > GNORM_UNITS:
+            raise ValueError(f"gradient clipping supports at most {GNORM_UNITS} units, got {len(units)}")
         if self.compact and self.capacity:
             raise RuntimeError("compact state: the units are fixed once the page pools are allocated")
         self.layout = ShardLayout(tuple((int(a), int(b)) for a, b in units), self._replication)
@@ -384,7 +425,8 @@ class Zero1Optimizer:
     def _on_configured(self, store: Any, rank: int, world: int, epoch: int) -> None:
         """Runs inside ``ProcessGroupB200.configure`` (quorum thread) with the quorum-scoped store."""
         with self._lock:
-            missing = [n for n in ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") if not self.comm.is_symmetric(n)]
+            names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ())
+            missing = [n for n in names if not self.comm.is_symmetric(n)]
             if missing:
                 # the kernels dereference peer pointers: every replica must construct its Zero1Optimizer before its first
                 # quorum (segments allocated later only become symmetric at the NEXT quorum change)
@@ -566,6 +608,19 @@ class Zero1Optimizer:
     def reduce_scatter(self, unit: int, scale: float, contribute: bool) -> Any:
         """Reduce unit ``unit`` of the gradient buffer across the quorum (comm stream, overlaps backward)."""
         lo, hi = self.layout.units[unit]
+        if self.max_grad_norm is not None:
+            gn = self._gnorm.data_ptr() + 8 * unit
+            after = self._commit_event
+            k = self.layout.replication
+
+            def launch(s: torch.cuda.Stream) -> None:
+                if after is not None:
+                    # the last commit kernel read the partials this launch overwrites (see zero1_commit_kernel)
+                    s.wait_event(after)
+                self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s,
+                                                gnorm=gn)
+
+            return self.pg._launch(launch, None)
         if self.comm.world == 1:
             if scale != 1.0 or not contribute:
                 self.grad[lo:hi].mul_(scale if contribute else 0.0)
@@ -589,7 +644,11 @@ class Zero1Optimizer:
             stream.wait_event(self._reshard_event)  # a verdict also tells peers "my pulls are done"
             self._reshard_event = None
         self._commit_layout = (self.comm.rank, self.comm.world)
-        seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream)
+        if self.max_grad_norm is not None:
+            seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream, gnorm="z1_gnorm",
+                                          nunits=len(self.layout.units), max_norm=self.max_grad_norm, norm=self._clip)
+        else:
+            seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream)
         self._commit_event = stream.record_event()
         return seq
 
@@ -599,6 +658,8 @@ class Zero1Optimizer:
         v = self.comm.verdict(seq)
         if v is None:
             raise RuntimeError(f"commit {seq}: the verdict kernel finished without posting a verdict")
+        if self.max_grad_norm is not None:
+            self._resolved_norm = self.comm.grad_norm(seq)
         return v
 
     def update(self, events: Optional[Sequence[torch.cuda.Event]] = None) -> None:
@@ -608,6 +669,7 @@ class Zero1Optimizer:
         k = self.layout.replication
         lr = self.param_groups[0]["lr"]
         hp = (lr, self.betas[0], self.betas[1], self.eps, self.weight_decay)
+        coef = self._clip.data_ptr() + 4 if self.max_grad_norm is not None else 0
         modes = (1, 0) if self._refresh_pending else (0,)
         self._refresh_pending = False
         for i, (lo, hi) in enumerate(self.layout.units):
@@ -615,11 +677,11 @@ class Zero1Optimizer:
                 if self.compact:
                     self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr(),
                                             self.m.data_ptr(), self.v.data_ptr(), hi - lo, hp, self.gate, k, mode,
-                                            self._upd_blocks, stream, self._table.data_ptr(), lo, self._page_shift)
+                                            self._upd_blocks, stream, self._table.data_ptr(), lo, self._page_shift, coef=coef)
                     continue
                 self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr() + lo * 4,
                                         self.m.data_ptr() + lo * 4, self.v.data_ptr() + lo * 4, hi - lo, hp,
-                                        self.gate, k, mode, self._upd_blocks, stream)
+                                        self.gate, k, mode, self._upd_blocks, stream, coef=coef)
             if events is not None:
                 events[i].record(stream)
 
@@ -631,6 +693,13 @@ class Zero1Optimizer:
                 self.t += 1
                 self._holdings = self.layout.held(rank, world)
             self._commit_layout = None
+            if self.max_grad_norm is not None and self._resolved_norm is not None:
+                norm, self._resolved_norm = self._resolved_norm, None
+                self.last_grad_norm = norm
+                if not math.isfinite(norm):
+                    self.nonfinite_steps += 1
+                    logger.warning("zero1: gradient norm is %s: the step was skipped on every replica (%d so far)",
+                                   norm, self.nonfinite_steps)
 
     # ------------------------------------------------------------------ introspection
     def state_bytes_held(self) -> int:
