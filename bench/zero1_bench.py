@@ -21,6 +21,12 @@ gradient-norm clipping, alternating the two ``--repeats`` times, and reports the
 card's name and power limit. Clipping adds squares to the reduce, per-rank partial loads to the commit and one multiply
 per element to the update; the peer loads hit local HBM there, so NVLink costs are not part of the comparison.
 
+``--virtual W --accum`` times rank 0's reduce launch of one unit in the gradient-accumulation modes off (today's launch),
+acc (a middle micro-batch: 32 B of fp32 accumulator read and written per 8 elements, no bf16 store, no push) and last
+(accumulator read, bf16 store and buddy push), alternating ``--repeats`` times, with the card's name and power limit.
+It first checks that an accumulated pair gives the off result bit for bit. The peer loads hit local HBM, so this
+compares the kernels' HBM behaviour, not NVLink.
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -198,6 +204,71 @@ def clip_ab(comm, nelem, k, rs_blocks, upd_blocks, iters, warmup, repeats, max_n
     return out
 
 
+def accum_ab(comms, nelem, k, rs_blocks, iters, warmup, repeats):
+    """Rank 0's reduce-scatter of one unit in the three accumulation modes, timed alternately: ``off`` (today's launch),
+    ``acc`` (a middle micro-batch: fp32 rank sum added into the accumulator) and ``last`` (accumulator + rank sum,
+    scaled, rounded to bf16 and pushed to the buddies). Before timing, a first + last pair over the same gradients with
+    half the scale must give the ``off`` result bit for bit (2s * scale/2 == s * scale exactly), and slice 0 must equal
+    the PyTorch reference bf16(fp32 rank sum * scale). At world 1 there is no ``off`` kernel (the optimizer scales on
+    the host), so only the reference is checked."""
+    from torchft_b200.parallel.zero1 import ShardLayout, accum_offsets
+
+    comm = comms[0]
+    peers = [c.segment("z1_grad")[: nelem * 2].view(torch.bfloat16) for c in comms]
+    for p in peers:
+        p.normal_()
+    L = ShardLayout(((0, nelem),), k)
+    _, n = accum_offsets(L, comm.rank, comm.world)
+    lo, hi = L.slice_bounds(0, comm.world, comm.rank)
+    acc = torch.zeros(n + 8, device=comm.device)
+    scale = 1.0 / comm.world
+    saved = [p.clone() for p in peers]
+    rank_sum = saved[0][lo:hi].float()
+    for p in saved[1:]:
+        rank_sum = rank_sum + p[lo:hi].float()
+    expect = (rank_sum * torch.tensor(scale, dtype=torch.float32, device=comm.device)).bfloat16()
+
+    def launch(mode, sc=scale):
+        return lambda: comm.zero1_reduce_scatter_("z1_grad", 0, nelem, sc, True, k, rs_blocks, acc=acc.data_ptr(),
+                                                  acc_mode=mode)
+
+    has_off = comm.world > 1
+    if has_off:
+        launch(0)()
+        torch.cuda.synchronize()
+        ref = [p.clone() for p in peers]
+        for p, x in zip(peers, saved):
+            p.copy_(x)
+    launch(1, scale / 2)()
+    launch(3, scale / 2)()
+    torch.cuda.synchronize()
+    same = all(torch.equal(p, r) for p, r in zip(peers, ref)) if has_off else None
+    matches_ref = torch.equal(peers[0][lo:hi], expect)
+    arms = ((("off", launch(0)),) if has_off else ()) + (("acc", launch(2)), ("last", launch(3)))
+    times = {name: [] for name, _ in arms}
+    for _ in range(repeats):
+        for name, fn in arms:
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    assert comm.errored() is None
+    out = {"timing": "local HBM (virtual ranks), not NVLink", "accum_equals_off": same, "accum_matches_reference": matches_ref,
+           "accum_bytes": 4 * n}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        out[f"reduce_{name}_ms"] = {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4), "max": round(ts[-1], 4)}
+    for name in ("acc", "last") if has_off else ():
+        out[f"{name}_over_off"] = round(out[f"reduce_{name}_ms"]["median"] / out["reduce_off_ms"]["median"], 4)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--mb", type=float, default=436.0, help="unit size in MB of bf16 gradients (one Llama-3-8B block = 436 MB)")
@@ -209,7 +280,8 @@ def main() -> None:
     ap.add_argument("--virtual", type=int, default=0, help="emulate this many ranks on ONE GPU (presignalled; for ncu)")
     ap.add_argument("--compact", action="store_true", help="--virtual: A/B the update on flat vs paged optimizer state")
     ap.add_argument("--clip", action="store_true", help="--virtual: A/B one unit's pipeline without and with gradient clipping")
-    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip: alternations of the two arms")
+    ap.add_argument("--accum", action="store_true", help="--virtual: A/B rank 0's reduce in accumulation modes off / acc / last")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum: alternations of the arms")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -220,9 +292,11 @@ def main() -> None:
         segments = {"z1_grad": S, "z1_param": S, **({"z1_gnorm": 8} if a.clip else {})}
         comms = SymmetricComm.virtual_world(a.virtual, segments, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
-        if a.compact or a.clip:
+        if a.compact or a.clip or a.accum:
             if a.compact:
                 res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
+            elif a.accum:
+                res.update(accum_ab(comms, nelem, a.replication, a.rs_blocks, a.iters, a.warmup, a.repeats))
             else:
                 res.update(clip_ab(comms[0], nelem, a.replication, a.rs_blocks, a.upd_blocks, a.iters, a.warmup, a.repeats))
             res.update(gpu_info())

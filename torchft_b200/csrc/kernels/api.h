@@ -33,11 +33,14 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
 // (per-CTA scratch `cta_sq` of >= blocks doubles and a zeroed `ticket`); at world 1 it scales in place. The commit sums
 // `gn[0..world-1][0..nunits-1]`, writes {norm, coef} to `norm`, posts the norm to the host ring and vetoes a non-finite
 // norm. The update multiplies the gradient by `*coef`.
+// Gradient accumulation (acc_mode 0 = off by default): `acc` is this rank's fp32 accumulator of the unit's primary
+// slice. acc_mode 1 (first micro-batch) stores the fp32 rank sum there, 2 (middle) adds it; neither writes the gradient
+// segment. 3 (last) reduces (acc + rank sum) * scale to bf16 like mode 0, with the gradient norm when `gn` is set.
 void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
                             int barrier_mode, cudaStream_t stream);
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
                          int replication, int blocks, int threads, cudaStream_t stream, double* gn = nullptr,
-                         double* cta_sq = nullptr, unsigned* ticket = nullptr);
+                         double* cta_sq = nullptr, unsigned* ticket = nullptr, float* acc = nullptr, int acc_mode = 0);
 void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64_t flag, uint32_t seq, int channel,
                          int host_ok, int exchange, cudaStream_t stream, const double* const* gn = nullptr,
                          int nunits = 0, float max_norm = 0.f, float* norm = nullptr);

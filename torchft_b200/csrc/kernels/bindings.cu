@@ -233,13 +233,14 @@ PYBIND11_MODULE(_K, m) {
   m.def(
       "zero1_reduce",
       [](const PeerTableH& pt, uintptr_t ok, uintptr_t mc_base, size_t off, size_t nelem, float scale, int replication,
-         int blocks, int threads, uintptr_t stream, uintptr_t gn, uintptr_t cta_sq, uintptr_t ticket) {
+         int blocks, int threads, uintptr_t stream, uintptr_t gn, uintptr_t cta_sq, uintptr_t ticket, uintptr_t acc,
+         int acc_mode) {
         zero1_reduce_launch(pt.pt, P<const int>(ok), P<void>(mc_base), off, nelem, scale, replication, blocks, threads, S(stream),
-                            P<double>(gn), P<double>(cta_sq), P<unsigned>(ticket));
+                            P<double>(gn), P<double>(cta_sq), P<unsigned>(ticket), P<float>(acc), acc_mode);
       },
       py::arg("pt"), py::arg("ok"), py::arg("mc_base"), py::arg("off"), py::arg("nelem"), py::arg("scale"),
       py::arg("replication"), py::arg("blocks"), py::arg("threads"), py::arg("stream"), py::arg("gn") = 0,
-      py::arg("cta_sq") = 0, py::arg("ticket") = 0);
+      py::arg("cta_sq") = 0, py::arg("ticket") = 0, py::arg("acc") = 0, py::arg("acc_mode") = 0);
   m.def(
       "zero1_commit",
       [](const PeerTableH& pt, const Status& st, uintptr_t gate, uint64_t flag, uint32_t seq, int channel,

@@ -30,6 +30,10 @@
 // kernel adds every rank's partials in rank order into the global norm and the clip coefficient -- vetoing the step on
 // every rank when the norm is not finite -- and the update kernel scales the gradient by that coefficient.
 //
+// Gradient accumulation (opt-in, ACC template mode / non-null accumulator): every micro-batch but the last reduces its
+// slice in fp32 into a per-rank accumulator of the primary slices only (no bf16 rounding, no gradient write, no push);
+// the last one adds the accumulator and finishes exactly like a single step (scale, bf16, buddy push, CLIP squares).
+//
 // The two big kernels contain NO inter-rank synchronisation at all: any grid size, no co-residency requirement, no
 // SM held by a spinning CTA while peers are skewed, profilable stand-alone. Ordering comes from the one-CTA handshake
 // kernels around them (bounded, abortable spins; epoch-tagged flags; error latched in the status block and mirrored
@@ -109,7 +113,27 @@ struct RSArgs {
   double* gn;
   double* cta_sq;
   unsigned* ticket;
+  // gradient accumulation (ACC != kAccOff): this rank's fp32 accumulator of the unit's primary slice; vector v of the
+  // slice lives at acc + (v - lo(rank)) * 8. acc_first (uniform per launch): store the sum instead of adding it.
+  float* acc;
+  int acc_first;
 };
+
+// Accumulation mode of the reduce kernel, for a step of M micro-batches:
+//   kAccOff  -- M = 1: scale, round to bf16, store to this rank and its k-1 buddies
+//   kAccAcc  -- micro-batches 0 .. M-2: the fp32 rank sum goes to the accumulator (micro-batch 0 stores, later ones
+//               add); nothing is rounded, written to the gradient segment or pushed
+//   kAccLast -- micro-batch M-1: (accumulator + rank sum) * scale, then exactly as kAccOff
+enum : int { kAccOff = 0, kAccAcc = 1, kAccLast = 2 };
+
+// 16-byte vectors in flight per thread. A P2P vector holds W x 16 B of loads in registers, the accumulator 32 B more;
+// the counts keep every instantiation inside the 128 registers of __launch_bounds__(512, 1) without spilling (W = 7
+// keeps three plain vectors in flight, not four).
+__host__ __device__ constexpr int reduce_unroll(int W, bool NVLS, int ACC) {
+  if (ACC == kAccOff) return NVLS ? 8 : (W >= 8 ? 2 : (W == 7 ? 3 : (W >= 3 ? 4 : 8)));
+  if (NVLS) return 6;
+  return W <= 1 ? 8 : (W <= 4 ? 4 : (W <= 6 ? 3 : 2));
+}
 
 __device__ __forceinline__ float sumsq8(const Vec16& v) {
   float f[8];
@@ -156,8 +180,39 @@ __device__ __forceinline__ void finish_unit_sumsq(const RSArgs& a, float sq) {
   }
 }
 
-template <int W, bool NVLS, bool CLIP>
+// What happens to vector v once its fp32 rank sum s is in registers (`av`: the accumulator's two 16-byte halves,
+// loaded when `load_acc`). kAccAcc stores acc + s (or s) back to the accumulator; the other modes scale (kAccLast: acc + s
+// first), round to bf16 and store to this rank and its buddies.
+template <int W, bool CLIP, int ACC>
+__device__ __forceinline__ void reduce_epilogue(const RSArgs& a, size_t v, size_t lo, float* s, const Vec16* av,
+                                                bool load_acc, bf16* const* dst, int k, float& sq) {
+  if constexpr (ACC != kAccOff) {
+    if (load_acc) {
+      float p[8];
+      Pack<float>::unpack(av[0], p);
+      Pack<float>::unpack(av[1], p + 4);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) s[i] = p[i] + s[i];  // ((s_1 + s_2) + ...) + s_m, in micro-batch order
+    }
+  }
+  if constexpr (ACC == kAccAcc) {
+    float* o = a.acc + (v - lo) * 8;
+    st_stream(o, Pack<float>::pack(s));
+    st_stream(o + 4, Pack<float>::pack(s + 4));
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s[i] *= a.scale;
+    const Vec16 out = P8::pack(s);
+    if constexpr (CLIP) sq += sumsq8(out);
+#pragma unroll
+    for (int j = 0; j < W; ++j)
+      if (j < k) st_stream(dst[j] + v * 8, out);
+  }
+}
+
+template <int W, bool NVLS, bool CLIP, int ACC>
 __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
+  static_assert(!(CLIP && ACC == kAccAcc), "an accumulating micro-batch produces no bf16 gradient to take the norm of");
   if (*a.ok == 0) return;
   const int rank = a.pt.rank;
   const Geo g(a.nelem, W);
@@ -171,11 +226,25 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
   const char* mcbase = a.mc + a.off;
   const int k = min(a.replication, W);
   const size_t lo = g.lo(rank), hi = g.hi(rank);
-  // CLIP at W = 7: three vectors per thread in flight instead of four, so the extra accumulator does not spill
-  constexpr int U = NVLS ? 8 : ((W >= 8) ? 2 : ((CLIP && W == 7) ? 3 : (W >= 3 ? 4 : 8)));
+  constexpr int U = reduce_unroll(W, NVLS, ACC);
+  constexpr int UA = ACC != kAccOff ? U : 1;  // accumulator vectors held in registers
+  const bool load_acc = ACC == kAccLast || (ACC == kAccAcc && !a.acc_first);
   const size_t stride = (size_t)gridDim.x * blockDim.x * U;
   float sq = 0.f;  // CLIP: squares of the bf16 values this thread stores
   for (size_t base = lo + (size_t)blockIdx.x * blockDim.x * U; base < hi; base += stride) {
+    Vec16 av[UA][2];
+    if constexpr (ACC != kAccOff) {
+      if (load_acc) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const size_t v = base + threadIdx.x + (size_t)u * blockDim.x;
+          if (v < hi) {
+            av[u][0] = ld_stream(a.acc + (v - lo) * 8);
+            av[u][1] = ld_stream(a.acc + (v - lo) * 8 + 4);
+          }
+        }
+      }
+    }
     if constexpr (NVLS) {
       Vec16 r[U];
 #pragma unroll
@@ -189,13 +258,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
         if (v < hi) {
           float f[8];
           P8::unpack(r[u], f);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) f[i] *= a.scale;
-          const Vec16 out = P8::pack(f);
-          if constexpr (CLIP) sq += sumsq8(out);
-#pragma unroll
-          for (int j = 0; j < W; ++j)
-            if (j < k) st_stream(dst[j] + v * 8, out);
+          reduce_epilogue<W, CLIP, ACC>(a, v, lo, f, av[ACC != kAccOff ? u : 0], load_acc, dst, k, sq);
         }
       }
     } else {
@@ -220,13 +283,7 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) acc[i] += f[i];
           }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i] *= a.scale;
-          const Vec16 out = P8::pack(acc);
-          if constexpr (CLIP) sq += sumsq8(out);
-#pragma unroll
-          for (int j = 0; j < W; ++j)
-            if (j < k) st_stream(dst[j] + v * 8, out);
+          reduce_epilogue<W, CLIP, ACC>(a, v, lo, acc, av[ACC != kAccOff ? u : 0], load_acc, dst, k, sq);
         }
       }
     }
@@ -453,25 +510,33 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   }
 }
 
-template <bool NVLS, bool CLIP>
+template <bool NVLS, bool CLIP, int ACC>
 void launch_rs(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
   switch (a.pt.world) {
     case 1:
-      // one rank: only the clipping path launches it (scale in place + the unit's sum of squares); never multicast
-      if constexpr (CLIP && !NVLS) {
-        zero1_reduce_kernel<1, false, true><<<blocks, threads, 0, s>>>(a);
+      // one rank: only clipping and accumulation launch it (in place, no peer access); never multicast
+      if constexpr ((CLIP || ACC != kAccOff) && !NVLS) {
+        zero1_reduce_kernel<1, false, CLIP, ACC><<<blocks, threads, 0, s>>>(a);
         break;
       }
       throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
-    case 2: zero1_reduce_kernel<2, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_reduce_kernel<3, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_reduce_kernel<4, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_reduce_kernel<5, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_reduce_kernel<6, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_reduce_kernel<7, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_reduce_kernel<8, NVLS, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 2: zero1_reduce_kernel<2, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 3: zero1_reduce_kernel<3, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 4: zero1_reduce_kernel<4, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 5: zero1_reduce_kernel<5, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 6: zero1_reduce_kernel<6, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 7: zero1_reduce_kernel<7, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
+    case 8: zero1_reduce_kernel<8, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
     default: throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
   }
+}
+
+template <bool CLIP, int ACC>
+void launch_rs_path(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
+  if (a.mc != nullptr)
+    launch_rs<true, CLIP, ACC>(a, blocks, threads, s);
+  else
+    launch_rs<false, CLIP, ACC>(a, blocks, threads, s);
 }
 
 template <bool NVLS, bool PAGED, bool CLIP>
@@ -513,22 +578,30 @@ void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, u
 
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
                          int replication, int blocks, int threads, cudaStream_t stream, double* gn, double* cta_sq,
-                         unsigned* ticket) {
+                         unsigned* ticket, float* acc, int acc_mode) {
   check_grid(blocks, threads, "zero1_reduce");
   if ((off & 15) || (nelem & 7)) throw std::runtime_error("zero1_reduce: unit must be 16 B aligned and a multiple of 8 elements");
   if (replication < 1) throw std::runtime_error("zero1_reduce: replication must be >= 1");
   if (gn != nullptr && (cta_sq == nullptr || ticket == nullptr))
     throw std::runtime_error("zero1_reduce: the gradient norm needs the per-CTA scratch and the ticket");
-  RSArgs a{pt, ok, reinterpret_cast<char*>(mc_base), off, nelem, scale, replication, gn, cta_sq, ticket};
-  if (gn != nullptr) {
-    if (mc_base != nullptr)
-      launch_rs<true, true>(a, blocks, threads, stream);
+  if (acc_mode < 0 || acc_mode > 3) throw std::runtime_error("zero1_reduce: acc_mode must be 0 (off), 1 (first), 2 (middle) or 3 (last)");
+  if (acc_mode != 0 && (acc == nullptr || (reinterpret_cast<uintptr_t>(acc) & 15)))
+    throw std::runtime_error("zero1_reduce: accumulation needs a 16 B aligned fp32 accumulator");
+  if ((acc_mode == 1 || acc_mode == 2) && gn != nullptr)
+    throw std::runtime_error("zero1_reduce: the gradient norm is taken on the last micro-batch only");
+  RSArgs a{pt, ok, reinterpret_cast<char*>(mc_base), off, nelem, scale, replication, gn, cta_sq, ticket,
+           acc_mode != 0 ? acc : nullptr, acc_mode == 1 ? 1 : 0};
+  if (acc_mode == 1 || acc_mode == 2) {
+    launch_rs_path<false, kAccAcc>(a, blocks, threads, stream);
+  } else if (acc_mode == 3) {
+    if (gn != nullptr)
+      launch_rs_path<true, kAccLast>(a, blocks, threads, stream);
     else
-      launch_rs<false, true>(a, blocks, threads, stream);
-  } else if (mc_base != nullptr) {
-    launch_rs<true, false>(a, blocks, threads, stream);
+      launch_rs_path<false, kAccLast>(a, blocks, threads, stream);
+  } else if (gn != nullptr) {
+    launch_rs_path<true, kAccOff>(a, blocks, threads, stream);
   } else {
-    launch_rs<false, false>(a, blocks, threads, stream);
+    launch_rs_path<false, kAccOff>(a, blocks, threads, stream);
   }
   TFT_CUDA_CHECK(cudaGetLastError());
 }

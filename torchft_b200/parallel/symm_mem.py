@@ -812,14 +812,27 @@ class SymmetricComm:
 
     def zero1_reduce_scatter_(self, segment: str, off: int, nelem: int, scale: float, contribute: bool,
                               replication: int, blocks: int, stream: Optional[torch.cuda.Stream] = None,
-                              gnorm: int = 0) -> None:
+                              gnorm: int = 0, acc: int = 0, acc_mode: int = 0) -> None:
         """Reduce-scatter ``nelem`` bf16 elements at byte offset ``off`` of ``segment`` in place: afterwards rank r
         (and its ``replication - 1`` successors) hold the scaled sum of slice r. Three launches on ``stream``:
         handshake ("my unit is ready") -> sync-free reduce kernel (any grid) -> handshake ("my pushes landed").
 
         ``gnorm`` (device address of one fp64, 0 = off): the kernel also writes there the sum of squares of the bf16
         values of slice r it produced (this rank's partial of the global gradient norm). At world 1 that is the one
-        reduce launch: it scales the unit in place, with no handshake."""
+        reduce launch: it scales the unit in place, with no handshake.
+
+        Gradient accumulation over micro-batches: ``acc`` is the device address of this rank's fp32 accumulator of
+        slice r (16 B aligned, one fp32 per element of the slice) and ``acc_mode`` says which micro-batch this is: 0
+        off, 1 first (store the fp32 sum of slice r there), 2 middle (add it), 3 last (scale accumulator + sum, round to
+        bf16 and store like mode 0; ``gnorm`` allowed). Modes 1 and 2 leave the gradient segment untouched and push
+        nothing. The handshakes are the same in every mode; the trailing one is what lets the peers overwrite their
+        gradients with the next micro-batch. At world 1 every mode but 0 is one launch with no handshake."""
+        if acc_mode not in (0, 1, 2, 3):
+            raise ValueError(f"acc_mode must be 0 (off), 1 (first), 2 (middle) or 3 (last), got {acc_mode}")
+        if acc_mode and not acc:
+            raise ValueError("gradient accumulation needs the accumulator's device address")
+        if acc_mode in (1, 2) and gnorm:
+            raise ValueError("the gradient norm is taken on the last micro-batch only (acc_mode 3)")
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -828,13 +841,14 @@ class SymmetricComm:
                 # healing / spare replica: its gradients count as zeros (reference manager.py:441-442)
                 self._K.memset_async(self._segments[segment].ptr + off, 0, nelem * 2, sp)
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
-            if gnorm:
-                scratch, ticket = self._z1_norm_scratch_ptrs()
+            if gnorm or acc_mode:
+                scratch, ticket = self._z1_norm_scratch_ptrs() if gnorm else (0, 0)
                 one = self._world == 1
                 if not one:
                     self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
                 self._K.zero1_reduce(self._tables[segment], self._z1_ok(2 if one else 0), self._mc_base(segment, nelem * 2),
-                                     off, nelem, scale, replication, blocks, self._threads, sp, gnorm, scratch, ticket)
+                                     off, nelem, scale, replication, blocks, self._threads, sp, gnorm, scratch, ticket,
+                                     acc if acc_mode else 0, acc_mode)
                 self.launches += 1
                 if not one:
                     self._handshake(0, True, _CH_ALLREDUCE, sp)

@@ -56,6 +56,10 @@ class FaultTolerantTrainer:
         max_grad_norm: FT-ZeRO-1: clip the global L2 norm of the reduced gradient to this, on the device; a step with a
             non-finite norm is skipped on every replica (``inf``: only that). ``None``: env
             ``TORCHFT_B200_Z1_MAX_GRAD_NORM``, unset = no clipping. Not available on the classic all-reduce pipeline.
+        grad_accum_steps: FT-ZeRO-1: micro-batches per optimizer step (``M``). ``step`` and friends then take
+            ``(M * B, S)`` inputs, run ``M`` forward/backward passes of ``B`` sequences and apply the gradient of the mean
+            loss over all of them; each micro-batch is reduce-scattered under its own backward into an fp32
+            accumulator of this replica's slices. Not available on the classic all-reduce pipeline.
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -68,7 +72,8 @@ class FaultTolerantTrainer:
                  activation_checkpoint: Optional[str] = None, init_sync: bool = False,
                  use_async_quorum: bool = True, overlap_optimizer: Optional[bool] = None,
                  optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2,
-                 compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None) -> None:
+                 compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None,
+                 grad_accum_steps: int = 1) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -83,6 +88,12 @@ class FaultTolerantTrainer:
         self.zero1 = bool(zero1)
         if max_grad_norm is not None and not self.zero1:
             raise ValueError("max_grad_norm needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if int(grad_accum_steps) != grad_accum_steps or grad_accum_steps < 1:
+            raise ValueError(f"grad_accum_steps must be an integer >= 1, got {grad_accum_steps}")
+        if grad_accum_steps > 1 and not self.zero1:
+            raise ValueError("grad_accum_steps > 1 needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        self.grad_accum_steps = int(grad_accum_steps)
+        self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
 
         # the replica group's own store (group world size 1 => this process hosts it)
         self._store = TCPStore("127.0.0.1", 0, is_master=True, wait_for_workers=False)
@@ -108,7 +119,8 @@ class FaultTolerantTrainer:
             # the optimizer owns the five symmetric flat buffers; FlatParams adopts two of them. Units (= gradient
             # buckets = update launches) are the forward stages, known once the parameters have offsets.
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
-                                       compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm)
+                                       compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
+                                       grad_accum_steps=self.grad_accum_steps)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:
@@ -199,7 +211,11 @@ class FaultTolerantTrainer:
     def _reduce_unit(self, bucket: int, start: int, end: int) -> Any:
         m = self.manager
         unit = self._bucket_unit[bucket]
-        return m.guarded(lambda: self.zopt.reduce_scatter(unit, 1.0 / max(m.num_participants(), 1), m.is_participating()))
+        if self.grad_accum_steps == 1:
+            return m.guarded(lambda: self.zopt.reduce_scatter(unit, 1.0 / max(m.num_participants(), 1), m.is_participating()))
+        micro, steps = self._micro, self.grad_accum_steps
+        return m.guarded(lambda: self.zopt.reduce_scatter(unit, 1.0 / (max(m.num_participants(), 1) * steps),
+                                                          m.is_participating(), micro))
 
     # ------------------------------------------------- classic pipeline pieces
     def _optimizer_step(self) -> None:
@@ -243,7 +259,10 @@ class FaultTolerantTrainer:
 
     # -------------------------------------------------------------------- step
     def step_device(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
-        """One fault-tolerant optimisation step on device-resident inputs; returns the loss tensor (device)."""
+        """One fault-tolerant optimisation step on device-resident inputs; returns the loss tensor (device). With
+        ``grad_accum_steps = M`` the inputs are ``(M * B, S)`` and the loss is the mean over the ``M`` micro-batches."""
+        if self.zero1 and self.grad_accum_steps > 1:
+            return self._step_accumulate(tokens, targets)
         if self.zero1:
             self.manager.start_quorum()       # async; its thread first books the previous step's device verdict
             self.flat.reset_grads()           # wgrad GEMMs write the flat gradient buffer directly: no memset
@@ -262,6 +281,36 @@ class FaultTolerantTrainer:
         if self.manager.should_commit():  # OptimizerWrapper.step() semantics (optim.py), with the update
             self._optimizer_step()        # cut per layer so the next forward overlaps it
         return loss
+
+    def _step_accumulate(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
+        """FT-ZeRO-1 step over ``M`` micro-batches: one quorum, ``M`` forward/backward passes whose reduce-scatters
+        accumulate on the comm stream, one commit and one update."""
+        M = self.grad_accum_steps
+        if tokens.shape[0] % M or tokens.shape[0] == 0 or targets.shape[0] != tokens.shape[0]:
+            raise ValueError(f"grad_accum_steps={M} must divide the batch dimension of tokens and targets, got "
+                             f"{tuple(tokens.shape)} and {tuple(targets.shape)}")
+        B = tokens.shape[0] // M
+        cur = torch.cuda.current_stream()
+        read_done = torch.cuda.Event()
+        losses = []
+        self.manager.start_quorum()              # once: the quorum is fixed for all micro-batches of the step
+        for m in range(M):
+            self._micro = m
+            self.flat.reset_grads()
+            loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B])  # overlaps micro-batch m-1's tail
+            if m > 0:
+                # backward overwrites the gradient buffer that the peers read in micro-batch m-1's reduce-scatters:
+                # wait until its last trailing handshake ("every peer is done reading mine") has passed
+                cur.wait_event(read_done)
+            loss.backward()
+            self.ddp.finish(wait=False)
+            if m < M - 1:
+                read_done.record(self.pg.comm_stream)
+            losses.append(loss.detach().float())
+        self.manager.commit_on_device(self.zopt)
+        self.zopt.update(self._opt_events)
+        self._opt_pending = True
+        return torch.stack(losses).mean()
 
     def _stage_inputs(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor) -> None:
         B, S = tokens_cpu.shape

@@ -43,7 +43,7 @@ Range = Tuple[int, int]
 
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
            "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges",
-           "clip_threshold"]
+           "clip_threshold", "accum_offsets", "accum_elements", "accum_mode"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
@@ -258,6 +258,36 @@ def pool_pages(layout: ShardLayout, min_world: int, page: int = 1 << PAGE_SHIFT,
     return best
 
 
+# --------------------------------------------------------------------------- gradient accumulation
+def accum_offsets(layout: ShardLayout, rank: int, world: int) -> Tuple[List[int], int]:
+    """Where each unit's primary slice of quorum rank ``rank`` lives in its fp32 accumulator: per-unit offsets in
+    elements, in unit order, and the elements the accumulator needs. The slices are packed back to back; each is a
+    multiple of 8 elements, so every offset is 32-byte aligned."""
+    offsets, n = [], 0
+    for u in range(len(layout.units)):
+        offsets.append(n)
+        lo, hi = layout.slice_bounds(u, world, rank)
+        n += hi - lo
+    return offsets, n
+
+
+def accum_elements(layout: ShardLayout, min_world: int, max_world: int = 8) -> int:
+    """Accumulator elements that hold any rank's primary slices at every world in ``[min_world, max_world]``."""
+    if not 1 <= min_world <= max_world:
+        raise ValueError(f"min_world must be in [1, {max_world}]")
+    return max(accum_offsets(layout, r, w)[1] for w in range(min_world, max_world + 1) for r in range(w))
+
+
+def accum_mode(micro: int, steps: int) -> int:
+    """``acc_mode`` of the reduce launch for micro-batch ``micro`` of ``steps``: 0 without accumulation (``steps`` = 1),
+    1 for the first micro-batch (stores), 2 for the middle ones (add), 3 for the last (reduces to bf16)."""
+    if steps < 1 or not 0 <= micro < steps:
+        raise ValueError(f"micro-batch {micro} is not in [0, {steps})")
+    if steps == 1:
+        return 0
+    return 1 if micro == 0 else (3 if micro == steps - 1 else 2)
+
+
 # --------------------------------------------------------------------------- the optimizer
 class Zero1Optimizer:
     """AdamW with fp32 master/m/v partitioned over the replicas of the current quorum (see module doc).
@@ -280,6 +310,13 @@ class Zero1Optimizer:
     every replica (counted in ``nonfinite_steps``): no state changes and ``t`` does not advance. ``grad_norm`` is the
     device scalar of the last commit, ``last_grad_norm`` the host value of the last resolved step.
 
+    With ``grad_accum_steps = M > 1`` one step reduces ``M`` micro-batches: :meth:`reduce_scatter` takes the micro-batch
+    index, micro-batches ``0 .. M-2`` add their fp32 reduced slice into an accumulator that covers only this rank's
+    primary slices (an ordinary device tensor of about ``4 * numel / min_world`` bytes, :meth:`accum_bytes`), and the
+    last one adds its own, scales by the caller's ``scale`` and rounds to bf16 once. The first micro-batch of a step
+    overwrites the accumulator, so nothing of an aborted step survives into the next. A step in which some unit was
+    not reduced ``M`` times is vetoed (:meth:`enqueue`).
+
     Args:
         pg: a ``ProcessGroupB200`` (symmetric segments must be allocated before its first ``configure``)
         numel: elements of the flat parameter vector (multiple of 8)
@@ -291,16 +328,24 @@ class Zero1Optimizer:
         page_shift: compact: pages of ``2**page_shift`` elements
         max_grad_norm: clip the global gradient norm to this (``inf``: only veto non-finite steps; ``None``: env
             ``TORCHFT_B200_Z1_MAX_GRAD_NORM``, unset = no clipping)
+        grad_accum_steps: micro-batches per step (``M``); the accumulator is sized for every world in
+            ``[min_world, 8]``
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
                  betas: Tuple[float, float] = (0.9, 0.95), eps: float = 1e-8, weight_decay: float = 0.1,
                  replication: int = 2, blocks: Optional[int] = None, compact: Optional[bool] = None, min_world: int = 1,
                  state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT,
-                 max_grad_norm: Optional[float] = None) -> None:
+                 max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1) -> None:
         from torchft_b200.ops import _native
 
         self.max_grad_norm = clip_threshold(max_grad_norm)
+        if int(grad_accum_steps) != grad_accum_steps or grad_accum_steps < 1:
+            raise ValueError(f"grad_accum_steps must be an integer >= 1, got {grad_accum_steps}")
+        self.grad_accum_steps = int(grad_accum_steps)
+        self._acc: Optional[torch.Tensor] = None      # accumulation: fp32 primary slices of this rank, packed
+        self._acc_offsets: List[int] = []             # ... element offset of each unit's slice in it
+        self._acc_for: Optional[Tuple[int, int]] = None  # ... the (rank, world) the offsets were computed for
         assert numel % 8 == 0
         self._K = _native.load()
         self.pg = pg
@@ -358,6 +403,7 @@ class Zero1Optimizer:
         self._commit_event: Optional[torch.cuda.Event] = None
         self.lost_elements = 0           # state elements that had to be re-seeded because no holder survived
         self.pulled_bytes = 0
+        self._micro_seen: List[int] = [0] * len(self.layout.units)  # accumulation: micro-batches reduced per unit
         if units is not None:
             self.set_units(units)
         pg.add_configure_hook(self._on_configured)
@@ -371,8 +417,34 @@ class Zero1Optimizer:
         if self.compact and self.capacity:
             raise RuntimeError("compact state: the units are fixed once the page pools are allocated")
         self.layout = ShardLayout(tuple((int(a), int(b)) for a, b in units), self._replication)
+        self._micro_seen = [0] * len(self.layout.units)
         if self.compact:
             self._alloc_pools()
+        if self.grad_accum_steps > 1:
+            self._alloc_accum()
+
+    def _alloc_accum(self) -> None:
+        """One fp32 accumulator for this rank's primary slices, large enough for every world in ``[min_world, 8]``.
+        Only this rank reads it, so it is an ordinary device tensor, not a symmetric segment."""
+        self._acc = None  # a re-allocation for new units frees the old one first
+        self._acc = torch.empty(accum_elements(self.layout, self.min_world), dtype=torch.float32, device=self.device)
+        self._acc_for = None
+
+    def _accum_for(self, rank: int, world: int) -> None:
+        """Point the accumulator offsets at this quorum's slice geometry; raises when the slices do not fit."""
+        if self._acc is None:
+            self._alloc_accum()
+        need = max(accum_offsets(self.layout, r, world)[1] for r in range(world))
+        if need > self._acc.numel():
+            # the same numbers on every rank: all of them raise alike
+            raise RuntimeError(f"zero1: gradient accumulation at a quorum of {world} needs {4 * need} accumulator bytes "
+                               f"per rank, {self.accum_bytes()} are allocated (sized for min_world={self.min_world})")
+        self._acc_offsets = accum_offsets(self.layout, rank, world)[0]
+        self._acc_for = (rank, world)
+
+    def accum_bytes(self) -> int:
+        """Device bytes of the gradient-accumulation buffer (0 without accumulation)."""
+        return 0 if self._acc is None else 4 * self._acc.numel()
 
     def _alloc_pools(self) -> None:
         import numpy as np
@@ -431,6 +503,8 @@ class Zero1Optimizer:
                 # the kernels dereference peer pointers: every replica must construct its Zero1Optimizer before its first
                 # quorum (segments allocated later only become symmetric at the NEXT quorum change)
                 raise RuntimeError(f"FT-ZeRO-1 segments {missing} are not mapped on every replica of this quorum")
+            if self.grad_accum_steps > 1:
+                self._accum_for(rank, world)
             me = {"t": self.t, "hold": self._holdings}
             if self.compact:
                 if world < self.min_world:
@@ -605,9 +679,13 @@ class Zero1Optimizer:
     def unit_of(self, lo: int, hi: int) -> int:
         return self.layout.units.index((lo, hi))
 
-    def reduce_scatter(self, unit: int, scale: float, contribute: bool) -> Any:
-        """Reduce unit ``unit`` of the gradient buffer across the quorum (comm stream, overlaps backward)."""
+    def reduce_scatter(self, unit: int, scale: float, contribute: bool, micro: int = 0) -> Any:
+        """Reduce unit ``unit`` of the gradient buffer across the quorum (comm stream, overlaps backward). With
+        gradient accumulation, ``micro`` is the micro-batch index; ``scale`` applies on the last micro-batch only."""
         lo, hi = self.layout.units[unit]
+        mode = accum_mode(micro, self.grad_accum_steps)
+        if mode:
+            return self._reduce_accum(unit, lo, hi, scale, contribute, micro, mode)
         if self.max_grad_norm is not None:
             gn = self._gnorm.data_ptr() + 8 * unit
             after = self._commit_event
@@ -630,13 +708,48 @@ class Zero1Optimizer:
             lambda s: self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s),
             None)
 
+    def _reduce_accum(self, unit: int, lo: int, hi: int, scale: float, contribute: bool, micro: int, mode: int) -> Any:
+        """One micro-batch's reduce of ``unit`` into (modes 1, 2) or out of (mode 3) the accumulator. The reduce kernel
+        runs at world 1 too (in place, no handshake): the scale belongs after the sum over micro-batches."""
+        rank, world = self.comm.rank, self.comm.world
+        if self._acc_for != (rank, world):
+            self._accum_for(rank, world)
+        acc = self._acc.data_ptr() + 4 * self._acc_offsets[unit]
+        gn = self._gnorm.data_ptr() + 8 * unit if self.max_grad_norm is not None and mode == 3 else 0
+        after = self._commit_event if self.max_grad_norm is not None else None
+        k = self.layout.replication
+
+        def launch(s: torch.cuda.Stream) -> None:
+            if after is not None:
+                # the last commit kernel read the partials this step's last micro-batch overwrites
+                s.wait_event(after)
+            self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s,
+                                            gnorm=gn, acc=acc, acc_mode=mode)
+
+        work = self.pg._launch(launch, None)
+        # micro-batches must arrive in order from 0; anything else poisons the unit until the next micro-batch 0
+        in_order = micro == 0 or self._micro_seen[unit] == micro
+        self._micro_seen[unit] = micro + 1 if in_order else -1
+        return work
+
     # -- committer protocol of Manager.commit_on_device ---------------------------------------------------------
     def bind_stream(self, stream: torch.cuda.Stream) -> None:
         """The stream the verdict and update kernels run on (the trainer's optimizer stream)."""
         self._commit_stream = stream
 
     def enqueue(self, host_ok: bool) -> int:
-        """Enqueue the verdict kernel behind this step's reduce-scatters (comm stream) and backward (current stream)."""
+        """Enqueue the verdict kernel behind this step's reduce-scatters (comm stream) and backward (current stream).
+
+        With gradient accumulation a unit that was not reduced for all ``M`` micro-batches (e.g. the Manager stopped
+        launching after an error) makes the local verdict negative; the kernel still runs, so the peers learn of it."""
+        if self.grad_accum_steps > 1:
+            seen, self._micro_seen = self._micro_seen, [0] * len(self.layout.units)
+            short = [u for u, n in enumerate(seen) if n != self.grad_accum_steps]
+            if short:
+                if host_ok:
+                    logger.warning("zero1: units %s were not reduced for all %d micro-batches: the step is vetoed",
+                                   short, self.grad_accum_steps)
+                host_ok = False
         stream = self._commit_stream
         stream.wait_stream(self.pg.comm_stream)
         stream.wait_stream(torch.cuda.current_stream(self.device))
