@@ -1,0 +1,328 @@
+"""FT-ZeRO-1 durable checkpoints on ONE GPU: save under the next step, restore at another world and into compact state,
+partial restarts next to a live replica, fallback and refusal on real files, and the trainer.
+
+Ranks are emulated in-process with ``SymmetricComm.virtual_world`` (pre-signalled, see ``test_zero1_gpu.py``); every
+rank launches on the current stream, the snapshot copies run on the optimizer's own stream.
+"""
+
+from __future__ import annotations
+
+import os
+import threading
+from datetime import timedelta
+
+import pytest
+import torch
+
+from test_zero1_accum_gpu import _PG
+
+pytestmark = pytest.mark.gpu
+
+# large enough that the snapshot copy is still running when the next step's update is enqueued
+UNITS = [(0, 8 * 131072), (8 * 131072, 8 * 131072 + 8 * 50021), (8 * 131072 + 8 * 50021, 8 * 131072 + 8 * 50028)]
+NUMEL = UNITS[-1][1]
+HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)
+SHIFT = 8
+K = 2
+
+
+def _init():
+    dev = torch.device("cuda", 0)
+    return (torch.randn(NUMEL, device=dev, generator=torch.Generator(device=dev).manual_seed(2)) * 0.05).bfloat16()
+
+
+def _raws(world, seed):
+    dev = torch.device("cuda", 0)
+    g = torch.Generator(device=dev).manual_seed(seed)
+    return [(torch.randn(NUMEL, device=dev, generator=g) * 0.01 * (r + 1)).bfloat16() for r in range(world)]
+
+
+class _Reps:
+    """``n`` virtual ranks, each with a ``Zero1Optimizer``, driven in the Manager's order through quorum changes."""
+
+    def __init__(self, n, compact=False, min_world=1, units=UNITS):
+        from torch.distributed import HashStore
+
+        from torchft_b200.parallel.symm_mem import SymmetricComm
+        from torchft_b200.parallel.zero1 import ShardLayout, pool_pages
+
+        n_state = (pool_pages(ShardLayout(tuple(units), K), min_world, 1 << SHIFT) << SHIFT) if compact else NUMEL
+        seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, **{x: n_state * 4 for x in ("z1_master", "z1_m", "z1_v")}}
+        self.comms = SymmetricComm.virtual_world(n, seg, presignal=True, timeout=timedelta(seconds=20))
+        self.opts = [self.make(c, compact, min_world, units) for c in self.comms]
+        for o in self.opts:
+            o.param.copy_(_init())
+            o.seed_master()
+        self.store = HashStore()
+        self.members = list(range(n))
+        self.pending = None
+
+    @staticmethod
+    def make(comm, compact=False, min_world=1, units=UNITS):
+        from torchft_b200.parallel.zero1 import Zero1Optimizer
+
+        return Zero1Optimizer(_PG(comm), NUMEL, units=units, lr=HP[0], betas=HP[1:3], eps=HP[3], weight_decay=HP[4],
+                              replication=K, blocks=4, compact=compact, min_world=min_world, page_shift=SHIFT)
+
+    def configure(self, members, epoch):
+        from torch.distributed import PrefixStore
+
+        from torchft_b200.parallel.symm_mem import SymmetricComm
+
+        self.settle()
+        SymmetricComm.virtual_quorum(self.comms, members, epoch)
+        errs = []
+
+        def run(rank, m):
+            try:
+                self.opts[m]._on_configured(PrefixStore(f"q/{epoch}", self.store), rank, len(members), epoch)
+            except Exception as e:  # noqa: BLE001
+                errs.append(e)
+
+        ts = [threading.Thread(target=run, args=(rank, m)) for rank, m in enumerate(members)]
+        [t.start() for t in ts]
+        [t.join() for t in ts]
+        assert not errs, errs
+        torch.cuda.synchronize()
+        self.members = list(members)
+
+    def settle(self):
+        if self.pending is not None:
+            for m, s in self.pending.items():
+                self.opts[m].resolved(self.opts[m].wait(s))
+            self.pending = None
+
+    def step(self, seed):
+        """One step without a host synchronisation: gradients, reduce-scatters, verdicts and updates are enqueued."""
+        self.settle()
+        world = len(self.members)
+        raws = _raws(world, seed)
+        for rank, i in enumerate(self.members):
+            self.opts[i].grad.copy_(raws[rank])
+        for i in self.members:
+            for u in range(len(UNITS)):
+                self.opts[i].reduce_scatter(u, 1.0 / world, True)
+        self.pending = {i: self.opts[i].enqueue(True) for i in self.members}
+        for i in self.members:
+            self.opts[i].update()
+
+    def save(self, directory, keep=2):
+        self.settle()
+        t = {self.opts[i].save(directory, {"step": self.opts[i].t, "batches_committed": 0}, keep=keep) for i in self.members}
+        assert len(t) == 1
+        return t.pop()
+
+    def full_state(self):
+        """(master, m, v) over the whole vector, assembled from the holders, and the weights."""
+        self.settle()
+        out = [torch.full((NUMEL,), float("nan"), device="cuda") for _ in range(3)]
+        for i in self.members:
+            for (lo, hi), arrs in self.opts[i].held_state().items():
+                for o, a in zip(out, arrs):
+                    o[lo:hi] = a
+        return out, self.opts[self.members[0]].param.clone()
+
+    def check_against(self, ref, param):
+        self.settle()
+        for i in self.members:
+            o = self.opts[i]
+            assert torch.equal(o.param, param), f"weights of member {i}"
+            for (lo, hi), arrs in o.held_state().items():
+                for name, a, r in zip(("master", "m", "v"), arrs, ref):
+                    assert torch.equal(a, r[lo:hi]), f"{name} of member {i} over {(lo, hi)}"
+
+
+def _chain(world):
+    """Quorums a live run of 4 goes through to reach ``world`` without losing state (k = 2)."""
+    return {4: [[0, 1, 2, 3]], 3: [[0, 1, 2]], 1: [[0, 2], [0]]}[world]
+
+
+@pytest.mark.parametrize("world,compact", [(4, False), (3, False), (1, False), (3, True)])
+def test_save_under_the_next_step_and_restore_at_another_world(tmp_path, world, compact):
+    live = _Reps(4)
+    live.configure([0, 1, 2, 3], 1)
+    live.step(11)
+    live.step(12)
+    ref, param = live.full_state()
+    assert not torch.isnan(ref[0]).any()
+    assert live.save(str(tmp_path)) == 2
+    live.step(13)  # immediately: the update of each unit waits for that unit's snapshot copy, not for the host
+    for o in live.opts:
+        o.wait_checkpoint()
+    live.settle()
+    assert all(o.t == 3 for o in live.opts)
+    assert sorted(os.listdir(tmp_path)) == [f"z1_step_2.w4.r{r}.bin" for r in range(4)]
+
+    back = _Reps(world, compact=compact, min_world=3 if compact else 1)
+    for o in back.opts:
+        o.master.fill_(float("nan"))  # a re-shard must fill every held element
+        assert o.restore(str(tmp_path)) == {"step": 2, "batches_committed": 0}
+        assert torch.equal(o.param, param) and o.t == 2
+    back.configure(list(range(world)), 1)
+    back.check_against(ref, param)
+    assert all(o.lost_elements == 0 for o in back.opts)
+    assert sum(o.disk_read_elements for o in back.opts) == sum(
+        sum(hi - lo for lo, hi in o.layout.held(r, world)) for r, o in enumerate(back.opts))
+
+    # a live run that changed 4 -> world at T = 2 and the restored one agree bit for bit two steps later
+    ctl = _Reps(4)
+    ctl.configure([0, 1, 2, 3], 1)
+    ctl.step(11)
+    ctl.step(12)
+    for e, members in enumerate(_chain(world)):
+        ctl.configure(members, 2 + e)
+    for seed in (21, 22):
+        ctl.step(seed)
+        back.step(seed)
+    st, p = ctl.full_state()
+    back.check_against(st, p)
+    assert all(o.t == 4 for o in back.opts) and all(ctl.opts[i].lost_elements == 0 for i in ctl.members)
+
+
+def test_partial_restart_pulls_from_the_live_replica_and_reads_the_rest(tmp_path):
+    from torchft_b200.parallel.zero1 import intersect_ranges, subtract_ranges, total
+
+    live = _Reps(4)
+    live.configure([0, 1, 2, 3], 1)
+    live.step(31)
+    live.step(32)
+    ref, param = live.full_state()
+    live.save(str(tmp_path))
+    for o in live.opts:
+        o.wait_checkpoint()
+    for r in (1, 2, 3):  # these processes restart; member 0 stays alive at T = 2
+        o = _Reps.make(live.comms[r])
+        o.param.zero_()
+        for a in (o.master, o.m, o.v):
+            a.fill_(float("nan"))
+        assert o.restore(str(tmp_path))["step"] == 2
+        live.opts[r] = o
+    live.configure([0, 1, 2, 3], 2)
+    live.check_against(ref, param)
+    L = live.opts[0].layout
+    for r in (1, 2, 3):
+        o = live.opts[r]
+        assert o.pulled_bytes == 12 * total(intersect_ranges(L.held(r, 4), L.held(0, 4)))
+        assert o.disk_read_elements == total(subtract_ranges(L.held(r, 4), L.held(0, 4))) > 0
+        assert o.lost_elements == 0
+    assert live.opts[0].pulled_bytes == 0 and live.opts[0].disk_read_elements == 0
+
+
+def test_missing_and_torn_files_fall_back_and_a_mismatch_refuses(tmp_path):
+    live = _Reps(2)
+    live.configure([0, 1], 1)
+    live.step(41)
+    live.save(str(tmp_path))
+    live.step(42)
+    live.save(str(tmp_path))
+    live.step(43)
+    live.save(str(tmp_path))  # keep = 2: step 1's files are pruned
+    for o in live.opts:
+        o.wait_checkpoint()
+    _, p2 = live.full_state()  # the weights of step 3
+    assert sorted(os.listdir(tmp_path)) == [f"z1_step_{t}.w2.r{r}.bin" for t in (2, 3) for r in (0, 1)]
+
+    def restore_one():
+        o = _Reps(1).opts[0]
+        return o.restore(str(tmp_path)), o
+
+    sd, o = restore_one()
+    assert sd["step"] == 3 and torch.equal(o.param, p2)
+    with open(tmp_path / "z1_step_3.w2.r1.bin", "r+b") as f:  # torn: step 3 is incomplete
+        f.truncate(os.path.getsize(tmp_path / "z1_step_3.w2.r1.bin") // 2)
+    sd, o = restore_one()
+    assert sd["step"] == 2 and o.t == 2
+    os.remove(tmp_path / "z1_step_2.w2.r0.bin")  # missing: nothing is complete
+    sd, o = restore_one()
+    assert sd is None and o.t == 0 and torch.equal(o.param, _init())
+    # another unit split (as with another optimizer_blocks) refuses before touching anything
+    other = _Reps(1, units=[(0, UNITS[1][0]), (UNITS[1][0], NUMEL)]).opts[0]
+    with pytest.raises(ValueError, match="units"):
+        other.restore(str(tmp_path))
+    assert other.t == 0 and torch.equal(other.param, _init())
+
+
+# ----------------------------------------------------------------------------- trainer
+def _trainer(tag, **kw):
+    from torchft_b200.bench_utils import local_lighthouse, loopback
+    from torchft_b200.parallel.trainer import FaultTolerantTrainer
+
+    lh = local_lighthouse()
+    tr = FaultTolerantTrainer("llama3_debug", loopback(lh.address()), replica_id=f"z1ckpt_{tag}_0",
+                              timeout=timedelta(seconds=30), **kw)
+    return tr, lh
+
+
+def _batches(cfg, n):
+    gen = torch.Generator().manual_seed(9)
+    return [(torch.randint(0, cfg.vocab_size, (2, 128), generator=gen).pin_memory(),
+             torch.randint(0, cfg.vocab_size, (2, 128), generator=gen).pin_memory()) for _ in range(n)]
+
+
+def test_trainer_resumes_bit_identically_where_the_durable_checkpointer_route_does_not(tmp_path):
+    from torchft_b200.checkpointing import DurableCheckpointer
+
+    sharded, classic = str(tmp_path / "sharded"), str(tmp_path / "classic")
+    tr, lh = _trainer("a")
+    try:
+        data = _batches(tr.cfg, 5)
+        for tok, tgt in data[:3]:
+            tr.step(tok, tgt)
+        assert tr.save_checkpoint(sharded) == 3
+        dc = DurableCheckpointer(tr.manager, tr.state_dict, tr.load_state_dict, classic)
+        assert dc.maybe_save(force=True)
+        dc.wait()
+        live = [tr.step(tok, tgt) for tok, tgt in data[3:]]
+        tr.wait_checkpoint()
+        with pytest.raises(RuntimeError, match="before the first step"):
+            tr.restore_checkpoint(sharded)
+        tr.join()
+        p_live = tr.zopt.param.clone()
+        assert tr.manager.current_step() == 5
+    finally:
+        tr.shutdown()
+        lh.shutdown()
+
+    tr, lh = _trainer("b")
+    try:
+        assert tr.restore_checkpoint(sharded) == 3
+        assert tr.manager.current_step() == 3
+        resumed = [tr.step(tok, tgt) for tok, tgt in data[3:]]
+        tr.join()
+        assert resumed == live
+        assert torch.equal(tr.zopt.param, p_live)
+        assert tr.manager.current_step() == 5 and tr.zopt.lost_elements == 0
+    finally:
+        tr.shutdown()
+        lh.shutdown()
+
+    # the route this exists to replace: weights and t come back, master / m / v do not, so training continues from
+    # the initial master weights with zero moments
+    tr, lh = _trainer("c")
+    try:
+        assert DurableCheckpointer(tr.manager, tr.state_dict, tr.load_state_dict, classic).restore() == 3
+        for tok, tgt in data[3:]:
+            tr.step(tok, tgt)
+        tr.join()
+        assert not torch.equal(tr.zopt.param, p_live)
+    finally:
+        tr.shutdown()
+        lh.shutdown()
+
+
+def test_trainer_refusals(tmp_path):
+    tr, lh = _trainer("classic", zero1=False)
+    try:
+        with pytest.raises(ValueError, match="FT-ZeRO-1"):
+            tr.save_checkpoint(str(tmp_path))
+        with pytest.raises(ValueError, match="FT-ZeRO-1"):
+            tr.restore_checkpoint(str(tmp_path))
+    finally:
+        tr.shutdown()
+        lh.shutdown()
+    tr, lh = _trainer("empty")
+    try:
+        assert tr.restore_checkpoint(str(tmp_path / "nothing")) is None
+    finally:
+        tr.shutdown()
+        lh.shutdown()

@@ -29,7 +29,7 @@ import os
 import re
 import threading
 import time
-from typing import Any, Callable, Dict, List, Optional
+from typing import Any, BinaryIO, Callable, Dict, List, Optional, Sequence
 
 import torch
 from torch.utils import _pytree as pytree
@@ -38,7 +38,7 @@ from torchft_b200.checkpointing._serialization import streaming_load, streaming_
 
 logger = logging.getLogger(__name__)
 
-__all__ = ["DurableCheckpointer"]
+__all__ = ["DurableCheckpointer", "BackgroundWriter", "atomic_write", "prune_steps"]
 
 _NAME = re.compile(r"^step_(\d+)\.rank_(\d+)\.pt$")
 
@@ -53,6 +53,57 @@ def _to_host(tree: Any) -> Any:
         return x
 
     return pytree.tree_map(leaf, tree)
+
+
+def atomic_write(path: str, write: Callable[[BinaryIO], None]) -> None:
+    """Write ``path`` through a temporary file next to it, fsync it and ``os.replace`` it into place (atomic on POSIX):
+    a reader sees the previous file or the complete new one, never a partial write under the final name."""
+    tmp = f"{path}.tmp.{os.getpid()}"
+    with open(tmp, "wb") as f:
+        write(f)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+
+
+def prune_steps(paths: Dict[int, Sequence[str]], keep: int) -> None:
+    """Remove the files of every step but the ``keep`` newest (``paths[step]``: that step's files)."""
+    for step in sorted(paths)[: -keep]:
+        for path in paths[step]:
+            try:
+                os.remove(path)
+            except OSError:
+                pass
+
+
+class BackgroundWriter:
+    """At most one write in flight, on a daemon thread; an exception it raises is re-raised by the next :meth:`wait`
+    (and so by the next :meth:`start`) instead of being lost."""
+
+    def __init__(self, what: str) -> None:
+        self._what = what
+        self._thread: Optional[threading.Thread] = None
+        self._error: Optional[BaseException] = None
+
+    def start(self, fn: Callable[..., None], *args: Any) -> None:
+        self.wait()
+        self._thread = threading.Thread(target=self._run, args=(fn, args), name="tft_ckpt_writer", daemon=True)
+        self._thread.start()
+
+    def _run(self, fn: Callable[..., None], args: Any) -> None:
+        try:
+            fn(*args)
+        except BaseException as e:  # noqa: BLE001 - reported on the next wait()
+            self._error = e
+
+    def wait(self) -> None:
+        """Block until the in-flight write (if any) has finished; re-raises its error."""
+        if self._thread is not None:
+            self._thread.join()
+            self._thread = None
+        if self._error is not None:
+            e, self._error = self._error, None
+            raise RuntimeError(f"{self._what} write failed: {e}") from e
 
 
 class DurableCheckpointer:
@@ -77,8 +128,7 @@ class DurableCheckpointer:
         self._keep = keep
         self._group_rank = int(group_rank if group_rank is not None else getattr(manager, "_group_rank", 0))
         self._last_saved_step = -1
-        self._writer: Optional[threading.Thread] = None
-        self._error: Optional[BaseException] = None
+        self._writer = BackgroundWriter("durable checkpoint")
         os.makedirs(directory, exist_ok=True)
 
     # ------------------------------------------------------------------ save
@@ -101,31 +151,22 @@ class DurableCheckpointer:
         self.wait()  # at most one write in flight; surfaces the previous write's error
         payload = {"user": _to_host(self._state_dict()), "torchft": dict(self._manager.state_dict())}
         self._last_saved_step = step
-        self._writer = threading.Thread(target=self._write, args=(step, payload), name="tft_durable_ckpt", daemon=True)
-        self._writer.start()
+        self._writer.start(self._write, step, payload)
         return True
 
     def _path(self, step: int) -> str:
         return os.path.join(self._dir, f"step_{step}.rank_{self._group_rank}.pt")
 
     def _write(self, step: int, payload: Dict[str, Any]) -> None:
-        try:
-            t0 = time.perf_counter()
-            final = self._path(step)
-            tmp = f"{final}.tmp.{os.getpid()}"
-            with open(tmp, "wb") as f:
-                streaming_save(payload, f)
-                f.flush()
-                os.fsync(f.fileno())
-            os.replace(tmp, final)
-            marker = os.path.join(self._dir, f"LATEST.rank_{self._group_rank}")
-            with open(marker + ".tmp", "w") as f:
-                f.write(os.path.basename(final))
-            os.replace(marker + ".tmp", marker)
-            self._prune()
-            logger.info("durable checkpoint step %d written in %.2fs -> %s", step, time.perf_counter() - t0, final)
-        except BaseException as e:  # noqa: BLE001 - reported on the next maybe_save()/wait()
-            self._error = e
+        t0 = time.perf_counter()
+        final = self._path(step)
+        atomic_write(final, lambda f: streaming_save(payload, f))
+        marker = os.path.join(self._dir, f"LATEST.rank_{self._group_rank}")
+        with open(marker + ".tmp", "w") as f:
+            f.write(os.path.basename(final))
+        os.replace(marker + ".tmp", marker)
+        self._prune()
+        logger.info("durable checkpoint step %d written in %.2fs -> %s", step, time.perf_counter() - t0, final)
 
     def _mine(self) -> List[int]:
         steps = []
@@ -136,20 +177,11 @@ class DurableCheckpointer:
         return sorted(steps)
 
     def _prune(self) -> None:
-        for step in self._mine()[: -self._keep]:
-            try:
-                os.remove(self._path(step))
-            except OSError:
-                pass
+        prune_steps({step: [self._path(step)] for step in self._mine()}, self._keep)
 
     def wait(self) -> None:
         """Block until the in-flight write (if any) is on disk; re-raises its error."""
-        if self._writer is not None:
-            self._writer.join()
-            self._writer = None
-        if self._error is not None:
-            e, self._error = self._error, None
-            raise RuntimeError(f"durable checkpoint write failed: {e}") from e
+        self._writer.wait()
 
     # --------------------------------------------------------------- restore
     def latest_step(self) -> Optional[int]:

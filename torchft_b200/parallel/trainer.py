@@ -94,6 +94,7 @@ class FaultTolerantTrainer:
             raise ValueError("grad_accum_steps > 1 needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         self.grad_accum_steps = int(grad_accum_steps)
         self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
+        self._steps_run = 0  # steps started by this trainer (a checkpoint restore must come first)
 
         # the replica group's own store (group world size 1 => this process hosts it)
         self._store = TCPStore("127.0.0.1", 0, is_master=True, wait_for_workers=False)
@@ -261,6 +262,7 @@ class FaultTolerantTrainer:
     def step_device(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
         """One fault-tolerant optimisation step on device-resident inputs; returns the loss tensor (device). With
         ``grad_accum_steps = M`` the inputs are ``(M * B, S)`` and the loss is the mean over the ``M`` micro-batches."""
+        self._steps_run += 1
         if self.zero1 and self.grad_accum_steps > 1:
             return self._step_accumulate(tokens, targets)
         if self.zero1:
@@ -346,6 +348,42 @@ class FaultTolerantTrainer:
         self._loss_event.record()
         return prev
 
+    # ----------------------------------------------------- durable checkpoints (FT-ZeRO-1)
+    def _require_zero1_ckpt(self) -> None:
+        if not self.zero1:
+            raise ValueError("save_checkpoint / restore_checkpoint need the FT-ZeRO-1 pipeline (backend='b200', "
+                             "zero1=True); the classic pipeline keeps its full optimizer state on every replica and "
+                             "checkpoints with checkpointing.DurableCheckpointer")
+
+    def save_checkpoint(self, directory: str, keep: int = 2) -> int:
+        """Write this replica's share of a durable checkpoint of the last committed step to ``directory`` (shared by
+        every replica of the job) and return its step ``T`` once the write is enqueued. Call it on every replica after
+        the same step. The copy to host memory runs under the next step's forward and backward; the file is written by
+        a background thread (:meth:`wait_checkpoint`). The ``keep`` newest steps this replica wrote are kept."""
+        self._require_zero1_ckpt()
+        ms = self.manager.state_dict()  # settles the last step's deferred verdict: the host learns T, no other sync
+        assert ms["step"] == self.zopt.t, (ms, self.zopt.t)
+        return self.zopt.save(directory, ms, self._opt_events, keep)
+
+    def wait_checkpoint(self) -> None:
+        """Block until the last :meth:`save_checkpoint` is on disk; raises if the write failed."""
+        self._require_zero1_ckpt()
+        self.zopt.wait_checkpoint()
+
+    def restore_checkpoint(self, directory: str) -> Optional[int]:
+        """Before the first step: resume from the newest complete checkpoint in ``directory``. Returns its step, or
+        ``None`` when there is none (a fresh run). Works at any number of replicas: ranges a live replica of the same
+        step still holds are pulled from it at the first quorum, the rest are read from the files. The data loader's
+        position is the caller's to restore from the returned step."""
+        self._require_zero1_ckpt()
+        if self._steps_run:
+            raise RuntimeError("restore_checkpoint must be called before the first step")
+        ms = self.zopt.restore(directory)
+        if ms is None:
+            return None
+        self.manager.load_state_dict(ms)
+        return int(ms["step"])
+
     def last_grad_norm(self) -> Optional[float]:
         """Global gradient norm of the most recently resolved step (FT-ZeRO-1 with clipping; ``None`` otherwise). Steps
         resolve lazily, so after step ``n`` this is usually the norm of step ``n - 1``."""
@@ -362,5 +400,7 @@ class FaultTolerantTrainer:
     def shutdown(self) -> None:
         if self._opt_stream is not None:
             self._opt_stream.synchronize()
+        if self.zopt is not None:
+            self.zopt.wait_checkpoint()  # a checkpoint write in flight lands (or raises) before the process moves on
         self.manager.shutdown(wait=False)
         self.pg.shutdown()

@@ -43,7 +43,7 @@ Range = Tuple[int, int]
 
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
            "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges",
-           "clip_threshold", "accum_offsets", "accum_elements", "accum_mode"]
+           "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
@@ -171,6 +171,40 @@ def plan_pulls(need: Sequence[Range], holdings: Dict[int, Sequence[Range]], me: 
             pulls.append((r, lo, hi))
         left = subtract_ranges(left, got)
     return pulls, left
+
+
+# --------------------------------------------------------------------------- durable checkpoints
+def newest_complete_step(headers: Sequence[Dict[str, Any]], numel: int) -> Optional[int]:
+    """The newest update count ``T`` whose checkpoint files together cover ``[0, numel)`` (``None``: there is none).
+    ``headers[i]`` has ``T`` and the written ``ranges`` (``[lo, hi, offset]``). Files of one ``T`` may come from quorums
+    of different sizes: holders at the same update count hold the same bits."""
+    by_t: Dict[int, List[Range]] = {}
+    for h in headers:
+        by_t.setdefault(int(h["T"]), []).extend((int(lo), int(hi)) for lo, hi, _ in h["ranges"])
+    for t in sorted(by_t, reverse=True):
+        if merge_ranges(by_t[t]) == [(0, numel)]:
+            return t
+    return None
+
+
+def ckpt_read_plan(need: Sequence[Range], files: Sequence[Tuple[Any, Sequence[Tuple[int, int, int]]]]
+                   ) -> List[Tuple[Any, int, int, int]]:
+    """Cover ``need`` from checkpoint files of one update count: ``[(file, offset, lo, hi), ...]`` reads elements
+    ``[lo, hi)`` of the flat vector from element ``offset`` of ``file``'s arrays. ``files[i] = (file, ranges)`` with the
+    written ``ranges`` as ``(lo, hi, offset)``; earlier files are preferred. Raises ``ValueError`` when the files do not
+    cover ``need``."""
+    reads: List[Tuple[Any, int, int, int]] = []
+    left = merge_ranges(need)
+    for f, ranges in files:
+        if not left:
+            break
+        for lo, hi, off in ranges:
+            for a, b in intersect_ranges(left, [(lo, hi)]):
+                reads.append((f, int(off) + a - int(lo), a, b))
+        left = subtract_ranges(left, [(lo, hi) for lo, hi, _ in ranges])
+    if left:
+        raise ValueError(f"the checkpoint files do not cover {left}")
+    return reads
 
 
 # --------------------------------------------------------------------------- compact (paged) state
@@ -317,6 +351,14 @@ class Zero1Optimizer:
     overwrites the accumulator, so nothing of an aborted step survives into the next. A step in which some unit was
     not reduced ``M`` times is vetoed (:meth:`enqueue`).
 
+    Durable checkpoints (:meth:`save` / :meth:`restore`, format in ``checkpointing/sharded.py``): every replica writes
+    the bf16 weights and (master, m, v) over its primary slices at one committed update count ``T``, so the files of
+    one quorum tile the flat vector. The snapshot is a device-to-host copy on its own stream, unit by unit behind that
+    unit's update; the next update of a unit waits for its copy, and a re-shard waits on the host for the whole
+    snapshot, so forward and backward of the next step run under the copy. :meth:`restore` reads the weights, sets
+    ``t = T`` and claims no state; the next re-shard reads the ranges that no live holder at ``T`` has from the files,
+    instead of re-seeding them. Without a save nothing is allocated and :meth:`update` launches and waits as before.
+
     Args:
         pg: a ``ProcessGroupB200`` (symmetric segments must be allocated before its first ``configure``)
         numel: elements of the flat parameter vector (multiple of 8)
@@ -404,6 +446,13 @@ class Zero1Optimizer:
         self.lost_elements = 0           # state elements that had to be re-seeded because no holder survived
         self.pulled_bytes = 0
         self._micro_seen: List[int] = [0] * len(self.layout.units)  # accumulation: micro-batches reduced per unit
+        self._configured = False         # a quorum has been configured (restore must come before)
+        self._ckpt: Any = None           # durable checkpoints: ShardedWriter (staging buffer, writer thread)
+        self._snap_stream: Optional[torch.cuda.Stream] = None
+        self._snap_events: Optional[List[torch.cuda.Event]] = None  # per unit: its snapshot copy has been enqueued
+        self._snap_done: Optional[torch.cuda.Event] = None          # ... and the whole snapshot
+        self._disk: Optional[Tuple[int, str, List[Any]]] = None  # restore: (T, directory, files) for the next re-shard
+        self.disk_read_elements = 0      # state elements re-shards read from a restored checkpoint's files
         if units is not None:
             self.set_units(units)
         pg.add_configure_hook(self._on_configured)
@@ -497,6 +546,9 @@ class Zero1Optimizer:
     def _on_configured(self, store: Any, rank: int, world: int, epoch: int) -> None:
         """Runs inside ``ProcessGroupB200.configure`` (quorum thread) with the quorum-scoped store."""
         with self._lock:
+            if self._snap_done is not None:
+                # a snapshot copy may still read the state that pulls, seeds, page reuse and heal are about to rewrite
+                self._snap_done.synchronize()
             names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ())
             missing = [n for n in names if not self.comm.is_symmetric(n)]
             if missing:
@@ -506,6 +558,8 @@ class Zero1Optimizer:
             if self.grad_accum_steps > 1:
                 self._accum_for(rank, world)
             me = {"t": self.t, "hold": self._holdings}
+            if self._disk is not None:
+                me["disk"] = [self._disk[0], self._disk[1]]  # every rank may read what no live holder has from it
             if self.compact:
                 if world < self.min_world:
                     raise RuntimeError(f"zero1: a quorum of {world} is below min_world={self.min_world}; the compact "
@@ -518,6 +572,7 @@ class Zero1Optimizer:
                     peers[r] = json.loads(bytes(store.get(f"z1/{r}")).decode())
             if self.compact:
                 self._reshard_compact(store, rank, world, peers)
+                self._configured, self._disk = True, None
                 return
             tmax = max(int(p["t"]) for p in peers.values())
             if self.t < tmax:
@@ -525,9 +580,14 @@ class Zero1Optimizer:
             valid = {r: [tuple(x) for x in p["hold"]] for r, p in peers.items() if int(p["t"]) == tmax and r != rank}
             need = subtract_ranges(self.layout.held(rank, world), self._holdings)
             pulls, lost = plan_pulls(need, valid, rank)
+            reads = self._disk_reads(lost, tmax, peers)
+            if reads:
+                lost = []
             with torch.cuda.stream(self._reshard_stream):
                 if pulls:
                     self._pull(pulls)
+                if reads:
+                    self._read_state(reads)
                 for lo, hi in lost:
                     # every holder vanished in one transition: re-seed from the replicated bf16 weights
                     self.master[lo:hi].copy_(self.param[lo:hi])
@@ -544,6 +604,7 @@ class Zero1Optimizer:
             self.t = tmax
             self._holdings = merge_ranges(list(self._holdings) + list(need))
             self._refresh_pending = world > 1
+            self._configured, self._disk = True, None
 
     def _pull(self, pulls: List[Tuple[int, int, int]]) -> None:
         """One heal_copy launch that gathers (master, m, v)[lo:hi] from the source ranks' segments."""
@@ -629,6 +690,9 @@ class Zero1Optimizer:
             raise RuntimeError(f"zero1: re-sharding to a quorum of {world} needs {peak} state pages on one rank, the "
                                f"pools hold {self.capacity} (raise min_world's range or state_pages)")
         need, pulls, lost = plans[rank]
+        reads = self._disk_reads(lost, tmax, peers)
+        if reads:
+            lost = []
         new_pages, src_pages, _ = pages[rank]
         mine_old = old[rank]
         free_first, allocate, free_last = reshard_page_steps(mine_old, new_pages, src_pages)
@@ -657,6 +721,8 @@ class Zero1Optimizer:
                             for c, d, mine in self._pieces(self._table_host, a, b):
                                 entries.append((ptrs[src] + (at + c - a) * 4, local.data_ptr() + mine * 4, (d - c) * 4))
                 device_copy(entries, s, chunk_bytes=1 << 20)
+            if reads:
+                self._read_state(reads)  # nobody live holds these at T: the restored checkpoint does
             self._seed(lost)  # nobody holds these: re-seed from the replicated bf16 weights
         s.synchronize()
         self.comm._store_barrier(store, "z1/pulled", world)  # every peer has finished reading our source pages
@@ -785,7 +851,10 @@ class Zero1Optimizer:
         coef = self._clip.data_ptr() + 4 if self.max_grad_norm is not None else 0
         modes = (1, 0) if self._refresh_pending else (0,)
         self._refresh_pending = False
+        snap, self._snap_events = self._snap_events, None
         for i, (lo, hi) in enumerate(self.layout.units):
+            if snap is not None:
+                stream.wait_event(snap[i])  # the last save's copy of this unit has read it
             for mode in modes:
                 if self.compact:
                     self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr(),
@@ -813,6 +882,154 @@ class Zero1Optimizer:
                     self.nonfinite_steps += 1
                     logger.warning("zero1: gradient norm is %s: the step was skipped on every replica (%d so far)",
                                    norm, self.nonfinite_steps)
+
+    # ------------------------------------------------------------------ durable checkpoints
+    @torch.no_grad()
+    def save(self, directory: str, manager_state: Optional[Dict[str, int]] = None,
+             events: Optional[Sequence[torch.cuda.Event]] = None, keep: int = 2) -> int:
+        """Snapshot this rank's primary slices (bf16 weights, master, m, v) at the update count ``t`` and write them to
+        ``directory`` in the background; returns ``t``. Every replica of the quorum calls it after the same step.
+
+        The last step's verdict must be resolved (``Manager.state_dict()`` does it). ``events[i]`` are the events
+        :meth:`update` recorded for unit ``i`` (default: everything enqueued on the commit stream so far);
+        ``manager_state`` is ``{"step", "batches_committed"}`` for the header. A save first waits for the previous
+        write and re-raises its error; :meth:`wait_checkpoint` waits for this one. ``keep`` newest steps of the files
+        this optimizer wrote are kept."""
+        if not self._configured:
+            raise RuntimeError("zero1: nothing to checkpoint before the first quorum")
+        if self._commit_layout is not None:
+            raise RuntimeError("zero1: the last step's verdict is not resolved; settle it first (Manager.state_dict())")
+        rank, world = self.comm.rank, self.comm.world
+        ranges = intersect_ranges(self.layout.primary(rank, world), self._holdings)
+        return self._save(directory, ranges, rank, world, manager_state, events, keep)
+
+    def _save(self, directory: str, ranges: Sequence[Range], rank: int, world: int,
+              manager_state: Optional[Dict[str, int]], events: Optional[Sequence[torch.cuda.Event]], keep: int) -> int:
+        from torchft_b200.checkpointing.sharded import ShardedWriter, sections
+
+        if self._ckpt is None or self._ckpt.directory != directory or self._ckpt.keep != keep:
+            if self._ckpt is not None:
+                self._ckpt.wait()
+            self._ckpt = ShardedWriter(directory, keep)
+        w = self._ckpt
+        w.wait()  # the previous write has left the staging buffer; surfaces its error
+        written, e = [], 0
+        for lo, hi in ranges:
+            written.append((lo, hi, e))
+            e += hi - lo
+        stage = w.staging(14 * e)
+        sec = sections(e)
+        if self._snap_stream is None:
+            self._snap_stream = torch.cuda.Stream(device=self.device)
+        s = self._snap_stream
+        after = None if events is not None else self._commit_stream.record_event()
+        u8 = torch.uint8
+        done: List[torch.cuda.Event] = []
+        with torch.cuda.stream(s):
+            for i, unit in enumerate(self.layout.units):
+                s.wait_event(events[i] if events is not None else after)  # unit i's update and weight pushes landed
+                for lo, hi, off in written:
+                    for a, b in intersect_ranges([(lo, hi)], [unit]):
+                        x = off + a - lo
+                        stage[2 * x:2 * (x + b - a)].copy_(self.param[a:b].view(u8), non_blocking=True)
+                        for name, arr in (("master", self.master), ("m", self.m), ("v", self.v)):
+                            base = sec[name] + 4 * x
+                            if not self.compact:
+                                stage[base:base + 4 * (b - a)].copy_(arr[a:b].view(u8), non_blocking=True)
+                                continue
+                            for c, d, at in self._pieces(self._table_host, a, b):  # maximal runs of consecutive slots
+                                stage[base + 4 * (c - a):base + 4 * (d - a)].copy_(arr[at:at + d - c].view(u8),
+                                                                                   non_blocking=True)
+                done.append(s.record_event())
+        self._snap_events, self._snap_done = done, done[-1]
+        ms = manager_state or {"step": self.t, "batches_committed": 0}
+        header = {"version": 1, "numel": self.numel, "units": [list(u) for u in self.layout.units], "T": self.t,
+                  "step": int(ms["step"]), "batches": int(ms["batches_committed"]), "world": world, "rank": rank,
+                  "k": self.layout.k(world), "compact": self.compact, "ranges": [list(r) for r in written],
+                  "elements": e, "sections": sec,
+                  "hparams": {"lr": self.param_groups[0]["lr"], "betas": list(self.betas), "eps": self.eps,
+                              "weight_decay": self.weight_decay, "max_grad_norm": self.max_grad_norm}}
+        w.submit(header, self._snap_done)
+        return self.t
+
+    def wait_checkpoint(self) -> None:
+        """Block until the last :meth:`save` is on disk; re-raises a failed write."""
+        if self._ckpt is not None:
+            self._ckpt.wait()
+
+    def snapshot_bytes(self) -> int:
+        """Pinned host bytes of the checkpoint staging buffer (0 before the first save)."""
+        stage = None if self._ckpt is None else self._ckpt.stage
+        return 0 if stage is None else stage.numel()
+
+    @torch.no_grad()
+    def restore(self, directory: str) -> Optional[Dict[str, int]]:
+        """Before the first quorum: load the newest complete checkpoint in ``directory``. Reads the full bf16 weights,
+        sets ``t`` to its update count ``T``, claims no state, and arms the next re-shard to read the ranges no live
+        holder at ``T`` has from the files. Returns the header's ``{"step", "batches_committed"}`` for the Manager, or
+        ``None`` when no update count is complete. Unreadable files are skipped; files written for another ``numel``
+        or other units raise ``ValueError`` before any state changes."""
+        from torchft_b200.checkpointing.sharded import check_compatible, scan
+
+        if self._configured:
+            raise RuntimeError("zero1: restore must be called before the first quorum")
+        headers = scan(directory)
+        check_compatible(headers, self.numel, self.layout.units)
+        T = newest_complete_step(headers, self.numel)
+        if T is None:
+            return None
+        files = [(h, [tuple(int(x) for x in r) for r in h["ranges"]]) for h in headers if int(h["T"]) == T]
+        self._read_ranges(ckpt_read_plan([(0, self.numel)], files), ("param",))
+        self._set_t(T)
+        self._holdings = []  # nothing held is current until the re-shard: the files or live peers at T provide it
+        self._disk = (T, directory, files)
+        self._reshard_stream.synchronize()  # the weights are in place before the first forward
+        first = files[0][0]
+        logger.info("zero1: restored the weights of update %d from %d checkpoint file(s) in %s", T, len(files), directory)
+        return {"step": int(first["step"]), "batches_committed": int(first["batches"])}
+
+    def _disk_reads(self, lost: Sequence[Range], tmax: int, peers: Dict[int, Dict[str, Any]]
+                    ) -> List[Tuple[Any, int, int, int]]:
+        """Reads that fill ``lost`` from a restored checkpoint at the quorum's update count: this rank's own, or one a
+        restored peer published (a live rank may now hold slices that only restored ranks held)."""
+        if not lost:
+            return []
+        if self._disk is not None and self._disk[0] == tmax:
+            return ckpt_read_plan(lost, self._disk[2])
+        for r in sorted(peers):
+            d = peers[r].get("disk")
+            if d and int(d[0]) == tmax:
+                from torchft_b200.checkpointing.sharded import scan
+
+                files = [(h, [tuple(int(x) for x in rg) for rg in h["ranges"]]) for h in scan(d[1]) if int(h["T"]) == tmax]
+                try:
+                    return ckpt_read_plan(lost, files)
+                except ValueError as e:
+                    logger.warning("zero1: checkpoint %s of update %d does not cover this rank's lost ranges: %s",
+                                   d[1], tmax, e)
+        return []
+
+    def _read_state(self, reads: Sequence[Tuple[Any, int, int, int]]) -> None:
+        self._read_ranges(reads, ("master", "m", "v"))
+        self.disk_read_elements += total([(lo, hi) for _, _, lo, hi in reads])
+
+    def _read_ranges(self, reads: Sequence[Tuple[Any, int, int, int]], arrays: Sequence[str]) -> None:
+        """``arrays`` over the flat ranges of ``reads`` from the files, through pinned bounce buffers, on the re-shard
+        stream (compact state: into the pool pages the table maps them to)."""
+        from torchft_b200.checkpointing.sharded import RangedReader
+
+        dst = {"param": self.param, "master": self.master, "m": self.m, "v": self.v}
+        rd = RangedReader(self._reshard_stream)
+        try:
+            for h, off, lo, hi in reads:
+                for name in arrays:
+                    if name == "param" or not self.compact:
+                        rd.read(h, name, off, dst[name][lo:hi])
+                        continue
+                    for a, b, at in self._pieces(self._table_host, lo, hi):
+                        rd.read(h, name, off + a - lo, dst[name][at:at + b - a])
+        finally:
+            rd.close()
 
     # ------------------------------------------------------------------ introspection
     def state_bytes_held(self) -> int:
