@@ -106,7 +106,8 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
 void rope_launch(const void* in, void* out, const void* cs, size_t T, int S, int heads, int D,
                  size_t in_stride, size_t out_stride, float sign, cudaStream_t s);
 void xent_launch(void* logits, const void* target, float* loss, size_t rows, int V,
-                 size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s);
+                 size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s,
+                 const float* scale = nullptr);
 void adamw_launch(void* p, float* master, float* m, float* v, const void* g, size_t n, float lr,
                   float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale,
                   const int* gate, int max_blocks, cudaStream_t s);

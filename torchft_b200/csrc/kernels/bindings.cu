@@ -400,10 +400,11 @@ PYBIND11_MODULE(_K, m) {
                     Hkv, dir, S(s));
   }, "RoPE + q/k/v split of a packed projection (dir 0) or its backward (dir 1), one launch");
   m.def("xent", [](uintptr_t logits, uintptr_t target, uintptr_t loss, size_t rows, int V,
-                   size_t row_stride, float grad_scale, long long ignore_index, uintptr_t s) {
+                   size_t row_stride, float grad_scale, long long ignore_index, uintptr_t s, uintptr_t scale) {
     xent_launch(P<void>(logits), P<void>(target), P<float>(loss), rows, V, row_stride, grad_scale,
-                ignore_index, S(s));
-  });
+                ignore_index, S(s), P<const float>(scale));
+  }, py::arg("logits"), py::arg("target"), py::arg("loss"), py::arg("rows"), py::arg("V"), py::arg("row_stride"),
+     py::arg("grad_scale"), py::arg("ignore_index"), py::arg("stream"), py::arg("scale") = 0);
   m.def("adamw", [](uintptr_t p, uintptr_t master, uintptr_t mm, uintptr_t v, uintptr_t g, size_t n,
                     float lr, float b1, float b2, float eps, float wd, float bc1, float bc2,
                     float gscale, uintptr_t gate, uintptr_t s, int max_blocks) {

@@ -396,15 +396,19 @@ __global__ void __launch_bounds__(256) rope_qkv_kernel(const RopeQKVArgs a) {
 // One CTA per row of logits [rows, V] (bf16). Writes loss[row] (fp32) and
 // overwrites the logits row with d(loss_sum * grad_scale)/dlogits in bf16.
 // Rows whose target == ignore_index get loss 0 and zero gradient.
+// `scale` (nullable) is a device factor on grad_scale, so a normaliser the host does not know (the count of
+// non-ignored targets) costs no host sync; a factor of exactly 1 leaves every result bit-identical.
 __global__ void __launch_bounds__(1024) xent_fwd_bwd_kernel(bf16* __restrict__ logits,
                                                             const long long* __restrict__ target,
                                                             float* __restrict__ loss, int V,
                                                             size_t row_stride, float grad_scale,
+                                                            const float* __restrict__ scale,
                                                             long long ignore_index) {
   __shared__ float red[32];
   const size_t row = blockIdx.x;
   bf16* lr = logits + row * row_stride;
   const long long tgt = target[row];
+  if (scale != nullptr) grad_scale *= *scale;
   const int nvec = V / 8;
   if (tgt == ignore_index) {
     for (int v = threadIdx.x; v < nvec; v += blockDim.x) st_stream(lr + v * 8, Vec16{0, 0, 0, 0});
@@ -840,6 +844,7 @@ void rmsnorm_tune(int bwd, int tpb, int prefetch, int ctas_per_sm_at_128) {
 void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int rows, int H,
                         float eps, cudaStream_t s) {
   if (H % 8 || H > 8 * kRmsMaxVec * 512) throw std::runtime_error("rmsnorm: H must be %8 and <= 16384");
+  if (rows == 0) return;  // a zero-CTA grid is an invalid launch
   int tpb, nv;
   rms_shape(H / 8, 0, tpb, nv);
   const int grid = rms_grid(rows, 0, tpb);
@@ -857,8 +862,11 @@ void rmsnorm_bwd_launch(const void* dy, const void* x, const void* w, const floa
   int tpb, nv;
   rms_shape(H / 8, 1, tpb, nv);
   const int grid = rms_grid(rows, 1, tpb);
-  RMS_DISPATCH(rmsnorm_bwd_kernel, 1, (const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd, (bf16*)dx, dw_partial,
-               (const bf16*)dres, rows, H);
+  // no rows: skip the (zero-CTA, invalid) row launch; the column sum over zero partials still writes dw = 0 (or leaves
+  // it unchanged when accumulating), the gradient of an empty batch
+  if (rows > 0)
+    RMS_DISPATCH(rmsnorm_bwd_kernel, 1, (const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd, (bf16*)dx, dw_partial,
+                 (const bf16*)dres, rows, H);
   colsum_kernel<<<(H + 31) / 32, 1024, 0, s>>>(dw_partial, grid, H, (bf16*)dw, accumulate);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
@@ -924,11 +932,11 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
 }
 
 void xent_launch(void* logits, const void* target, float* loss, size_t rows, int V,
-                 size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s) {
+                 size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s, const float* scale) {
   if (row_stride % 8) throw std::runtime_error("xent: row stride must be a multiple of 8");
   if (rows == 0) return;
   xent_fwd_bwd_kernel<<<(unsigned)rows, 1024, 0, s>>>((bf16*)logits, (const long long*)target, loss,
-                                                      V, row_stride, grad_scale, ignore_index);
+                                                      V, row_stride, grad_scale, scale, ignore_index);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

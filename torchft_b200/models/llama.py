@@ -164,7 +164,7 @@ class Llama(nn.Module):
         return x
 
     def forward(self, tokens: torch.Tensor, targets: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Returns the mean next-token loss when ``targets`` is given, else logits."""
+        """Returns the mean next-token loss over the targets that are not -100 when ``targets`` is given, else logits."""
         x = self.hidden(tokens)
         B, S, d = x.shape
         if self.stage_hook is not None:
@@ -172,7 +172,7 @@ class Llama(nn.Module):
         if targets is None:
             return fused.rmsnorm(x, self.norm, self.cfg.norm_eps) @ self.output.t()
         h = fused.rmsnorm(x, self.norm, self.cfg.norm_eps).view(B * S, d)
-        return fused.linear_cross_entropy(h, self.output, targets.reshape(-1), chunk=self.cfg.loss_chunk, count_valid=False)
+        return fused.linear_cross_entropy(h, self.output, targets.reshape(-1), chunk=self.cfg.loss_chunk)
 
 
 class FlatParams:

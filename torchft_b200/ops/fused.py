@@ -177,9 +177,13 @@ class _LinearCrossEntropy(torch.autograd.Function):
         K = _native.load()
         T, H = h.shape
         V = weight.shape[0]
-        # count_valid costs one host sync; training loops with no ignored
-        # targets (the synthetic-data bench) pass count_valid=False.
-        n_valid = max(int((target != ignore_index).sum().item()), 1) if count_valid else T
+        # count_valid: divide by the number of non-ignored targets, counted on the device (no host sync). The kernels
+        # keep grad_scale = 1/T and scale it by the device factor T / n_valid, which is exactly 1.0 when no target is
+        # ignored, so that case is bit-identical to count_valid=False (divide by T).
+        scale = None
+        if count_valid:
+            n_valid = (target != ignore_index).sum().clamp_(min=1).float()
+            scale = torch.full((), float(T), dtype=torch.float32, device=h.device).div_(n_valid)
         need_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         dh = torch.empty_like(h) if need_grad else None
         slot = getattr(weight, "_flat_grad", None)
@@ -194,7 +198,7 @@ class _LinearCrossEntropy(torch.autograd.Function):
             logits = hc @ weight.t()  # [c, V] bf16, cuBLAS
             K.xent(
                 logits.data_ptr(), target[lo:hi].data_ptr(), losses[lo:hi].data_ptr(), hi - lo, V,
-                logits.stride(0), 1.0 / n_valid, ignore_index, sp,
+                logits.stride(0), 1.0 / max(T, 1), ignore_index, sp, scale.data_ptr() if scale is not None else 0,
             )
             if need_grad:
                 torch.mm(logits, weight, out=dh[lo:hi])
@@ -202,7 +206,8 @@ class _LinearCrossEntropy(torch.autograd.Function):
             del logits
         ctx.save_for_backward(dh, dW)
         ctx.need = need_grad
-        return losses.sum() / n_valid
+        loss = losses.sum() / max(T, 1)
+        return loss * scale if scale is not None else loss
 
     @staticmethod
     def backward(ctx, g: torch.Tensor):  # type: ignore[override]
@@ -215,7 +220,10 @@ class _LinearCrossEntropy(torch.autograd.Function):
 
 def linear_cross_entropy(h: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, chunk: int = 2048,
                          ignore_index: int = -100, count_valid: bool = True) -> torch.Tensor:
-    """Mean cross entropy of ``h @ weight.T`` against ``target`` (int64)."""
+    """Mean cross entropy of ``h @ weight.T`` against ``target`` (int64).
+
+    With ``count_valid`` (the default) the mean is over targets that are not ``ignore_index``, counted on the device
+    without a host sync; with ``count_valid=False`` the sum is divided by the number of rows."""
     assert h.dim() == 2 and target.dim() == 1 and h.shape[0] == target.shape[0]
     return _LinearCrossEntropy.apply(h.contiguous(), weight, target.contiguous(), chunk, ignore_index, count_valid)
 
@@ -279,6 +287,10 @@ class FlatAdamW:
         underneath the (tensor-core-bound) GEMMs. ``streams_events`` = ``(stream, events)``."""
         K = _native.load()
         stream, events = streams_events
+        # the kernel's 16-byte vector path needs p + 2*lo to be 16-byte aligned
+        bad = [lo for lo, _ in ranges if lo % 8]
+        if bad:
+            raise ValueError(f"step_ranges: range starts must be multiples of 8 elements, got {bad}")
         self.t += 1
         lr = self.param_groups[0]["lr"]
         b1, b2 = self.betas
@@ -333,7 +345,7 @@ class _NormLinear(torch.autograd.Function):
         H = x.shape[-1]
         rows = x.numel() // H
         sp = _native.stream_ptr()
-        dy2 = dy.reshape(rows, -1)
+        dy2 = dy.reshape(rows, W.shape[0])
         n = torch.empty_like(x)
         K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, ctx.eps, sp)
         dW = _wgrad(dy2, n.view(rows, H), W)
@@ -383,7 +395,7 @@ class _NormLinearRes(torch.autograd.Function):
         H = x.shape[-1]
         rows = x.numel() // H
         sp = _native.stream_ptr()
-        dy2 = dy.reshape(rows, -1)
+        dy2 = dy.reshape(rows, W.shape[0])
         n = torch.empty_like(x)
         K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, ctx.eps, sp)
         dW = _wgrad(dy2, n.view(rows, H), W)
@@ -419,7 +431,7 @@ class _SwiGLULinear(torch.autograd.Function):
         a = torch.empty((T, F), dtype=gu.dtype, device=gu.device)
         K.swiglu_fwd(gu.data_ptr(), a.data_ptr(), T, F, _native.stream_ptr())
         # residual add rides in the GEMM epilogue (beta = 1) instead of a separate elementwise pass
-        out = a @ W2.t() if res is None else torch.addmm(res.reshape(T, -1), a, W2.t())
+        out = a @ W2.t() if res is None else torch.addmm(res.reshape(T, W2.shape[0]), a, W2.t())
         ctx.save_for_backward(gu, W2)
         ctx.has_res = res is not None
         return out.view(gu.shape[:-1] + (W2.shape[0],))
@@ -432,7 +444,7 @@ class _SwiGLULinear(torch.autograd.Function):
         F = F2 // 2
         T = gu.numel() // F2
         sp = _native.stream_ptr()
-        d2 = dout.reshape(T, -1)
+        d2 = dout.reshape(T, W2.shape[0])
         a = torch.empty((T, F), dtype=gu.dtype, device=gu.device)
         K.swiglu_fwd(gu.data_ptr(), a.data_ptr(), T, F, sp)
         dW2 = _wgrad(d2, a, W2)
@@ -457,7 +469,7 @@ class _Linear(torch.autograd.Function):
         if res is None:
             return x @ W.t()
         x2 = x.reshape(-1, x.shape[-1])
-        return torch.addmm(res.reshape(x2.shape[0], -1), x2, W.t()).view(x.shape[:-1] + (W.shape[0],))
+        return torch.addmm(res.reshape(x2.shape[0], W.shape[0]), x2, W.t()).view(x.shape[:-1] + (W.shape[0],))
 
     @staticmethod
     def backward(ctx, dy: torch.Tensor):  # type: ignore[override]
