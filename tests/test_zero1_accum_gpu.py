@@ -9,25 +9,24 @@ Ranks are emulated in-process with ``SymmetricComm.virtual_world`` (see ``test_z
 
 from __future__ import annotations
 
-import threading
 from datetime import timedelta
 
 import pytest
 import torch
 
+from _zero1_replicas import Replicas, ref_adamw
+
 pytestmark = pytest.mark.gpu
 
 UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
 NUMEL = UNITS[-1][1]
-HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)  # lr, b1, b2, eps, wd
-SHIFT = 8  # paged state: 256-element pages
 MAX_NORM = 50.0
 
 
-def _world(world, presignal=True, extra=None):
+def _world(world, presignal=True):
     from torchft_b200.parallel.symm_mem import SymmetricComm
 
-    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS), **(extra or {})}
+    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS)}
     return SymmetricComm.virtual_world(world, seg, presignal=presignal, timeout=timedelta(seconds=20))
 
 
@@ -205,113 +204,9 @@ def test_norm_of_the_accumulated_gradient(world, k):
 
 
 # ----------------------------------------------------------------------------- Zero1Optimizer
-class _PG:
-    """The slice of ``ProcessGroupB200`` that ``Zero1Optimizer`` uses, over one virtual-world rank whose segments exist;
-    collectives run on the current stream."""
-
-    def __init__(self, comm):
-        self.comm = comm
-        self.comm_stream = torch.cuda.current_stream()
-
-    def alloc_symmetric(self, name, nbytes):
-        seg = self.comm.segment(name)
-        assert seg.numel() >= nbytes
-        return seg[:nbytes]
-
-    def add_configure_hook(self, fn):
-        pass
-
-    def _launch(self, fn, result):
-        fn(self.comm_stream)
-        return None
-
-
-def _ref_adamw(master, m, v, g, t):
-    lr, b1, b2, eps, wd = HP
-    m.mul_(b1).add_(g, alpha=1 - b1)
-    v.mul_(b2).addcmul_(g, g, value=1 - b2)
-    bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t
-    denom = v.sqrt() / (bc2 ** 0.5) + eps
-    master.mul_(1 - lr * wd).addcdiv_(m, denom, value=-lr / bc1)
-
-
-class _Replicas:
-    """``n`` pre-signalled virtual ranks, each with a ``Zero1Optimizer`` accumulating ``M`` micro-batches, driven in the
-    Manager's order (enqueue / update / wait / resolved) through quorum changes."""
-
-    def __init__(self, n, M, compact=False, max_norm=None, min_world=3, k=2):
-        from torch.distributed import HashStore
-
-        from torchft_b200.parallel.zero1 import GNORM_UNITS, ShardLayout, Zero1Optimizer, pool_pages
-
-        self.M, self.k = M, k
-        n_state = (pool_pages(ShardLayout(tuple(UNITS), k), min_world, 1 << SHIFT) << SHIFT) if compact else NUMEL
-        extra = {x: n_state * 4 for x in ("z1_master", "z1_m", "z1_v")}
-        extra["z1_gnorm"] = GNORM_UNITS * 8
-        self.comms = _world(n, extra=extra)
-        dev = torch.device("cuda", 0)
-        self.init = (torch.randn(NUMEL, device=dev, generator=torch.Generator(device=dev).manual_seed(2)) * 0.05).bfloat16()
-        self.opts = []
-        for c in self.comms:
-            o = Zero1Optimizer(_PG(c), NUMEL, units=UNITS, lr=HP[0], betas=HP[1:3], eps=HP[3], weight_decay=HP[4],
-                               replication=k, blocks=4, compact=compact, min_world=min_world, page_shift=SHIFT,
-                               max_grad_norm=max_norm, grad_accum_steps=M)
-            o.param.copy_(self.init)
-            o.seed_master()
-            self.opts.append(o)
-        self.store = HashStore()
-        self.members = list(range(n))
-        self.pending = None
-
-    def configure(self, members, epoch):
-        from torch.distributed import PrefixStore
-
-        from torchft_b200.parallel.symm_mem import SymmetricComm
-
-        self.settle()
-        SymmetricComm.virtual_quorum(self.comms, members, epoch)
-        errs = []
-
-        def run(rank, m):
-            try:
-                self.opts[m]._on_configured(PrefixStore(f"q/{epoch}", self.store), rank, len(members), epoch)
-            except Exception as e:  # noqa: BLE001
-                errs.append(e)
-
-        ts = [threading.Thread(target=run, args=(rank, m)) for rank, m in enumerate(members)]
-        [t.start() for t in ts]
-        [t.join() for t in ts]
-        assert not errs, errs
-        torch.cuda.synchronize()
-        self.members = list(members)
-
-    def settle(self):
-        if self.pending is not None:
-            for m, s in self.pending.items():
-                self.opts[m].resolved(self.opts[m].wait(s))
-            self.pending = None
-
-    def step(self, raws, skip=None):
-        """One step: micro-batch m writes ``raws[m][rank]`` into quorum rank ``rank``'s gradient, then every member
-        reduces every unit. ``skip = (unit, micro)`` leaves that reduce out on every member."""
-        self.settle()
-        world = len(self.members)
-        for m, raw in enumerate(raws):
-            for rank, i in enumerate(self.members):
-                self.opts[i].grad.copy_(raw[rank])
-            torch.cuda.synchronize()
-            for i in self.members:
-                for u in range(len(UNITS)):
-                    if skip != (u, m):
-                        self.opts[i].reduce_scatter(u, _scale(world, self.M), True, m)
-            torch.cuda.synchronize()
-        self.pending = {i: self.opts[i].enqueue(True) for i in self.members}
-        for i in self.members:
-            self.opts[i].update()
-        torch.cuda.synchronize()
-
-    def verdicts(self):
-        return {i: self.opts[i].comm.verdict(s) for i, s in self.pending.items()}
+def _replicas(n, M, compact=False, max_norm=None, min_world=3, k=2):
+    """``n`` replicas accumulating ``M`` micro-batches, driven through quorum changes."""
+    return Replicas(n, UNITS, k=k, compact=compact, min_world=min_world, max_norm=max_norm, M=M)
 
 
 @pytest.mark.parametrize("compact", [False, True])
@@ -319,7 +214,7 @@ def test_optimizer_accumulates_through_a_change_of_world(compact):
     from torchft_b200.parallel.zero1 import ShardLayout, accum_elements, accum_offsets
 
     M, k = 3, 2
-    reps = _Replicas(4, M, compact=compact)
+    reps = _replicas(4, M, compact=compact)
     L = ShardLayout(tuple(UNITS), k)
     assert all(o.accum_bytes() == 4 * accum_elements(L, 3) for o in reps.opts)
     dev = torch.device("cuda", 0)
@@ -343,7 +238,7 @@ def test_optimizer_accumulates_through_a_change_of_world(compact):
             reps.step(raws)
             reduced = _reduced(raws)
             t += 1
-            _ref_adamw(rm, rmm, rv, reduced.float(), t)
+            ref_adamw(rm, rmm, rv, reduced.float(), t)
             assert reps.verdicts() == {i: True for i in members}
             for rank, i in enumerate(members):
                 o = reps.opts[i]
@@ -362,7 +257,7 @@ def test_optimizer_accumulates_through_a_change_of_world(compact):
 
 def test_a_unit_short_of_micro_batches_vetoes_the_step():
     M, world = 3, 4
-    reps = _Replicas(world, M)
+    reps = _replicas(world, M)
     reps.configure([0, 1, 2, 3], 1)
     reps.step(_raws(world, M, 5))
     reps.settle()
@@ -383,7 +278,7 @@ def test_a_unit_short_of_micro_batches_vetoes_the_step():
 
 def test_clipped_accumulation_matches_adamw_and_an_inf_in_an_early_micro_batch_vetoes():
     M, world, k = 3, 4, 2
-    reps = _Replicas(world, M, max_norm=MAX_NORM)
+    reps = _replicas(world, M, max_norm=MAX_NORM)
     reps.configure([0, 1, 2, 3], 1)
     dev = torch.device("cuda", 0)
     rm, rmm, rv = reps.init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)
@@ -411,7 +306,7 @@ def test_clipped_accumulation_matches_adamw_and_an_inf_in_an_early_micro_batch_v
         assert torch.equal(reps.opts[0]._clip[1], coef)
         clipped.append(bool(coef < 1))
         t += 1
-        _ref_adamw(rm, rmm, rv, reduced.float() * coef, t)
+        ref_adamw(rm, rmm, rv, reduced.float() * coef, t)
     reps.settle()
     assert any(clipped) and not all(clipped), clipped
     for rank, o in enumerate(reps.opts):
@@ -426,7 +321,7 @@ def test_accumulator_too_small_for_the_quorum_raises():
 
     from torchft_b200.parallel.symm_mem import SymmetricComm
 
-    reps = _Replicas(4, 2, min_world=3)
+    reps = _replicas(4, 2, min_world=3)
     SymmetricComm.virtual_quorum(reps.comms, [0, 1], 9)
     with pytest.raises(RuntimeError, match="accumulator bytes"):
         reps.opts[0]._on_configured(PrefixStore("q/9", reps.store), 0, 2, 9)

@@ -14,7 +14,7 @@ from test_zero1_cpu import NUMEL, UNITS, _mask, _Sim
 from torchft_b200.checkpointing.sharded import (check_compatible, encode_header, file_name, read_header, scan,
                                                 sections)
 from torchft_b200.parallel.zero1 import (ShardLayout, ckpt_read_plan, intersect_ranges, merge_ranges,
-                                         newest_complete_step, plan_pulls, subtract_ranges, total)
+                                         newest_complete_step, plan_quorum, total)
 
 
 def _files(L, world, t=1):
@@ -71,18 +71,35 @@ def test_newest_complete_step_falls_back_and_accepts_mixed_worlds():
         ckpt_read_plan([(0, NUMEL)], [(f, f["ranges"]) for f in w3[:2]])
 
 
+def test_plan_quorum_reads_its_own_restore_else_the_first_checkpoint_that_covers():
+    L = ShardLayout(UNITS, 1)
+
+    def tagged(tag, files):
+        return [(dict(h, tag=tag), r) for h, r in files]
+
+    part, full = tagged("part", _files(L, 2)[:1]), tagged("full", _files(L, 2))  # part: rank 0's file of a quorum of 2
+    fresh = lambda world: {r: {"t": 1, "hold": []} for r in range(world)}  # noqa: E731  (restored: t = T, holds nothing)
+    sources = lambda p: {h["tag"] for h, _, _, _ in p.reads}  # noqa: E731
+    plans = plan_quorum(L, 2, fresh(2), ckpt={0: part, 1: full})
+    assert sources(plans[0]) == {"part"} and sources(plans[1]) == {"full"}
+    assert all(not p.lost and merge_ranges([(lo, hi) for _, _, lo, hi in p.reads]) == L.held(r, 2) for r, p in plans.items())
+    plans = plan_quorum(L, 3, fresh(3), ckpt={0: part, 1: full})
+    assert sources(plans[2]) == {"full"} and not plans[2].lost  # rank 0's restore does not cover its slices
+    plans = plan_quorum(L, 2, fresh(2), ckpt={0: part})
+    assert not plans[1].reads and plans[1].lost == L.held(1, 2) and plans[1].counted
+
+
 # ----------------------------------------------------------------------------- the disk in the random walk
 class _DiskSim(_Sim):
     """``_Sim`` with durable checkpoints: ``save`` writes every member's ``primary ∩ hold`` at its own ``t``; a restarted
     member restores the newest complete step (``t = T``, holds nothing) and is armed; at the next quorum, ranges that
     no live holder at ``tmax`` has are read from the files when a member is armed at ``T == tmax`` (any rank may read
-    them), and re-seeded otherwise. ``Zero1Optimizer._on_configured`` in the same planners."""
+    them), and re-seeded otherwise. The optimizer's planner decides, as in ``Zero1Optimizer._on_configured``."""
 
     def __init__(self, n, k):
         super().__init__(n, k)
         self.files = []   # (header, ranges, values)
         self.armed = {}   # member -> T
-        self.read = 0
 
     def save(self):
         world = len(self.members)
@@ -102,30 +119,9 @@ class _DiskSim(_Sim):
         self.armed[m] = T
 
     def configure(self, members):
-        self.members = list(members)
-        world = len(members)
         tmax = max(self.t[m] for m in members)
-        disk = any(T == tmax for m, T in self.armed.items() if m in members)
-        files = [(i, r) for i, (h, r, _) in enumerate(self.files) if h["T"] == tmax] if disk else []
-        valid = {i: self.hold[m] for i, m in enumerate(members) if self.t[m] == tmax}
-        plans = {}
-        for i, m in enumerate(members):
-            mine = self.hold[m] if self.t[m] == tmax else []
-            need = subtract_ranges(self.L.held(i, world), mine)
-            pulls, lost = plan_pulls(need, {j: h for j, h in valid.items() if j != i}, i)
-            reads = ckpt_read_plan(lost, files) if disk and lost else []
-            plans[m] = (pulls, [] if reads else lost, reads, need, mine)
-        for m, (pulls, lost, reads, need, mine) in plans.items():
-            for src, lo, hi in pulls:
-                self.state[m][lo:hi] = self.state[members[src]][lo:hi]
-            for f, off, lo, hi in reads:
-                self.state[m][lo:hi] = self.files[f][2][off:off + hi - lo]
-                self.read += hi - lo
-            for lo, hi in lost:
-                self.state[m][lo:hi] = -1000.0
-                self.lost += hi - lo
-            self.hold[m] = merge_ranges(list(mine) + list(need))
-            self.t[m] = tmax
+        files = [(vals, r) for h, r, vals in self.files if h["T"] == tmax]
+        super().configure(members, ckpt={i: files for i, m in enumerate(members) if self.armed.get(m) == tmax})
         for m in members:
             self.armed.pop(m, None)
 

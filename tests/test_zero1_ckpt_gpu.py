@@ -8,27 +8,19 @@ rank launches on the current stream, the snapshot copies run on the optimizer's 
 from __future__ import annotations
 
 import os
-import threading
 from datetime import timedelta
 
 import pytest
 import torch
 
-from test_zero1_accum_gpu import _PG
+from _zero1_replicas import Replicas, seeded_weights
 
 pytestmark = pytest.mark.gpu
 
 # large enough that the snapshot copy is still running when the next step's update is enqueued
 UNITS = [(0, 8 * 131072), (8 * 131072, 8 * 131072 + 8 * 50021), (8 * 131072 + 8 * 50021, 8 * 131072 + 8 * 50028)]
 NUMEL = UNITS[-1][1]
-HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)
-SHIFT = 8
 K = 2
-
-
-def _init():
-    dev = torch.device("cuda", 0)
-    return (torch.randn(NUMEL, device=dev, generator=torch.Generator(device=dev).manual_seed(2)) * 0.05).bfloat16()
 
 
 def _raws(world, seed):
@@ -37,74 +29,15 @@ def _raws(world, seed):
     return [(torch.randn(NUMEL, device=dev, generator=g) * 0.01 * (r + 1)).bfloat16() for r in range(world)]
 
 
-class _Reps:
-    """``n`` virtual ranks, each with a ``Zero1Optimizer``, driven in the Manager's order through quorum changes."""
+class _Reps(Replicas):
+    """``n`` replicas of ``K`` holders per slice, stepped without a host synchronisation."""
 
     def __init__(self, n, compact=False, min_world=1, units=UNITS):
-        from torch.distributed import HashStore
-
-        from torchft_b200.parallel.symm_mem import SymmetricComm
-        from torchft_b200.parallel.zero1 import ShardLayout, pool_pages
-
-        n_state = (pool_pages(ShardLayout(tuple(units), K), min_world, 1 << SHIFT) << SHIFT) if compact else NUMEL
-        seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, **{x: n_state * 4 for x in ("z1_master", "z1_m", "z1_v")}}
-        self.comms = SymmetricComm.virtual_world(n, seg, presignal=True, timeout=timedelta(seconds=20))
-        self.opts = [self.make(c, compact, min_world, units) for c in self.comms]
-        for o in self.opts:
-            o.param.copy_(_init())
-            o.seed_master()
-        self.store = HashStore()
-        self.members = list(range(n))
-        self.pending = None
-
-    @staticmethod
-    def make(comm, compact=False, min_world=1, units=UNITS):
-        from torchft_b200.parallel.zero1 import Zero1Optimizer
-
-        return Zero1Optimizer(_PG(comm), NUMEL, units=units, lr=HP[0], betas=HP[1:3], eps=HP[3], weight_decay=HP[4],
-                              replication=K, blocks=4, compact=compact, min_world=min_world, page_shift=SHIFT)
-
-    def configure(self, members, epoch):
-        from torch.distributed import PrefixStore
-
-        from torchft_b200.parallel.symm_mem import SymmetricComm
-
-        self.settle()
-        SymmetricComm.virtual_quorum(self.comms, members, epoch)
-        errs = []
-
-        def run(rank, m):
-            try:
-                self.opts[m]._on_configured(PrefixStore(f"q/{epoch}", self.store), rank, len(members), epoch)
-            except Exception as e:  # noqa: BLE001
-                errs.append(e)
-
-        ts = [threading.Thread(target=run, args=(rank, m)) for rank, m in enumerate(members)]
-        [t.start() for t in ts]
-        [t.join() for t in ts]
-        assert not errs, errs
-        torch.cuda.synchronize()
-        self.members = list(members)
-
-    def settle(self):
-        if self.pending is not None:
-            for m, s in self.pending.items():
-                self.opts[m].resolved(self.opts[m].wait(s))
-            self.pending = None
+        super().__init__(n, units, k=K, compact=compact, min_world=min_world)
 
     def step(self, seed):
-        """One step without a host synchronisation: gradients, reduce-scatters, verdicts and updates are enqueued."""
-        self.settle()
-        world = len(self.members)
-        raws = _raws(world, seed)
-        for rank, i in enumerate(self.members):
-            self.opts[i].grad.copy_(raws[rank])
-        for i in self.members:
-            for u in range(len(UNITS)):
-                self.opts[i].reduce_scatter(u, 1.0 / world, True)
-        self.pending = {i: self.opts[i].enqueue(True) for i in self.members}
-        for i in self.members:
-            self.opts[i].update()
+        """Gradients, reduce-scatters, verdicts and updates of one step are enqueued; nothing waits for the device."""
+        super().step([_raws(len(self.members), seed)], sync=False)
 
     def save(self, directory, keep=2):
         self.settle()
@@ -191,7 +124,7 @@ def test_partial_restart_pulls_from_the_live_replica_and_reads_the_rest(tmp_path
     for o in live.opts:
         o.wait_checkpoint()
     for r in (1, 2, 3):  # these processes restart; member 0 stays alive at T = 2
-        o = _Reps.make(live.comms[r])
+        o = live.make(live.comms[r])
         o.param.zero_()
         for a in (o.master, o.m, o.v):
             a.fill_(float("nan"))
@@ -234,12 +167,12 @@ def test_missing_and_torn_files_fall_back_and_a_mismatch_refuses(tmp_path):
     assert sd["step"] == 2 and o.t == 2
     os.remove(tmp_path / "z1_step_2.w2.r0.bin")  # missing: nothing is complete
     sd, o = restore_one()
-    assert sd is None and o.t == 0 and torch.equal(o.param, _init())
+    assert sd is None and o.t == 0 and torch.equal(o.param, seeded_weights(NUMEL))
     # another unit split (as with another optimizer_blocks) refuses before touching anything
     other = _Reps(1, units=[(0, UNITS[1][0]), (UNITS[1][0], NUMEL)]).opts[0]
     with pytest.raises(ValueError, match="units"):
         other.restore(str(tmp_path))
-    assert other.t == 0 and torch.equal(other.param, _init())
+    assert other.t == 0 and torch.equal(other.param, seeded_weights(NUMEL))
 
 
 # ----------------------------------------------------------------------------- trainer

@@ -13,30 +13,21 @@ from datetime import timedelta
 import pytest
 import torch
 
+from _zero1_replicas import HP, SHIFT, Replicas, ref_adamw
+
 pytestmark = pytest.mark.gpu
 
 UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
 NUMEL = UNITS[-1][1]
-HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)  # lr, b1, b2, eps, wd
-SHIFT = 8  # paged state: 256-element pages
 MAX_NORM = 50.0
 STEP_SCALES = (1.0, 0.01, 1.0)  # norms of a few hundred, a few units, a few hundred: clipped, not clipped, clipped
 
 
-def _world(world, presignal=True, extra=None):
+def _world(world, presignal=True):
     from torchft_b200.parallel.symm_mem import SymmetricComm
 
-    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS), **(extra or {})}
+    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS)}
     return SymmetricComm.virtual_world(world, seg, presignal=presignal, timeout=timedelta(seconds=20))
-
-
-def _ref_adamw(master, m, v, g, t):
-    lr, b1, b2, eps, wd = HP
-    m.mul_(b1).add_(g, alpha=1 - b1)
-    v.mul_(b2).addcmul_(g, g, value=1 - b2)
-    bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t
-    denom = v.sqrt() / (bc2 ** 0.5) + eps
-    master.mul_(1 - lr * wd).addcdiv_(m, denom, value=-lr / bc1)
 
 
 def _coef(max_norm, norm):
@@ -172,7 +163,7 @@ def test_clipped_pipeline_matches_reference(world, k):
         coef = _coef(MAX_NORM, torch.tensor(norm, dtype=torch.float32, device=dev))
         clipped.append(bool(coef < 1))
         assert rec["verdict"] == [True] * world and rec["t"] == [step] * world
-        _ref_adamw(rm, rmm, rv, reduced.float() * coef, step)
+        ref_adamw(rm, rmm, rv, reduced.float() * coef, step)
     assert any(clipped) and not all(clipped), clipped
     last = recs[-1]
     for r in range(1, world):
@@ -269,43 +260,8 @@ def _check_paged_vs_flat(world, k, flat, paged):
 
 
 # ----------------------------------------------------------------------------- Zero1Optimizer
-class _PG:
-    """The slice of ``ProcessGroupB200`` that ``Zero1Optimizer`` uses, over one virtual-world rank whose segments exist;
-    collectives run on the current stream."""
-
-    def __init__(self, comm):
-        self.comm = comm
-        self.comm_stream = torch.cuda.current_stream()
-
-    def alloc_symmetric(self, name, nbytes):
-        seg = self.comm.segment(name)
-        assert seg.numel() >= nbytes
-        return seg[:nbytes]
-
-    def add_configure_hook(self, fn):
-        pass
-
-    def _launch(self, fn, result):
-        fn(self.comm_stream)
-        return None
-
-
 def _optimizers(world, max_norm):
-    from torchft_b200.parallel.zero1 import GNORM_UNITS, Zero1Optimizer
-
-    extra = {x: NUMEL * 4 for x in ("z1_master", "z1_m", "z1_v")}
-    extra["z1_gnorm"] = GNORM_UNITS * 8
-    comms = _world(world, extra=extra)
-    dev = torch.device("cuda", 0)
-    init = (torch.randn(NUMEL, device=dev, generator=torch.Generator(device=dev).manual_seed(2)) * 0.05).bfloat16()
-    opts = []
-    for c in comms:
-        o = Zero1Optimizer(_PG(c), NUMEL, units=UNITS, lr=HP[0], betas=HP[1:3], eps=HP[3], weight_decay=HP[4],
-                           replication=2, blocks=4, max_grad_norm=max_norm)
-        o.param.copy_(init)
-        o.seed_master()
-        opts.append(o)
-    return opts
+    return Replicas(world, UNITS, max_norm=max_norm).opts
 
 
 def test_optimizer_reports_norms_one_step_late_and_counts_nonfinite_steps():

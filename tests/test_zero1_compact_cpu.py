@@ -8,9 +8,8 @@ import pytest
 
 from test_zero1_cpu import NUMEL, UNITS, _Sim
 from torchft_b200.models.llama import CONFIGS
-from torchft_b200.parallel.zero1 import (ShardLayout, backed_ranges, intersect_ranges, merge_ranges, page_ranges,
-                                         plan_reshard, pool_pages, reshard_page_steps, reshard_pages, subtract_ranges,
-                                         total)
+from torchft_b200.parallel.zero1 import (ShardLayout, intersect_ranges, merge_ranges, page_ranges, plan_quorum,
+                                         pool_pages, total)
 
 SHIFT = 8  # 256-element pages: the 12 168-element test vector spans 48 of them
 PAGE = 1 << SHIFT
@@ -18,9 +17,9 @@ PAGE = 1 << SHIFT
 
 class _CompactSim:
     """The state protocol of ``_Sim`` with every replica's state in a page pool behind a page table, re-sharded the way
-    ``Zero1Optimizer`` does it in compact mode, through the same planners and page-step sets (``reshard_page_steps``,
-    ``backed_ranges``). Ranks run each phase one after the other, every rank's frees and allocations before anybody
-    pulls, so a page freed too early is reused and poisoned before a peer reads it."""
+    ``Zero1Optimizer`` does it in compact mode, by the same planner (``plan_quorum``) and its page steps. Ranks run
+    each phase one after the other, every rank's frees and allocations before anybody pulls, so a page freed too early
+    is reused and poisoned before a peer reads it."""
 
     POISON = -7.0
 
@@ -63,39 +62,36 @@ class _CompactSim:
         world = len(members)
         if world < self.min_world:
             raise RuntimeError(f"quorum of {world} is below min_world")
-        info = {i: (self.t[m], self.hold[m]) for i, m in enumerate(members)}
-        old = {i: self._pages(m) for i, m in enumerate(members)}
-        tmax, plans = plan_reshard(self.L, info, world)
-        pages = reshard_pages(self.L, plans, old, world, SHIFT)
-        worst = max(pk for _, _, pk in pages.values())
+        published = {i: {"t": self.t[m], "hold": self.hold[m], "pages": [(p, s, 1) for p, s in sorted(self.table[m].items())]}
+                     for i, m in enumerate(members)}
+        plans = plan_quorum(self.L, world, published, SHIFT)
+        worst = max(p.peak for p in plans.values())
         if worst > self.cap:
             raise RuntimeError(f"needs {worst} pages")
-        sources = {i: merge_ranges([(lo, hi) for p in plans.values() for s, lo, hi in p[1] if s == i]) for i in range(world)}
-        steps = {i: reshard_page_steps(old[i], pages[i][0], pages[i][1]) for i in range(world)}
+        sources = {i: merge_ranges([(lo, hi) for p in plans.values() for s, lo, hi in p.pulls if s == i]) for i in range(world)}
         for i, m in enumerate(members):  # 1. free what is neither kept nor a source, 2. allocate the new pages
-            first, allocate, _ = steps[i]
-            assert not intersect_ranges(first, page_ranges(sources[i], SHIFT)), "a page freed while a peer sources from it"
-            self._free_pages(m, first)
-            self.hold[m] = backed_ranges(self.hold[m], subtract_ranges(old[i], first), SHIFT)
+            p = plans[i]
+            assert not intersect_ranges(p.free_first, page_ranges(sources[i], SHIFT)), "a page freed while a peer sources from it"
+            self._free_pages(m, p.free_first)
+            self.hold[m] = p.hold_mid
             self.free[m].sort(reverse=True)
-            for lo, hi in allocate:
-                for p in range(lo, hi):
-                    self.table[m][p] = slot = self.free[m].pop()
+            for lo, hi in p.allocate:
+                for pg in range(lo, hi):
+                    self.table[m][pg] = slot = self.free[m].pop()
                     self.pool[m][slot * PAGE:(slot + 1) * PAGE] = self.POISON
             self.peak = max(self.peak, len(self.table[m]))
         if abort_after_alloc:
             return
         for i, m in enumerate(members):  # 3. pull through both page tables, seed what nobody holds
-            need, pulls, lost = plans[i]
-            for src, lo, hi in pulls:
+            p = plans[i]
+            for src, lo, hi in p.pulls:
                 self.pool[m][self._idx(m, lo, hi)] = self.read(members[src], lo, hi)
-            for lo, hi in lost:
-                self.pool[m][self._idx(m, lo, hi)] = -1000.0 if tmax > 0 else 0.0
-                self.lost += (hi - lo) if tmax > 0 else 0
+            for lo, hi in p.lost:
+                self.pool[m][self._idx(m, lo, hi)] = -1000.0 if p.counted else 0.0
+                self.lost += (hi - lo) if p.counted else 0
         for i, m in enumerate(members):  # 6. after the barrier: drop the pages kept only for peers
-            self._free_pages(m, steps[i][2])
-            self.hold[m] = self.L.held(i, world)
-            self.t[m] = tmax
+            self._free_pages(m, plans[i].free_last)
+            self.hold[m], self.t[m] = plans[i].hold, plans[i].tmax
             assert self._pages(m) == page_ranges(self.hold[m], SHIFT)
         self.members = list(members)
 

@@ -10,12 +10,12 @@ from datetime import timedelta
 import pytest
 import torch
 
+from _zero1_replicas import HP, SHIFT, Replicas
+
 pytestmark = pytest.mark.gpu
 
 UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
 NUMEL = UNITS[-1][1]
-HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)  # lr, b1, b2, eps, wd
-SHIFT = 8  # 256-element pages: unit and slice bounds fall inside pages
 
 
 def _world(world, segments, presignal=True):
@@ -114,84 +114,35 @@ def _check_paged_vs_flat(world, k, presignal):
 
 
 # ----------------------------------------------------------------------------- Zero1Optimizer, compact vs full-size
-class _PG:
-    """The slice of ``ProcessGroupB200`` that ``Zero1Optimizer`` uses, over one virtual-world rank whose segments exist."""
-
-    def __init__(self, comm):
-        self.comm = comm
-        self.comm_stream = torch.cuda.current_stream()
-
-    def alloc_symmetric(self, name, nbytes):
-        seg = self.comm.segment(name)
-        assert seg.numel() >= nbytes
-        return seg[:nbytes]
-
-    def add_configure_hook(self, fn):
-        pass
-
-
 def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_split_commit():
-    from torch.distributed import HashStore, PrefixStore
+    import json
+
+    from torch.distributed import PrefixStore
 
     from torchft_b200.parallel.symm_mem import SymmetricComm
-    from torchft_b200.parallel.zero1 import ShardLayout, Zero1Optimizer, pool_pages
+    from torchft_b200.parallel.zero1 import ShardLayout, page_ranges, pool_pages
 
     dev = torch.device("cuda", 0)
     n, k, min_world = 4, 2, 3
     cap = pool_pages(ShardLayout(tuple(UNITS), k), min_world, 1 << SHIFT)
     assert cap < NUMEL >> SHIFT  # the pools really are smaller than the vector
-    seg = {"z1_param": NUMEL * 2, "z1_grad": NUMEL * 2}
-    flat_c = _world(n, {**seg, **{x: NUMEL * 4 for x in ("z1_master", "z1_m", "z1_v")}})
-    comp_c = _world(n, {**seg, **{x: (cap << SHIFT) * 4 for x in ("z1_master", "z1_m", "z1_v")}})
     g = torch.Generator(device=dev).manual_seed(3)
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
-    store = HashStore()
-
-    def make(kind, r):
-        c = (comp_c if kind == "compact" else flat_c)[r]
-        o = Zero1Optimizer(_PG(c), NUMEL, units=UNITS, lr=HP[0], betas=HP[1:3], eps=HP[3], weight_decay=HP[4],
-                           replication=k, blocks=4, compact=kind == "compact", min_world=min_world, page_shift=SHIFT)
-        return o
-
-    opts = {kind: {} for kind in ("flat", "compact")}
-    for r in range(n):
-        for kind in opts:
-            o = make(kind, r)
-            o.param.copy_(init)
-            o.seed_master()
-            opts[kind][r] = o
+    reps = {kind: Replicas(n, UNITS, k=k, compact=kind == "compact", min_world=min_world, init=init)
+            for kind in ("flat", "compact")}
+    opts = {kind: r.opts for kind, r in reps.items()}
     assert opts["compact"][0].state_bytes_allocated() == 12 * (cap << SHIFT)
     assert opts["flat"][0].state_bytes_allocated() == 12 * NUMEL
 
     def configure(members, epoch):
-        for kind, comms in (("flat", flat_c), ("compact", comp_c)):
-            SymmetricComm.virtual_quorum(comms, members, epoch)
-            errs = []
-
-            def run(rank, m):
-                try:
-                    opts[kind][m]._on_configured(PrefixStore(f"{kind}/{epoch}", store), rank, len(members), epoch)
-                except Exception as e:  # noqa: BLE001
-                    errs.append(e)
-
-            ts = [threading.Thread(target=run, args=(rank, m)) for rank, m in enumerate(members)]
-            [t.start() for t in ts]
-            [t.join() for t in ts]
-            assert not errs, errs
-        torch.cuda.synchronize()
+        for r in reps.values():
+            r.configure(members, epoch)
 
     def step(members, veto=None):
         gstep = torch.randn(NUMEL, device=dev, generator=g).bfloat16()  # the reduced gradient, identical everywhere
-        for kind in opts:
-            for m in members:
-                opts[kind][m].grad.copy_(gstep)
-            torch.cuda.synchronize()
-            seqs = {m: opts[kind][m].enqueue(m != veto) for m in members}
-            for m in members:
-                opts[kind][m].update()
-            torch.cuda.synchronize()
-            for m in members:
-                opts[kind][m].resolved(opts[kind][m].wait(seqs[m]))
+        for r in reps.values():
+            r.step([[gstep] * len(members)], veto=veto, reduce=False)
+            r.settle()
         for m in members:
             f, c = opts["flat"][m], opts["compact"][m]
             assert f.t == c.t and f._holdings == c._holdings
@@ -207,11 +158,11 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
     configure([0, 1, 3], 2)                        # kill: 4 -> 3
     assert opts["compact"][0].lost_elements == 0
     step([0, 1, 3])
-    for kind in opts:                              # rejoin: 3 -> 4, member 2 restarts from the healed weights
-        o = make(kind, 2)
-        o.param.copy_(opts[kind][0].param)
+    for r in reps.values():                        # rejoin: 3 -> 4, member 2 restarts from the healed weights
+        o = r.make(r.comms[2])
+        o.param.copy_(r.opts[0].param)
         o.seed_master()
-        opts[kind][2] = o
+        r.opts[2] = o
     configure([0, 1, 2, 3], 3)
     step([0, 1, 2, 3])
     step([0, 1, 2, 3], veto=1)                     # split commit: member 1 misses the update the others apply
@@ -223,12 +174,8 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
         assert opts["compact"][m].state_bytes_held() == opts["flat"][m].state_bytes_held()
     # a re-shard to [0, 1, 3] that fails at the barrier: member 3 publishes and then dies, members 0 and 1 have already
     # freed and allocated pages. They keep their update count and may claim only ranges their kept pages still back.
-    import json
-
-    from torchft_b200.parallel.zero1 import page_ranges
-
-    c3 = opts["compact"][3]
-    qs = PrefixStore("compact/5", store)
+    comp_c, c3 = reps["compact"].comms, opts["compact"][3]
+    qs = PrefixStore("q/5", reps["compact"].store)
     qs.set("z1/2", json.dumps({"t": c3.t, "hold": c3._holdings, "pages": c3._page_runs()}))
     SymmetricComm.virtual_quorum(comp_c, [0, 1, 3], 5)
     for m in (0, 1):
@@ -251,7 +198,7 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
     # a quorum below min_world is refused before any state moves
     SymmetricComm.virtual_quorum(comp_c, [0, 1], 7)
     with pytest.raises(RuntimeError, match="min_world"):
-        opts["compact"][0]._on_configured(PrefixStore("compact/7", store), 0, 2, 7)
+        opts["compact"][0]._on_configured(PrefixStore("q/7", reps["compact"].store), 0, 2, 7)
 
 
 def _raises(fn, *args):

@@ -10,8 +10,8 @@ import numpy as np
 import pytest
 from torch.distributed import TCPStore
 
-from torchft_b200.parallel.zero1 import (ShardLayout, intersect_ranges, merge_ranges, plan_pulls, subtract_ranges,
-                                         total)
+from torchft_b200.parallel.zero1 import (ShardLayout, intersect_ranges, merge_ranges, page_ranges, plan_quorum,
+                                         subtract_ranges, total)
 
 
 def _mask(rs, n):
@@ -59,7 +59,8 @@ def test_layout_every_element_has_exactly_k_holders_and_one_primary(world, k):
 
 
 class _Sim:
-    """Numpy emulation of N replicas running the FT-ZeRO-1 state protocol (update = +1 on held ranges)."""
+    """Numpy emulation of N replicas running the FT-ZeRO-1 state protocol (update = +1 on held ranges), re-sharded by
+    the optimizer's own planner (``plan_quorum``); only the state arrays and the counters are the emulation's."""
 
     def __init__(self, n, k):
         self.L = ShardLayout(UNITS, k)
@@ -68,26 +69,24 @@ class _Sim:
         self.t = {r: 0 for r in range(n)}
         self.members = list(range(n))
         self.lost = 0
+        self.read = 0
 
-    def configure(self, members):
+    def configure(self, members, ckpt=None):
+        """``ckpt``: checkpoint files for ``plan_quorum``, whose file objects are the arrays of values they store."""
         self.members = list(members)
-        world = len(members)
-        tmax = max(self.t[m] for m in members)
-        valid = {i: self.hold[m] for i, m in enumerate(members) if self.t[m] == tmax}
-        plans = {}
-        for i, m in enumerate(members):
-            mine = self.hold[m] if self.t[m] == tmax else []
-            need = subtract_ranges(self.L.held(i, world), mine)
-            pulls, lost = plan_pulls(need, {j: h for j, h in valid.items() if j != i}, i)
-            plans[m] = (pulls, lost, need, mine)
-        for m, (pulls, lost, need, mine) in plans.items():  # all pulls read pre-update state
-            for src, lo, hi in pulls:
+        published = {i: {"t": self.t[m], "hold": self.hold[m]} for i, m in enumerate(members)}
+        plans = plan_quorum(self.L, len(members), published, ckpt=ckpt)
+        for i, m in enumerate(members):  # a source never writes the ranges it is read from: they are current there
+            p = plans[i]
+            for src, lo, hi in p.pulls:
                 self.state[m][lo:hi] = self.state[members[src]][lo:hi]
-            for lo, hi in lost:
-                self.state[m][lo:hi] = -1000.0
-                self.lost += hi - lo
-            self.hold[m] = merge_ranges(list(mine) + list(need))
-            self.t[m] = tmax
+            for vals, off, lo, hi in p.reads:
+                self.state[m][lo:hi] = vals[off:off + hi - lo]
+                self.read += hi - lo
+            for lo, hi in p.lost:
+                self.state[m][lo:hi] = -1000.0 if p.counted else 0.0
+                self.lost += (hi - lo) if p.counted else 0
+            self.hold[m], self.t[m] = p.hold, p.tmax
 
     def step(self, commit_on=None):
         world = len(self.members)
@@ -144,6 +143,38 @@ def test_k1_loses_state_and_k2_loses_only_on_adjacent_double_failure():
     s.configure([m for m in range(8) if m not in (2, 3)])  # slice 2 lived on exactly {2, 3}
     # both new holders of the orphaned ranges re-seed them
     assert s.lost == 2 * total([ShardLayout(UNITS, 2).slice_bounds(u, 8, 2) for u in range(len(UNITS))])
+
+
+@pytest.mark.parametrize("paged", [False, True])
+def test_plan_quorum_holdings_after_and_losses_at_t0(paged):
+    """What a rank claims after a re-shard is what its state really keeps. Full-size state keeps every range it held at
+    ``tmax``, also those outside the new layout, and peers may pull them at a later quorum; paged state keeps exactly its
+    new slices, not the whole pages they touch. A slice nobody holds at t = 0 is seeded, and not counted as lost."""
+    shift = 8
+    L = ShardLayout(UNITS, 2)
+
+    def pub(t, holds):
+        pages = lambda h: [(lo, 0, hi - lo) for lo, hi in page_ranges(h, shift)]  # noqa: E731
+        return {r: {"t": t, "hold": h, **({"pages": pages(h)} if paged else {})} for r, h in enumerate(holds)}
+
+    old = [L.held(r, 4) for r in range(4)]
+    plans = plan_quorum(L, 3, pub(5, old[:3]), shift if paged else None)  # member 3 is gone after update 5
+    for r, p in plans.items():
+        new = L.held(r, 3)
+        assert p.tmax == 5 and p.counted
+        assert p.need == subtract_ranges(new, old[r]) and not p.lost
+        assert p.hold == (new if paged else merge_ranges(old[r] + new))
+    assert any(subtract_ranges(old[r], L.held(r, 3)) for r in range(3)), "the test needs ranges the new layout drops"
+    if paged:
+        assert any(page_ranges(L.held(r, 3), shift) != [(lo >> shift, hi >> shift) for lo, hi in L.held(r, 3)]
+                   for r in range(3)), "the test needs slices that end inside a page"
+    # the first quorum of paged state, or a quorum of restarted replicas: nobody holds anything at t = 0
+    for p in plan_quorum(L, 3, pub(0, [[]] * 3), shift if paged else None).values():
+        assert p.lost == p.need and not p.pulls and not p.counted
+    # a split commit: rank 1 missed update 6, so what it held is not current
+    plans = plan_quorum(L, 3, pub(6, [L.held(r, 3) for r in range(3)]) | {1: pub(5, [L.held(1, 3)] * 2)[1]},
+                        shift if paged else None)
+    assert plans[1].need == L.held(1, 3) and plans[1].hold == L.held(1, 3) and not plans[1].lost
 
 
 # ----------------------------------------------------------------------------- Manager.commit_on_device

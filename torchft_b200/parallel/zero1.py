@@ -42,7 +42,7 @@ logger = logging.getLogger(__name__)
 Range = Tuple[int, int]
 
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
-           "plan_reshard", "reshard_pages", "reshard_page_steps", "backed_ranges", "pool_pages", "page_ranges",
+           "plan_reshard", "reshard_pages", "reshard_page_steps", "RankPlan", "plan_quorum", "backed_ranges", "pool_pages", "page_ranges",
            "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
@@ -262,6 +262,66 @@ def reshard_pages(layout: ShardLayout, plans: Dict[int, Tuple[List[Range], List[
     return out
 
 
+@dataclass
+class RankPlan:
+    """One rank's part of a quorum change (:func:`plan_quorum`), in the order the re-shard applies it."""
+
+    tmax: int                                # the update count the quorum agrees on
+    need: List[Range]                        # held in the new layout and not current here
+    pulls: List[Tuple[int, int, int]]        # ``(source rank, lo, hi)``: the parts of ``need`` a peer at ``tmax`` has
+    reads: List[Tuple[Any, int, int, int]]   # ``(file, offset, lo, hi)``: what no peer has, from a checkpoint at tmax
+    lost: List[Range]                        # what nobody has: re-seeded from the bf16 weights
+    counted: bool                            # whether ``lost`` is a loss (at t = 0 the seed IS the state)
+    hold: List[Range]                        # the ranges the rank claims afterwards
+    hold_mid: List[Range]                    # ... while the re-shard runs (paged: after ``free_first``)
+    free_first: List[Range] = ()             # paged: old pages neither kept nor read by a peer
+    allocate: List[Range] = ()               # paged: new pages it did not have
+    free_last: List[Range] = ()              # paged: old pages kept only for peers, freed once every peer has pulled
+    peak: int = 0                            # paged: the most pages it has allocated at once
+
+
+def _ckpt_reads(lost: Sequence[Range], rank: int, ckpt: Dict[int, Any]) -> List[Tuple[Any, int, int, int]]:
+    if not lost:
+        return []
+    for q in sorted(ckpt, key=lambda q: (q != rank, q)):  # its own restore first
+        try:
+            return ckpt_read_plan(lost, ckpt[q])
+        except ValueError:
+            continue
+    return []
+
+
+def plan_quorum(layout: ShardLayout, world: int, published: Dict[int, Dict[str, Any]], shift: Optional[int] = None,
+                ckpt: Optional[Dict[int, Any]] = None) -> Dict[int, RankPlan]:
+    """Every rank's re-shard for a new quorum of ``world``, from what each rank published: ``published[r]`` has its
+    update count ``t``, its holdings ``hold`` and, for paged state (``shift`` = log2 of the page size), its page table
+    as ``pages`` runs ``(page, slot, count)``. Only holdings at the highest ``t`` count; a rank that missed an update
+    holds nothing. ``ckpt[r]`` are the files at that update count of the checkpoint rank ``r`` restored from, as
+    ``(file, ranges)`` for :func:`ckpt_read_plan`: a rank reads what no peer has from its own, else from the first one
+    that covers it. Every rank of :class:`Zero1Optimizer` plans every rank, so it knows which of its ranges its peers
+    are about to read.
+
+    Full-size state keeps every range it held at the highest ``t`` (also those outside the new layout: peers may pull
+    them later). Paged state holds exactly its new slices; while its re-shard runs it claims only the held ranges its
+    kept pages still back, so a re-shard that dies before its barrier leaves no claim on a page it gave back."""
+    tmax, base = plan_reshard(layout, {r: (p["t"], [tuple(x) for x in p["hold"]]) for r, p in published.items()}, world)
+    if shift is not None:
+        old = {r: merge_ranges([(pg, pg + n) for pg, _, n in p["pages"]]) for r, p in published.items()}
+        pages = reshard_pages(layout, base, old, world, shift)
+    plans: Dict[int, RankPlan] = {}
+    for r, (need, pulls, lost) in base.items():
+        hold = [tuple(x) for x in published[r]["hold"]]
+        mine = hold if int(published[r]["t"]) == tmax else []
+        reads = _ckpt_reads(lost, r, ckpt or {})
+        p = plans[r] = RankPlan(tmax, need, pulls, reads, [] if reads else lost, tmax > 0,
+                                layout.held(r, world) if shift is not None else merge_ranges(mine + need), hold)
+        if shift is not None:
+            new, src, p.peak = pages[r]
+            p.free_first, p.allocate, p.free_last = reshard_page_steps(old[r], new, src)
+            p.hold_mid = backed_ranges(hold, subtract_ranges(old[r], p.free_first), shift)
+    return plans
+
+
 def pool_pages(layout: ShardLayout, min_world: int, page: int = 1 << PAGE_SHIFT, max_world: int = 8) -> int:
     """Pages per state array that let every rank hold its slices at every world in ``[min_world, max_world]`` and ride
     through every single-member loss or join between those worlds (the re-shard peak), for steady-state holders
@@ -276,19 +336,16 @@ def pool_pages(layout: ShardLayout, min_world: int, page: int = 1 << PAGE_SHIFT,
 
     best = max(total(p) for w in range(min_world, max_world + 1) for p in held_pages(w))
     for w in range(min_world, max_world + 1):
-        old = [layout.held(r, w) for r in range(w)]
-        old_pg = held_pages(w)
+        old = [{"t": 1, "hold": layout.held(r, w), "pages": [(lo, 0, hi - lo) for lo, hi in pg]}
+               for r, pg in enumerate(held_pages(w))]
         transitions = []
         if w - 1 >= min_world:  # member ``d`` is lost
-            transitions += [[(1, old[r], old_pg[r]) for r in range(w) if r != d] for d in range(w)]
+            transitions += [[old[r] for r in range(w) if r != d] for d in range(w)]
         if w + 1 <= max_world:  # a member with no state joins at quorum rank ``j``
-            transitions += [[(1, old[r], old_pg[r]) for r in range(j)] + [(0, [], [])] + [(1, old[r], old_pg[r]) for r in range(j, w)]
-                            for j in range(w + 1)]
+            transitions += [old[:j] + [{"t": 0, "hold": [], "pages": []}] + old[j:] for j in range(w + 1)]
         for members in transitions:
-            nw = len(members)
-            _, plans = plan_reshard(layout, {r: (t, h) for r, (t, h, _) in enumerate(members)}, nw)
-            pages = reshard_pages(layout, plans, {r: pg for r, (_, _, pg) in enumerate(members)}, nw, shift)
-            best = max(best, max(pk for _, _, pk in pages.values()))
+            plans = plan_quorum(layout, len(members), dict(enumerate(members)), shift)
+            best = max(best, max(p.peak for p in plans.values()))
     return best
 
 
@@ -418,11 +475,16 @@ class Zero1Optimizer:
             self._clip = torch.zeros(2, dtype=torch.float32, device=self.device)  # [norm, coef] of the last commit
             self.grad_norm = self._clip[0]
             self._resolved_norm: Optional[float] = None
+        # element e of the flat vector lives at pool index (table[e >> shift] << shift) | (e & mask) of paged state; full-size
+        # state has no table and keeps it at e (see _pieces)
+        self._table: Optional[torch.Tensor] = None
+        self._table_host: Any = None
         if not self.compact:
             self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
             self.m = pg.alloc_symmetric("z1_m", numel * 4).view(torch.float32)
             self.v = pg.alloc_symmetric("z1_v", numel * 4).view(torch.float32)
         else:
+            self.master = self.m = self.v = torch.empty(0, dtype=torch.float32, device=self.device)  # set_units allocates
             if not 1 <= self.min_world <= 8:
                 raise ValueError("min_world must be in [1, 8]")
             self._page_shift = int(page_shift)
@@ -517,14 +579,10 @@ class Zero1Optimizer:
     # ------------------------------------------------------------------ init / heal
     @torch.no_grad()
     def seed_master(self) -> None:
-        """Call once after the bf16 weights were initialised (same seed on every replica). Compact state is seeded
-        from the weights at the first quorum, when the rank's slices are known."""
-        if self.compact:
-            self._seed(self._holdings)
-            return
-        self.master.copy_(self.param)
-        self.m.zero_()
-        self.v.zero_()
+        """Call once after the bf16 weights were initialised (same seed on every replica): seeds what this rank holds,
+        i.e. all of full-size state. Compact state holds nothing yet and is seeded from the weights at the first
+        quorum, when the rank's slices are known."""
+        self._seed(self._holdings)
 
     def state_dict(self) -> Dict[str, Any]:
         """What a healing replica needs from ANY peer: the replicated bf16 weights and the update count.
@@ -544,7 +602,14 @@ class Zero1Optimizer:
 
     # ------------------------------------------------------------------ re-shard on quorum change
     def _on_configured(self, store: Any, rank: int, world: int, epoch: int) -> None:
-        """Runs inside ``ProcessGroupB200.configure`` (quorum thread) with the quorum-scoped store."""
+        """Runs inside ``ProcessGroupB200.configure`` (quorum thread) with the quorum-scoped store. Every rank publishes
+        ``{t, hold, pages?, disk?}``, plans every rank's re-shard (:func:`plan_quorum`) and applies its own: pulls
+        (one copy launch), checkpoint reads and re-seeds on the re-shard stream, which the next commit waits for.
+        Full-size state returns without waiting for them. Paged state frees the pages that are neither kept nor a
+        source first and allocates its new ones, and after its pulls it meets its peers at a store barrier before it
+        frees the pages it kept for them, so its re-shard completes here."""
+        from torchft_b200.checkpointing.p2p_transport import device_copy
+
         with self._lock:
             if self._snap_done is not None:
                 # a snapshot copy may still read the state that pulls, seeds, page reuse and heal are about to rewrite
@@ -570,52 +635,79 @@ class Zero1Optimizer:
             for r in range(world):
                 if r != rank:
                     peers[r] = json.loads(bytes(store.get(f"z1/{r}")).decode())
+            ckpt = self._ckpt_files(rank, peers)
+            plans = plan_quorum(self.layout, world, peers, self._page_shift if self.compact else None, ckpt)
+            plan = plans[rank]
+            if plan.lost and ckpt:
+                logger.warning("zero1: no checkpoint of update %d covers this rank's lost ranges %s", plan.tmax, plan.lost)
+            s = self._reshard_stream
+            s.wait_stream(self._commit_stream)  # no update of the old quorum may still touch state that is about to move
             if self.compact:
-                self._reshard_compact(store, rank, world, peers)
-                self._configured, self._disk = True, None
-                return
-            tmax = max(int(p["t"]) for p in peers.values())
-            if self.t < tmax:
-                self._holdings = []  # we missed an update: nothing we hold is current
-            valid = {r: [tuple(x) for x in p["hold"]] for r, p in peers.items() if int(p["t"]) == tmax and r != rank}
-            need = subtract_ranges(self.layout.held(rank, world), self._holdings)
-            pulls, lost = plan_pulls(need, valid, rank)
-            reads = self._disk_reads(lost, tmax, peers)
-            if reads:
-                lost = []
-            with torch.cuda.stream(self._reshard_stream):
-                if pulls:
-                    self._pull(pulls)
-                if reads:
-                    self._read_state(reads)
-                for lo, hi in lost:
-                    # every holder vanished in one transition: re-seed from the replicated bf16 weights
-                    self.master[lo:hi].copy_(self.param[lo:hi])
-                    self.m[lo:hi].zero_()
-                    self.v[lo:hi].zero_()
-                if self.t != tmax:
-                    self.gate[1:2].fill_(tmax)
-                self._reshard_event = self._reshard_stream.record_event()
-            if lost:
-                self.lost_elements += total(lost)
+                peak = max(p.peak for p in plans.values())
+                if peak > self.capacity:
+                    # every rank sees the same plans and raises alike, before anything is freed
+                    raise RuntimeError(f"zero1: re-sharding to a quorum of {world} needs {peak} state pages on one rank, "
+                                       f"the pools hold {self.capacity} (raise min_world's range or state_pages)")
+                self._free_pages(plan.free_first)
+                # from here on a failure (a peer dying before the barrier) leaves this rank at its old t: it must not
+                # claim ranges whose pages it gave back, or a later quorum would pull (or keep) state that is gone
+                self._holdings = plan.hold_mid
+                self._alloc_pages(plan.allocate)
+                with torch.cuda.stream(s):
+                    self._table.copy_(torch.from_numpy(self._table_host))
+            with torch.cuda.stream(s):
+                if plan.pulls:
+                    tables = {src: self._peer_table(peers[src].get("pages")) for src, _, _ in plan.pulls}
+                    entries: List[Tuple[int, int, int]] = []
+                    for name, local in (("z1_master", self.master), ("z1_m", self.m), ("z1_v", self.v)):
+                        ptrs = self.comm.peer_pointers(name)
+                        for src, lo, hi in plan.pulls:
+                            for a, b, at in self._pieces(tables[src], lo, hi):
+                                for c, d, mine in self._pieces(self._table_host, a, b):
+                                    entries.append((ptrs[src] + (at + c - a) * 4, local.data_ptr() + mine * 4, (d - c) * 4))
+                    device_copy(entries, s, chunk_bytes=1 << 20)
+                if plan.reads:
+                    self._read_state(plan.reads)  # nobody live holds these at T: the restored checkpoint does
+                self._seed(plan.lost)  # nobody holds these: re-seed from the replicated bf16 weights
+            if self.compact:
+                s.synchronize()
+                self.comm._store_barrier(store, "z1/pulled", world)  # every peer has finished reading our source pages
+                self._free_pages(plan.free_last)
+                with torch.cuda.stream(s):
+                    self._table.copy_(torch.from_numpy(self._table_host))
+            with torch.cuda.stream(s):
+                if self.t != plan.tmax:
+                    self.gate[1:2].fill_(plan.tmax)
+                self._reshard_event = s.record_event()
+            if plan.lost and plan.counted:
+                self.lost_elements += total(plan.lost)
                 logger.warning("zero1: %d state elements had no surviving holder and were re-seeded from the weights "
-                               "(moments reset)", total(lost))
-            self.pulled_bytes += 12 * total([(lo, hi) for _, lo, hi in pulls])
-            self.t = tmax
-            self._holdings = merge_ranges(list(self._holdings) + list(need))
+                               "(moments reset)", total(plan.lost))
+            self.pulled_bytes += 12 * total([(lo, hi) for _, lo, hi in plan.pulls])
+            self.t = plan.tmax
+            self._holdings = plan.hold
             self._refresh_pending = world > 1
             self._configured, self._disk = True, None
 
-    def _pull(self, pulls: List[Tuple[int, int, int]]) -> None:
-        """One heal_copy launch that gathers (master, m, v)[lo:hi] from the source ranks' segments."""
-        from torchft_b200.checkpointing.p2p_transport import device_copy
+    def _ckpt_files(self, rank: int, peers: Dict[int, Dict[str, Any]]) -> Dict[int, Any]:
+        """The checkpoint files at the quorum's update count that ranks restored from, for :func:`plan_quorum`: this
+        rank's own restore, or else the directory every restored peer published (a live rank may now hold slices that
+        only restored ranks held)."""
+        from torchft_b200.checkpointing.sharded import scan
 
-        entries: List[Tuple[int, int, int]] = []
-        for name, local in (("z1_master", self.master), ("z1_m", self.m), ("z1_v", self.v)):
-            ptrs = self.comm.peer_pointers(name)
-            for src, lo, hi in pulls:
-                entries.append((ptrs[src] + lo * 4, local.data_ptr() + lo * 4, (hi - lo) * 4))
-        device_copy(entries, torch.cuda.current_stream(), chunk_bytes=1 << 20)
+        tmax = max(int(p["t"]) for p in peers.values())
+        if self._disk is not None and self._disk[0] == tmax:
+            return {rank: self._disk[2]}
+        scanned: Dict[str, Any] = {}
+        out = {}
+        for r, p in peers.items():
+            d = p.get("disk")
+            if d and int(d[0]) == tmax:
+                if d[1] not in scanned:
+                    scanned[d[1]] = [(h, [tuple(int(x) for x in rg) for rg in h["ranges"]]) for h in scan(d[1])
+                                     if int(h["T"]) == tmax]
+                out[r] = scanned[d[1]]
+        return out
 
     # ------------------------------------------------------------------ compact (paged) state
     def _page_runs(self) -> List[Tuple[int, int, int]]:
@@ -629,8 +721,22 @@ class Zero1Optimizer:
                 runs.append([pg, slot, 1])
         return [tuple(r) for r in runs]
 
+    def _peer_table(self, runs: Optional[Sequence[Sequence[int]]]) -> Any:
+        """A page table from published ``(page, slot, count)`` runs (``None``: full-size state, no table)."""
+        import numpy as np
+
+        if runs is None:
+            return None
+        t = np.full(len(self._table_host), -1, dtype=np.int64)
+        for pg, slot, n in runs:
+            t[pg:pg + n] = np.arange(slot, slot + n)
+        return t
+
     def _pieces(self, table: Any, lo: int, hi: int) -> List[Tuple[int, int, int]]:
-        """``[lo, hi)`` cut at page boundaries as ``(elem_lo, elem_hi, pool_index)``, pieces in consecutive slots merged."""
+        """``[lo, hi)`` cut at page boundaries as ``(elem_lo, elem_hi, pool_index)``, pieces in consecutive slots merged.
+        Without a ``table`` (full-size state) element ``e`` is at index ``e``: one piece."""
+        if table is None:
+            return [(lo, hi, lo)] if hi > lo else []
         out: List[Tuple[int, int, int]] = []
         sh, mask = self._page_shift, self._page - 1
         e = lo
@@ -670,77 +776,6 @@ class Zero1Optimizer:
                 self.m[at:at + b - a].zero_()
                 self.v[at:at + b - a].zero_()
 
-    def _reshard_compact(self, store: Any, rank: int, world: int, peers: Dict[int, Dict[str, Any]]) -> None:
-        """Move to this quorum's slices inside the page pools. Every rank derives every peer's plan from the published
-        ``{t, hold, pages}``, so it knows which of its old pages are sources: it frees the pages that are neither kept
-        nor a source, allocates its new pages, pulls (one copy launch), waits for its pulls, meets its peers at a store
-        barrier, and only then frees the pages it kept for them."""
-        import numpy as np
-
-        from torchft_b200.checkpointing.p2p_transport import device_copy
-
-        sh = self._page_shift
-        info = {r: (int(p["t"]), [tuple(x) for x in p["hold"]]) for r, p in peers.items()}
-        old = {r: merge_ranges([(pg, pg + n) for pg, _, n in p["pages"]]) for r, p in peers.items()}
-        tmax, plans = plan_reshard(self.layout, info, world)
-        pages = reshard_pages(self.layout, plans, old, world, sh)
-        peak = max(pk for _, _, pk in pages.values())
-        if peak > self.capacity:
-            # every rank sees the same plans and raises alike, before anything is freed
-            raise RuntimeError(f"zero1: re-sharding to a quorum of {world} needs {peak} state pages on one rank, the "
-                               f"pools hold {self.capacity} (raise min_world's range or state_pages)")
-        need, pulls, lost = plans[rank]
-        reads = self._disk_reads(lost, tmax, peers)
-        if reads:
-            lost = []
-        new_pages, src_pages, _ = pages[rank]
-        mine_old = old[rank]
-        free_first, allocate, free_last = reshard_page_steps(mine_old, new_pages, src_pages)
-        s = self._reshard_stream
-        s.wait_stream(self._commit_stream)  # no update of the old quorum may still touch a page that is about to move
-        self._free_pages(free_first)
-        # from here on a failure (a peer dying before the barrier) leaves this rank at its old t: it must not claim
-        # ranges whose pages it gave back, or a later quorum would pull (or keep) state that is no longer there
-        kept = subtract_ranges(mine_old, free_first)
-        self._holdings = backed_ranges(self._holdings, kept, sh)
-        self._alloc_pages(allocate)
-        with torch.cuda.stream(s):
-            self._table.copy_(torch.from_numpy(self._table_host))
-            if pulls:
-                ptabs = {}
-                for src in {p[0] for p in pulls}:
-                    t = np.full(len(self._table_host), -1, dtype=np.int64)
-                    for pg, slot, n in peers[src]["pages"]:
-                        t[pg:pg + n] = np.arange(slot, slot + n)
-                    ptabs[src] = t
-                entries: List[Tuple[int, int, int]] = []
-                for name, local in (("z1_master", self.master), ("z1_m", self.m), ("z1_v", self.v)):
-                    ptrs = self.comm.peer_pointers(name)
-                    for src, lo, hi in pulls:
-                        for a, b, at in self._pieces(ptabs[src], lo, hi):
-                            for c, d, mine in self._pieces(self._table_host, a, b):
-                                entries.append((ptrs[src] + (at + c - a) * 4, local.data_ptr() + mine * 4, (d - c) * 4))
-                device_copy(entries, s, chunk_bytes=1 << 20)
-            if reads:
-                self._read_state(reads)  # nobody live holds these at T: the restored checkpoint does
-            self._seed(lost)  # nobody holds these: re-seed from the replicated bf16 weights
-        s.synchronize()
-        self.comm._store_barrier(store, "z1/pulled", world)  # every peer has finished reading our source pages
-        self._free_pages(free_last)
-        with torch.cuda.stream(s):
-            self._table.copy_(torch.from_numpy(self._table_host))
-            if self.t != tmax:
-                self.gate[1:2].fill_(tmax)
-            self._reshard_event = s.record_event()
-        if lost and tmax > 0:  # at t = 0 every replica has the same seed: a slice nobody holds yet is not lost
-            self.lost_elements += total(lost)
-            logger.warning("zero1: %d state elements had no surviving holder and were re-seeded from the weights "
-                           "(moments reset)", total(lost))
-        self.pulled_bytes += 12 * total([(lo, hi) for _, lo, hi in pulls])
-        self.t = tmax
-        self._holdings = self.layout.held(rank, world)
-        self._refresh_pending = world > 1
-
     # ------------------------------------------------------------------ per-step pipeline
     def unit_of(self, lo: int, hi: int) -> int:
         return self.layout.units.index((lo, hi))
@@ -750,52 +785,35 @@ class Zero1Optimizer:
         gradient accumulation, ``micro`` is the micro-batch index; ``scale`` applies on the last micro-batch only."""
         lo, hi = self.layout.units[unit]
         mode = accum_mode(micro, self.grad_accum_steps)
-        if mode:
-            return self._reduce_accum(unit, lo, hi, scale, contribute, micro, mode)
-        if self.max_grad_norm is not None:
-            gn = self._gnorm.data_ptr() + 8 * unit
-            after = self._commit_event
-            k = self.layout.replication
-
-            def launch(s: torch.cuda.Stream) -> None:
-                if after is not None:
-                    # the last commit kernel read the partials this launch overwrites (see zero1_commit_kernel)
-                    s.wait_event(after)
-                self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s,
-                                                gnorm=gn)
-
-            return self.pg._launch(launch, None)
-        if self.comm.world == 1:
+        clip = self.max_grad_norm is not None
+        if self.comm.world == 1 and not clip and not mode:
             if scale != 1.0 or not contribute:
                 self.grad[lo:hi].mul_(scale if contribute else 0.0)
             return None
-        k = self.layout.replication
-        return self.pg._launch(
-            lambda s: self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s),
-            None)
-
-    def _reduce_accum(self, unit: int, lo: int, hi: int, scale: float, contribute: bool, micro: int, mode: int) -> Any:
-        """One micro-batch's reduce of ``unit`` into (modes 1, 2) or out of (mode 3) the accumulator. The reduce kernel
-        runs at world 1 too (in place, no handshake): the scale belongs after the sum over micro-batches."""
-        rank, world = self.comm.rank, self.comm.world
-        if self._acc_for != (rank, world):
-            self._accum_for(rank, world)
-        acc = self._acc.data_ptr() + 4 * self._acc_offsets[unit]
-        gn = self._gnorm.data_ptr() + 8 * unit if self.max_grad_norm is not None and mode == 3 else 0
-        after = self._commit_event if self.max_grad_norm is not None else None
+        # with accumulation the kernel runs at world 1 too (in place, no handshake): the scale belongs after the sum
+        # over micro-batches, which it adds into (modes 1, 2) or out of (mode 3) this rank's accumulator
+        acc = 0
+        if mode:
+            rank, world = self.comm.rank, self.comm.world
+            if self._acc_for != (rank, world):
+                self._accum_for(rank, world)
+            acc = self._acc.data_ptr() + 4 * self._acc_offsets[unit]
+        gn = self._gnorm.data_ptr() + 8 * unit if clip and mode in (0, 3) else 0
+        after = self._commit_event if clip else None
         k = self.layout.replication
 
         def launch(s: torch.cuda.Stream) -> None:
             if after is not None:
-                # the last commit kernel read the partials this step's last micro-batch overwrites
+                # the last commit kernel read the partials this step overwrites (see zero1_commit_kernel)
                 s.wait_event(after)
             self.comm.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, scale, contribute, k, self._rs_blocks, s,
                                             gnorm=gn, acc=acc, acc_mode=mode)
 
         work = self.pg._launch(launch, None)
-        # micro-batches must arrive in order from 0; anything else poisons the unit until the next micro-batch 0
-        in_order = micro == 0 or self._micro_seen[unit] == micro
-        self._micro_seen[unit] = micro + 1 if in_order else -1
+        if mode:
+            # micro-batches must arrive in order from 0; anything else poisons the unit until the next micro-batch 0
+            in_order = micro == 0 or self._micro_seen[unit] == micro
+            self._micro_seen[unit] = micro + 1 if in_order else -1
         return work
 
     # -- committer protocol of Manager.commit_on_device ---------------------------------------------------------
@@ -823,11 +841,9 @@ class Zero1Optimizer:
             stream.wait_event(self._reshard_event)  # a verdict also tells peers "my pulls are done"
             self._reshard_event = None
         self._commit_layout = (self.comm.rank, self.comm.world)
-        if self.max_grad_norm is not None:
-            seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream, gnorm="z1_gnorm",
-                                          nunits=len(self.layout.units), max_norm=self.max_grad_norm, norm=self._clip)
-        else:
-            seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream)
+        clip = {} if self.max_grad_norm is None else dict(gnorm="z1_gnorm", nunits=len(self.layout.units),
+                                                           max_norm=self.max_grad_norm, norm=self._clip)
+        seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream, **clip)
         self._commit_event = stream.record_event()
         return seq
 
@@ -855,17 +871,22 @@ class Zero1Optimizer:
         for i, (lo, hi) in enumerate(self.layout.units):
             if snap is not None:
                 stream.wait_event(snap[i])  # the last save's copy of this unit has read it
+            state = self._update_state(lo)
             for mode in modes:
-                if self.compact:
-                    self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr(),
-                                            self.m.data_ptr(), self.v.data_ptr(), hi - lo, hp, self.gate, k, mode,
-                                            self._upd_blocks, stream, self._table.data_ptr(), lo, self._page_shift, coef=coef)
-                    continue
-                self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, self.master.data_ptr() + lo * 4,
-                                        self.m.data_ptr() + lo * 4, self.v.data_ptr() + lo * 4, hi - lo, hp,
-                                        self.gate, k, mode, self._upd_blocks, stream, coef=coef)
+                self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, nelem=hi - lo, hyper=hp,
+                                        gate=self.gate, replication=k, mode=mode, blocks=self._upd_blocks, stream=stream,
+                                        coef=coef, **state)
             if events is not None:
                 events[i].record(stream)
+
+    def _update_state(self, lo: int) -> Dict[str, int]:
+        """The state arguments of ``zero1_update_`` for the unit that starts at element ``lo``. Full-size state passes
+        the arrays at ``lo`` and no table, which selects the kernel without page lookups; paged state passes the pools
+        and the page table, through which the kernel finds each element."""
+        ptrs = {"master": self.master.data_ptr(), "m": self.m.data_ptr(), "v": self.v.data_ptr()}
+        if self._table is None:
+            return {name: p + 4 * lo for name, p in ptrs.items()}
+        return {**ptrs, "table": self._table.data_ptr(), "state_off": lo, "page_shift": self._page_shift}
 
     def resolved(self, verdict: bool) -> None:
         """The Manager learned the verdict of the last :meth:`commit` (lazily, on the quorum thread)."""
@@ -934,9 +955,6 @@ class Zero1Optimizer:
                         stage[2 * x:2 * (x + b - a)].copy_(self.param[a:b].view(u8), non_blocking=True)
                         for name, arr in (("master", self.master), ("m", self.m), ("v", self.v)):
                             base = sec[name] + 4 * x
-                            if not self.compact:
-                                stage[base:base + 4 * (b - a)].copy_(arr[a:b].view(u8), non_blocking=True)
-                                continue
                             for c, d, at in self._pieces(self._table_host, a, b):  # maximal runs of consecutive slots
                                 stage[base + 4 * (c - a):base + 4 * (d - a)].copy_(arr[at:at + d - c].view(u8),
                                                                                    non_blocking=True)
@@ -988,27 +1006,6 @@ class Zero1Optimizer:
         logger.info("zero1: restored the weights of update %d from %d checkpoint file(s) in %s", T, len(files), directory)
         return {"step": int(first["step"]), "batches_committed": int(first["batches"])}
 
-    def _disk_reads(self, lost: Sequence[Range], tmax: int, peers: Dict[int, Dict[str, Any]]
-                    ) -> List[Tuple[Any, int, int, int]]:
-        """Reads that fill ``lost`` from a restored checkpoint at the quorum's update count: this rank's own, or one a
-        restored peer published (a live rank may now hold slices that only restored ranks held)."""
-        if not lost:
-            return []
-        if self._disk is not None and self._disk[0] == tmax:
-            return ckpt_read_plan(lost, self._disk[2])
-        for r in sorted(peers):
-            d = peers[r].get("disk")
-            if d and int(d[0]) == tmax:
-                from torchft_b200.checkpointing.sharded import scan
-
-                files = [(h, [tuple(int(x) for x in rg) for rg in h["ranges"]]) for h in scan(d[1]) if int(h["T"]) == tmax]
-                try:
-                    return ckpt_read_plan(lost, files)
-                except ValueError as e:
-                    logger.warning("zero1: checkpoint %s of update %d does not cover this rank's lost ranges: %s",
-                                   d[1], tmax, e)
-        return []
-
     def _read_state(self, reads: Sequence[Tuple[Any, int, int, int]]) -> None:
         self._read_ranges(reads, ("master", "m", "v"))
         self.disk_read_elements += total([(lo, hi) for _, _, lo, hi in reads])
@@ -1023,10 +1020,7 @@ class Zero1Optimizer:
         try:
             for h, off, lo, hi in reads:
                 for name in arrays:
-                    if name == "param" or not self.compact:
-                        rd.read(h, name, off, dst[name][lo:hi])
-                        continue
-                    for a, b, at in self._pieces(self._table_host, lo, hi):
+                    for a, b, at in self._pieces(None if name == "param" else self._table_host, lo, hi):
                         rd.read(h, name, off + a - lo, dst[name][at:at + b - a])
         finally:
             rd.close()
@@ -1037,18 +1031,15 @@ class Zero1Optimizer:
 
     def state_bytes_allocated(self) -> int:
         """Device bytes of the fp32 master/m/v arrays (compact: the page pools)."""
-        return 12 * (self.capacity * self._page if self.compact else self.numel)
+        return 12 * self.master.numel()
 
     def held_state(self) -> Dict[Range, Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
         """Copies of (master, m, v) over each range this rank holds, keyed by ``(lo, hi)`` (for inspection and tests)."""
         out = {}
         torch.cuda.synchronize(self.device)
         for lo, hi in self._holdings:
-            if not self.compact:
-                out[(lo, hi)] = (self.master[lo:hi].clone(), self.m[lo:hi].clone(), self.v[lo:hi].clone())
-                continue
-            idx = torch.cat([torch.arange(at, at + b - a, device=self.device) for a, b, at in self._pieces(self._table_host, lo, hi)])
-            out[(lo, hi)] = (self.master[idx], self.m[idx], self.v[idx])
+            pieces = self._pieces(self._table_host, lo, hi)
+            out[(lo, hi)] = tuple(torch.cat([x[at:at + b - a] for a, b, at in pieces]) for x in (self.master, self.m, self.v))
         return out
 
     def zero_grad(self, set_to_none: bool = False) -> None:  # gradients are overwritten by the wgrad GEMMs
