@@ -27,6 +27,11 @@ acc (a middle micro-batch: 32 B of fp32 accumulator read and written per 8 eleme
 It first checks that an accumulated pair gives the off result bit for bit. The peer loads hit local HBM, so this
 compares the kernels' HBM behaviour, not NVLink.
 
+``--virtual W --sched`` times the update of one unit (rank 0's launch) without a learning-rate schedule and with a
+table of rates and two weight-decay exemptions, alternating the two ``--repeats`` times, with the card's name and power
+limit. The scheduled launch adds one uniform table load per thread and a few integer compares per 8 elements to a kernel
+bound by HBM; it first checks that a constant table and no exemptions give the plain launch's bits.
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -204,6 +209,55 @@ def clip_ab(comm, nelem, k, rs_blocks, upd_blocks, iters, warmup, repeats, max_n
     return out
 
 
+def sched_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats):
+    """The update of one unit without a schedule and with a 1000-entry rate table and two exempt ranges, alternately."""
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
+    dev = comm.device
+    grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
+    grad.normal_()
+    gate = torch.ones(2, dtype=torch.int32, device=dev)
+    gate[1] = 500
+    init = torch.randn(nelem, device=dev)
+    table = torch.full((1000,), HP[0], dtype=torch.float32, device=dev)
+
+    def state():
+        return [init.clone(), torch.zeros(nelem, device=dev), torch.zeros(nelem, device=dev)]
+
+    def launch(st, **kw):
+        return lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), st[0].data_ptr(), st[1].data_ptr(),
+                                          st[2].data_ptr(), nelem, HP, gate, k, 0, upd_blocks, **kw)
+
+    # bit check: a table of the constant rate and no exemptions is the plain launch
+    a, b = state(), state()
+    launch(a)()
+    launch(b, lr_table=table.data_ptr(), lr_steps=table.numel())()
+    torch.cuda.synchronize()
+    same = all(torch.equal(x, y) for x, y in zip(a, b))
+    nd = [(nelem // 8 // 8 * 8, nelem // 8 // 8 * 8 + 4096), (nelem // 2 // 8 * 8, nelem // 2 // 8 * 8 + 4096)]
+    st = state()
+    arms = (("off", launch(st)), ("sched", launch(st, lr_table=table.data_ptr(), lr_steps=table.numel(), no_decay=nd)))
+    times = {name: [] for name, _ in arms}
+    for _ in range(repeats):
+        for name, fn in arms:
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    out = {"timing": "local HBM (virtual ranks), not NVLink", "constant_table_equals_off": same, "no_decay_ranges": nd}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        out[f"adamw_allgather_{name}_ms"] = {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4),
+                                             "max": round(ts[-1], 4)}
+    out["sched_over_off"] = round(out["adamw_allgather_sched_ms"]["median"] / out["adamw_allgather_off_ms"]["median"], 4)
+    return out
+
+
 def accum_ab(comms, nelem, k, rs_blocks, iters, warmup, repeats):
     """Rank 0's reduce-scatter of one unit in the three accumulation modes, timed alternately: ``off`` (today's launch),
     ``acc`` (a middle micro-batch: fp32 rank sum added into the accumulator) and ``last`` (accumulator + rank sum,
@@ -281,7 +335,9 @@ def main() -> None:
     ap.add_argument("--compact", action="store_true", help="--virtual: A/B the update on flat vs paged optimizer state")
     ap.add_argument("--clip", action="store_true", help="--virtual: A/B one unit's pipeline without and with gradient clipping")
     ap.add_argument("--accum", action="store_true", help="--virtual: A/B rank 0's reduce in accumulation modes off / acc / last")
-    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum: alternations of the arms")
+    ap.add_argument("--sched", action="store_true", help="--virtual: A/B the update without and with a learning-rate "
+                    "table and weight-decay exemptions")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum / --sched: alternations of the arms")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -292,9 +348,11 @@ def main() -> None:
         segments = {"z1_grad": S, "z1_param": S, **({"z1_gnorm": 8} if a.clip else {})}
         comms = SymmetricComm.virtual_world(a.virtual, segments, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
-        if a.compact or a.clip or a.accum:
+        if a.compact or a.clip or a.accum or a.sched:
             if a.compact:
                 res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
+            elif a.sched:
+                res.update(sched_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
             elif a.accum:
                 res.update(accum_ab(comms, nelem, a.replication, a.rs_blocks, a.iters, a.warmup, a.repeats))
             else:

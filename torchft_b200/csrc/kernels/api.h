@@ -36,6 +36,11 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
 // Gradient accumulation (acc_mode 0 = off by default): `acc` is this rank's fp32 accumulator of the unit's primary
 // slice. acc_mode 1 (first micro-batch) stores the fp32 rank sum there, 2 (middle) adds it; neither writes the gradient
 // segment. 3 (last) reduces (acc + rank sum) * scale to bf16 like mode 0, with the gradient norm when `gn` is set.
+// Learning-rate schedule (lr_tab null by default = the constant `lr`): lr_tab[i] is the fp32 rate of committed update
+// i + 1, and the update reads lr_tab[clamp(gate[1], 1, lr_steps) - 1] for both the step and the decoupled decay.
+// Weight-decay exemptions: `no_decay` holds n_no_decay <= kMaxNoDecay unit-relative element ranges as (lo, hi) pairs,
+// multiples of 8, whose elements get no decay.
+constexpr int kMaxNoDecay = 4;
 void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
                             int barrier_mode, cudaStream_t stream);
 void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
@@ -47,7 +52,9 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream,
-                         const int* table = nullptr, size_t soff = 0, int page_shift = 0, const float* coef = nullptr);
+                         const int* table = nullptr, size_t soff = 0, int page_shift = 0, const float* coef = nullptr,
+                         const float* lr_tab = nullptr, int lr_steps = 0, int n_no_decay = 0,
+                         const size_t* no_decay = nullptr);
 
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);

@@ -34,6 +34,10 @@
 // slice in fp32 into a per-rank accumulator of the primary slices only (no bf16 rounding, no gradient write, no push);
 // the last one adds the accumulator and finishes exactly like a single step (scale, bf16, buddy push, CLIP squares).
 //
+// Learning-rate schedule and weight-decay exemptions (opt-in, non-null table / non-zero count, no template flag): the
+// update kernel reads the rate of the committed update count gate[1] from a device table, and vectors inside up to
+// kMaxNoDecay unit-relative ranges take no decay.
+//
 // The two big kernels contain NO inter-rank synchronisation at all: any grid size, no co-residency requirement, no
 // SM held by a spinning CTA while peers are skewed, profilable stand-alone. Ordering comes from the one-CTA handshake
 // kernels around them (bounded, abortable spins; epoch-tagged flags; error latched in the status block and mirrored
@@ -416,6 +420,13 @@ struct UpdArgs {
   size_t soff;
   int page_shift;
   const float* coef;   // CLIP: the clip coefficient the commit kernel wrote; the gradient is scaled by it (mode 0)
+  // learning-rate schedule (lr_tab != nullptr): lr_tab[i] is the fp32 rate of committed update i + 1; update t uses
+  // lr_tab[clamp(t, 1, lr_steps) - 1] in place of lr (past the table the last rate holds)
+  const float* lr_tab;
+  int lr_steps;
+  // weight-decay exemptions: n_nd ranges [nd_lo, nd_hi) of 8-element vectors, relative to the unit, get no decay
+  int n_nd;
+  size_t nd_lo[kMaxNoDecay], nd_hi[kMaxNoDecay];
 };
 
 template <int W, bool NVLS, bool PAGED, bool CLIP>
@@ -428,11 +439,15 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   if constexpr (CLIP) {
     if (a.mode == 0) cf = __ldg(a.coef);
   }
-  const float tf = (float)a.gate[1];
+  const int t = a.gate[1];
+  const float tf = (float)t;
+  // the rate follows the committed update count on the device, like the bias correction: one uniform load
+  // (a refresh may run at t = 0 and does not use it)
+  const float lr = a.lr_tab != nullptr ? __ldg(a.lr_tab + (min(max(t, 1), a.lr_steps) - 1)) : a.lr;
   const float bc1 = 1.f - powf(a.b1, tf), bc2 = 1.f - powf(a.b2, tf);
-  const float step_size = a.lr / bc1;
+  const float step_size = lr / bc1;
   const float inv_bc2_sqrt = rsqrtf(bc2);
-  const float decay = 1.f - a.lr * a.wd;
+  const float decay = 1.f - lr * a.wd;
   // dst[0] = this rank; dst[j] = rank + j. Ranks rank+1 .. rank+k-1 hold the primary slice too and compute the same
   // bits themselves, so the primary only pushes to dst[k .. W-1] (mode 0). A refresh pushes to everybody.
   bf16* dst[W];
@@ -478,12 +493,18 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
         Pack<float>::unpack(m1, m + 4);
         Pack<float>::unpack(v0, vv);
         Pack<float>::unpack(v1, vv + 4);
+        float dcy = decay;
+        if (a.n_nd > 0) {  // uniform: without exemptions no vector pays for the compares
+#pragma unroll
+          for (int r = 0; r < kMaxNoDecay; ++r)
+            if (r < a.n_nd && v >= a.nd_lo[r] && v < a.nd_hi[r]) dcy = 1.f;
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           m[i] = a.b1 * m[i] + (1.f - a.b1) * gr[i];
           vv[i] = a.b2 * vv[i] + (1.f - a.b2) * gr[i] * gr[i];
           const float denom = sqrtf(vv[i]) * inv_bc2_sqrt + a.eps;
-          w[i] = w[i] * decay - step_size * __fdividef(m[i], denom);
+          w[i] = w[i] * dcy - step_size * __fdividef(m[i], denom);
         }
         st_stream(a.master + si, Pack<float>::pack(w));
         st_stream(a.master + si + 4, Pack<float>::pack(w + 4));
@@ -628,13 +649,26 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
                          float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream, const int* table,
-                         size_t soff, int page_shift, const float* coef) {
+                         size_t soff, int page_shift, const float* coef, const float* lr_tab, int lr_steps,
+                         int n_no_decay, const size_t* no_decay) {
   check_grid(blocks, threads, "zero1_update");
   if ((poff & 15) || (nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
   if (table != nullptr && (page_shift < 3 || page_shift > 30 || (soff & 7)))
     throw std::runtime_error("zero1_update: pages must be 2^3 .. 2^30 elements and the unit 8-element aligned");
+  if (lr_tab != nullptr && (lr_steps < 1 || (reinterpret_cast<uintptr_t>(lr_tab) & 3)))
+    throw std::runtime_error("zero1_update: a learning-rate table needs lr_steps >= 1 and 4 B alignment");
+  if (n_no_decay < 0 || n_no_decay > kMaxNoDecay || (n_no_decay > 0 && no_decay == nullptr))
+    throw std::runtime_error("zero1_update: at most " + std::to_string(kMaxNoDecay) + " weight-decay exemptions per unit");
   UpdArgs a{pt, reinterpret_cast<char*>(mc_base), gate, poff, reinterpret_cast<const bf16*>(grad), master, m, v,
-            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift, coef};
+            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift, coef, lr_tab, lr_tab != nullptr ? lr_steps : 0,
+            n_no_decay, {}, {}};
+  for (int r = 0; r < n_no_decay; ++r) {
+    const size_t lo = no_decay[2 * r], hi = no_decay[2 * r + 1];
+    if ((lo & 7) || (hi & 7) || lo >= hi || hi > nelem)
+      throw std::runtime_error("zero1_update: weight-decay exemptions must be non-empty 8-element aligned ranges inside the unit");
+    a.nd_lo[r] = lo / 8;
+    a.nd_hi[r] = hi / 8;
+  }
   if (table != nullptr) {
     if (mc_base != nullptr)
       launch_upd<true, true>(a, blocks, threads, stream);

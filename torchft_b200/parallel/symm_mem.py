@@ -28,7 +28,7 @@ import threading
 import time
 from dataclasses import dataclass
 from datetime import timedelta
-from typing import Any, Dict, List, Optional, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -900,14 +900,27 @@ class SymmetricComm:
     def zero1_update_(self, segment: str, poff: int, grad: int, master: int, m: int, v: int, nelem: int,
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,
                       blocks: int, stream: Optional[torch.cuda.Stream] = None, table: int = 0, state_off: int = 0,
-                      page_shift: int = 0, coef: int = 0) -> None:
+                      page_shift: int = 0, coef: int = 0, lr_table: int = 0, lr_steps: int = 0,
+                      no_decay: Sequence[Tuple[int, int]] = ()) -> None:
         """Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights into
         ``segment`` on the ranks that do not hold it (``mode`` 1: ungated re-broadcast of bf16(master) to everybody, no
         state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed.
 
         ``table`` (device pointer to int32 page slots, 0 = flat state) selects paged state: ``master``/``m``/``v`` are
         then page pools and element ``state_off + i`` of the unit lives in pool page ``table[(state_off + i) >> page_shift]``.
-        ``coef`` (device address of an fp32, 0 = none): the gradient is multiplied by it (the clip coefficient)."""
+        ``coef`` (device address of an fp32, 0 = none): the gradient is multiplied by it (the clip coefficient).
+        ``lr_table`` (device address of ``lr_steps`` fp32 rates, 0 = the constant ``hyper`` rate): update ``t`` (the
+        device step count) uses entry ``min(max(t, 1), lr_steps) - 1`` for the step and the decay. ``no_decay``: at most
+        ``ZERO1_MAX_NO_DECAY`` unit-relative element ranges, multiples of 8, whose elements get no weight decay."""
+        if lr_table and lr_steps < 1:
+            raise ValueError(f"a learning-rate table needs lr_steps >= 1, got {lr_steps}")
+        nd = [(int(lo), int(hi)) for lo, hi in no_decay]
+        if len(nd) > self._K.ZERO1_MAX_NO_DECAY:
+            raise ValueError(f"at most {self._K.ZERO1_MAX_NO_DECAY} weight-decay exemptions per unit, got {len(nd)}")
+        for lo, hi in nd:
+            if lo % 8 or hi % 8 or not 0 <= lo < hi <= nelem:
+                raise ValueError(f"weight-decay exemption [{lo}, {hi}) is not an 8-element aligned range of the unit "
+                                 f"of {nelem} elements")
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -916,7 +929,8 @@ class SymmetricComm:
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp,
-                                 table, state_off, page_shift, coef)
+                                 table, state_off, page_shift, coef, lr_table, lr_steps if lr_table else 0,
+                                 [x for r in nd for x in r])
             self.launches += 1
             pushes = self._world > 1 and (mode == 1 or self._world > replication)
             if pushes:

@@ -27,9 +27,10 @@ from __future__ import annotations
 import dataclasses
 import os
 from datetime import timedelta
-from typing import Any, Dict, List, Optional, Tuple
+from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
+from torch import nn
 from torch.distributed import TCPStore
 
 from torchft_b200.ddp import FlatDistributedDataParallel
@@ -37,6 +38,20 @@ from torchft_b200.manager import Manager
 from torchft_b200.models.llama import CONFIGS, FlatParams, Llama, LlamaConfig
 from torchft_b200.optim import OptimizerWrapper
 from torchft_b200.ops.fused import FlatAdamW
+from torchft_b200.parallel.zero1 import intersect_ranges, merge_ranges
+
+
+def no_decay_ranges(flat: FlatParams, module: nn.Module, select: Callable[[str, nn.Parameter], bool]
+                    ) -> List[Tuple[int, int]]:
+    """The flat element ranges of ``module``'s parameters for which ``select(name, p)`` holds, each with the
+    ``FlatParams.ALIGN`` padding behind it (the padding is never read, so exempting it changes nothing), merged."""
+    where = {id(p): o for p, o in zip(flat.params, flat.offsets)}
+    out = []
+    for name, p in module.named_parameters():
+        if id(p) in where and select(name, p):
+            o = where[id(p)]
+            out.append((o, min(o + (p.numel() + FlatParams.ALIGN - 1) // FlatParams.ALIGN * FlatParams.ALIGN, flat.numel)))
+    return merge_ranges(out)
 
 
 class FaultTolerantTrainer:
@@ -60,6 +75,12 @@ class FaultTolerantTrainer:
             ``(M * B, S)`` inputs, run ``M`` forward/backward passes of ``B`` sequences and apply the gradient of the mean
             loss over all of them; each micro-batch is reduce-scattered under its own backward into an fp32
             accumulator of this replica's slices. Not available on the classic all-reduce pipeline.
+        lr_lambda: FT-ZeRO-1: learning-rate schedule as a ``LambdaLR`` lambda stepped once per committed step: committed
+            update ``t`` uses ``lr * lr_lambda(min(t, lr_steps) - 1)``; vetoed steps do not advance it. Tabulated once
+            at construction. Not available on the classic all-reduce pipeline.
+        lr_steps: FT-ZeRO-1: length of that table (required with ``lr_lambda``); later updates keep its last rate
+        no_decay: FT-ZeRO-1: ``(name, parameter) -> bool`` selecting the parameters that get no weight decay, e.g.
+            ``lambda name, p: p.ndim == 1`` for the norm gains. Not available on the classic all-reduce pipeline.
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -73,7 +94,9 @@ class FaultTolerantTrainer:
                  use_async_quorum: bool = True, overlap_optimizer: Optional[bool] = None,
                  optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2,
                  compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None,
-                 grad_accum_steps: int = 1) -> None:
+                 grad_accum_steps: int = 1, lr_lambda: Optional[Callable[[int], float]] = None,
+                 lr_steps: Optional[int] = None,
+                 no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -93,6 +116,10 @@ class FaultTolerantTrainer:
         if grad_accum_steps > 1 and not self.zero1:
             raise ValueError("grad_accum_steps > 1 needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         self.grad_accum_steps = int(grad_accum_steps)
+        if (lr_lambda is not None or no_decay is not None) and not self.zero1:
+            raise ValueError("lr_lambda and no_decay need the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if lr_lambda is not None and lr_steps is None:
+            raise ValueError("lr_lambda needs lr_steps, the length of the schedule")
         self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
         self._steps_run = 0  # steps started by this trainer (a checkpoint restore must come first)
 
@@ -121,7 +148,8 @@ class FaultTolerantTrainer:
             # buckets = update launches) are the forward stages, known once the parameters have offsets.
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
                                        compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
-                                       grad_accum_steps=self.grad_accum_steps)
+                                       grad_accum_steps=self.grad_accum_steps, lr_lambda=lr_lambda,
+                                       lr_steps=lr_steps or 0)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:
@@ -131,7 +159,11 @@ class FaultTolerantTrainer:
         self._stage_ranges = self._compute_stage_ranges()
 
         if self.zero1:
-            self.zopt.set_units(self._stage_ranges)
+            nd = None
+            if no_decay is not None:
+                nd = [r for unit in self._stage_ranges
+                      for r in intersect_ranges(no_decay_ranges(self.flat, self.model, no_decay), [unit])]
+            self.zopt.set_units(self._stage_ranges, no_decay=nd)
             self.zopt.seed_master()
             self.inner_optim: Any = self.zopt
         else:
@@ -388,6 +420,13 @@ class FaultTolerantTrainer:
         """Global gradient norm of the most recently resolved step (FT-ZeRO-1 with clipping; ``None`` otherwise). Steps
         resolve lazily, so after step ``n`` this is usually the norm of step ``n - 1``."""
         return self.zopt.last_grad_norm if self.zopt is not None else None
+
+    def last_lr(self) -> Optional[float]:
+        """The fp32 learning rate of the most recently resolved committed update (FT-ZeRO-1; ``None`` before the first
+        one and on the classic pipeline). Steps resolve lazily, like :meth:`last_grad_norm`."""
+        if self.zopt is None or self.zopt.t < 1:
+            return None
+        return self.zopt.lr_at(self.zopt.t)
 
     def last_loss(self) -> Optional[float]:
         """Loss of the most recent :meth:`step_async` (waits for it)."""

@@ -33,7 +33,7 @@ import math
 import os
 import threading
 from dataclasses import dataclass
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -43,10 +43,12 @@ Range = Tuple[int, int]
 
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
            "plan_reshard", "reshard_pages", "reshard_page_steps", "RankPlan", "plan_quorum", "backed_ranges", "pool_pages", "page_ranges",
-           "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan"]
+           "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan",
+           "lr_schedule_table", "split_no_decay", "schedule_digest"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
+MAX_NO_DECAY = 4  # weight-decay exemptions per unit and update launch (kMaxNoDecay of csrc/kernels/api.h)
 
 
 def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
@@ -62,6 +64,53 @@ def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
     if not max_grad_norm > 0:
         raise ValueError(f"max_grad_norm must be > 0 (inf: compute the norm without scaling), got {max_grad_norm}")
     return max_grad_norm
+
+
+# --------------------------------------------------------------------------- learning-rate schedule, decay exemptions
+def lr_schedule_table(lr: float, lr_lambda: Callable[[int], float], lr_steps: int) -> Any:
+    """The fp32 rates of committed updates ``1 .. lr_steps`` as a numpy array: entry ``i`` is
+    ``fp32(lr * lr_lambda(i))``, evaluated in Python double -- what ``LambdaLR(opt, lr_lambda)`` sets after ``i``
+    scheduler steps. Raises ``ValueError`` for ``lr_steps < 1`` and for a rate that is negative or not finite."""
+    import numpy as np
+
+    if int(lr_steps) != lr_steps or lr_steps < 1:
+        raise ValueError(f"a learning-rate schedule needs lr_steps >= 1, got {lr_steps}")
+    rates = [float(lr) * float(lr_lambda(i)) for i in range(int(lr_steps))]
+    bad = next((i for i, x in enumerate(rates) if not (math.isfinite(x) and x >= 0)), None)
+    if bad is not None:
+        raise ValueError(f"the learning rate of update {bad + 1} is {rates[bad]}: it must be finite and >= 0")
+    return np.asarray(rates, dtype=np.float32)
+
+
+def split_no_decay(units: Sequence[Range], ranges: Sequence[Range], cap: int = MAX_NO_DECAY) -> List[List[Range]]:
+    """Flat element ranges exempt from weight decay, as unit-relative ranges per unit (``units`` in their own order).
+    Ranges that touch inside one unit are merged. Raises ``ValueError`` for a range that is not 8-element aligned, that
+    is not inside one unit, or for more than ``cap`` ranges in one unit."""
+    out: List[List[Range]] = [[] for _ in units]
+    for lo, hi in sorted((int(a), int(b)) for a, b in ranges):
+        if lo % 8 or hi % 8 or lo >= hi:
+            raise ValueError(f"weight-decay exemption [{lo}, {hi}) must be a non-empty range of multiples of 8 elements")
+        u = next((i for i, (a, b) in enumerate(units) if a <= lo < b), None)
+        if u is None or hi > units[u][1]:
+            raise ValueError(f"weight-decay exemption [{lo}, {hi}) is not inside one unit")
+        out[u].append((lo, hi))
+    for u, rs in enumerate(out):
+        base = units[u][0]
+        out[u] = [(lo - base, hi - base) for lo, hi in merge_ranges(rs)]
+        if len(out[u]) > cap:
+            raise ValueError(f"unit {u} {tuple(units[u])} has {len(out[u])} weight-decay exemptions, at most {cap} fit "
+                             f"one update launch")
+    return out
+
+
+def schedule_digest(table: Any, no_decay: Sequence[Range]) -> str:
+    """A digest of the learning-rate table's fp32 bytes (``None``: constant rate) and the merged exempt ranges, which
+    every replica of a quorum must share."""
+    import hashlib
+
+    h = hashlib.sha256(b"none" if table is None else table.tobytes())
+    h.update(json.dumps(merge_ranges(no_decay)).encode())
+    return h.hexdigest()
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -429,16 +478,29 @@ class Zero1Optimizer:
             ``TORCHFT_B200_Z1_MAX_GRAD_NORM``, unset = no clipping)
         grad_accum_steps: micro-batches per step (``M``); the accumulator is sized for every world in
             ``[min_world, 8]``
+        lr_lambda: learning-rate schedule: committed update ``t`` (1-based, the device's count) uses
+            ``fp32(lr * lr_lambda(min(t, lr_steps) - 1))``, what ``LambdaLR`` gives when stepped after every committed
+            step. The rates are tabulated once here (``lr`` is then the base rate, read once); ``None``: the constant
+            ``param_groups[0]["lr"]``, read at every :meth:`update`.
+        lr_steps: entries of the table; later updates keep the last rate
+        no_decay: flat element ranges (multiples of 8, each inside one unit, at most ``MAX_NO_DECAY`` per unit) whose
+            elements get no weight decay
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
                  betas: Tuple[float, float] = (0.9, 0.95), eps: float = 1e-8, weight_decay: float = 0.1,
                  replication: int = 2, blocks: Optional[int] = None, compact: Optional[bool] = None, min_world: int = 1,
                  state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT,
-                 max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1) -> None:
+                 max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1,
+                 lr_lambda: Optional[Callable[[int], float]] = None, lr_steps: int = 0,
+                 no_decay: Sequence[Range] = ()) -> None:
         from torchft_b200.ops import _native
 
         self.max_grad_norm = clip_threshold(max_grad_norm)
+        # learning-rate schedule: fp32 rate of committed update i + 1 at index i (host copy and device table)
+        self._lr_host = lr_schedule_table(lr, lr_lambda, lr_steps) if lr_lambda is not None else None
+        self.no_decay: List[Range] = [(int(a), int(b)) for a, b in no_decay]  # split by unit in set_units
+        self._nd_units: Optional[List[List[Range]]] = None  # ... unit-relative ranges per unit
         if int(grad_accum_steps) != grad_accum_steps or grad_accum_steps < 1:
             raise ValueError(f"grad_accum_steps must be an integer >= 1, got {grad_accum_steps}")
         self.grad_accum_steps = int(grad_accum_steps)
@@ -455,6 +517,11 @@ class Zero1Optimizer:
         self.layout: ShardLayout = ShardLayout(((0, numel),), self._replication)
         self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay
         self.param_groups = [{"lr": lr, "betas": betas, "eps": eps, "weight_decay": weight_decay}]
+        self._lr_tab: Optional[torch.Tensor] = None
+        if self._lr_host is not None:
+            # a synchronous copy: the table is on the device before any update can be enqueued on any stream
+            self._lr_tab = torch.from_numpy(self._lr_host).to(self.device)
+            torch.cuda.current_stream(self.device).synchronize()
         # the big kernels are sync-free, so their grids are free parameters: the reduce-scatter is NVLink-latency bound
         # and shares the SMs with backward; the update is HBM-bound and likes many short CTAs (cf. the AdamW cap sweep)
         self._rs_blocks = int(os.environ.get("TORCHFT_B200_Z1_RS_BLOCKS", 128))
@@ -517,17 +584,24 @@ class Zero1Optimizer:
         self.disk_read_elements = 0      # state elements re-shards read from a restored checkpoint's files
         if units is not None:
             self.set_units(units)
+        elif self.no_decay:
+            self._nd_units = split_no_decay(self.layout.units, self.no_decay)
         pg.add_configure_hook(self._on_configured)
 
-    def set_units(self, units: Sequence[Range]) -> None:
-        """Fix the unit ranges (forward order, tiling ``[0, numel)``); call before the first quorum."""
+    def set_units(self, units: Sequence[Range], no_decay: Optional[Sequence[Range]] = None) -> None:
+        """Fix the unit ranges (forward order, tiling ``[0, numel)``); call before the first quorum. ``no_decay``
+        replaces the constructor's weight-decay exemptions (flat element ranges); each must lie inside one unit."""
         assert all(lo % 8 == 0 and hi % 8 == 0 for lo, hi in units)
         assert merge_ranges(units) == [(0, self.numel)] and total(units) == self.numel, "units must tile the flat buffer exactly"
         if self.max_grad_norm is not None and len(units) > GNORM_UNITS:
             raise ValueError(f"gradient clipping supports at most {GNORM_UNITS} units, got {len(units)}")
         if self.compact and self.capacity:
             raise RuntimeError("compact state: the units are fixed once the page pools are allocated")
-        self.layout = ShardLayout(tuple((int(a), int(b)) for a, b in units), self._replication)
+        units = tuple((int(a), int(b)) for a, b in units)
+        nd = self.no_decay if no_decay is None else [(int(a), int(b)) for a, b in no_decay]
+        self._nd_units = split_no_decay(units, nd)  # raises before anything changes
+        self.no_decay = nd
+        self.layout = ShardLayout(units, self._replication)
         self._micro_seen = [0] * len(self.layout.units)
         if self.compact:
             self._alloc_pools()
@@ -623,6 +697,9 @@ class Zero1Optimizer:
             if self.grad_accum_steps > 1:
                 self._accum_for(rank, world)
             me = {"t": self.t, "hold": self._holdings}
+            sched = self._schedule_digest()
+            if sched is not None:
+                me["sched"] = sched
             if self._disk is not None:
                 me["disk"] = [self._disk[0], self._disk[1]]  # every rank may read what no live holder has from it
             if self.compact:
@@ -635,6 +712,12 @@ class Zero1Optimizer:
             for r in range(world):
                 if r != rank:
                     peers[r] = json.loads(bytes(store.get(f"z1/{r}")).decode())
+            digests = {r: p.get("sched") for r, p in peers.items()}
+            if len(set(digests.values())) > 1:
+                # holders of one slice would apply different rates or decays to the same bits and drift apart without a
+                # sign; every rank reads the same records and raises alike, before anything is freed or pulled
+                raise RuntimeError(f"zero1: the replicas of this quorum disagree on the learning-rate schedule or the "
+                                   f"weight-decay exemptions (digest per rank: {digests})")
             ckpt = self._ckpt_files(rank, peers)
             plans = plan_quorum(self.layout, world, peers, self._page_shift if self.compact else None, ckpt)
             plan = plans[rank]
@@ -688,6 +771,12 @@ class Zero1Optimizer:
             self._holdings = plan.hold
             self._refresh_pending = world > 1
             self._configured, self._disk = True, None
+
+    def _schedule_digest(self) -> Optional[str]:
+        """What this rank publishes of its schedule and exemptions (``None`` without either: the record stays as it was)."""
+        if self._lr_host is None and not self.no_decay:
+            return None
+        return schedule_digest(self._lr_host, self.no_decay)
 
     def _ckpt_files(self, rank: int, peers: Dict[int, Dict[str, Any]]) -> Dict[int, Any]:
         """The checkpoint files at the quorum's update count that ranks restored from, for :func:`plan_quorum`: this
@@ -865,6 +954,9 @@ class Zero1Optimizer:
         lr = self.param_groups[0]["lr"]
         hp = (lr, self.betas[0], self.betas[1], self.eps, self.weight_decay)
         coef = self._clip.data_ptr() + 4 if self.max_grad_norm is not None else 0
+        # with a schedule the kernel reads the rate of the device's update count from the table; lr is unused
+        sched = {} if self._lr_tab is None else {"lr_table": self._lr_tab.data_ptr(), "lr_steps": self._lr_tab.numel()}
+        nd = self._nd_units if self.no_decay else None
         modes = (1, 0) if self._refresh_pending else (0,)
         self._refresh_pending = False
         snap, self._snap_events = self._snap_events, None
@@ -875,7 +967,7 @@ class Zero1Optimizer:
             for mode in modes:
                 self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, nelem=hi - lo, hyper=hp,
                                         gate=self.gate, replication=k, mode=mode, blocks=self._upd_blocks, stream=stream,
-                                        coef=coef, **state)
+                                        coef=coef, no_decay=nd[i] if nd else (), **sched, **state)
             if events is not None:
                 events[i].record(stream)
 
@@ -1026,6 +1118,15 @@ class Zero1Optimizer:
             rd.close()
 
     # ------------------------------------------------------------------ introspection
+    def lr_at(self, t: int) -> float:
+        """The fp32 learning rate committed update ``t`` (1-based) applies: the table's entry ``min(max(t, 1),
+        lr_steps) - 1`` with a schedule, else ``param_groups[0]["lr"]`` rounded to fp32."""
+        import numpy as np
+
+        if self._lr_host is None:
+            return float(np.float32(self.param_groups[0]["lr"]))
+        return float(self._lr_host[min(max(int(t), 1), len(self._lr_host)) - 1])
+
     def state_bytes_held(self) -> int:
         return 12 * total(self.layout.held(self.comm.rank, max(self.comm.world, 1)))
 
