@@ -12,6 +12,8 @@ from datetime import timedelta
 import pytest
 import torch
 
+import _q8_emulation as E
+
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
 
@@ -73,6 +75,34 @@ def test_allreduce_paths_exact(world, dtype):
         _ok(comms)
         for z in zs:
             assert torch.equal(z.float(), want - xs[0].float())
+    # random normal values: the sum is exact only in the kernels' order, rank 0 first, in fp32, then the scale and one
+    # round-to-nearest-even cast, on every rank and for both plans
+    n = 100_003
+    xs = [torch.randn(n, device=DEV, generator=g).to(dtype) for _ in range(world)]
+    want = _rank_order_sum(xs, 0.5).to(dtype)
+    for plan in ((0, 16), (1, 8)):
+        views = [c.segment("buf")[: n * xs[0].element_size()].view(dtype) for c in comms]
+        for v, x in zip(views, xs):
+            v.copy_(x)
+        ys = [x.clone() for x in xs]
+
+        def both(r, c, s):
+            c._force_plan = plan
+            c.allreduce_(views[r], scale=0.5, stream=s)
+            c.allreduce_(ys[r], scale=0.5, stream=s)
+            c._force_plan = None
+
+        _run(comms, both)
+        _ok(comms)
+        for v, y in zip(views, ys):
+            assert torch.equal(v, want) and torch.equal(y, want), plan
+
+
+def _rank_order_sum(xs, scale):
+    acc = xs[0].float()
+    for x in xs[1:]:
+        acc = acc + x.float()
+    return acc * scale
 
 
 @pytest.mark.parametrize("world", [2, 3, 8])
@@ -131,6 +161,14 @@ def test_reduce_scatter_exact(world):
         mn = torch.stack([x.float() for x in ins]).min(0).values
         for r in range(world):
             assert torch.equal(outs[r].float(), mn[r * n:(r + 1) * n])
+    for n, dtype in ((1001, torch.float32), (65_536, torch.bfloat16), (4104, torch.float16)):
+        ins = [torch.randn(world * n, device=DEV, generator=g).to(dtype) for _ in range(world)]
+        outs = [torch.empty(n, dtype=dtype, device=DEV) for _ in range(world)]
+        _run(comms, lambda r, c, s: c.reduce_scatter_(outs[r], ins[r], scale=0.25, stream=s))
+        _ok(comms)
+        want = _rank_order_sum(ins, 0.25).to(dtype)
+        for r in range(world):
+            assert torch.equal(outs[r], want[r * n:(r + 1) * n]), (n, dtype, r)
 
 
 def test_send_recv_multi_piece_fifo():
@@ -163,7 +201,9 @@ def test_q8_allreduce_and_reduce_scatter_within_reference_tolerance(world):
         _run(comms, lambda r, c, s: c.q8_allreduce_(outs[r], a[r], b[r], scale=1.0 / world, stream=s))
         _ok(comms)
         ref = sum(x.float() - y.float() for x, y in zip(a, b)) / world
+        exact, _ = E.allreduce([E.pseudo_grad(x, y) for x, y in zip(a, b)], 1.0 / world)
         for o in outs:
+            assert E.equal_bits(o, E.cast(exact, dtype)), E.first_mismatch(o, E.cast(exact, dtype))
             assert ((o.float() - ref).abs().mean() / ref.abs().mean()).item() <= 0.04  # collectives_test.py:186
         assert all(torch.equal(outs[0], o) for o in outs)
         se = ((n + world - 1) // world + 7) // 8 * 8
@@ -171,8 +211,10 @@ def test_q8_allreduce_and_reduce_scatter_within_reference_tolerance(world):
         _run(comms, lambda r, c, s: c.q8_reduce_scatter_(rs[r], a[r], se, scale=1.0 / world, stream=s))
         _ok(comms)
         tot = sum(x.float() for x in a) / world
+        exact = E.reduce_scatter([E.load(x) for x in a], se, 1.0 / world)
         for r in range(world):
             valid = max(0, min(se, n - r * se))
+            assert E.equal_bits(rs[r][:valid], E.cast(exact[r], dtype))
             if valid:
                 want = tot[r * se: r * se + valid]
                 assert ((rs[r][:valid].float() - want).abs().mean() / want.abs().mean()).item() <= 0.05  # :207
@@ -195,7 +237,10 @@ def test_q8_allreduce_large_message_pipeline_with_scratch_segment(world):
         assert [c.launches - x for c, x in zip(comms, before)] == [5] * world  # 3 kernels + 2 handshakes, ONE pass
         quiet = None if world == 2 else 1
         ref = sum(x.float() - y.float() for r, (x, y) in enumerate(zip(a, b)) if r != quiet) / world
+        exact, _, _ = E.allreduce_scratch([E.pseudo_grad(x, y) for x, y in zip(a, b)], 1.0 / world,
+                                          [r != quiet for r in range(world)])
         for o in outs:
+            assert E.equal_bits(o, E.cast(exact, dtype)), E.first_mismatch(o, E.cast(exact, dtype))
             assert ((o.float() - ref).abs().mean() / ref.abs().mean()).item() <= 0.04
         assert all(torch.equal(outs[0], o) for o in outs)
 

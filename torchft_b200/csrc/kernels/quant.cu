@@ -113,8 +113,8 @@ __device__ __forceinline__ Vec16 quant16(const float* f, float m) {
   return Vec16{w[0], w[1], w[2], w[3]};
 }
 
-// 16 e4m3 bytes -> 16 floats times dequant scale s.
-__device__ __forceinline__ void dequant16(const Vec16& v, float s, float* f) {
+// 16 e4m3 bytes -> 16 floats (exact: every e4m3 value is a half).
+__device__ __forceinline__ void decode16(const Vec16& v, float* f) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -122,23 +122,46 @@ __device__ __forceinline__ void dequant16(const Vec16& v, float s, float* f) {
     const __half2_raw b = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> 16), __NV_E4M3);
     const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&a));
     const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&b));
-    f[4 * i] = fa.x * s;
-    f[4 * i + 1] = fa.y * s;
-    f[4 * i + 2] = fb.x * s;
-    f[4 * i + 3] = fb.y * s;
+    f[4 * i] = fa.x;
+    f[4 * i + 1] = fa.y;
+    f[4 * i + 2] = fb.x;
+    f[4 * i + 3] = fb.y;
   }
 }
 
+// 16 e4m3 bytes -> 16 floats times dequant scale s.
+__device__ __forceinline__ void dequant16(const Vec16& v, float s, float* f) {
+  decode16(v, f);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) f[i] = __fmul_rn(f[i], s);
+}
+
+// acc += code * s with a separately rounded multiply and add: the sum of a reduction is then fixed bit for bit (no
+// contraction into an FMA left to the compiler), so every rank and the tests' CPU emulation agree on it.
+__device__ __forceinline__ void dequant16_add(const Vec16& v, float s, float* acc) {
+  float f[16];
+  decode16(v, f);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) acc[i] = __fadd_rn(acc[i], __fmul_rn(f[i], s));
+}
+
+// Floor of a group's absmax. With amax >= 2^-116 the dequant scale s = amax/448 >= 2^-124.8 is a normal fp32 (so FTZ
+// cannot zero it; 2^-117 is the smallest power of two that would do) and m = 448/amax <= 2^124.8 is finite (an
+// infinite m turns the group's zeros into 0 * inf = NaN). A power of two keeps s and m exact scalings of fl(1/448) and
+// 448. Groups below the floor get codes below 448; their largest element still dequantises to itself +-1/16.
+constexpr float kAmaxFloor = 0x1p-116f;
+
 // Quantise one group held as 16 floats/lane across a warp; returns dequant scale.
+// A group whose absmax is inf (or an inf next to NaN) gets scale NaN: it dequantises to NaN, like the unquantised sum
+// of an inf would be non-finite, instead of saturating to a finite +-448 * scale. NaN elements of an otherwise finite
+// group are ignored by fmaxf and become NaN codes.
 __device__ __forceinline__ float group_quant(const float* f, Vec16* q) {
   float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < 16; ++i) amax = fmaxf(amax, fabsf(f[i]));
-  amax = warp_max(amax);
-  // inf/nan absmax: keep finite scale semantics of the reference (scale=1)
-  const bool bad = !(amax < INFINITY);
-  const float s = bad ? 1.f : amax * (1.f / kFp8Max);
-  const float m = (amax > 0.f && !bad) ? kFp8Max / amax : (bad ? 1.f : 0.f);
+  amax = fmaxf(warp_max(amax), kAmaxFloor);
+  const float s = amax < INFINITY ? __fmul_rn(amax, 1.f / kFp8Max) : __int_as_float(0x7fc00000);
+  const float m = __fdiv_rn(kFp8Max, amax);  // exact division (fast math would approximate it); 0 for an inf amax
   *q = quant16(f, m);
   return s;
 }
@@ -223,13 +246,10 @@ __global__ void __launch_bounds__(512) q8_reduce_kernel(const char* const* srcs,
     for (int k = 0; k < world; ++k) {
       const int p = (first + k) % world;  // fixed order starting at `first` (ref: quantization.py:405-407)
       const float s = reinterpret_cast<const float*>(srcs[p])[g];
-      float f[16];
-      dequant16(ld_stream(srcs[p] + poff + g * kGroup + lane * 16), s, f);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[i] += f[i];
+      dequant16_add(ld_stream(srcs[p] + poff + g * kGroup + lane * 16), s, acc);
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) acc[i] *= post_scale;
+    for (int i = 0; i < 16; ++i) acc[i] = __fmul_rn(acc[i], post_scale);
     Vec16 q;
     const float s = group_quant(acc, &q);
     if (lane == 0) reinterpret_cast<float*>(dst)[g] = s;
@@ -320,14 +340,9 @@ __global__ void __launch_bounds__(512, 1) q8_allreduce_kernel(Q8Args a) {
       float acc[16];
       dequant16(qv[0], sv[0], acc);
 #pragma unroll
-      for (int p = 1; p < W; ++p) {
-        float f[16];
-        dequant16(qv[p], sv[p], f);
+      for (int p = 1; p < W; ++p) dequant16_add(qv[p], sv[p], acc);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i] += f[i];
-      }
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[i] *= a.post_scale;
+      for (int i = 0; i < 16; ++i) acc[i] = __fmul_rn(acc[i], a.post_scale);
       if (a.mode == 1) {
         const size_t base = (size_t)rank * a.slice_elems;
         const size_t valid = a.nelem > base ? min(a.slice_elems, a.nelem - base) : 0;
@@ -403,15 +418,10 @@ __global__ void __launch_bounds__(512) q8_slice_reduce_kernel(Q8Ptrs q, int worl
     dequant16(qv[0], sv[0], acc);
 #pragma unroll
     for (int k = 1; k < kMaxRanks; ++k) {
-      if (k < world) {
-        float f[16];
-        dequant16(qv[k], sv[k], f);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i] += f[i];
-      }
+      if (k < world) dequant16_add(qv[k], sv[k], acc);
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) acc[i] *= post_scale;
+    for (int i = 0; i < 16; ++i) acc[i] = __fmul_rn(acc[i], post_scale);
     Vec16 out;
     const float sc = group_quant(acc, &out);
     if (lane == 0) reinterpret_cast<float*>(r_out)[l] = sc;
