@@ -32,6 +32,12 @@ table of rates and two weight-decay exemptions, alternating the two ``--repeats`
 limit. The scheduled launch adds one uniform table load per thread and a few integer compares per 8 elements to a kernel
 bound by HBM; it first checks that a constant table and no exemptions give the plain launch's bits.
 
+``--virtual W --moments`` times the update of one unit (rank 0's launch) with fp32 and with bf16 moments, alternating
+the two ``--repeats`` times, on flat state or (with ``--compact``) on page pools in slot order, with the card's name and
+power limit. It reports medians, spread and the bytes the launch moves, computed from the shapes: per updated element
+2 (gradient) + 8 (master in and out) + 2 (weight) + 4 x the moment size, i.e. 28 B with fp32 and 20 B with bf16 moments,
+plus 2 B per primary element and peer the weights are pushed to (local HBM here, NVLink on real ranks).
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -258,6 +264,68 @@ def sched_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats):
     return out
 
 
+def moments_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats, paged, shift=16):
+    """The update of one unit with fp32 and with bf16 moments, timed alternately, on flat state or on page pools."""
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
+    dev = comm.device
+    grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
+    grad.normal_()
+    gate = torch.ones(2, dtype=torch.int32, device=dev)
+    npages = (nelem + (1 << shift) - 1) >> shift
+    n_state = npages << shift if paged else nelem
+    table = torch.arange(npages, dtype=torch.int32, device=dev)
+    paging = dict(table=table.data_ptr(), page_shift=shift) if paged else {}
+
+    def arm(dtype):
+        st = [torch.randn(n_state, device=dev), torch.zeros(n_state, device=dev, dtype=dtype),
+              torch.zeros(n_state, device=dev, dtype=dtype)]
+        return st, lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), st[0].data_ptr(), st[1].data_ptr(),
+                                              st[2].data_ptr(), nelem, HP, gate, k, 0, upd_blocks, moment_dtype=dtype,
+                                              **paging)
+
+    arms = {"fp32": arm(torch.float32), "bf16": arm(torch.bfloat16)}
+    for st, _ in arms.values():
+        st[0].copy_(arms["fp32"][0][0])
+    for _, fn in arms.values():
+        fn()
+    torch.cuda.synchronize()
+    # from zero moments both launches compute the weights from the same fp32 moments
+    same_weights = torch.equal(arms["fp32"][0][0], arms["bf16"][0][0])
+    times = {name: [] for name in arms}
+    for _ in range(repeats):
+        for name, (_, fn) in arms.items():
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    assert comm.errored() is None
+    W, kk = comm.world, min(k, comm.world)
+    nvec = nelem // 8
+    per = (nvec + W - 1) // W
+    primary = 8 * min(per, nvec)  # rank 0's primary slice; it also updates the kk - 1 slices it backs up
+    updated = sum(8 * (min((s + 1) * per, nvec) - min(s * per, nvec)) for s in {(0 - j) % W for j in range(kk)})
+    out = {"timing": "local HBM (virtual ranks), not NVLink", "state": "paged_ordered" if paged else "flat",
+           "first_update_weights_equal": same_weights, "elements_updated": updated,
+           "pushed_bytes": 2 * primary * (W - kk)}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        per_elem = 2 + 8 + 2 + 4 * (2 if name == "bf16" else 4)
+        moved = per_elem * updated + out["pushed_bytes"]
+        out[f"adamw_allgather_{name}_moments"] = {
+            "ms": {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4), "max": round(ts[-1], 4)},
+            "state_bytes_per_element": per_elem, "bytes_moved": moved,
+            "gb_per_s_at_median": round(moved / ts[len(ts) // 2] / 1e6, 1)}
+    out["bf16_over_fp32"] = round(out["adamw_allgather_bf16_moments"]["ms"]["median"]
+                                  / out["adamw_allgather_fp32_moments"]["ms"]["median"], 4)
+    return out
+
+
 def accum_ab(comms, nelem, k, rs_blocks, iters, warmup, repeats):
     """Rank 0's reduce-scatter of one unit in the three accumulation modes, timed alternately: ``off`` (today's launch),
     ``acc`` (a middle micro-batch: fp32 rank sum added into the accumulator) and ``last`` (accumulator + rank sum,
@@ -337,7 +405,10 @@ def main() -> None:
     ap.add_argument("--accum", action="store_true", help="--virtual: A/B rank 0's reduce in accumulation modes off / acc / last")
     ap.add_argument("--sched", action="store_true", help="--virtual: A/B the update without and with a learning-rate "
                     "table and weight-decay exemptions")
-    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum / --sched: alternations of the arms")
+    ap.add_argument("--moments", action="store_true", help="--virtual: A/B the update with fp32 and bf16 moments "
+                    "(with --compact: on paged state)")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum / --sched / --moments: alternations "
+                    "of the arms")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -348,8 +419,10 @@ def main() -> None:
         segments = {"z1_grad": S, "z1_param": S, **({"z1_gnorm": 8} if a.clip else {})}
         comms = SymmetricComm.virtual_world(a.virtual, segments, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
-        if a.compact or a.clip or a.accum or a.sched:
-            if a.compact:
+        if a.compact or a.clip or a.accum or a.sched or a.moments:
+            if a.moments:
+                res.update(moments_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats, a.compact))
+            elif a.compact:
                 res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))
             elif a.sched:
                 res.update(sched_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))

@@ -11,7 +11,7 @@ It tries ``--seq`` first without and then with activation checkpointing, and hal
 fits; every attempt runs in a fresh process and records the device's free memory before it starts (``cudaMemGetInfo``
 sees the whole device, so memory other processes hold counts against the attempt). Step times come from the aliased peers' buffers in local HBM, not from NVLink, and are not multi-GPU step times.
 
-    python bench/zero1_fit.py --model llama3_8b --world 8 --min-world 7 --replication 2 --seq 8192
+    python bench/zero1_fit.py --model llama3_8b --world 8 --min-world 7 --replication 2 --seq 8192 [--moments bf16]
 """
 
 from __future__ import annotations
@@ -95,7 +95,8 @@ def _run(args, cfg, seq, ckpt, dev, base, comms):
     pg = _AliasedGroup(comms)
     model = Llama(cfg, device="meta")
     numel = sum((p.numel() + FlatParams.ALIGN - 1) // FlatParams.ALIGN * FlatParams.ALIGN for p in model.parameters())
-    opt = Zero1Optimizer(pg, numel, replication=args.replication, compact=True, min_world=args.min_world)
+    opt = Zero1Optimizer(pg, numel, replication=args.replication, compact=True, min_world=args.min_world,
+                         moment_dtype={"fp32": torch.float32, "bf16": torch.bfloat16}[args.moments])
     flat = FlatParams(model, grad_alloc=lambda n: opt.grad, device=dev, param_alloc=lambda n: opt.param)
     model.init_weights(0)
     units = FaultTolerantTrainer._compute_stage_ranges(SimpleNamespace(flat=flat, model=model))
@@ -134,7 +135,7 @@ def _run(args, cfg, seq, ckpt, dev, base, comms):
     assert opt.t == args.steps and opt.lost_elements == 0
     res = {
         "model": args.model, "world": args.world, "min_world": args.min_world, "replication": opt.layout.replication,
-        "seq": seq, "batch": args.batch, "activation_checkpoint": ckpt,
+        "seq": seq, "batch": args.batch, "activation_checkpoint": ckpt, "moments": args.moments,
         "pool_pages": opt.capacity, "state_gib_allocated": round(opt.state_bytes_allocated() / 2**30, 2),
         "state_gib_held": round(opt.state_bytes_held() / 2**30, 2),
         "device_used_before_gib": round(base / 2**30, 2),
@@ -153,6 +154,7 @@ def main() -> None:
     ap.add_argument("--world", type=int, default=8)
     ap.add_argument("--min-world", type=int, default=7)
     ap.add_argument("--replication", type=int, default=2)
+    ap.add_argument("--moments", default="fp32", choices=["fp32", "bf16"], help="type of the AdamW moments m and v")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--batch", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)

@@ -119,6 +119,29 @@ def collectives_selfcheck(world: int = 4, nelem: int = 1 << 18, device: Optional
     errs["zero1_replicas_differ"] = float(sum(int(not torch.equal(pr[0], pr[r])) for r in range(1, world)))
     errs["zero1_reduced"] = max(float((gr[r][lo:hi].float() - red[lo:hi]).abs().max())
                                 for r in range(world) for lo, hi in L.held(r, world))
+    # the same update with bf16 moments: from zero moments the weights are the fp32-moment launch's, and the stored
+    # moments are the stochastic rounding of single fp32 products, which the numpy specification reproduces bit for bit
+    import numpy as np
+
+    from torchft_b200.parallel.zero1 import bf16_sr
+
+    w_fp32 = pr[0].clone()
+    master = [init.float() for _ in comms]
+    mb = [torch.zeros(nelem, device=dev, dtype=torch.bfloat16) for _ in comms]
+    vb = [torch.zeros(nelem, device=dev, dtype=torch.bfloat16) for _ in comms]
+    for r, c in enumerate(comms):
+        c.zero1_update_("z1_param", 0, gr[r].data_ptr(), master[r].data_ptr(), mb[r].data_ptr(), vb[r].data_ptr(), nelem,
+                        hp, gates[r], 2, 0, 8, moment_dtype=torch.bfloat16)
+    torch.cuda.synchronize()
+    errs["zero1_bf16_moments_weights_differ"] = float(sum(int(not torch.equal(w_fp32, pr[r])) for r in range(world)))
+    g32 = red.cpu().numpy()
+    c1, c2 = np.float32(1) - np.float32(hp[1]), np.float32(1) - np.float32(hp[2])
+    e = np.arange(nelem, dtype=np.uint64)
+    want_m, want_v = bf16_sr(c1 * g32, e, 1, 0), bf16_sr((c2 * g32) * g32, e, 1, 1)
+    bits = lambda x: x.view(torch.int16).cpu().numpy().view(np.uint16)  # noqa: E731
+    errs["zero1_bf16_moment_bits_differ"] = float(sum(
+        int((bits(x[r][lo:hi]) != want[lo:hi]).sum()) for r in range(world) for lo, hi in L.held(r, world)
+        for x, want in ((mb, want_m), (vb, want_v))))
     # heal copy (NVLink pull kernel; here between two local buffers)
     from torchft_b200.checkpointing.p2p_transport import device_copy
 
@@ -131,5 +154,6 @@ def collectives_selfcheck(world: int = 4, nelem: int = 1 << 18, device: Optional
     assert errs["allreduce_twoshot"] < 0.05 and errs["allreduce_oneshot"] < 0.05, errs
     assert errs["q8_allreduce_finite"] == 1.0 and errs["heal_copy"] == 0.0, errs
     assert errs["zero1_reduced"] == 0.0 and errs["zero1_replicas_differ"] == 0 and errs["zero1_weights"] < 2e-2, errs
+    assert errs["zero1_bf16_moments_weights_differ"] == 0 and errs["zero1_bf16_moment_bits_differ"] == 0, errs
     assert _native.kernel_launches() > 0
     return errs

@@ -9,7 +9,8 @@ File ``z1_step_{T}.w{W}.r{r}.bin``::
     b"TFTZ1CKP" | u64 header bytes (little endian) | JSON header | zero pad to 16 bytes | payload
 
 The payload holds four arrays over the ``elements`` written elements, back to back: ``param`` (bf16), ``master``,
-``m`` and ``v`` (fp32), at the byte offsets ``sections`` gives relative to the payload start. Each written range
+``m`` and ``v`` (fp32; bf16 when the header says ``"moments": "bf16"``, a file without the key has fp32 moments), at the
+byte offsets ``sections`` gives relative to the payload start. Each written range
 ``[lo, hi)`` of the flat vector is stored at element offset ``off`` of every array (``ranges``: ``[lo, hi, off]``).
 Ranges are multiples of 8 elements, so every array and every range in it starts 16-byte aligned. The payload is read
 with ranged ``pread`` calls only, never loaded whole.
@@ -31,7 +32,7 @@ from torchft_b200.checkpointing.durable import BackgroundWriter, atomic_write, p
 
 logger = logging.getLogger(__name__)
 
-__all__ = ["FORMAT_VERSION", "file_name", "sections", "encode_header", "read_header", "scan", "check_compatible",
+__all__ = ["FORMAT_VERSION", "file_name", "sections", "moment_size", "file_dtype", "payload_bytes", "encode_header", "read_header", "scan", "check_compatible",
            "ShardedWriter", "RangedReader"]
 
 FORMAT_VERSION = 1
@@ -44,13 +45,33 @@ def file_name(step: int, world: int, rank: int) -> str:
     return f"z1_step_{step}.w{world}.r{rank}.bin"
 
 
-def sections(elements: int) -> Dict[str, int]:
-    """Byte offset of each array in the payload of a file holding ``elements`` elements (14 bytes each)."""
+def sections(elements: int, moment_size: int = 4) -> Dict[str, int]:
+    """Byte offset of each array in the payload of a file holding ``elements`` elements: 14 bytes each with fp32
+    moments, 10 with bf16 moments (``moment_size`` 2)."""
     out, at = {}, 0
     for name, size in _ITEM.items():
         out[name] = at
-        at += size * elements
+        at += (moment_size if name in ("m", "v") else size) * elements
     return out
+
+
+def moment_size(header: Dict[str, Any]) -> int:
+    """Bytes per element of ``m`` and ``v`` in the file ``header`` describes; raises ``ValueError`` for an unknown type."""
+    kind = header.get("moments", "fp32")
+    if kind not in ("fp32", "bf16"):
+        raise ValueError(f"unknown moment type {kind!r}")
+    return 2 if kind == "bf16" else 4
+
+
+def file_dtype(header: Dict[str, Any], array: str) -> torch.dtype:
+    """The dtype ``array`` is stored in."""
+    if array in ("m", "v"):
+        return torch.bfloat16 if moment_size(header) == 2 else torch.float32
+    return torch.bfloat16 if array == "param" else torch.float32
+
+
+def payload_bytes(header: Dict[str, Any]) -> int:
+    return (6 + 2 * moment_size(header)) * int(header["elements"])
 
 
 def encode_header(header: Dict[str, Any]) -> bytes:
@@ -79,7 +100,7 @@ def read_header(path: str) -> Optional[Dict[str, Any]]:
             elements = int(h["elements"])
             if sum(hi - lo for lo, hi, _ in h["ranges"]) != elements:
                 raise ValueError("ranges do not add up to the element count")
-            need = data + 14 * elements
+            need = data + payload_bytes(h)
             size = os.fstat(f.fileno()).st_size
             if size < need:
                 raise ValueError(f"truncated: {size} bytes, the header describes {need}")
@@ -139,7 +160,7 @@ class ShardedWriter:
         return self.stage
 
     def submit(self, header: Dict[str, Any], copied: Any) -> str:
-        """Write ``header`` and ``14 * elements`` bytes of staging once the event ``copied`` has fired."""
+        """Write ``header`` and the payload it describes from staging once the event ``copied`` has fired."""
         path = os.path.join(self.directory, file_name(int(header["T"]), int(header["world"]), int(header["rank"])))
         self._writer.start(self._write, path, header, copied)
         return path
@@ -148,7 +169,7 @@ class ShardedWriter:
         t0 = time.perf_counter()
         copied.synchronize()
         assert self.stage is not None
-        payload = memoryview(self.stage.numpy())[: 14 * int(header["elements"])]
+        payload = memoryview(self.stage.numpy())[: payload_bytes(header)]
         chunk = 256 << 20
 
         def write(f: Any) -> None:
@@ -191,8 +212,8 @@ class RangedReader:
         fd = self._fds.get(path)
         if fd is None:
             fd = self._fds[path] = os.open(path, os.O_RDONLY)
-        size = _ITEM[array]
-        assert dst.element_size() == size, (array, dst.dtype)
+        assert dst.dtype == file_dtype(header, array), (array, dst.dtype)
+        size = dst.element_size()
         pos = int(header["data"]) + int(header["sections"][array]) + elem_off * size
         out = dst.view(torch.uint8)
         n = out.numel()

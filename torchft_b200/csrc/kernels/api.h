@@ -40,6 +40,9 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
 // i + 1, and the update reads lr_tab[clamp(gate[1], 1, lr_steps) - 1] for both the step and the decoupled decay.
 // Weight-decay exemptions: `no_decay` holds n_no_decay <= kMaxNoDecay unit-relative element ranges as (lo, hi) pairs,
 // multiples of 8, whose elements get no decay.
+// Moment type (moment_dtype: a DType code, 0 = fp32 by default or 1 = bf16): with bf16 `m` and `v` are bf16 arrays, 16 B aligned, and the
+// update stores them with stochastic rounding whose bits depend only on (soff + local element index, gate[1], which
+// moment); flat launches then pass the unit's first global element as `soff`. `master` stays fp32.
 constexpr int kMaxNoDecay = 4;
 void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
                             int barrier_mode, cudaStream_t stream);
@@ -50,11 +53,11 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
                          int host_ok, int exchange, cudaStream_t stream, const double* const* gn = nullptr,
                          int nunits = 0, float max_norm = 0.f, float* norm = nullptr);
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
-                         float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
+                         void* m, void* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream,
                          const int* table = nullptr, size_t soff = 0, int page_shift = 0, const float* coef = nullptr,
                          const float* lr_tab = nullptr, int lr_steps = 0, int n_no_decay = 0,
-                         const size_t* no_decay = nullptr);
+                         const size_t* no_decay = nullptr, int moment_dtype = 0);
 
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);

@@ -166,6 +166,7 @@ PYBIND11_MODULE(_K, m) {
   m.attr("SIGNAL_PAD_BYTES") = sizeof(SignalPad);
   m.attr("Q8_GROUP") = 512;
   m.attr("ZERO1_MAX_NO_DECAY") = kMaxNoDecay;
+  m.attr("ZERO1_BF16_MOMENTS") = true;  // zero1_update takes moment_dtype = bf16
 
   py::class_<Status>(m, "Status")
       .def(py::init<>())
@@ -266,18 +267,18 @@ PYBIND11_MODULE(_K, m) {
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,
          uintptr_t v, size_t nelem, float lr, float b1, float b2, float eps, float wd, int replication, int mode,
          int blocks, int threads, uintptr_t stream, uintptr_t table, size_t soff, int page_shift, uintptr_t coef,
-         uintptr_t lr_tab, int lr_steps, const std::vector<size_t>& no_decay) {
+         uintptr_t lr_tab, int lr_steps, const std::vector<size_t>& no_decay, int moment_dtype) {
         if (no_decay.size() & 1) throw std::runtime_error("zero1_update: no_decay is a flat list of (lo, hi) pairs");
-        zero1_update_launch(pt.pt, P<void>(mc_base), P<const int>(gate), poff, P<void>(grad), P<float>(master), P<float>(mm),
-                            P<float>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream),
+        zero1_update_launch(pt.pt, P<void>(mc_base), P<const int>(gate), poff, P<void>(grad), P<float>(master), P<void>(mm),
+                            P<void>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream),
                             P<const int>(table), soff, page_shift, P<const float>(coef), P<const float>(lr_tab), lr_steps,
-                            (int)(no_decay.size() / 2), no_decay.empty() ? nullptr : no_decay.data());
+                            (int)(no_decay.size() / 2), no_decay.empty() ? nullptr : no_decay.data(), moment_dtype);
       },
       py::arg("pt"), py::arg("mc_base"), py::arg("gate"), py::arg("poff"), py::arg("grad"), py::arg("master"),
       py::arg("m"), py::arg("v"), py::arg("nelem"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"),
       py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("blocks"), py::arg("threads"), py::arg("stream"),
       py::arg("table") = 0, py::arg("soff") = 0, py::arg("page_shift") = 0, py::arg("coef") = 0, py::arg("lr_tab") = 0,
-      py::arg("lr_steps") = 0, py::arg("no_decay") = std::vector<size_t>{});
+      py::arg("lr_steps") = 0, py::arg("no_decay") = std::vector<size_t>{}, py::arg("moment_dtype") = 0);
 
   m.def(
       "push_exchange",

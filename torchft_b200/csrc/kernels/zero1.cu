@@ -38,6 +38,11 @@
 // update kernel reads the rate of the committed update count gate[1] from a device table, and vectors inside up to
 // kMaxNoDecay unit-relative ranges take no decay.
 //
+// bf16 moments (opt-in, MT template type of the update kernel): m and v are stored as bf16, 8 B of state per parameter
+// instead of 12. The arithmetic stays fp32; the moments are rounded stochastically on the way out (bf16_sr) with bits
+// that are a pure function of (global element index, gate[1], which moment), so every holder of a slice stores the
+// same bits at any grid size, world and paging.
+//
 // The two big kernels contain NO inter-rank synchronisation at all: any grid size, no co-residency requirement, no
 // SM held by a spinning CTA while peers are skewed, profilable stand-alone. Ordering comes from the one-CTA handshake
 // kernels around them (bounded, abortable spins; epoch-tagged flags; error latched in the status block and mirrored
@@ -398,6 +403,31 @@ __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
 }
 
 // ---------------------------------------------------------------------------
+// Stochastic rounding of the bf16 moments. parallel/zero1.py (sr_bits, bf16_sr) is the specification; the two must
+// return the same bits.
+// ---------------------------------------------------------------------------
+// The 32 random bits of element e at update t: murmur3's 32-bit finaliser over a linear mix of the index halves, the
+// update count and a fixed seed. The low half rounds m, the high half rounds v.
+__device__ __forceinline__ uint32_t sr_bits(uint64_t e, uint32_t t) {
+  uint32_t x = (uint32_t)e * 0x9E3779B1u + (uint32_t)(e >> 32) * 0x85EBCA77u + t * 0xC2B2AE3Du + 0x27D4EB2Fu;
+  x ^= x >> 16;
+  x *= 0x85EBCA6Bu;
+  x ^= x >> 13;
+  x *= 0xC2B2AE35u;
+  x ^= x >> 16;
+  return x;
+}
+
+// fp32 -> bf16 bits: add the 16-bit r to the fp32 bits and keep the upper half. The add is on the magnitude, so it
+// rounds away from zero with probability (discarded fraction), which is unbiased for both signs; a value bf16
+// represents exactly comes back unchanged for every r. Inf and NaN are not added to; a NaN keeps a mantissa bit.
+__device__ __forceinline__ uint32_t bf16_sr(float x, uint32_t r) {
+  const uint32_t u = __float_as_uint(x);
+  if ((u & 0x7f800000u) == 0x7f800000u) return (u >> 16) | ((u & 0x007fffffu) ? 0x0040u : 0u);
+  return (u + r) >> 16;
+}
+
+// ---------------------------------------------------------------------------
 // Gated AdamW on the held slices + all-gather of the new bf16 weights (no synchronisation).
 // ---------------------------------------------------------------------------
 struct UpdArgs {
@@ -407,15 +437,16 @@ struct UpdArgs {
   size_t poff;         // byte offset of the unit inside the parameter segment
   const bf16* grad;    // local reduced gradients of the unit
   float* master;       // local fp32 state of the unit (full-size arrays; only held slices are valid)
-  float* m;
-  float* v;
+  void* m;             // moments: fp32 or bf16 arrays (the kernel's MT), indexed like master
+  void* v;
   size_t nelem;
   float lr, b1, b2, eps, wd;
   int replication;
   int mode;            // 0 = gated update + push, 1 = refresh (re-broadcast bf16(master) of the primary slice, ungated)
   // paged state (PAGED = true): master/m/v are page pools; element e of the flat vector (e = soff + local index)
   // lives at pool[table[e >> page_shift] << page_shift | (e & (page - 1))]. A page is a multiple of 8 elements, so
-  // the two 16-byte vectors of one 8-element group never straddle a page.
+  // the two 16-byte vectors of one 8-element group never straddle a page. bf16 moments hash soff + local index, so
+  // flat launches pass the unit's first element there too.
   const int* table;
   size_t soff;
   int page_shift;
@@ -429,8 +460,11 @@ struct UpdArgs {
   size_t nd_lo[kMaxNoDecay], nd_hi[kMaxNoDecay];
 };
 
-template <int W, bool NVLS, bool PAGED, bool CLIP>
+template <int W, bool NVLS, bool PAGED, bool CLIP, typename MT>
 __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
+  constexpr bool BF16M = sizeof(MT) == 2;
+  MT* const mp = reinterpret_cast<MT*>(a.m);
+  MT* const vp = reinterpret_cast<MT*>(a.v);
   if (a.mode == 0 && a.gate[0] == 0) return;  // uniform over the grid AND (unanimous verdict) over the quorum
   const int rank = a.pt.rank;
   const Geo g(a.nelem, W);
@@ -477,10 +511,18 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
       float w[8];
       const Vec16 w0 = ld_stream(a.master + si), w1 = ld_stream(a.master + si + 4);
       if (a.mode == 0) {
-        // all 7 x 16 B loads in flight before any use
+        // all 7 x 16 B loads (5 with bf16 moments) in flight before any use
         const Vec16 gv = ld_stream(a.grad + v * 8);
-        const Vec16 m0 = ld_stream(a.m + si), m1 = ld_stream(a.m + si + 4);
-        const Vec16 v0 = ld_stream(a.v + si), v1 = ld_stream(a.v + si + 4);
+        Vec16 m0, m1, v0, v1;
+        if constexpr (BF16M) {
+          m0 = ld_stream(mp + si);
+          v0 = ld_stream(vp + si);
+        } else {
+          m0 = ld_stream(mp + si);
+          m1 = ld_stream(mp + si + 4);
+          v0 = ld_stream(vp + si);
+          v1 = ld_stream(vp + si + 4);
+        }
         float gr[8], m[8], vv[8];
         P8::unpack(gv, gr);
         if constexpr (CLIP) {
@@ -489,10 +531,15 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
         }
         Pack<float>::unpack(w0, w);
         Pack<float>::unpack(w1, w + 4);
-        Pack<float>::unpack(m0, m);
-        Pack<float>::unpack(m1, m + 4);
-        Pack<float>::unpack(v0, vv);
-        Pack<float>::unpack(v1, vv + 4);
+        if constexpr (BF16M) {
+          P8::unpack(m0, m);
+          P8::unpack(v0, vv);
+        } else {
+          Pack<float>::unpack(m0, m);
+          Pack<float>::unpack(m1, m + 4);
+          Pack<float>::unpack(v0, vv);
+          Pack<float>::unpack(v1, vv + 4);
+        }
         float dcy = decay;
         if (a.n_nd > 0) {  // uniform: without exemptions no vector pays for the compares
 #pragma unroll
@@ -508,10 +555,24 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
         }
         st_stream(a.master + si, Pack<float>::pack(w));
         st_stream(a.master + si + 4, Pack<float>::pack(w + 4));
-        st_stream(a.m + si, Pack<float>::pack(m));
-        st_stream(a.m + si + 4, Pack<float>::pack(m + 4));
-        st_stream(a.v + si, Pack<float>::pack(vv));
-        st_stream(a.v + si + 4, Pack<float>::pack(vv + 4));
+        if constexpr (BF16M) {
+          // the weights above used the fp32 moments; what is stored is their stochastic rounding
+          const uint64_t e0 = a.soff + v * 8;
+          uint32_t mo[4], vo[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const uint32_t r0 = sr_bits(e0 + 2 * i, (uint32_t)t), r1 = sr_bits(e0 + 2 * i + 1, (uint32_t)t);
+            mo[i] = bf16_sr(m[2 * i], r0 & 0xffffu) | (bf16_sr(m[2 * i + 1], r1 & 0xffffu) << 16);
+            vo[i] = bf16_sr(vv[2 * i], r0 >> 16) | (bf16_sr(vv[2 * i + 1], r1 >> 16) << 16);
+          }
+          st_stream(mp + si, Vec16{mo[0], mo[1], mo[2], mo[3]});
+          st_stream(vp + si, Vec16{vo[0], vo[1], vo[2], vo[3]});
+        } else {
+          st_stream(mp + si, Pack<float>::pack(m));
+          st_stream(mp + si + 4, Pack<float>::pack(m + 4));
+          st_stream(vp + si, Pack<float>::pack(vv));
+          st_stream(vp + si + 4, Pack<float>::pack(vv + 4));
+        }
       } else {
         Pack<float>::unpack(w0, w);
         Pack<float>::unpack(w1, w + 4);
@@ -560,27 +621,35 @@ void launch_rs_path(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
     launch_rs<false, CLIP, ACC>(a, blocks, threads, s);
 }
 
-template <bool NVLS, bool PAGED, bool CLIP>
+template <bool NVLS, bool PAGED, bool CLIP, typename MT>
 void launch_upd_w(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
   switch (a.pt.world) {
-    case 1: zero1_update_kernel<1, false, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 2: zero1_update_kernel<2, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_update_kernel<3, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_update_kernel<4, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_update_kernel<5, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_update_kernel<6, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_update_kernel<7, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_update_kernel<8, NVLS, PAGED, CLIP><<<blocks, threads, 0, s>>>(a); break;
+    case 1: zero1_update_kernel<1, false, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 2: zero1_update_kernel<2, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 3: zero1_update_kernel<3, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 4: zero1_update_kernel<4, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 5: zero1_update_kernel<5, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 6: zero1_update_kernel<6, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 7: zero1_update_kernel<7, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
+    case 8: zero1_update_kernel<8, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
     default: throw std::runtime_error("zero1_update: world size must be in [1, 8]");
   }
 }
 
-template <bool NVLS, bool PAGED>
-void launch_upd(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
+template <bool NVLS, bool PAGED, typename MT>
+void launch_upd_clip(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
   if (a.coef != nullptr)
-    launch_upd_w<NVLS, PAGED, true>(a, blocks, threads, s);
+    launch_upd_w<NVLS, PAGED, true, MT>(a, blocks, threads, s);
   else
-    launch_upd_w<NVLS, PAGED, false>(a, blocks, threads, s);
+    launch_upd_w<NVLS, PAGED, false, MT>(a, blocks, threads, s);
+}
+
+template <bool NVLS, bool PAGED>
+void launch_upd(const UpdArgs& a, bool bf16_moments, int blocks, int threads, cudaStream_t s) {
+  if (bf16_moments)
+    launch_upd_clip<NVLS, PAGED, bf16>(a, blocks, threads, s);
+  else
+    launch_upd_clip<NVLS, PAGED, float>(a, blocks, threads, s);
 }
 
 void check_grid(int blocks, int threads, const char* who) {
@@ -647,11 +716,15 @@ void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64
 }
 
 void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
-                         float* m, float* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
+                         void* m, void* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
                          int replication, int mode, int blocks, int threads, cudaStream_t stream, const int* table,
                          size_t soff, int page_shift, const float* coef, const float* lr_tab, int lr_steps,
-                         int n_no_decay, const size_t* no_decay) {
+                         int n_no_decay, const size_t* no_decay, int moment_dtype) {
   check_grid(blocks, threads, "zero1_update");
+  if (moment_dtype != kF32 && moment_dtype != kBF16) throw std::runtime_error("zero1_update: moments are fp32 or bf16");
+  const bool bf16m = moment_dtype == kBF16;
+  if (((reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15) || (bf16m && (soff & 7)))
+    throw std::runtime_error("zero1_update: m and v must be 16 B aligned (bf16 moments: and the unit's first element a multiple of 8)");
   if ((poff & 15) || (nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
   if (table != nullptr && (page_shift < 3 || page_shift > 30 || (soff & 7)))
     throw std::runtime_error("zero1_update: pages must be 2^3 .. 2^30 elements and the unit 8-element aligned");
@@ -671,13 +744,13 @@ void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, si
   }
   if (table != nullptr) {
     if (mc_base != nullptr)
-      launch_upd<true, true>(a, blocks, threads, stream);
+      launch_upd<true, true>(a, bf16m, blocks, threads, stream);
     else
-      launch_upd<false, true>(a, blocks, threads, stream);
+      launch_upd<false, true>(a, bf16m, blocks, threads, stream);
   } else if (mc_base != nullptr) {
-    launch_upd<true, false>(a, blocks, threads, stream);
+    launch_upd<true, false>(a, bf16m, blocks, threads, stream);
   } else {
-    launch_upd<false, false>(a, blocks, threads, stream);
+    launch_upd<false, false>(a, bf16m, blocks, threads, stream);
   }
   TFT_CUDA_CHECK(cudaGetLastError());
 }

@@ -901,7 +901,7 @@ class SymmetricComm:
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,
                       blocks: int, stream: Optional[torch.cuda.Stream] = None, table: int = 0, state_off: int = 0,
                       page_shift: int = 0, coef: int = 0, lr_table: int = 0, lr_steps: int = 0,
-                      no_decay: Sequence[Tuple[int, int]] = ()) -> None:
+                      no_decay: Sequence[Tuple[int, int]] = (), moment_dtype: torch.dtype = torch.float32) -> None:
         """Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights into
         ``segment`` on the ranks that do not hold it (``mode`` 1: ungated re-broadcast of bf16(master) to everybody, no
         state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed.
@@ -911,7 +911,12 @@ class SymmetricComm:
         ``coef`` (device address of an fp32, 0 = none): the gradient is multiplied by it (the clip coefficient).
         ``lr_table`` (device address of ``lr_steps`` fp32 rates, 0 = the constant ``hyper`` rate): update ``t`` (the
         device step count) uses entry ``min(max(t, 1), lr_steps) - 1`` for the step and the decay. ``no_decay``: at most
-        ``ZERO1_MAX_NO_DECAY`` unit-relative element ranges, multiples of 8, whose elements get no weight decay."""
+        ``ZERO1_MAX_NO_DECAY`` unit-relative element ranges, multiples of 8, whose elements get no weight decay.
+        ``moment_dtype`` ``torch.bfloat16``: ``m`` and ``v`` point at bf16 arrays, stored with stochastic rounding whose
+        bits depend only on the global element index ``state_off + i``, the device step count and the moment; flat
+        state then passes the unit's first element as ``state_off`` too."""
+        if moment_dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"the moments are fp32 or bf16, got {moment_dtype}")
         if lr_table and lr_steps < 1:
             raise ValueError(f"a learning-rate table needs lr_steps >= 1, got {lr_steps}")
         nd = [(int(lo), int(hi)) for lo, hi in no_decay]
@@ -930,7 +935,7 @@ class SymmetricComm:
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp,
                                  table, state_off, page_shift, coef, lr_table, lr_steps if lr_table else 0,
-                                 [x for r in nd for x in r])
+                                 [x for r in nd for x in r], _native.DTYPE_CODE[moment_dtype])
             self.launches += 1
             pushes = self._world > 1 and (mode == 1 or self._world > replication)
             if pushes:

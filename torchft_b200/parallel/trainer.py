@@ -81,6 +81,9 @@ class FaultTolerantTrainer:
         lr_steps: FT-ZeRO-1: length of that table (required with ``lr_lambda``); later updates keep its last rate
         no_decay: FT-ZeRO-1: ``(name, parameter) -> bool`` selecting the parameters that get no weight decay, e.g.
             ``lambda name, p: p.ndim == 1`` for the norm gains. Not available on the classic all-reduce pipeline.
+        moment_dtype: FT-ZeRO-1: ``torch.bfloat16`` keeps the AdamW moments in bf16 (8 instead of 12 bytes of optimizer
+            state per parameter), rounded stochastically so that the holders of a slice stay bit-identical; ``None``:
+            env ``TORCHFT_B200_Z1_MOMENTS=bf16``, unset = fp32. Not available on the classic all-reduce pipeline.
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -96,7 +99,8 @@ class FaultTolerantTrainer:
                  compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None,
                  grad_accum_steps: int = 1, lr_lambda: Optional[Callable[[int], float]] = None,
                  lr_steps: Optional[int] = None,
-                 no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None) -> None:
+                 no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None,
+                 moment_dtype: Optional[torch.dtype] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -118,6 +122,8 @@ class FaultTolerantTrainer:
         self.grad_accum_steps = int(grad_accum_steps)
         if (lr_lambda is not None or no_decay is not None) and not self.zero1:
             raise ValueError("lr_lambda and no_decay need the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if moment_dtype is not None and not self.zero1:
+            raise ValueError("moment_dtype needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         if lr_lambda is not None and lr_steps is None:
             raise ValueError("lr_lambda needs lr_steps, the length of the schedule")
         self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
@@ -149,7 +155,7 @@ class FaultTolerantTrainer:
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
                                        compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
                                        grad_accum_steps=self.grad_accum_steps, lr_lambda=lr_lambda,
-                                       lr_steps=lr_steps or 0)
+                                       lr_steps=lr_steps or 0, moment_dtype=moment_dtype)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:

@@ -44,11 +44,13 @@ Range = Tuple[int, int]
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
            "plan_reshard", "reshard_pages", "reshard_page_steps", "RankPlan", "plan_quorum", "backed_ranges", "pool_pages", "page_ranges",
            "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan",
-           "lr_schedule_table", "split_no_decay", "schedule_digest"]
+           "lr_schedule_table", "split_no_decay", "schedule_digest", "check_moment_agreement", "moment_type", "sr_bits", "bf16_sr"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
+CONVERT_CHUNK = 1 << 24  # restore into the other moment type: elements converted per device temporary
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
 MAX_NO_DECAY = 4  # weight-decay exemptions per unit and update launch (kMaxNoDecay of csrc/kernels/api.h)
+SR_SEED = 0x27D4EB2F  # bf16 moments: the fixed seed of the rounding bits (sr_bits of csrc/kernels/zero1.cu)
 
 
 def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
@@ -111,6 +113,63 @@ def schedule_digest(table: Any, no_decay: Sequence[Range]) -> str:
     h = hashlib.sha256(b"none" if table is None else table.tobytes())
     h.update(json.dumps(merge_ranges(no_decay)).encode())
     return h.hexdigest()
+
+
+# --------------------------------------------------------------------------- bf16 moments
+def moment_type(moment_dtype: Optional[torch.dtype]) -> torch.dtype:
+    """The dtype :class:`Zero1Optimizer` keeps ``m`` and ``v`` in: ``moment_dtype``, or env ``TORCHFT_B200_Z1_MOMENTS``
+    (``fp32`` or ``bf16``; unset or empty: fp32) when it is ``None``. Anything else raises ``ValueError``."""
+    if moment_dtype is None:
+        env = os.environ.get("TORCHFT_B200_Z1_MOMENTS", "").strip().lower()
+        moment_dtype = {"": torch.float32, "fp32": torch.float32, "bf16": torch.bfloat16}.get(env)
+        if moment_dtype is None:
+            raise ValueError(f"TORCHFT_B200_Z1_MOMENTS must be fp32 or bf16, got {env!r}")
+    if moment_dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"moment_dtype must be torch.float32 or torch.bfloat16, got {moment_dtype}")
+    return moment_dtype
+
+
+def sr_bits(e: Any, t: Any) -> Any:
+    """The 32 rounding bits of global element ``e`` at committed update ``t`` (numpy ``uint32``, broadcast over both):
+    murmur3's 32-bit finaliser over ``lo32(e) * 0x9E3779B1 + hi32(e) * 0x85EBCA77 + t * 0xC2B2AE3D + SR_SEED`` (mod
+    2**32). The low half rounds ``m``, the high half ``v``. A pure function: no state, and no dependence on rank, world,
+    grid, paging or thread, so every holder of an element draws the same bits at the same update."""
+    import numpy as np
+
+    e = np.asarray(e, dtype=np.uint64)
+    t = (np.asarray(t, dtype=np.int64) & 0xFFFFFFFF).astype(np.uint32)
+    lo, hi = (e & np.uint64(0xFFFFFFFF)).astype(np.uint32), (e >> np.uint64(32)).astype(np.uint32)
+    with np.errstate(over="ignore"):
+        x = lo * np.uint32(0x9E3779B1) + hi * np.uint32(0x85EBCA77) + t * np.uint32(0xC2B2AE3D) + np.uint32(SR_SEED)
+        x = x ^ (x >> np.uint32(16))
+        x = x * np.uint32(0x85EBCA6B)
+        x = x ^ (x >> np.uint32(13))
+        x = x * np.uint32(0xC2B2AE35)
+        x = x ^ (x >> np.uint32(16))
+    return x
+
+
+def bf16_sr(x: Any, e: Any, t: Any, which: int, r: Any = None) -> Any:
+    """fp32 ``x`` rounded stochastically to bf16, as numpy ``uint16`` bit patterns: the 16 rounding bits ``r`` (default:
+    the low half of ``sr_bits(e, t)`` for ``which = 0``, the moment ``m``, and the high half for ``which = 1``, ``v``)
+    are added to ``x``'s fp32 bits and the upper 16 bits are kept. The add is on the magnitude, so ``x`` rounds away from
+    zero with probability equal to the discarded fraction -- unbiased for both signs -- and a value bf16 represents
+    exactly is returned unchanged for every ``r``. Inf and NaN are not added to; a NaN keeps a mantissa bit. This is the
+    specification of the update kernel's rounding: ``bf16_sr`` of ``zero1.cu`` returns the same bits."""
+    import numpy as np
+
+    if which not in (0, 1):
+        raise ValueError(f"which is 0 (m) or 1 (v), got {which}")
+    u = np.asarray(x, dtype=np.float32).view(np.uint32)
+    if r is None:
+        bits = sr_bits(e, t)
+        r = (bits >> np.uint32(16)) if which else (bits & np.uint32(0xFFFF))
+    r = np.asarray(r, dtype=np.uint32)
+    special = (u & np.uint32(0x7F800000)) == np.uint32(0x7F800000)
+    nan = np.where((u & np.uint32(0x007FFFFF)) != 0, np.uint32(0x40), np.uint32(0))
+    with np.errstate(over="ignore"):
+        out = np.where(special, (u >> np.uint32(16)) | nan, (u + r) >> np.uint32(16))
+    return out.astype(np.uint16)
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -201,6 +260,17 @@ class ShardLayout:
         return [(s + j) % world for j in range(self.k(world))]
 
 
+def check_moment_agreement(records: Dict[int, Dict[str, Any]]) -> None:
+    """``RuntimeError`` when the published ``z1/{rank}`` records of a quorum name different moment types (``moments``;
+    absent: fp32). Holders of one slice would round the same moments differently and drift apart without a sign, and a
+    pull would copy the wrong number of bytes; every rank reads the same records and raises alike, before anything is
+    freed or pulled."""
+    kinds = {r: p.get("moments", "fp32") for r, p in records.items()}
+    if len(set(kinds.values())) > 1:
+        raise RuntimeError(f"zero1: the replicas of this quorum disagree on the type of the optimizer moments "
+                           f"(per rank: {kinds})")
+
+
 def plan_pulls(need: Sequence[Range], holdings: Dict[int, Sequence[Range]], me: int) -> Tuple[List[Tuple[int, int, int]], List[Range]]:
     """Cover ``need`` from peers' ``holdings``: ``[(src_rank, lo, hi), ...]`` plus the ranges nobody holds.
 
@@ -226,12 +296,16 @@ def plan_pulls(need: Sequence[Range], holdings: Dict[int, Sequence[Range]], me: 
 def newest_complete_step(headers: Sequence[Dict[str, Any]], numel: int) -> Optional[int]:
     """The newest update count ``T`` whose checkpoint files together cover ``[0, numel)`` (``None``: there is none).
     ``headers[i]`` has ``T`` and the written ``ranges`` (``[lo, hi, offset]``). Files of one ``T`` may come from quorums
-    of different sizes: holders at the same update count hold the same bits."""
+    of different sizes: holders at the same update count hold the same bits. An update count whose files name
+    different moment types (``moments``; absent: fp32) does not count."""
     by_t: Dict[int, List[Range]] = {}
+    kinds: Dict[int, set] = {}
     for h in headers:
         by_t.setdefault(int(h["T"]), []).extend((int(lo), int(hi)) for lo, hi, _ in h["ranges"])
+        kinds.setdefault(int(h["T"]), set()).add(h.get("moments", "fp32"))
     for t in sorted(by_t, reverse=True):
-        if merge_ranges(by_t[t]) == [(0, numel)]:
+        # one quorum writes one moment type; an update count with files of both is not one quorum's and is passed over
+        if merge_ranges(by_t[t]) == [(0, numel)] and len(kinds[t]) == 1:
             return t
     return None
 
@@ -430,7 +504,7 @@ def accum_mode(micro: int, steps: int) -> int:
 
 # --------------------------------------------------------------------------- the optimizer
 class Zero1Optimizer:
-    """AdamW with fp32 master/m/v partitioned over the replicas of the current quorum (see module doc).
+    """AdamW with fp32 master and fp32 or bf16 m/v partitioned over the replicas of the current quorum (see module doc).
 
     All five flat buffers live in NVLink-symmetric segments of the process group: ``param`` and ``grad``
     (bf16; written/read by peers every step) and ``master``/``m``/``v`` (fp32; read by peers only when
@@ -485,6 +559,11 @@ class Zero1Optimizer:
         lr_steps: entries of the table; later updates keep the last rate
         no_decay: flat element ranges (multiples of 8, each inside one unit, at most ``MAX_NO_DECAY`` per unit) whose
             elements get no weight decay
+        moment_dtype: ``torch.float32`` (default) or ``torch.bfloat16`` for ``m`` and ``v`` (``None``: env
+            ``TORCHFT_B200_Z1_MOMENTS=bf16``). bf16 moments take 8 instead of 12 bytes of state per element; the update
+            computes in fp32 and rounds them stochastically (:func:`bf16_sr`) with bits that depend only on the element
+            index and the committed update count, so the holders of a slice stay bit-identical. ``master`` stays fp32.
+            Every replica of a quorum must use the same type. A checkpoint of the other type is converted on restore.
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
@@ -493,9 +572,11 @@ class Zero1Optimizer:
                  state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT,
                  max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1,
                  lr_lambda: Optional[Callable[[int], float]] = None, lr_steps: int = 0,
-                 no_decay: Sequence[Range] = ()) -> None:
+                 no_decay: Sequence[Range] = (), moment_dtype: Optional[torch.dtype] = None) -> None:
         from torchft_b200.ops import _native
 
+        self.moment_dtype = moment_type(moment_dtype)
+        self._msize = 2 if self.moment_dtype == torch.bfloat16 else 4  # bytes per element of m and of v
         self.max_grad_norm = clip_threshold(max_grad_norm)
         # learning-rate schedule: fp32 rate of committed update i + 1 at index i (host copy and device table)
         self._lr_host = lr_schedule_table(lr, lr_lambda, lr_steps) if lr_lambda is not None else None
@@ -548,10 +629,11 @@ class Zero1Optimizer:
         self._table_host: Any = None
         if not self.compact:
             self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
-            self.m = pg.alloc_symmetric("z1_m", numel * 4).view(torch.float32)
-            self.v = pg.alloc_symmetric("z1_v", numel * 4).view(torch.float32)
+            self.m = pg.alloc_symmetric("z1_m", numel * self._msize).view(self.moment_dtype)
+            self.v = pg.alloc_symmetric("z1_v", numel * self._msize).view(self.moment_dtype)
         else:
-            self.master = self.m = self.v = torch.empty(0, dtype=torch.float32, device=self.device)  # set_units allocates
+            self.master = torch.empty(0, dtype=torch.float32, device=self.device)  # set_units allocates
+            self.m = self.v = torch.empty(0, dtype=self.moment_dtype, device=self.device)
             if not 1 <= self.min_world <= 8:
                 raise ValueError("min_world must be in [1, 8]")
             self._page_shift = int(page_shift)
@@ -643,8 +725,8 @@ class Zero1Optimizer:
             logger.warning("zero1: compact state pools of %d pages are not smaller than full-size state (min_world=%d "
                            "means a rank may have to hold everything): no memory is saved", self.capacity, self.min_world)
         self.master = self.pg.alloc_symmetric("z1_master", n * 4).view(torch.float32)[:n]
-        self.m = self.pg.alloc_symmetric("z1_m", n * 4).view(torch.float32)[:n]
-        self.v = self.pg.alloc_symmetric("z1_v", n * 4).view(torch.float32)[:n]
+        self.m = self.pg.alloc_symmetric("z1_m", n * self._msize).view(self.moment_dtype)[:n]
+        self.v = self.pg.alloc_symmetric("z1_v", n * self._msize).view(self.moment_dtype)[:n]
         npages = (self.numel + self._page - 1) >> self._page_shift
         self._table_host = np.full(npages, -1, dtype=np.int32)  # page of the flat vector -> pool slot (-1: not held)
         self._table = torch.full((npages,), -1, dtype=torch.int32, device=self.device)
@@ -700,6 +782,8 @@ class Zero1Optimizer:
             sched = self._schedule_digest()
             if sched is not None:
                 me["sched"] = sched
+            if self._msize == 2:
+                me["moments"] = "bf16"  # fp32 moments publish no key: their record stays as it was
             if self._disk is not None:
                 me["disk"] = [self._disk[0], self._disk[1]]  # every rank may read what no live holder has from it
             if self.compact:
@@ -718,6 +802,7 @@ class Zero1Optimizer:
                 # sign; every rank reads the same records and raises alike, before anything is freed or pulled
                 raise RuntimeError(f"zero1: the replicas of this quorum disagree on the learning-rate schedule or the "
                                    f"weight-decay exemptions (digest per rank: {digests})")
+            check_moment_agreement(peers)
             ckpt = self._ckpt_files(rank, peers)
             plans = plan_quorum(self.layout, world, peers, self._page_shift if self.compact else None, ckpt)
             plan = plans[rank]
@@ -747,7 +832,8 @@ class Zero1Optimizer:
                         for src, lo, hi in plan.pulls:
                             for a, b, at in self._pieces(tables[src], lo, hi):
                                 for c, d, mine in self._pieces(self._table_host, a, b):
-                                    entries.append((ptrs[src] + (at + c - a) * 4, local.data_ptr() + mine * 4, (d - c) * 4))
+                                    sz = local.element_size()
+                                    entries.append((ptrs[src] + (at + c - a) * sz, local.data_ptr() + mine * sz, (d - c) * sz))
                     device_copy(entries, s, chunk_bytes=1 << 20)
                 if plan.reads:
                     self._read_state(plan.reads)  # nobody live holds these at T: the restored checkpoint does
@@ -766,11 +852,15 @@ class Zero1Optimizer:
                 self.lost_elements += total(plan.lost)
                 logger.warning("zero1: %d state elements had no surviving holder and were re-seeded from the weights "
                                "(moments reset)", total(plan.lost))
-            self.pulled_bytes += 12 * total([(lo, hi) for _, lo, hi in plan.pulls])
+            self.pulled_bytes += self._state_item() * total([(lo, hi) for _, lo, hi in plan.pulls])
             self.t = plan.tmax
             self._holdings = plan.hold
             self._refresh_pending = world > 1
             self._configured, self._disk = True, None
+
+    def _state_item(self) -> int:
+        """Bytes of (master, m, v) per element: 12 with fp32 moments, 8 with bf16."""
+        return self.master.element_size() + self.m.element_size() + self.v.element_size()
 
     def _schedule_digest(self) -> Optional[str]:
         """What this rank publishes of its schedule and exemptions (``None`` without either: the record stays as it was)."""
@@ -967,7 +1057,8 @@ class Zero1Optimizer:
             for mode in modes:
                 self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, nelem=hi - lo, hyper=hp,
                                         gate=self.gate, replication=k, mode=mode, blocks=self._upd_blocks, stream=stream,
-                                        coef=coef, no_decay=nd[i] if nd else (), **sched, **state)
+                                        coef=coef, no_decay=nd[i] if nd else (), moment_dtype=self.moment_dtype,
+                                        **sched, **state)
             if events is not None:
                 events[i].record(stream)
 
@@ -975,9 +1066,11 @@ class Zero1Optimizer:
         """The state arguments of ``zero1_update_`` for the unit that starts at element ``lo``. Full-size state passes
         the arrays at ``lo`` and no table, which selects the kernel without page lookups; paged state passes the pools
         and the page table, through which the kernel finds each element."""
-        ptrs = {"master": self.master.data_ptr(), "m": self.m.data_ptr(), "v": self.v.data_ptr()}
         if self._table is None:
-            return {name: p + 4 * lo for name, p in ptrs.items()}
+            # the global element index of the unit's start is what bf16 moments hash for their rounding bits
+            return {"master": self.master.data_ptr() + 4 * lo, "m": self.m.data_ptr() + self._msize * lo,
+                    "v": self.v.data_ptr() + self._msize * lo, "state_off": lo}
+        ptrs = {"master": self.master.data_ptr(), "m": self.m.data_ptr(), "v": self.v.data_ptr()}
         return {**ptrs, "table": self._table.data_ptr(), "state_off": lo, "page_shift": self._page_shift}
 
     def resolved(self, verdict: bool) -> None:
@@ -1030,8 +1123,8 @@ class Zero1Optimizer:
         for lo, hi in ranges:
             written.append((lo, hi, e))
             e += hi - lo
-        stage = w.staging(14 * e)
-        sec = sections(e)
+        sec = sections(e, self._msize)
+        stage = w.staging((6 + 2 * self._msize) * e)  # bf16 weights, fp32 master, m and v per primary element
         if self._snap_stream is None:
             self._snap_stream = torch.cuda.Stream(device=self.device)
         s = self._snap_stream
@@ -1046,10 +1139,11 @@ class Zero1Optimizer:
                         x = off + a - lo
                         stage[2 * x:2 * (x + b - a)].copy_(self.param[a:b].view(u8), non_blocking=True)
                         for name, arr in (("master", self.master), ("m", self.m), ("v", self.v)):
-                            base = sec[name] + 4 * x
+                            sz = arr.element_size()
+                            base = sec[name] + sz * x
                             for c, d, at in self._pieces(self._table_host, a, b):  # maximal runs of consecutive slots
-                                stage[base + 4 * (c - a):base + 4 * (d - a)].copy_(arr[at:at + d - c].view(u8),
-                                                                                   non_blocking=True)
+                                stage[base + sz * (c - a):base + sz * (d - a)].copy_(arr[at:at + d - c].view(u8),
+                                                                                     non_blocking=True)
                 done.append(s.record_event())
         self._snap_events, self._snap_done = done, done[-1]
         ms = manager_state or {"step": self.t, "batches_committed": 0}
@@ -1059,6 +1153,8 @@ class Zero1Optimizer:
                   "elements": e, "sections": sec,
                   "hparams": {"lr": self.param_groups[0]["lr"], "betas": list(self.betas), "eps": self.eps,
                               "weight_decay": self.weight_decay, "max_grad_norm": self.max_grad_norm}}
+        if self._msize == 2:
+            header["moments"] = "bf16"  # a header without the key describes fp32 moments
         w.submit(header, self._snap_done)
         return self.t
 
@@ -1105,15 +1201,25 @@ class Zero1Optimizer:
     def _read_ranges(self, reads: Sequence[Tuple[Any, int, int, int]], arrays: Sequence[str]) -> None:
         """``arrays`` over the flat ranges of ``reads`` from the files, through pinned bounce buffers, on the re-shard
         stream (compact state: into the pool pages the table maps them to)."""
-        from torchft_b200.checkpointing.sharded import RangedReader
+        from torchft_b200.checkpointing.sharded import RangedReader, file_dtype
 
         dst = {"param": self.param, "master": self.master, "m": self.m, "v": self.v}
         rd = RangedReader(self._reshard_stream)
         try:
             for h, off, lo, hi in reads:
                 for name in arrays:
+                    convert = file_dtype(h, name) != dst[name].dtype
                     for a, b, at in self._pieces(None if name == "param" else self._table_host, lo, hi):
-                        rd.read(h, name, off + a - lo, dst[name][at:at + b - a])
+                        if not convert:
+                            rd.read(h, name, off + a - lo, dst[name][at:at + b - a])
+                            continue
+                        # moments saved in the other type: fp32 -> bf16 rounds to nearest, bf16 -> fp32 is exact
+                        for c in range(a, b, CONVERT_CHUNK):
+                            n = min(CONVERT_CHUNK, b - c)
+                            with torch.cuda.stream(self._reshard_stream):
+                                tmp = torch.empty(n, dtype=file_dtype(h, name), device=self.device)
+                                rd.read(h, name, off + c - lo, tmp)
+                                dst[name][at + c - a:at + c - a + n].copy_(tmp)
         finally:
             rd.close()
 
@@ -1128,11 +1234,11 @@ class Zero1Optimizer:
         return float(self._lr_host[min(max(int(t), 1), len(self._lr_host)) - 1])
 
     def state_bytes_held(self) -> int:
-        return 12 * total(self.layout.held(self.comm.rank, max(self.comm.world, 1)))
+        return self._state_item() * total(self.layout.held(self.comm.rank, max(self.comm.world, 1)))
 
     def state_bytes_allocated(self) -> int:
-        """Device bytes of the fp32 master/m/v arrays (compact: the page pools)."""
-        return 12 * self.master.numel()
+        """Device bytes of the master/m/v arrays (compact: the page pools)."""
+        return self._state_item() * self.master.numel()
 
     def held_state(self) -> Dict[Range, Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
         """Copies of (master, m, v) over each range this rank holds, keyed by ``(lo, hi)`` (for inspection and tests)."""
