@@ -474,11 +474,13 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
     if (a.mode == 0) cf = __ldg(a.coef);
   }
   const int t = a.gate[1];
-  const float tf = (float)t;
   // the rate follows the committed update count on the device, like the bias correction: one uniform load
   // (a refresh may run at t = 0 and does not use it)
   const float lr = a.lr_tab != nullptr ? __ldg(a.lr_tab + (min(max(t, 1), a.lr_steps) - 1)) : a.lr;
-  const float bc1 = 1.f - powf(a.b1, tf), bc2 = 1.f - powf(a.b2, tf);
+  // 1 - b^t in fp64 from the fp32 betas the moving averages use, rounded once. --use_fast_math turns powf into
+  // __log2f/exp2f, whose absolute error in log2(b) becomes a relative error of up to ~1e-4 in 1 - b^t at b = 0.999; the
+  // fp64 pow is not approximated and leaves the fp32 result correctly rounded but for near-ties.
+  const float bc1 = (float)(1.0 - pow((double)a.b1, (double)t)), bc2 = (float)(1.0 - pow((double)a.b2, (double)t));
   const float step_size = lr / bc1;
   const float inv_bc2_sqrt = rsqrtf(bc2);
   const float decay = 1.f - lr * a.wd;
@@ -549,7 +551,9 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           m[i] = a.b1 * m[i] + (1.f - a.b1) * gr[i];
-          vv[i] = a.b2 * vv[i] + (1.f - a.b2) * gr[i] * gr[i];
+          // spelled out as the flat AdamW kernel (model_ops.cu) compiles it, so both store the same bits: left to
+          // itself the compiler fuses b2 * v here and g * ((1 - b2) * g) there
+          vv[i] = __fmaf_rn(gr[i], __fmul_rn(1.f - a.b2, gr[i]), __fmul_rn(a.b2, vv[i]));
           const float denom = sqrtf(vv[i]) * inv_bc2_sqrt + a.eps;
           w[i] = w[i] * dcy - step_size * __fdividef(m[i], denom);
         }

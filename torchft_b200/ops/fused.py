@@ -9,6 +9,7 @@ from __future__ import annotations
 
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 
 from torchft_b200.ops import _native
@@ -273,11 +274,17 @@ class FlatAdamW:
         self.t += 1
         lr = self.param_groups[0]["lr"]
         b1, b2 = self.betas
+        bc1, bc2 = self._bias_corrections()
         K.adamw(
             self.p.data_ptr(), self.master.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self.g.data_ptr(),
-            self.p.numel(), lr, b1, b2, self.eps, self.weight_decay, 1.0 - b1 ** self.t, 1.0 - b2 ** self.t,
+            self.p.numel(), lr, b1, b2, self.eps, self.weight_decay, bc1, bc2,
             grad_scale, gate.data_ptr() if gate is not None else 0, _native.stream_ptr(),
         )
+
+    def _bias_corrections(self) -> Tuple[float, float]:
+        """1 - b^t of the fp32 betas the kernel's moving averages use (fp64 here, rounded to fp32 by the binding): at
+        b2 = 0.999 the double beta's 1 - b^t is hundreds of fp32 ulps away from the fp32 beta's."""
+        return tuple(1.0 - float(np.float32(b)) ** self.t for b in self.betas)
 
     def step_ranges(self, ranges, streams_events, grad_scale: float = 1.0, gate: Optional[torch.Tensor] = None,
                     max_blocks: int = 0) -> None:
@@ -294,7 +301,7 @@ class FlatAdamW:
         self.t += 1
         lr = self.param_groups[0]["lr"]
         b1, b2 = self.betas
-        bc1, bc2 = 1.0 - b1 ** self.t, 1.0 - b2 ** self.t
+        bc1, bc2 = self._bias_corrections()
         gp = gate.data_ptr() if gate is not None else 0
         p, w, m, v, g = (t.data_ptr() for t in (self.p, self.master, self.m, self.v, self.g))
         for (lo, hi), ev in zip(ranges, events):
