@@ -24,40 +24,18 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
                            int barrier_mode, cudaStream_t stream);
 
 // zero1.cu -------------------------------------------------------------------
-// FT-ZeRO-1: one-CTA handshake (flag exchange with every peer, result mirrored to a device word), sync-free
-// reduce-scatter body (+ buddy push), device-side commit verdict, sync-free gated AdamW fused with the all-gather of the
-// new bf16 weights. mc_base != nullptr selects the NVLS (multimem) data path. A non-null `table` selects paged
-// optimizer state: master/m/v are pools of 2^page_shift-element pages, element soff + i of the unit lives in page
-// table[(soff + i) >> page_shift]; a null table keeps flat addressing (state indexed like the unit).
-// Gradient clipping (all null by default = off): the reduce writes the unit's fp64 sum of squares of its slice to `gn`
-// (per-CTA scratch `cta_sq` of >= blocks doubles and a zeroed `ticket`); at world 1 it scales in place. The commit sums
-// `gn[0..world-1][0..nunits-1]`, writes {norm, coef} to `norm`, posts the norm to the host ring and vetoes a non-finite
-// norm. The update multiplies the gradient by `*coef`.
-// Gradient accumulation (acc_mode 0 = off by default): `acc` is this rank's fp32 accumulator of the unit's primary
-// slice. acc_mode 1 (first micro-batch) stores the fp32 rank sum there, 2 (middle) adds it; neither writes the gradient
-// segment. 3 (last) reduces (acc + rank sum) * scale to bf16 like mode 0, with the gradient norm when `gn` is set.
-// Learning-rate schedule (lr_tab null by default = the constant `lr`): lr_tab[i] is the fp32 rate of committed update
-// i + 1, and the update reads lr_tab[clamp(gate[1], 1, lr_steps) - 1] for both the step and the decoupled decay.
-// Weight-decay exemptions: `no_decay` holds n_no_decay <= kMaxNoDecay unit-relative element ranges as (lo, hi) pairs,
-// multiples of 8, whose elements get no decay.
-// Moment type (moment_dtype: a DType code, 0 = fp32 by default or 1 = bf16): with bf16 `m` and `v` are bf16 arrays, 16 B aligned, and the
-// update stores them with stochastic rounding whose bits depend only on (soff + local element index, gate[1], which
-// moment); flat launches then pass the unit's first global element as `soff`. `master` stays fp32.
-constexpr int kMaxNoDecay = 4;
-void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
-                            int barrier_mode, cudaStream_t stream);
-void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
-                         int replication, int blocks, int threads, cudaStream_t stream, double* gn = nullptr,
-                         double* cta_sq = nullptr, unsigned* ticket = nullptr, float* acc = nullptr, int acc_mode = 0);
-void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64_t flag, uint32_t seq, int channel,
-                         int host_ok, int exchange, cudaStream_t stream, const double* const* gn = nullptr,
-                         int nunits = 0, float max_norm = 0.f, float* norm = nullptr);
-void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
-                         void* m, void* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
-                         int replication, int mode, int blocks, int threads, cudaStream_t stream,
-                         const int* table = nullptr, size_t soff = 0, int page_shift = 0, const float* coef = nullptr,
-                         const float* lr_tab = nullptr, int lr_steps = 0, int n_no_decay = 0,
-                         const size_t* no_decay = nullptr, int moment_dtype = 0);
+// FT-ZeRO-1: one-CTA handshake, sync-free reduce-scatter body (+ buddy push), device-side commit verdict, sync-free
+// gated AdamW fused with the all-gather of the new bf16 weights. The argument structs and their fields: zero1.cuh.
+namespace zero1 {
+struct HsArgs;
+struct RSArgs;
+struct CommitArgs;
+struct UpdArgs;
+}  // namespace zero1
+void zero1_handshake_launch(const zero1::HsArgs& a, cudaStream_t stream);
+void zero1_reduce_launch(zero1::RSArgs a, int acc_mode, int blocks, int threads, cudaStream_t stream);
+void zero1_commit_launch(const zero1::CommitArgs& a, cudaStream_t stream);
+void zero1_update_launch(zero1::UpdArgs a, int moment_dtype, int blocks, int threads, cudaStream_t stream);
 
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);

@@ -7,6 +7,7 @@
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <algorithm>
 #include <cstring>
 #include <stdexcept>
 #include <string>
@@ -14,6 +15,7 @@
 
 #include "api.h"
 #include "common.cuh"
+#include "zero1.cuh"
 
 namespace py = pybind11;
 using namespace tft;
@@ -228,57 +230,106 @@ PYBIND11_MODULE(_K, m) {
       "zero1_handshake",
       [](const PeerTableH& pt, const Status& st, uintptr_t ok_out, uint64_t flag, int channel, bool release, int barrier_mode,
          uintptr_t stream) {
-        zero1_handshake_launch(pt.pt, st.dev(), P<int>(ok_out), flag, channel, release ? 1 : 0, barrier_mode, S(stream));
+        zero1::HsArgs a{};
+        a.pt = pt.pt;
+        a.st = st.dev();
+        a.ok_out = P<int>(ok_out);
+        a.flag = flag;
+        a.channel = channel;
+        a.release = release;
+        a.barrier_mode = barrier_mode;
+        zero1_handshake_launch(a, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("ok_out"), py::arg("flag"), py::arg("channel"), py::arg("release"),
       py::arg("barrier_mode"), py::arg("stream"));
   m.def(
       "zero1_reduce",
       [](const PeerTableH& pt, uintptr_t ok, uintptr_t mc_base, size_t off, size_t nelem, float scale, int replication,
-         int blocks, int threads, uintptr_t stream, uintptr_t gn, uintptr_t cta_sq, uintptr_t ticket, uintptr_t acc,
-         int acc_mode) {
-        zero1_reduce_launch(pt.pt, P<const int>(ok), P<void>(mc_base), off, nelem, scale, replication, blocks, threads, S(stream),
-                            P<double>(gn), P<double>(cta_sq), P<unsigned>(ticket), P<float>(acc), acc_mode);
+         uintptr_t gn, uintptr_t cta_sq, uintptr_t ticket, uintptr_t acc, int acc_mode, int blocks, int threads,
+         uintptr_t stream) {
+        zero1::RSArgs a{};
+        a.pt = pt.pt;
+        a.ok = P<const int>(ok);
+        a.mc = P<char>(mc_base);
+        a.off = off;
+        a.nelem = nelem;
+        a.scale = scale;
+        a.replication = replication;
+        a.gn = P<double>(gn);
+        a.cta_sq = P<double>(cta_sq);
+        a.ticket = P<unsigned>(ticket);
+        a.acc = P<float>(acc);
+        zero1_reduce_launch(a, acc_mode, blocks, threads, S(stream));
       },
       py::arg("pt"), py::arg("ok"), py::arg("mc_base"), py::arg("off"), py::arg("nelem"), py::arg("scale"),
-      py::arg("replication"), py::arg("blocks"), py::arg("threads"), py::arg("stream"), py::arg("gn") = 0,
-      py::arg("cta_sq") = 0, py::arg("ticket") = 0, py::arg("acc") = 0, py::arg("acc_mode") = 0);
+      py::arg("replication"), py::arg("gn"), py::arg("cta_sq"), py::arg("ticket"), py::arg("acc"), py::arg("acc_mode"),
+      py::arg("blocks"), py::arg("threads"), py::arg("stream"));
   m.def(
       "zero1_commit",
-      [](const PeerTableH& pt, const Status& st, uintptr_t gate, uint64_t flag, uint32_t seq, int channel,
-         bool host_ok, bool exchange, uintptr_t stream, const std::vector<uintptr_t>& gnorm, int nunits, float max_norm,
-         uintptr_t norm) {
-        if (gnorm.empty()) {
-          zero1_commit_launch(pt.pt, st.dev(), P<int>(gate), flag, seq, channel, host_ok ? 1 : 0, exchange ? 1 : 0,
-                              S(stream));
-          return;
-        }
-        if ((int)gnorm.size() != pt.pt.world) throw std::runtime_error("zero1_commit: need one z1_gnorm pointer per rank");
-        const double* gn[kMaxRanks] = {};
-        for (size_t r = 0; r < gnorm.size(); ++r) gn[r] = P<const double>(gnorm[r]);
-        zero1_commit_launch(pt.pt, st.dev(), P<int>(gate), flag, seq, channel, host_ok ? 1 : 0, exchange ? 1 : 0,
-                            S(stream), gn, nunits, max_norm, P<float>(norm));
+      [](const PeerTableH& pt, const Status& st, uintptr_t gate, uint64_t flag, uint32_t seq, int channel, bool host_ok,
+         bool exchange, const std::vector<uintptr_t>& gnorm, int nunits, float max_norm, uintptr_t norm, uintptr_t stream) {
+        if (!gnorm.empty() && (int)gnorm.size() != pt.pt.world)
+          throw std::runtime_error("zero1_commit: need one z1_gnorm pointer per rank");
+        zero1::CommitArgs a{};
+        a.pt = pt.pt;
+        a.st = st.dev();
+        a.gate = P<int>(gate);
+        a.flag = flag;
+        a.seq = seq;
+        a.channel = channel;
+        a.host_ok = host_ok;
+        a.exchange = exchange;
+        for (size_t r = 0; r < gnorm.size(); ++r) a.gn[r] = P<const double>(gnorm[r]);
+        a.nunits = nunits;
+        a.max_norm = max_norm;
+        a.norm = P<float>(norm);
+        zero1_commit_launch(a, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("gate"), py::arg("flag"), py::arg("seq"), py::arg("channel"),
-      py::arg("host_ok"), py::arg("exchange"), py::arg("stream"), py::arg("gnorm") = std::vector<uintptr_t>{},
-      py::arg("nunits") = 0, py::arg("max_norm") = 0.f, py::arg("norm") = 0);
+      py::arg("host_ok"), py::arg("exchange"), py::arg("gnorm"), py::arg("nunits"), py::arg("max_norm"), py::arg("norm"),
+      py::arg("stream"));
   m.def(
       "zero1_update",
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,
          uintptr_t v, size_t nelem, float lr, float b1, float b2, float eps, float wd, int replication, int mode,
-         int blocks, int threads, uintptr_t stream, uintptr_t table, size_t soff, int page_shift, uintptr_t coef,
-         uintptr_t lr_tab, int lr_steps, const std::vector<size_t>& no_decay, int moment_dtype) {
+         uintptr_t table, size_t soff, int page_shift, uintptr_t coef, uintptr_t lr_tab, int lr_steps,
+         const std::vector<size_t>& no_decay, int moment_dtype, int blocks, int threads, uintptr_t stream) {
         if (no_decay.size() & 1) throw std::runtime_error("zero1_update: no_decay is a flat list of (lo, hi) pairs");
-        zero1_update_launch(pt.pt, P<void>(mc_base), P<const int>(gate), poff, P<void>(grad), P<float>(master), P<void>(mm),
-                            P<void>(v), nelem, lr, b1, b2, eps, wd, replication, mode, blocks, threads, S(stream),
-                            P<const int>(table), soff, page_shift, P<const float>(coef), P<const float>(lr_tab), lr_steps,
-                            (int)(no_decay.size() / 2), no_decay.empty() ? nullptr : no_decay.data(), moment_dtype);
+        zero1::UpdArgs a{};
+        a.pt = pt.pt;
+        a.mc = P<char>(mc_base);
+        a.gate = P<const int>(gate);
+        a.poff = poff;
+        a.grad = P<const __nv_bfloat16>(grad);
+        a.master = P<float>(master);
+        a.m = P<void>(mm);
+        a.v = P<void>(v);
+        a.nelem = nelem;
+        a.lr = lr;
+        a.b1 = b1;
+        a.b2 = b2;
+        a.eps = eps;
+        a.wd = wd;
+        a.replication = replication;
+        a.mode = mode;
+        a.table = P<const int>(table);
+        a.soff = soff;
+        a.page_shift = page_shift;
+        a.coef = P<const float>(coef);
+        a.lr_tab = P<const float>(lr_tab);
+        a.lr_steps = lr_steps;
+        a.n_nd = (int)(no_decay.size() / 2);
+        for (int r = 0; r < std::min(a.n_nd, kMaxNoDecay); ++r) {  // the launcher rejects more
+          a.nd_lo[r] = no_decay[2 * r];
+          a.nd_hi[r] = no_decay[2 * r + 1];
+        }
+        zero1_update_launch(a, moment_dtype, blocks, threads, S(stream));
       },
       py::arg("pt"), py::arg("mc_base"), py::arg("gate"), py::arg("poff"), py::arg("grad"), py::arg("master"),
       py::arg("m"), py::arg("v"), py::arg("nelem"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"),
-      py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("blocks"), py::arg("threads"), py::arg("stream"),
-      py::arg("table") = 0, py::arg("soff") = 0, py::arg("page_shift") = 0, py::arg("coef") = 0, py::arg("lr_tab") = 0,
-      py::arg("lr_steps") = 0, py::arg("no_decay") = std::vector<size_t>{}, py::arg("moment_dtype") = 0);
+      py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("table"), py::arg("soff"), py::arg("page_shift"),
+      py::arg("coef"), py::arg("lr_tab"), py::arg("lr_steps"), py::arg("no_decay"), py::arg("moment_dtype"),
+      py::arg("blocks"), py::arg("threads"), py::arg("stream"));
 
   m.def(
       "push_exchange",

@@ -50,13 +50,21 @@
 //
 // Per rank and step this moves the same NVLink bytes as a two-shot all-reduce but divides the 28 B/param optimizer
 // HBM traffic (and the state a replica must hold) by N/k.
+#include <algorithm>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "api.h"
 #include "common.cuh"
+#include "zero1.cuh"
 
 namespace tft {
+
+using zero1::CommitArgs;
+using zero1::HsArgs;
+using zero1::RSArgs;
+using zero1::UpdArgs;
 
 namespace {
 
@@ -88,19 +96,8 @@ struct Geo {
 };
 
 // ---------------------------------------------------------------------------
-// Handshake: one CTA, one flag exchange with every peer. `ok_out` (device) receives 1/0 so the
-// sync-free kernels that follow on the same stream can turn themselves into no-ops after a failure.
+// Handshake: one CTA, one flag exchange with every peer.
 // ---------------------------------------------------------------------------
-struct HsArgs {
-  PeerTable pt;
-  StatusBlock* st;
-  int* ok_out;
-  uint64_t flag;     // consumes flag+1
-  int channel;
-  int release;       // this rank wrote peer-visible data in an earlier kernel of this stream
-  int barrier_mode;
-};
-
 __global__ void __launch_bounds__(32, 1) zero1_handshake_kernel(HsArgs a) {
   const bool ok = block_barrier(a.pt, a.channel, a.flag + 1, a.st, a.release != 0, /*acquire=*/true, a.barrier_mode);
   if (threadIdx.x == 0) *a.ok_out = ok ? 1 : 0;
@@ -109,25 +106,6 @@ __global__ void __launch_bounds__(32, 1) zero1_handshake_kernel(HsArgs a) {
 // ---------------------------------------------------------------------------
 // Reduce-scatter body (no synchronisation).
 // ---------------------------------------------------------------------------
-struct RSArgs {
-  PeerTable pt;       // data[] = every rank's gradient segment
-  const int* ok;      // result of the handshake in front of this kernel
-  char* mc;           // multicast VA of the gradient segment (nullptr = P2P loads)
-  size_t off;         // byte offset of the unit inside the segment
-  size_t nelem;       // elements in the unit (multiple of 8)
-  float scale;
-  int replication;    // k
-  // CLIP: this rank's fp64 slot of the unit in its z1_gnorm segment, one fp64 per CTA of scratch and the last-CTA-done
-  // ticket (zero between launches: the last CTA resets it)
-  double* gn;
-  double* cta_sq;
-  unsigned* ticket;
-  // gradient accumulation (ACC != kAccOff): this rank's fp32 accumulator of the unit's primary slice; vector v of the
-  // slice lives at acc + (v - lo(rank)) * 8. acc_first (uniform per launch): store the sum instead of adding it.
-  float* acc;
-  int acc_first;
-};
-
 // Accumulation mode of the reduce kernel, for a step of M micro-batches:
 //   kAccOff  -- M = 1: scale, round to bf16, store to this rank and its k-1 buddies
 //   kAccAcc  -- micro-batches 0 .. M-2: the fp32 rank sum goes to the accumulator (micro-batch 0 stores, later ones
@@ -304,23 +282,6 @@ __global__ void __launch_bounds__(512, 1) zero1_reduce_kernel(RSArgs a) {
 // Commit verdict on the device (replaces current-stream synchronize + should_commit RPC for
 // replica groups of one rank, upstream torchft/manager.py:884-903).
 // ---------------------------------------------------------------------------
-struct CommitArgs {
-  PeerTable pt;        // pads only
-  StatusBlock* st;
-  int* gate;           // device: gate[0] = verdict of this step, gate[1] = optimizer step count t
-  uint64_t flag;       // consumes flag+1
-  uint32_t seq;        // commit sequence number (slot in the host ring)
-  int channel;
-  int host_ok;         // host-side part of the verdict (enough participants, no host-latched error)
-  int exchange;        // 1 = AND the verdict over the quorum through the signal pads
-  // gradient clipping (gn[rank] != nullptr): every rank's z1_gnorm segment (nunits fp64 partials each), the clip
-  // threshold, and the device pair norm[0] = global L2 norm, norm[1] = clip coefficient
-  const double* gn[kMaxRanks];
-  int nunits;
-  float max_norm;
-  float* norm;
-};
-
 // One rank's per-unit partials summed in unit order, 16 loads in flight at a time.
 __device__ __forceinline__ double rank_sumsq(const double* p, int n) {
   double s = 0.0;
@@ -430,36 +391,6 @@ __device__ __forceinline__ uint32_t bf16_sr(float x, uint32_t r) {
 // ---------------------------------------------------------------------------
 // Gated AdamW on the held slices + all-gather of the new bf16 weights (no synchronisation).
 // ---------------------------------------------------------------------------
-struct UpdArgs {
-  PeerTable pt;        // data[] = every rank's PARAMETER segment
-  char* mc;            // multicast VA of the parameter segment (nullptr = P2P stores)
-  const int* gate;     // gate[0] verdict, gate[1] step count (already incremented for this step)
-  size_t poff;         // byte offset of the unit inside the parameter segment
-  const bf16* grad;    // local reduced gradients of the unit
-  float* master;       // local fp32 state of the unit (full-size arrays; only held slices are valid)
-  void* m;             // moments: fp32 or bf16 arrays (the kernel's MT), indexed like master
-  void* v;
-  size_t nelem;
-  float lr, b1, b2, eps, wd;
-  int replication;
-  int mode;            // 0 = gated update + push, 1 = refresh (re-broadcast bf16(master) of the primary slice, ungated)
-  // paged state (PAGED = true): master/m/v are page pools; element e of the flat vector (e = soff + local index)
-  // lives at pool[table[e >> page_shift] << page_shift | (e & (page - 1))]. A page is a multiple of 8 elements, so
-  // the two 16-byte vectors of one 8-element group never straddle a page. bf16 moments hash soff + local index, so
-  // flat launches pass the unit's first element there too.
-  const int* table;
-  size_t soff;
-  int page_shift;
-  const float* coef;   // CLIP: the clip coefficient the commit kernel wrote; the gradient is scaled by it (mode 0)
-  // learning-rate schedule (lr_tab != nullptr): lr_tab[i] is the fp32 rate of committed update i + 1; update t uses
-  // lr_tab[clamp(t, 1, lr_steps) - 1] in place of lr (past the table the last rate holds)
-  const float* lr_tab;
-  int lr_steps;
-  // weight-decay exemptions: n_nd ranges [nd_lo, nd_hi) of 8-element vectors, relative to the unit, get no decay
-  int n_nd;
-  size_t nd_lo[kMaxNoDecay], nd_hi[kMaxNoDecay];
-};
-
 template <int W, bool NVLS, bool PAGED, bool CLIP, typename MT>
 __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   constexpr bool BF16M = sizeof(MT) == 2;
@@ -596,64 +527,11 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   }
 }
 
-template <bool NVLS, bool CLIP, int ACC>
-void launch_rs(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
-  switch (a.pt.world) {
-    case 1:
-      // one rank: only clipping and accumulation launch it (in place, no peer access); never multicast
-      if constexpr ((CLIP || ACC != kAccOff) && !NVLS) {
-        zero1_reduce_kernel<1, false, CLIP, ACC><<<blocks, threads, 0, s>>>(a);
-        break;
-      }
-      throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
-    case 2: zero1_reduce_kernel<2, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_reduce_kernel<3, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_reduce_kernel<4, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_reduce_kernel<5, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_reduce_kernel<6, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_reduce_kernel<7, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_reduce_kernel<8, NVLS, CLIP, ACC><<<blocks, threads, 0, s>>>(a); break;
-    default: throw std::runtime_error("zero1_reduce: world size must be in [2, 8]");
-  }
-}
-
-template <bool CLIP, int ACC>
-void launch_rs_path(const RSArgs& a, int blocks, int threads, cudaStream_t s) {
-  if (a.mc != nullptr)
-    launch_rs<true, CLIP, ACC>(a, blocks, threads, s);
-  else
-    launch_rs<false, CLIP, ACC>(a, blocks, threads, s);
-}
-
-template <bool NVLS, bool PAGED, bool CLIP, typename MT>
-void launch_upd_w(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
-  switch (a.pt.world) {
-    case 1: zero1_update_kernel<1, false, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 2: zero1_update_kernel<2, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 3: zero1_update_kernel<3, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 4: zero1_update_kernel<4, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 5: zero1_update_kernel<5, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 6: zero1_update_kernel<6, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 7: zero1_update_kernel<7, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    case 8: zero1_update_kernel<8, NVLS, PAGED, CLIP, MT><<<blocks, threads, 0, s>>>(a); break;
-    default: throw std::runtime_error("zero1_update: world size must be in [1, 8]");
-  }
-}
-
-template <bool NVLS, bool PAGED, typename MT>
-void launch_upd_clip(const UpdArgs& a, int blocks, int threads, cudaStream_t s) {
-  if (a.coef != nullptr)
-    launch_upd_w<NVLS, PAGED, true, MT>(a, blocks, threads, s);
-  else
-    launch_upd_w<NVLS, PAGED, false, MT>(a, blocks, threads, s);
-}
-
-template <bool NVLS, bool PAGED>
-void launch_upd(const UpdArgs& a, bool bf16_moments, int blocks, int threads, cudaStream_t s) {
-  if (bf16_moments)
-    launch_upd_clip<NVLS, PAGED, bf16>(a, blocks, threads, s);
-  else
-    launch_upd_clip<NVLS, PAGED, float>(a, blocks, threads, s);
+// Calls f(std::integral_constant<decltype(V), V>{}) for the V of Vs equal to the runtime value v: the one place where a
+// launcher's runtime selector becomes a template argument. Returns false when v is none of Vs.
+template <auto... Vs, typename T, typename F>
+bool dispatch(T v, F&& f) {
+  return ((v == Vs && (f(std::integral_constant<decltype(Vs), Vs>{}), true)) || ...);
 }
 
 void check_grid(int blocks, int threads, const char* who) {
@@ -663,99 +541,88 @@ void check_grid(int blocks, int threads, const char* who) {
 
 }  // namespace
 
-void zero1_handshake_launch(const PeerTable& pt, StatusBlock* st, int* ok_out, uint64_t flag, int channel, int release,
-                            int barrier_mode, cudaStream_t stream) {
-  HsArgs a{pt, st, ok_out, flag, channel, release, barrier_mode};
+void zero1_handshake_launch(const HsArgs& a, cudaStream_t stream) {
   zero1_handshake_kernel<<<1, 32, 0, stream>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-void zero1_reduce_launch(const PeerTable& pt, const int* ok, void* mc_base, size_t off, size_t nelem, float scale,
-                         int replication, int blocks, int threads, cudaStream_t stream, double* gn, double* cta_sq,
-                         unsigned* ticket, float* acc, int acc_mode) {
+void zero1_reduce_launch(RSArgs a, int acc_mode, int blocks, int threads, cudaStream_t stream) {
   check_grid(blocks, threads, "zero1_reduce");
-  if ((off & 15) || (nelem & 7)) throw std::runtime_error("zero1_reduce: unit must be 16 B aligned and a multiple of 8 elements");
-  if (replication < 1) throw std::runtime_error("zero1_reduce: replication must be >= 1");
-  if (gn != nullptr && (cta_sq == nullptr || ticket == nullptr))
+  if ((a.off & 15) || (a.nelem & 7)) throw std::runtime_error("zero1_reduce: unit must be 16 B aligned and a multiple of 8 elements");
+  if (a.replication < 1) throw std::runtime_error("zero1_reduce: replication must be >= 1");
+  if (a.gn != nullptr && (a.cta_sq == nullptr || a.ticket == nullptr))
     throw std::runtime_error("zero1_reduce: the gradient norm needs the per-CTA scratch and the ticket");
   if (acc_mode < 0 || acc_mode > 3) throw std::runtime_error("zero1_reduce: acc_mode must be 0 (off), 1 (first), 2 (middle) or 3 (last)");
-  if (acc_mode != 0 && (acc == nullptr || (reinterpret_cast<uintptr_t>(acc) & 15)))
+  if (acc_mode != 0 && (a.acc == nullptr || (reinterpret_cast<uintptr_t>(a.acc) & 15)))
     throw std::runtime_error("zero1_reduce: accumulation needs a 16 B aligned fp32 accumulator");
-  if ((acc_mode == 1 || acc_mode == 2) && gn != nullptr)
+  if ((acc_mode == 1 || acc_mode == 2) && a.gn != nullptr)
     throw std::runtime_error("zero1_reduce: the gradient norm is taken on the last micro-batch only");
-  RSArgs a{pt, ok, reinterpret_cast<char*>(mc_base), off, nelem, scale, replication, gn, cta_sq, ticket,
-           acc_mode != 0 ? acc : nullptr, acc_mode == 1 ? 1 : 0};
-  if (acc_mode == 1 || acc_mode == 2) {
-    launch_rs_path<false, kAccAcc>(a, blocks, threads, stream);
-  } else if (acc_mode == 3) {
-    if (gn != nullptr)
-      launch_rs_path<true, kAccLast>(a, blocks, threads, stream);
-    else
-      launch_rs_path<false, kAccLast>(a, blocks, threads, stream);
-  } else if (gn != nullptr) {
-    launch_rs_path<true, kAccOff>(a, blocks, threads, stream);
-  } else {
-    launch_rs_path<false, kAccOff>(a, blocks, threads, stream);
-  }
+  if (acc_mode == 0) a.acc = nullptr;
+  a.acc_first = acc_mode == 1 ? 1 : 0;
+  const int acc = acc_mode == 0 ? kAccOff : (acc_mode == 3 ? kAccLast : kAccAcc);
+  const char* bad_world = "zero1_reduce: world size must be in [2, 8]";
+  const bool known_world = dispatch<1, 2, 3, 4, 5, 6, 7, 8>(a.pt.world, [&](auto W) {
+    dispatch<false, true>(a.mc != nullptr, [&](auto NVLS) {
+      dispatch<false, true>(a.gn != nullptr, [&](auto CLIP) {
+        dispatch<kAccOff, kAccAcc, kAccLast>(acc, [&](auto ACC) {
+          // one rank: only clipping and accumulation launch it (in place, no peer access); never multicast. CLIP with
+          // kAccAcc was rejected above.
+          if constexpr ((W > 1 || ((CLIP || ACC != kAccOff) && !NVLS)) && !(CLIP && ACC == kAccAcc))
+            zero1_reduce_kernel<W, NVLS, CLIP, ACC><<<blocks, threads, 0, stream>>>(a);
+          else
+            throw std::runtime_error(bad_world);
+        });
+      });
+    });
+  });
+  if (!known_world) throw std::runtime_error(bad_world);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-void zero1_commit_launch(const PeerTable& pt, StatusBlock* st, int* gate, uint64_t flag, uint32_t seq, int channel,
-                         int host_ok, int exchange, cudaStream_t stream, const double* const* gn, int nunits,
-                         float max_norm, float* norm) {
-  CommitArgs a{pt, st, gate, flag, seq, channel, host_ok, exchange, {}, 0, 0.f, nullptr};
-  if (gn != nullptr) {
-    if (norm == nullptr || nunits < 1) throw std::runtime_error("zero1_commit: the gradient norm needs units and an output pair");
-    if (!(max_norm > 0.f)) throw std::runtime_error("zero1_commit: max_norm must be > 0");
-    for (int r = 0; r < pt.world; ++r) {
-      if (gn[r] == nullptr) throw std::runtime_error("zero1_commit: one z1_gnorm pointer per rank");
-      a.gn[r] = gn[r];
-    }
-    a.nunits = nunits;
-    a.max_norm = max_norm;
-    a.norm = norm;
+void zero1_commit_launch(const CommitArgs& a, cudaStream_t stream) {
+  if (std::any_of(a.gn, a.gn + a.pt.world, [](const double* p) { return p != nullptr; })) {
+    if (a.norm == nullptr || a.nunits < 1) throw std::runtime_error("zero1_commit: the gradient norm needs units and an output pair");
+    if (!(a.max_norm > 0.f)) throw std::runtime_error("zero1_commit: max_norm must be > 0");
+    if (std::count(a.gn, a.gn + a.pt.world, nullptr) != 0) throw std::runtime_error("zero1_commit: one z1_gnorm pointer per rank");
   }
   zero1_commit_kernel<<<1, 32, 0, stream>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-void zero1_update_launch(const PeerTable& pt, void* mc_base, const int* gate, size_t poff, const void* grad, float* master,
-                         void* m, void* v, size_t nelem, float lr, float b1, float b2, float eps, float wd,
-                         int replication, int mode, int blocks, int threads, cudaStream_t stream, const int* table,
-                         size_t soff, int page_shift, const float* coef, const float* lr_tab, int lr_steps,
-                         int n_no_decay, const size_t* no_decay, int moment_dtype) {
+void zero1_update_launch(UpdArgs a, int moment_dtype, int blocks, int threads, cudaStream_t stream) {
   check_grid(blocks, threads, "zero1_update");
   if (moment_dtype != kF32 && moment_dtype != kBF16) throw std::runtime_error("zero1_update: moments are fp32 or bf16");
-  const bool bf16m = moment_dtype == kBF16;
-  if (((reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15) || (bf16m && (soff & 7)))
+  if (((reinterpret_cast<uintptr_t>(a.m) | reinterpret_cast<uintptr_t>(a.v)) & 15) || (moment_dtype == kBF16 && (a.soff & 7)))
     throw std::runtime_error("zero1_update: m and v must be 16 B aligned (bf16 moments: and the unit's first element a multiple of 8)");
-  if ((poff & 15) || (nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
-  if (table != nullptr && (page_shift < 3 || page_shift > 30 || (soff & 7)))
+  if ((a.poff & 15) || (a.nelem & 7)) throw std::runtime_error("zero1_update: unit must be 16 B aligned and a multiple of 8 elements");
+  if (a.table != nullptr && (a.page_shift < 3 || a.page_shift > 30 || (a.soff & 7)))
     throw std::runtime_error("zero1_update: pages must be 2^3 .. 2^30 elements and the unit 8-element aligned");
-  if (lr_tab != nullptr && (lr_steps < 1 || (reinterpret_cast<uintptr_t>(lr_tab) & 3)))
+  if (a.lr_tab != nullptr && (a.lr_steps < 1 || (reinterpret_cast<uintptr_t>(a.lr_tab) & 3)))
     throw std::runtime_error("zero1_update: a learning-rate table needs lr_steps >= 1 and 4 B alignment");
-  if (n_no_decay < 0 || n_no_decay > kMaxNoDecay || (n_no_decay > 0 && no_decay == nullptr))
+  if (a.lr_tab == nullptr) a.lr_steps = 0;
+  if (a.n_nd < 0 || a.n_nd > kMaxNoDecay)
     throw std::runtime_error("zero1_update: at most " + std::to_string(kMaxNoDecay) + " weight-decay exemptions per unit");
-  UpdArgs a{pt, reinterpret_cast<char*>(mc_base), gate, poff, reinterpret_cast<const bf16*>(grad), master, m, v,
-            nelem, lr, b1, b2, eps, wd, replication, mode, table, soff, page_shift, coef, lr_tab, lr_tab != nullptr ? lr_steps : 0,
-            n_no_decay, {}, {}};
-  for (int r = 0; r < n_no_decay; ++r) {
-    const size_t lo = no_decay[2 * r], hi = no_decay[2 * r + 1];
-    if ((lo & 7) || (hi & 7) || lo >= hi || hi > nelem)
+  for (int r = 0; r < a.n_nd; ++r) {
+    const size_t lo = a.nd_lo[r], hi = a.nd_hi[r];
+    if ((lo & 7) || (hi & 7) || lo >= hi || hi > a.nelem)
       throw std::runtime_error("zero1_update: weight-decay exemptions must be non-empty 8-element aligned ranges inside the unit");
     a.nd_lo[r] = lo / 8;
     a.nd_hi[r] = hi / 8;
   }
-  if (table != nullptr) {
-    if (mc_base != nullptr)
-      launch_upd<true, true>(a, bf16m, blocks, threads, stream);
-    else
-      launch_upd<false, true>(a, bf16m, blocks, threads, stream);
-  } else if (mc_base != nullptr) {
-    launch_upd<true, false>(a, bf16m, blocks, threads, stream);
-  } else {
-    launch_upd<false, false>(a, bf16m, blocks, threads, stream);
-  }
+  const bool known_world = dispatch<1, 2, 3, 4, 5, 6, 7, 8>(a.pt.world, [&](auto W) {
+    dispatch<false, true>(a.mc != nullptr, [&](auto NVLS) {
+      dispatch<false, true>(a.table != nullptr, [&](auto PAGED) {
+        dispatch<false, true>(a.coef != nullptr, [&](auto CLIP) {
+          dispatch<kF32, kBF16>(moment_dtype, [&](auto MD) {
+            // one rank pushes to nobody: never multicast
+            using MT = std::conditional_t<MD == kBF16, bf16, float>;
+            zero1_update_kernel<W, (W > 1 && NVLS), PAGED, CLIP, MT><<<blocks, threads, 0, stream>>>(a);
+          });
+        });
+      });
+    });
+  });
+  if (!known_world) throw std::runtime_error("zero1_update: world size must be in [1, 8]");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -781,6 +781,8 @@ class SymmetricComm:
         self._p2p(False, t, src, stream)
 
     # ------------------------------------------------------------------ FT-ZeRO-1 (csrc/kernels/zero1.cu)
+    # The _K.zero1_* calls pass their arguments positionally, in the field order of the kernel's argument struct
+    # (csrc/kernels/zero1.cuh): pybind11 resolves each keyword by interning its name, several microseconds per update.
     def peer_pointers(self, name: str) -> List[int]:
         """Mapped base address of segment ``name`` on every quorum rank (index = rank)."""
         return list(self._ptrs[name])
@@ -827,12 +829,6 @@ class SymmetricComm:
         bf16 and store like mode 0; ``gnorm`` allowed). Modes 1 and 2 leave the gradient segment untouched and push
         nothing. The handshakes are the same in every mode; the trailing one is what lets the peers overwrite their
         gradients with the next micro-batch. At world 1 every mode but 0 is one launch with no handshake."""
-        if acc_mode not in (0, 1, 2, 3):
-            raise ValueError(f"acc_mode must be 0 (off), 1 (first), 2 (middle) or 3 (last), got {acc_mode}")
-        if acc_mode and not acc:
-            raise ValueError("gradient accumulation needs the accumulator's device address")
-        if acc_mode in (1, 2) and gnorm:
-            raise ValueError("the gradient norm is taken on the last micro-batch only (acc_mode 3)")
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -841,23 +837,15 @@ class SymmetricComm:
                 # healing / spare replica: its gradients count as zeros (reference manager.py:441-442)
                 self._K.memset_async(self._segments[segment].ptr + off, 0, nelem * 2, sp)
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
-            if gnorm or acc_mode:
-                scratch, ticket = self._z1_norm_scratch_ptrs() if gnorm else (0, 0)
-                one = self._world == 1
-                if not one:
-                    self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
-                self._K.zero1_reduce(self._tables[segment], self._z1_ok(2 if one else 0), self._mc_base(segment, nelem * 2),
-                                     off, nelem, scale, replication, blocks, self._threads, sp, gnorm, scratch, ticket,
-                                     acc if acc_mode else 0, acc_mode)
-                self.launches += 1
-                if not one:
-                    self._handshake(0, True, _CH_ALLREDUCE, sp)
-                return
-            self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
-            self._K.zero1_reduce(self._tables[segment], self._z1_ok(0), self._mc_base(segment, nelem * 2), off, nelem, scale,
-                                 replication, blocks, self._threads, sp)
+            scratch, ticket = self._z1_norm_scratch_ptrs() if gnorm else (0, 0)
+            one = self._world == 1
+            if not one:
+                self._handshake(0, not contribute, _CH_ALLREDUCE, sp)
+            self._K.zero1_reduce(self._tables[segment], self._z1_ok(2 if one else 0), self._mc_base(segment, nelem * 2), off,
+                                 nelem, scale, replication, gnorm, scratch, ticket, acc, acc_mode, blocks, self._threads, sp)
             self.launches += 1
-            self._handshake(0, True, _CH_ALLREDUCE, sp)
+            if not one:
+                self._handshake(0, True, _CH_ALLREDUCE, sp)
 
     def zero1_commit_(self, gate: torch.Tensor, host_ok: bool, exchange: bool,
                       stream: Optional[torch.cuda.Stream] = None, gnorm: Optional[str] = None, nunits: int = 0,
@@ -877,12 +865,9 @@ class SymmetricComm:
             seq = self._commit_seq
             if gnorm is not None:
                 assert norm is not None and norm.dtype == torch.float32 and norm.numel() >= 2
-                self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
-                                     bool(host_ok), bool(exchange), _native.stream_ptr(stream), self._ptrs[gnorm],
-                                     int(nunits), float(max_norm), norm.data_ptr())
-            else:
-                self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
-                                     bool(host_ok), bool(exchange), _native.stream_ptr(stream))
+            self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
+                                 bool(host_ok), bool(exchange), self._ptrs[gnorm] if gnorm is not None else [], int(nunits),
+                                 float(max_norm), norm.data_ptr() if norm is not None else 0, _native.stream_ptr(stream))
             self.launches += 1
             return seq
 
@@ -915,17 +900,6 @@ class SymmetricComm:
         ``moment_dtype`` ``torch.bfloat16``: ``m`` and ``v`` point at bf16 arrays, stored with stochastic rounding whose
         bits depend only on the global element index ``state_off + i``, the device step count and the moment; flat
         state then passes the unit's first element as ``state_off`` too."""
-        if moment_dtype not in (torch.float32, torch.bfloat16):
-            raise ValueError(f"the moments are fp32 or bf16, got {moment_dtype}")
-        if lr_table and lr_steps < 1:
-            raise ValueError(f"a learning-rate table needs lr_steps >= 1, got {lr_steps}")
-        nd = [(int(lo), int(hi)) for lo, hi in no_decay]
-        if len(nd) > self._K.ZERO1_MAX_NO_DECAY:
-            raise ValueError(f"at most {self._K.ZERO1_MAX_NO_DECAY} weight-decay exemptions per unit, got {len(nd)}")
-        for lo, hi in nd:
-            if lo % 8 or hi % 8 or not 0 <= lo < hi <= nelem:
-                raise ValueError(f"weight-decay exemption [{lo}, {hi}) is not an 8-element aligned range of the unit "
-                                 f"of {nelem} elements")
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -933,9 +907,9 @@ class SymmetricComm:
             sp = _native.stream_ptr(stream)
             blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
-                                 m, v, nelem, lr, b1, b2, eps, wd, replication, mode, blocks, self._threads, sp,
-                                 table, state_off, page_shift, coef, lr_table, lr_steps if lr_table else 0,
-                                 [x for r in nd for x in r], _native.DTYPE_CODE[moment_dtype])
+                                 m, v, nelem, lr, b1, b2, eps, wd, replication, mode, table, state_off, page_shift, coef,
+                                 lr_table, lr_steps, [int(x) for lo, hi in no_decay for x in (lo, hi)],
+                                 _native.DTYPE_CODE[moment_dtype], blocks, self._threads, sp)
             self.launches += 1
             pushes = self._world > 1 and (mode == 1 or self._world > replication)
             if pushes:
