@@ -38,6 +38,11 @@ power limit. It reports medians, spread and the bytes the launch moves, computed
 2 (gradient) + 8 (master in and out) + 2 (weight) + 4 x the moment size, i.e. 28 B with fp32 and 20 B with bf16 moments,
 plus 2 B per primary element and peer the weights are pushed to (local HBM here, NVLink on real ranks).
 
+``--virtual W --ema`` times the update of one unit (rank 0's launch) without and with an EMA of the weights, for fp32
+and for bf16 moments (the EMA has the moments' type), alternating the four arms ``--repeats`` times, on flat state or
+(with ``--compact``) on page pools in slot order, with the card's name and power limit. The EMA adds 2 x its size per
+updated element (read and written): 36 B instead of 28 with fp32 moments, 24 B instead of 20 with bf16.
+
 Per unit of S bytes of bf16 gradients and W ranks with k holders per slice, each rank moves over NVLink:
   reduce-scatter  in  (W-1)/W * S      (+ (k-1)/W * S out for the buddy push)
   update          out (W-1)/W * S      (bf16 weights to every peer)        [NVLS: S/W in, S/W out]
@@ -326,6 +331,79 @@ def moments_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats, paged, shift=
     return out
 
 
+def ema_ab(comm, nelem, k, upd_blocks, iters, warmup, repeats, paged, shift=16):
+    """The update of one unit without and with an EMA of the weights, for fp32 and for bf16 moments (the EMA takes the
+    moments' type), the four arms timed alternately, on flat state or on page pools in slot order. Before timing, one
+    launch of each pair from the same state must give the same weights: the EMA does not change the update."""
+    from torchft_b200.parallel.zero1 import ema_coefficient
+
+    upd_blocks = upd_blocks or comm._K.NUM_SMS * 16
+    dev = comm.device
+    grad = comm.segment("z1_grad")[: nelem * 2].view(torch.bfloat16)
+    grad.normal_()
+    gate = torch.ones(2, dtype=torch.int32, device=dev)
+    npages = (nelem + (1 << shift) - 1) >> shift
+    n_state = npages << shift if paged else nelem
+    table = torch.arange(npages, dtype=torch.int32, device=dev)
+    paging = dict(table=table.data_ptr(), page_shift=shift) if paged else {}
+    c = ema_coefficient(0.999)
+    init = torch.randn(n_state, device=dev)
+
+    def state(dtype):
+        return [init.clone(), torch.zeros(n_state, device=dev, dtype=dtype), torch.zeros(n_state, device=dev, dtype=dtype),
+                init.to(dtype)]
+
+    def launch(st, dtype, ema):
+        kw = dict(ema=st[3].data_ptr(), ema_c=c) if ema else {}
+        return lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), st[0].data_ptr(), st[1].data_ptr(),
+                                          st[2].data_ptr(), nelem, HP, gate, k, 0, upd_blocks, moment_dtype=dtype,
+                                          **paging, **kw)
+
+    arms, same = {}, {}
+    for name, dtype in (("fp32", torch.float32), ("bf16", torch.bfloat16)):
+        off, on = state(dtype), state(dtype)
+        launch(off, dtype, False)()
+        launch(on, dtype, True)()
+        torch.cuda.synchronize()
+        same[name] = torch.equal(off[0], on[0])
+        assert same[name], f"{name} moments: the update with an EMA computed other weights than the one without"
+        arms[f"{name}_off"], arms[f"{name}_ema"] = launch(off, dtype, False), launch(on, dtype, True)
+    times = {name: [] for name in arms}
+    for _ in range(repeats):
+        for name, fn in arms.items():
+            for _ in range(warmup):
+                fn()
+            torch.cuda.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            torch.cuda.synchronize()
+            times[name].append(s.elapsed_time(e) / iters)
+    assert comm.errored() is None
+    W, kk = comm.world, min(k, comm.world)
+    nvec = nelem // 8
+    per = (nvec + W - 1) // W
+    primary = 8 * min(per, nvec)
+    updated = sum(8 * (min((s + 1) * per, nvec) - min(s * per, nvec)) for s in {(0 - j) % W for j in range(kk)})
+    out = {"timing": "local HBM (virtual ranks), not NVLink", "state": "paged_ordered" if paged else "flat",
+           "first_update_weights_equal": same, "elements_updated": updated, "pushed_bytes": 2 * primary * (W - kk)}
+    for name, ts in times.items():
+        ts = sorted(ts)
+        msize = 2 if name.startswith("bf16") else 4
+        per_elem = 2 + 8 + 2 + 4 * msize + (2 * msize if name.endswith("ema") else 0)  # the EMA is read and written
+        moved = per_elem * updated + out["pushed_bytes"]
+        out[f"adamw_allgather_{name}"] = {
+            "ms": {"median": round(ts[len(ts) // 2], 4), "min": round(ts[0], 4), "max": round(ts[-1], 4)},
+            "state_bytes_per_element": per_elem, "bytes_moved": moved,
+            "gb_per_s_at_median": round(moved / ts[len(ts) // 2] / 1e6, 1)}
+    for name in ("fp32", "bf16"):
+        out[f"{name}_ema_over_off"] = round(out[f"adamw_allgather_{name}_ema"]["ms"]["median"]
+                                            / out[f"adamw_allgather_{name}_off"]["ms"]["median"], 4)
+    return out
+
+
 def accum_ab(comms, nelem, k, rs_blocks, iters, warmup, repeats):
     """Rank 0's reduce-scatter of one unit in the three accumulation modes, timed alternately: ``off`` (today's launch),
     ``acc`` (a middle micro-batch: fp32 rank sum added into the accumulator) and ``last`` (accumulator + rank sum,
@@ -407,8 +485,10 @@ def main() -> None:
                     "table and weight-decay exemptions")
     ap.add_argument("--moments", action="store_true", help="--virtual: A/B the update with fp32 and bf16 moments "
                     "(with --compact: on paged state)")
-    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum / --sched / --moments: alternations "
-                    "of the arms")
+    ap.add_argument("--ema", action="store_true", help="--virtual: A/B the update without and with an EMA of the weights, "
+                    "for fp32 and bf16 moments (with --compact: on paged state)")
+    ap.add_argument("--repeats", type=int, default=5, help="--compact / --clip / --accum / --sched / --moments / --ema: "
+                    "alternations of the arms")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     nelem = int(a.mb * (1 << 20)) // 2 // 4096 * 4096
@@ -419,8 +499,10 @@ def main() -> None:
         segments = {"z1_grad": S, "z1_param": S, **({"z1_gnorm": 8} if a.clip else {})}
         comms = SymmetricComm.virtual_world(a.virtual, segments, presignal=True)
         res = {"mode": f"virtual{a.virtual}", "unit_mb": S / 2**20}
-        if a.compact or a.clip or a.accum or a.sched or a.moments:
-            if a.moments:
+        if a.compact or a.clip or a.accum or a.sched or a.moments or a.ema:
+            if a.ema:
+                res.update(ema_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats, a.compact))
+            elif a.moments:
                 res.update(moments_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats, a.compact))
             elif a.compact:
                 res.update(compact_ab(comms[0], nelem, a.replication, a.upd_blocks, a.iters, a.warmup, a.repeats))

@@ -10,7 +10,8 @@ File ``z1_step_{T}.w{W}.r{r}.bin``::
 
 The payload holds four arrays over the ``elements`` written elements, back to back: ``param`` (bf16), ``master``,
 ``m`` and ``v`` (fp32; bf16 when the header says ``"moments": "bf16"``, a file without the key has fp32 moments), at the
-byte offsets ``sections`` gives relative to the payload start. Each written range
+byte offsets ``sections`` gives relative to the payload start. A file written with an EMA of the weights has
+``"ema": {"decay": d}`` in its header and a fifth array ``ema`` of the moments' type behind ``v``. Each written range
 ``[lo, hi)`` of the flat vector is stored at element offset ``off`` of every array (``ranges``: ``[lo, hi, off]``).
 Ranges are multiples of 8 elements, so every array and every range in it starts 16-byte aligned. The payload is read
 with ranged ``pread`` calls only, never loaded whole.
@@ -45,13 +46,15 @@ def file_name(step: int, world: int, rank: int) -> str:
     return f"z1_step_{step}.w{world}.r{rank}.bin"
 
 
-def sections(elements: int, moment_size: int = 4) -> Dict[str, int]:
+def sections(elements: int, moment_size: int = 4, ema: bool = False) -> Dict[str, int]:
     """Byte offset of each array in the payload of a file holding ``elements`` elements: 14 bytes each with fp32
-    moments, 10 with bf16 moments (``moment_size`` 2)."""
+    moments, 10 with bf16 moments (``moment_size`` 2), and ``moment_size`` more for the ``ema`` section."""
     out, at = {}, 0
     for name, size in _ITEM.items():
         out[name] = at
         at += (moment_size if name in ("m", "v") else size) * elements
+    if ema:
+        out["ema"] = at
     return out
 
 
@@ -65,13 +68,13 @@ def moment_size(header: Dict[str, Any]) -> int:
 
 def file_dtype(header: Dict[str, Any], array: str) -> torch.dtype:
     """The dtype ``array`` is stored in."""
-    if array in ("m", "v"):
+    if array in ("m", "v", "ema"):
         return torch.bfloat16 if moment_size(header) == 2 else torch.float32
     return torch.bfloat16 if array == "param" else torch.float32
 
 
 def payload_bytes(header: Dict[str, Any]) -> int:
-    return (6 + 2 * moment_size(header)) * int(header["elements"])
+    return (6 + (3 if "ema" in header else 2) * moment_size(header)) * int(header["elements"])
 
 
 def encode_header(header: Dict[str, Any]) -> bytes:

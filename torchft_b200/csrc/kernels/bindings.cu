@@ -169,6 +169,7 @@ PYBIND11_MODULE(_K, m) {
   m.attr("Q8_GROUP") = 512;
   m.attr("ZERO1_MAX_NO_DECAY") = kMaxNoDecay;
   m.attr("ZERO1_BF16_MOMENTS") = true;  // zero1_update takes moment_dtype = bf16
+  m.attr("ZERO1_EMA") = true;           // zero1_update takes an EMA of the weights and mode 2
 
   py::class_<Status>(m, "Status")
       .def(py::init<>())
@@ -293,7 +294,8 @@ PYBIND11_MODULE(_K, m) {
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,
          uintptr_t v, size_t nelem, float lr, float b1, float b2, float eps, float wd, int replication, int mode,
          uintptr_t table, size_t soff, int page_shift, uintptr_t coef, uintptr_t lr_tab, int lr_steps,
-         const std::vector<size_t>& no_decay, int moment_dtype, int blocks, int threads, uintptr_t stream) {
+         const std::vector<size_t>& no_decay, int moment_dtype, uintptr_t ema, float ema_c, int blocks, int threads,
+         uintptr_t stream) {
         if (no_decay.size() & 1) throw std::runtime_error("zero1_update: no_decay is a flat list of (lo, hi) pairs");
         zero1::UpdArgs a{};
         a.pt = pt.pt;
@@ -323,13 +325,15 @@ PYBIND11_MODULE(_K, m) {
           a.nd_lo[r] = no_decay[2 * r];
           a.nd_hi[r] = no_decay[2 * r + 1];
         }
+        a.ema = P<void>(ema);
+        a.ema_c = ema_c;
         zero1_update_launch(a, moment_dtype, blocks, threads, S(stream));
       },
       py::arg("pt"), py::arg("mc_base"), py::arg("gate"), py::arg("poff"), py::arg("grad"), py::arg("master"),
       py::arg("m"), py::arg("v"), py::arg("nelem"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"),
       py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("table"), py::arg("soff"), py::arg("page_shift"),
       py::arg("coef"), py::arg("lr_tab"), py::arg("lr_steps"), py::arg("no_decay"), py::arg("moment_dtype"),
-      py::arg("blocks"), py::arg("threads"), py::arg("stream"));
+      py::arg("ema"), py::arg("ema_c"), py::arg("blocks"), py::arg("threads"), py::arg("stream"));
 
   m.def(
       "push_exchange",

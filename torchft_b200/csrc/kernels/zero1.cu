@@ -43,6 +43,10 @@
 // that are a pure function of (global element index, gate[1], which moment), so every holder of a slice stores the
 // same bits at any grid size, world and paging.
 //
+// EMA of the weights (opt-in, EMA template flag / non-null ema): the holders of a slice also keep a moving average of
+// the new fp32 master weights, of the moments' type (bf16: rounded stochastically with bits of their own), advanced by
+// every committed update; mode 2 broadcasts bf16(EMA) of the primary slices into every replica's parameter buffer.
+//
 // The two big kernels contain NO inter-rank synchronisation at all: any grid size, no co-residency requirement, no
 // SM held by a spinning CTA while peers are skewed, profilable stand-alone. Ordering comes from the one-CTA handshake
 // kernels around them (bounded, abortable spins; epoch-tagged flags; error latched in the status block and mirrored
@@ -379,6 +383,18 @@ __device__ __forceinline__ uint32_t sr_bits(uint64_t e, uint32_t t) {
   return x;
 }
 
+// The bits of a bf16 EMA (low half): the same mix and finaliser with another seed, so element e's EMA is not rounded
+// with the bits that round its moments. parallel/zero1.py (sr_bits_ema) is the specification.
+__device__ __forceinline__ uint32_t sr_bits_ema(uint64_t e, uint32_t t) {
+  uint32_t x = (uint32_t)e * 0x9E3779B1u + (uint32_t)(e >> 32) * 0x85EBCA77u + t * 0xC2B2AE3Du + 0x165667B1u;
+  x ^= x >> 16;
+  x *= 0x85EBCA6Bu;
+  x ^= x >> 13;
+  x *= 0xC2B2AE35u;
+  x ^= x >> 16;
+  return x;
+}
+
 // fp32 -> bf16 bits: add the 16-bit r to the fp32 bits and keep the upper half. The add is on the magnitude, so it
 // rounds away from zero with probability (discarded fraction), which is unbiased for both signs; a value bf16
 // represents exactly comes back unchanged for every r. Inf and NaN are not added to; a NaN keeps a mantissa bit.
@@ -391,11 +407,12 @@ __device__ __forceinline__ uint32_t bf16_sr(float x, uint32_t r) {
 // ---------------------------------------------------------------------------
 // Gated AdamW on the held slices + all-gather of the new bf16 weights (no synchronisation).
 // ---------------------------------------------------------------------------
-template <int W, bool NVLS, bool PAGED, bool CLIP, typename MT>
+template <int W, bool NVLS, bool PAGED, bool CLIP, typename MT, bool EMA>
 __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   constexpr bool BF16M = sizeof(MT) == 2;
   MT* const mp = reinterpret_cast<MT*>(a.m);
   MT* const vp = reinterpret_cast<MT*>(a.v);
+  MT* const ep = reinterpret_cast<MT*>(a.ema);  // EMA: the moving average, of the moments' type
   if (a.mode == 0 && a.gate[0] == 0) return;  // uniform over the grid AND (unanimous verdict) over the quorum
   const int rank = a.pt.rank;
   const Geo g(a.nelem, W);
@@ -442,11 +459,15 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
         if (v + nthreads < hi) slot = __ldg(a.table + ((a.soff + (v + nthreads) * 8) >> a.page_shift));
       }
       float w[8];
-      const Vec16 w0 = ld_stream(a.master + si), w1 = ld_stream(a.master + si + 4);
+      Vec16 w0, w1;
+      if (!EMA || a.mode != 2) {  // mode 2 reads the EMA instead
+        w0 = ld_stream(a.master + si);
+        w1 = ld_stream(a.master + si + 4);
+      }
       if (a.mode == 0) {
-        // all 7 x 16 B loads (5 with bf16 moments) in flight before any use
+        // all 7 x 16 B loads (5 with bf16 moments; EMA: 2 more, 1 in bf16) in flight before any use
         const Vec16 gv = ld_stream(a.grad + v * 8);
-        Vec16 m0, m1, v0, v1;
+        Vec16 m0, m1, v0, v1, e0, e1;
         if constexpr (BF16M) {
           m0 = ld_stream(mp + si);
           v0 = ld_stream(vp + si);
@@ -455,6 +476,10 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
           m1 = ld_stream(mp + si + 4);
           v0 = ld_stream(vp + si);
           v1 = ld_stream(vp + si + 4);
+        }
+        if constexpr (EMA) {
+          e0 = ld_stream(ep + si);
+          if constexpr (!BF16M) e1 = ld_stream(ep + si + 4);
         }
         float gr[8], m[8], vv[8];
         P8::unpack(gv, gr);
@@ -507,6 +532,38 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
           st_stream(mp + si + 4, Pack<float>::pack(m + 4));
           st_stream(vp + si, Pack<float>::pack(vv));
           st_stream(vp + si + 4, Pack<float>::pack(vv + 4));
+        }
+        if constexpr (EMA) {
+          // ema + c * (w' - ema), each operation rounded on its own (no FMA): what numpy float32 computes
+          float e[8];
+          if constexpr (BF16M) {
+            P8::unpack(e0, e);
+          } else {
+            Pack<float>::unpack(e0, e);
+            Pack<float>::unpack(e1, e + 4);
+          }
+#pragma unroll
+          for (int i = 0; i < 8; ++i) e[i] = __fadd_rn(e[i], __fmul_rn(a.ema_c, __fsub_rn(w[i], e[i])));
+          if constexpr (BF16M) {
+            const uint64_t x0 = a.soff + v * 8;
+            uint32_t eo[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+              eo[i] = bf16_sr(e[2 * i], sr_bits_ema(x0 + 2 * i, (uint32_t)t) & 0xffffu) |
+                      (bf16_sr(e[2 * i + 1], sr_bits_ema(x0 + 2 * i + 1, (uint32_t)t) & 0xffffu) << 16);
+            st_stream(ep + si, Vec16{eo[0], eo[1], eo[2], eo[3]});
+          } else {
+            st_stream(ep + si, Pack<float>::pack(e));
+            st_stream(ep + si + 4, Pack<float>::pack(e + 4));
+          }
+        }
+      } else if (EMA && a.mode == 2) {
+        // fp32 EMA: rounded to nearest by the pack below; a bf16 EMA comes back with its own bits
+        if constexpr (BF16M) {
+          P8::unpack(ld_stream(ep + si), w);
+        } else {
+          Pack<float>::unpack(ld_stream(ep + si), w);
+          Pack<float>::unpack(ld_stream(ep + si + 4), w + 4);
         }
       } else {
         Pack<float>::unpack(w0, w);
@@ -600,6 +657,10 @@ void zero1_update_launch(UpdArgs a, int moment_dtype, int blocks, int threads, c
   if (a.lr_tab != nullptr && (a.lr_steps < 1 || (reinterpret_cast<uintptr_t>(a.lr_tab) & 3)))
     throw std::runtime_error("zero1_update: a learning-rate table needs lr_steps >= 1 and 4 B alignment");
   if (a.lr_tab == nullptr) a.lr_steps = 0;
+  if (a.mode < 0 || a.mode > 2) throw std::runtime_error("zero1_update: mode is 0 (update), 1 (refresh) or 2 (EMA broadcast)");
+  if (a.mode == 2 && a.ema == nullptr) throw std::runtime_error("zero1_update: mode 2 broadcasts the EMA and needs one");
+  if (a.ema != nullptr && ((reinterpret_cast<uintptr_t>(a.ema) & 15) || !(a.ema_c > 0.f && a.ema_c < 1.f)))
+    throw std::runtime_error("zero1_update: the EMA must be 16 B aligned and its coefficient 1 - decay in (0, 1)");
   if (a.n_nd < 0 || a.n_nd > kMaxNoDecay)
     throw std::runtime_error("zero1_update: at most " + std::to_string(kMaxNoDecay) + " weight-decay exemptions per unit");
   for (int r = 0; r < a.n_nd; ++r) {
@@ -614,9 +675,11 @@ void zero1_update_launch(UpdArgs a, int moment_dtype, int blocks, int threads, c
       dispatch<false, true>(a.table != nullptr, [&](auto PAGED) {
         dispatch<false, true>(a.coef != nullptr, [&](auto CLIP) {
           dispatch<kF32, kBF16>(moment_dtype, [&](auto MD) {
-            // one rank pushes to nobody: never multicast
-            using MT = std::conditional_t<MD == kBF16, bf16, float>;
-            zero1_update_kernel<W, (W > 1 && NVLS), PAGED, CLIP, MT><<<blocks, threads, 0, stream>>>(a);
+            dispatch<false, true>(a.ema != nullptr, [&](auto EMA) {
+              // one rank pushes to nobody: never multicast
+              using MT = std::conditional_t<MD == kBF16, bf16, float>;
+              zero1_update_kernel<W, (W > 1 && NVLS), PAGED, CLIP, MT, EMA><<<blocks, threads, 0, stream>>>(a);
+            });
           });
         });
       });

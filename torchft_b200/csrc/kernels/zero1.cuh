@@ -79,7 +79,8 @@ struct UpdArgs {
   size_t nelem;        // elements in the unit (multiple of 8)
   float lr, b1, b2, eps, wd;
   int replication;
-  int mode;            // 0 = gated update + push, 1 = refresh (re-broadcast bf16(master) of the primary slice, ungated)
+  int mode;            // 0 = gated update + push, 1 = refresh (re-broadcast bf16(master) of the primary slice, ungated),
+                       // 2 = the same broadcast of bf16(ema) (needs ema)
   // paged state (table != nullptr): master/m/v are pools of 2^page_shift-element pages (2^3 .. 2^30); element e of the
   // flat vector (e = soff + local index) lives at pool[table[e >> page_shift] << page_shift | (e & (page - 1))]. A page
   // is a multiple of 8 elements, so the two 16-byte vectors of one 8-element group never straddle a page. soff is a
@@ -97,6 +98,13 @@ struct UpdArgs {
   // element ranges, multiples of 8; the launcher checks them and converts them to the 8-element vectors the kernel reads.
   int n_nd;
   size_t nd_lo[kMaxNoDecay], nd_hi[kMaxNoDecay];
+  // exponential moving average of the weights (ema != nullptr; last, so the fields above keep their offsets): 16 B
+  // aligned, of the moment type and indexed like master. Every committed update (mode 0) also stores
+  // ema' = ema + ema_c * (w' - ema) with the new fp32 master w' and ema_c = fp32(1 - decay); a bf16 EMA is rounded
+  // stochastically with bits that depend only on (soff + local element index, gate[1]). Mode 2 is mode 1 with bf16(ema)
+  // in place of bf16(master); the launcher rejects it without an EMA.
+  void* ema;
+  float ema_c;
 };
 
 }  // namespace zero1

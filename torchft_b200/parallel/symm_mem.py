@@ -886,10 +886,12 @@ class SymmetricComm:
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,
                       blocks: int, stream: Optional[torch.cuda.Stream] = None, table: int = 0, state_off: int = 0,
                       page_shift: int = 0, coef: int = 0, lr_table: int = 0, lr_steps: int = 0,
-                      no_decay: Sequence[Tuple[int, int]] = (), moment_dtype: torch.dtype = torch.float32) -> None:
+                      no_decay: Sequence[Tuple[int, int]] = (), moment_dtype: torch.dtype = torch.float32,
+                      ema: int = 0, ema_c: float = 0.0) -> None:
         """Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights into
         ``segment`` on the ranks that do not hold it (``mode`` 1: ungated re-broadcast of bf16(master) to everybody, no
-        state change). A sync-free kernel (any grid) followed by one handshake when anything was pushed.
+        state change; ``mode`` 2: the same with bf16(ema)). A sync-free kernel (any grid) followed by one handshake when
+        anything was pushed.
 
         ``table`` (device pointer to int32 page slots, 0 = flat state) selects paged state: ``master``/``m``/``v`` are
         then page pools and element ``state_off + i`` of the unit lives in pool page ``table[(state_off + i) >> page_shift]``.
@@ -899,7 +901,9 @@ class SymmetricComm:
         ``ZERO1_MAX_NO_DECAY`` unit-relative element ranges, multiples of 8, whose elements get no weight decay.
         ``moment_dtype`` ``torch.bfloat16``: ``m`` and ``v`` point at bf16 arrays, stored with stochastic rounding whose
         bits depend only on the global element index ``state_off + i``, the device step count and the moment; flat
-        state then passes the unit's first element as ``state_off`` too."""
+        state then passes the unit's first element as ``state_off`` too. ``ema`` (device address, 0 = none): an array of
+        the moment type indexed like ``master``; every committed update also stores ``ema + ema_c * (w' - ema)`` with the
+        new fp32 master ``w'`` (bf16: rounded stochastically like the moments, with bits of its own)."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
@@ -909,11 +913,22 @@ class SymmetricComm:
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, table, state_off, page_shift, coef,
                                  lr_table, lr_steps, [int(x) for lo, hi in no_decay for x in (lo, hi)],
-                                 _native.DTYPE_CODE[moment_dtype], blocks, self._threads, sp)
+                                 _native.DTYPE_CODE[moment_dtype], ema, float(ema_c), blocks, self._threads, sp)
             self.launches += 1
-            pushes = self._world > 1 and (mode == 1 or self._world > replication)
+            # modes 1 and 2 broadcast to everybody; an update pushes only to the ranks that do not hold the slice
+            pushes = self._world > 1 and (mode != 0 or self._world > replication)
             if pushes:
                 self._handshake(1, True, _CH_HEAL, sp)
+
+    def zero1_barrier_(self, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """One handshake on the channel of :meth:`zero1_update_`: no kernel enqueued on ``stream`` after it runs before
+        every rank of the quorum has run what it enqueued on its own stream before its call. Every rank calls it at the
+        same point of its sequence of FT-ZeRO-1 launches. Nothing at world 1; the host never waits."""
+        with self._lock:
+            if not self._configured:
+                raise RuntimeError("SymmetricComm is not configured")
+            if self._world > 1:
+                self._handshake(1, True, _CH_HEAL, _native.stream_ptr(stream))
 
     # ------------------------------------------------------------------ status
     def abort(self) -> None:

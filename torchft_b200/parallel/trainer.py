@@ -24,10 +24,11 @@ the full bf16 model and its training state (on an 80 GB H100: up to ~3 B paramet
 
 from __future__ import annotations
 
+import contextlib
 import dataclasses
 import os
 from datetime import timedelta
-from typing import Any, Callable, Dict, List, Optional, Tuple
+from typing import Any, Callable, Dict, Iterator, List, Optional, Tuple
 
 import torch
 from torch import nn
@@ -84,6 +85,10 @@ class FaultTolerantTrainer:
         moment_dtype: FT-ZeRO-1: ``torch.bfloat16`` keeps the AdamW moments in bf16 (8 instead of 12 bytes of optimizer
             state per parameter), rounded stochastically so that the holders of a slice stay bit-identical; ``None``:
             env ``TORCHFT_B200_Z1_MOMENTS=bf16``, unset = fp32. Not available on the classic all-reduce pipeline.
+        ema_decay: FT-ZeRO-1: keep an exponential moving average of the fp32 master weights with this decay, as
+            partitioned optimizer state of the moments' type, advanced by every committed update (``None``: env
+            ``TORCHFT_B200_Z1_EMA_DECAY``, unset = no EMA). :meth:`ema_weights` evaluates it. Not available on the
+            classic all-reduce pipeline.
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -100,7 +105,7 @@ class FaultTolerantTrainer:
                  grad_accum_steps: int = 1, lr_lambda: Optional[Callable[[int], float]] = None,
                  lr_steps: Optional[int] = None,
                  no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None,
-                 moment_dtype: Optional[torch.dtype] = None) -> None:
+                 moment_dtype: Optional[torch.dtype] = None, ema_decay: Optional[float] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -124,6 +129,9 @@ class FaultTolerantTrainer:
             raise ValueError("lr_lambda and no_decay need the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         if moment_dtype is not None and not self.zero1:
             raise ValueError("moment_dtype needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if ema_decay is not None and not self.zero1:
+            raise ValueError("ema_decay needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        self._in_ema = False  # inside ema_weights(): the model holds the EMA weights
         if lr_lambda is not None and lr_steps is None:
             raise ValueError("lr_lambda needs lr_steps, the length of the schedule")
         self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
@@ -155,7 +163,7 @@ class FaultTolerantTrainer:
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
                                        compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
                                        grad_accum_steps=self.grad_accum_steps, lr_lambda=lr_lambda,
-                                       lr_steps=lr_steps or 0, moment_dtype=moment_dtype)
+                                       lr_steps=lr_steps or 0, moment_dtype=moment_dtype, ema_decay=ema_decay)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:
@@ -300,6 +308,7 @@ class FaultTolerantTrainer:
     def step_device(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
         """One fault-tolerant optimisation step on device-resident inputs; returns the loss tensor (device). With
         ``grad_accum_steps = M`` the inputs are ``(M * B, S)`` and the loss is the mean over the ``M`` micro-batches."""
+        self._not_in_ema("step")
         self._steps_run += 1
         if self.zero1 and self.grad_accum_steps > 1:
             return self._step_accumulate(tokens, targets)
@@ -363,6 +372,7 @@ class FaultTolerantTrainer:
 
     def step(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor) -> float:
         """End-to-end step: pinned-host inputs -> H2D -> train step -> D2H loss (blocks until the loss is on the host)."""
+        self._not_in_ema("step")
         self._stage_inputs(tokens_cpu, targets_cpu)
         loss = self.step_device(self._tok, self._tgt)
         return float(loss.item())
@@ -372,6 +382,7 @@ class FaultTolerantTrainer:
         of ITS loss into pinned memory, and returns the PREVIOUS step's loss (``None`` on the first call). The host
         never waits for the step it just launched, so the GPU queue stays full; every step still performs its
         H2D input copy and its D2H loss read."""
+        self._not_in_ema("step_async")
         prev: Optional[float] = None
         if self._loss_event is not None:
             self._loss_event.synchronize()
@@ -399,6 +410,7 @@ class FaultTolerantTrainer:
         the same step. The copy to host memory runs under the next step's forward and backward; the file is written by
         a background thread (:meth:`wait_checkpoint`). The ``keep`` newest steps this replica wrote are kept."""
         self._require_zero1_ckpt()
+        self._not_in_ema("save_checkpoint")
         ms = self.manager.state_dict()  # settles the last step's deferred verdict: the host learns T, no other sync
         assert ms["step"] == self.zopt.t, (ms, self.zopt.t)
         return self.zopt.save(directory, ms, self._opt_events, keep)
@@ -421,6 +433,28 @@ class FaultTolerantTrainer:
             return None
         self.manager.load_state_dict(ms)
         return int(ms["step"])
+
+    # ----------------------------------------------------- EMA of the weights (FT-ZeRO-1)
+    @contextlib.contextmanager
+    def ema_weights(self) -> Iterator[None]:
+        """Evaluate the EMA of the weights: inside the context ``self.model`` holds bf16(EMA) (e.g. ``with
+        torch.no_grad(): trainer.model(tokens)``); on exit it holds the training weights again, bit for bit. Every
+        replica enters after the same step. :meth:`step`, :meth:`step_device`, :meth:`step_async` and
+        :meth:`save_checkpoint` raise inside it."""
+        if self.zopt is None or self.zopt.ema is None:
+            raise RuntimeError("ema_weights needs the FT-ZeRO-1 pipeline with an ema_decay")
+        self._not_in_ema("ema_weights")
+        self.join()  # the last step's update has finished before its EMA is read
+        with self.zopt.ema_weights():
+            self._in_ema = True
+            try:
+                yield
+            finally:
+                self._in_ema = False
+
+    def _not_in_ema(self, what: str) -> None:
+        if self._in_ema:
+            raise RuntimeError(f"{what} inside ema_weights(): the model holds the EMA weights, not the training weights")
 
     def last_grad_norm(self) -> Optional[float]:
         """Global gradient norm of the most recently resolved step (FT-ZeRO-1 with clipping; ``None`` otherwise). Steps

@@ -27,13 +27,14 @@ different weights for more than one (discarded or slightly stale) step.
 
 from __future__ import annotations
 
+import contextlib
 import json
 import logging
 import math
 import os
 import threading
 from dataclasses import dataclass
-from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -44,13 +45,16 @@ Range = Tuple[int, int]
 __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "intersect_ranges", "plan_pulls",
            "plan_reshard", "reshard_pages", "reshard_page_steps", "RankPlan", "plan_quorum", "backed_ranges", "pool_pages", "page_ranges",
            "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan",
-           "lr_schedule_table", "split_no_decay", "schedule_digest", "check_moment_agreement", "moment_type", "sr_bits", "bf16_sr"]
+           "lr_schedule_table", "split_no_decay", "schedule_digest", "check_moment_agreement", "moment_type", "sr_bits", "bf16_sr",
+           "sr_bits_ema", "bf16_sr_ema", "ema_decay_value", "ema_coefficient", "ema_step", "ema_record", "check_ema_agreement",
+           "split_ema_reads"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 CONVERT_CHUNK = 1 << 24  # restore into the other moment type: elements converted per device temporary
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
 MAX_NO_DECAY = 4  # weight-decay exemptions per unit and update launch (kMaxNoDecay of csrc/kernels/api.h)
 SR_SEED = 0x27D4EB2F  # bf16 moments: the fixed seed of the rounding bits (sr_bits of csrc/kernels/zero1.cu)
+SR_SEED_EMA = 0x165667B1  # bf16 EMA of the weights: the seed of its rounding bits (sr_bits_ema of zero1.cu)
 
 
 def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
@@ -129,9 +133,9 @@ def moment_type(moment_dtype: Optional[torch.dtype]) -> torch.dtype:
     return moment_dtype
 
 
-def sr_bits(e: Any, t: Any) -> Any:
+def sr_bits(e: Any, t: Any, seed: int = SR_SEED) -> Any:
     """The 32 rounding bits of global element ``e`` at committed update ``t`` (numpy ``uint32``, broadcast over both):
-    murmur3's 32-bit finaliser over ``lo32(e) * 0x9E3779B1 + hi32(e) * 0x85EBCA77 + t * 0xC2B2AE3D + SR_SEED`` (mod
+    murmur3's 32-bit finaliser over ``lo32(e) * 0x9E3779B1 + hi32(e) * 0x85EBCA77 + t * 0xC2B2AE3D + seed`` (mod
     2**32). The low half rounds ``m``, the high half ``v``. A pure function: no state, and no dependence on rank, world,
     grid, paging or thread, so every holder of an element draws the same bits at the same update."""
     import numpy as np
@@ -140,13 +144,19 @@ def sr_bits(e: Any, t: Any) -> Any:
     t = (np.asarray(t, dtype=np.int64) & 0xFFFFFFFF).astype(np.uint32)
     lo, hi = (e & np.uint64(0xFFFFFFFF)).astype(np.uint32), (e >> np.uint64(32)).astype(np.uint32)
     with np.errstate(over="ignore"):
-        x = lo * np.uint32(0x9E3779B1) + hi * np.uint32(0x85EBCA77) + t * np.uint32(0xC2B2AE3D) + np.uint32(SR_SEED)
+        x = lo * np.uint32(0x9E3779B1) + hi * np.uint32(0x85EBCA77) + t * np.uint32(0xC2B2AE3D) + np.uint32(seed)
         x = x ^ (x >> np.uint32(16))
         x = x * np.uint32(0x85EBCA6B)
         x = x ^ (x >> np.uint32(13))
         x = x * np.uint32(0xC2B2AE35)
         x = x ^ (x >> np.uint32(16))
     return x
+
+
+def sr_bits_ema(e: Any, t: Any) -> Any:
+    """The rounding bits of a bf16 EMA of the weights: :func:`sr_bits` with the seed ``SR_SEED_EMA``, of which the low
+    half rounds element ``e``'s EMA at update ``t``. The other seed keeps them apart from the bits of ``e``'s moments."""
+    return sr_bits(e, t, SR_SEED_EMA)
 
 
 def bf16_sr(x: Any, e: Any, t: Any, which: int, r: Any = None) -> Any:
@@ -170,6 +180,77 @@ def bf16_sr(x: Any, e: Any, t: Any, which: int, r: Any = None) -> Any:
     with np.errstate(over="ignore"):
         out = np.where(special, (u >> np.uint32(16)) | nan, (u + r) >> np.uint32(16))
     return out.astype(np.uint16)
+
+
+def bf16_sr_ema(x: Any, e: Any, t: Any) -> Any:
+    """fp32 ``x`` rounded to bf16 as the update kernel rounds a bf16 EMA of element ``e`` at update ``t``:
+    :func:`bf16_sr` with the low half of ``sr_bits_ema(e, t)``."""
+    import numpy as np
+
+    return bf16_sr(x, e, t, 0, r=sr_bits_ema(e, t) & np.uint32(0xFFFF))
+
+
+# --------------------------------------------------------------------------- EMA of the weights
+def ema_decay_value(ema_decay: Optional[float]) -> Optional[float]:
+    """The decay of the EMA :class:`Zero1Optimizer` keeps: ``ema_decay``, or env ``TORCHFT_B200_Z1_EMA_DECAY`` when it
+    is ``None`` (unset or empty: no EMA). A decay outside ``(0, 1)``, or one whose ``fp32(1 - decay)`` is 0 or 1,
+    raises ``ValueError``."""
+    import numpy as np
+
+    if ema_decay is None:
+        env = os.environ.get("TORCHFT_B200_Z1_EMA_DECAY", "").strip()
+        if not env:
+            return None
+        ema_decay = float(env)
+    d = float(ema_decay)
+    if not (0.0 < d < 1.0 and 0.0 < float(np.float32(1.0 - d)) < 1.0):
+        raise ValueError(f"ema_decay must be in (0, 1) with fp32(1 - ema_decay) in (0, 1), got {ema_decay}")
+    return d
+
+
+def ema_coefficient(decay: float) -> float:
+    """``c = fp32(1 - decay)``, rounded once on the host: the update kernel's step is ``ema + c * (w' - ema)``."""
+    import numpy as np
+
+    return float(np.float32(1.0 - float(decay)))
+
+
+def ema_step(ema: Any, w: Any, c: float) -> Any:
+    """The update kernel's EMA step in numpy float32, bit for bit: ``ema + c * (w - ema)``, each of the three operations
+    rounded to fp32 on its own (the kernel spells them ``__fsub_rn`` / ``__fmul_rn`` / ``__fadd_rn``). A bf16 EMA stores
+    ``bf16_sr_ema(ema_step(...), e, t)``."""
+    import numpy as np
+
+    ema, w = np.asarray(ema, dtype=np.float32), np.asarray(w, dtype=np.float32)
+    return ema + np.float32(c) * (w - ema)
+
+
+def ema_record(c: Optional[float]) -> Optional[str]:
+    """What a rank publishes of its EMA in its ``z1/{rank}`` record: ``c`` as the hex of its fp32 value (``None``: no
+    EMA, no key)."""
+    import numpy as np
+
+    return None if c is None else float(np.float32(c)).hex()
+
+
+def check_ema_agreement(records: Dict[int, Dict[str, Any]]) -> None:
+    """``RuntimeError`` when the published ``z1/{rank}`` records of a quorum disagree on the EMA of the weights
+    (``ema``: its coefficient; absent: no EMA). Holders with different decays would drift apart without a sign, and a
+    holder without an EMA could not serve one to a peer that keeps it; every rank reads the same records and raises
+    alike, before anything is freed or pulled."""
+    kinds = {r: p.get("ema") for r, p in records.items()}
+    if len(set(kinds.values())) > 1:
+        raise RuntimeError(f"zero1: the replicas of this quorum disagree on the EMA of the weights (coefficient per "
+                           f"rank, None = no EMA: {kinds})")
+
+
+def split_ema_reads(reads: Sequence[Tuple[Any, int, int, int]]) -> Tuple[List[Tuple[Any, int, int, int]], List[Range]]:
+    """The EMA part of a checkpoint read plan (``(header, offset, lo, hi)`` from :func:`ckpt_read_plan`): the reads
+    whose file has an ``ema`` section, and the merged ranges whose file has none, which are seeded from the master
+    weights read with them."""
+    have = [r for r in reads if "ema" in r[0]]
+    seed = merge_ranges([(lo, hi) for h, _, lo, hi in reads if "ema" not in h])
+    return have, seed
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -564,6 +645,12 @@ class Zero1Optimizer:
             computes in fp32 and rounds them stochastically (:func:`bf16_sr`) with bits that depend only on the element
             index and the committed update count, so the holders of a slice stay bit-identical. ``master`` stays fp32.
             Every replica of a quorum must use the same type. A checkpoint of the other type is converted on restore.
+        ema_decay: keep an exponential moving average of the fp32 master weights with this decay ``d`` in ``(0, 1)``
+            (``None``: env ``TORCHFT_B200_Z1_EMA_DECAY``, unset = no EMA). It is partitioned state like ``m`` and ``v``
+            and of their type (bf16: rounded stochastically with bits of its own): the holders of a slice advance it in
+            the update kernel after every committed update, ``ema + fp32(1 - d) * (w' - ema)``; re-shards, heals and
+            checkpoints carry it; it is seeded from the weights wherever the master weights are. :meth:`ema_weights`
+            swaps it into ``param`` for evaluation. Every replica of a quorum must use the same decay.
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
@@ -572,11 +659,16 @@ class Zero1Optimizer:
                  state_pages: Optional[int] = None, page_shift: int = PAGE_SHIFT,
                  max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1,
                  lr_lambda: Optional[Callable[[int], float]] = None, lr_steps: int = 0,
-                 no_decay: Sequence[Range] = (), moment_dtype: Optional[torch.dtype] = None) -> None:
+                 no_decay: Sequence[Range] = (), moment_dtype: Optional[torch.dtype] = None,
+                 ema_decay: Optional[float] = None) -> None:
         from torchft_b200.ops import _native
 
         self.moment_dtype = moment_type(moment_dtype)
         self._msize = 2 if self.moment_dtype == torch.bfloat16 else 4  # bytes per element of m and of v
+        self.ema_decay = ema_decay_value(ema_decay)
+        self._ema_c = None if self.ema_decay is None else ema_coefficient(self.ema_decay)
+        self.ema: Optional[torch.Tensor] = None  # EMA of the weights, of the moment type, indexed like master
+        self._ema_active = False                 # inside ema_weights(): param holds bf16(EMA)
         self.max_grad_norm = clip_threshold(max_grad_norm)
         # learning-rate schedule: fp32 rate of committed update i + 1 at index i (host copy and device table)
         self._lr_host = lr_schedule_table(lr, lr_lambda, lr_steps) if lr_lambda is not None else None
@@ -631,9 +723,13 @@ class Zero1Optimizer:
             self.master = pg.alloc_symmetric("z1_master", numel * 4).view(torch.float32)
             self.m = pg.alloc_symmetric("z1_m", numel * self._msize).view(self.moment_dtype)
             self.v = pg.alloc_symmetric("z1_v", numel * self._msize).view(self.moment_dtype)
+            if self.ema_decay is not None:
+                self.ema = pg.alloc_symmetric("z1_ema", numel * self._msize).view(self.moment_dtype)
         else:
             self.master = torch.empty(0, dtype=torch.float32, device=self.device)  # set_units allocates
             self.m = self.v = torch.empty(0, dtype=self.moment_dtype, device=self.device)
+            if self.ema_decay is not None:
+                self.ema = self.m
             if not 1 <= self.min_world <= 8:
                 raise ValueError("min_world must be in [1, 8]")
             self._page_shift = int(page_shift)
@@ -727,6 +823,8 @@ class Zero1Optimizer:
         self.master = self.pg.alloc_symmetric("z1_master", n * 4).view(torch.float32)[:n]
         self.m = self.pg.alloc_symmetric("z1_m", n * self._msize).view(self.moment_dtype)[:n]
         self.v = self.pg.alloc_symmetric("z1_v", n * self._msize).view(self.moment_dtype)[:n]
+        if self.ema_decay is not None:
+            self.ema = self.pg.alloc_symmetric("z1_ema", n * self._msize).view(self.moment_dtype)[:n]
         npages = (self.numel + self._page - 1) >> self._page_shift
         self._table_host = np.full(npages, -1, dtype=np.int32)  # page of the flat vector -> pool slot (-1: not held)
         self._table = torch.full((npages,), -1, dtype=torch.int32, device=self.device)
@@ -770,7 +868,8 @@ class Zero1Optimizer:
             if self._snap_done is not None:
                 # a snapshot copy may still read the state that pulls, seeds, page reuse and heal are about to rewrite
                 self._snap_done.synchronize()
-            names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ())
+            names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ()) \
+                + (("z1_ema",) if self.ema is not None else ())
             missing = [n for n in names if not self.comm.is_symmetric(n)]
             if missing:
                 # the kernels dereference peer pointers: every replica must construct its Zero1Optimizer before its first
@@ -784,6 +883,8 @@ class Zero1Optimizer:
                 me["sched"] = sched
             if self._msize == 2:
                 me["moments"] = "bf16"  # fp32 moments publish no key: their record stays as it was
+            if self._ema_c is not None:
+                me["ema"] = ema_record(self._ema_c)  # likewise without an EMA
             if self._disk is not None:
                 me["disk"] = [self._disk[0], self._disk[1]]  # every rank may read what no live holder has from it
             if self.compact:
@@ -803,6 +904,7 @@ class Zero1Optimizer:
                 raise RuntimeError(f"zero1: the replicas of this quorum disagree on the learning-rate schedule or the "
                                    f"weight-decay exemptions (digest per rank: {digests})")
             check_moment_agreement(peers)
+            check_ema_agreement(peers)
             ckpt = self._ckpt_files(rank, peers)
             plans = plan_quorum(self.layout, world, peers, self._page_shift if self.compact else None, ckpt)
             plan = plans[rank]
@@ -827,7 +929,7 @@ class Zero1Optimizer:
                 if plan.pulls:
                     tables = {src: self._peer_table(peers[src].get("pages")) for src, _, _ in plan.pulls}
                     entries: List[Tuple[int, int, int]] = []
-                    for name, local in (("z1_master", self.master), ("z1_m", self.m), ("z1_v", self.v)):
+                    for name, local in self._state_arrays(prefix="z1_"):
                         ptrs = self.comm.peer_pointers(name)
                         for src, lo, hi in plan.pulls:
                             for a, b, at in self._pieces(tables[src], lo, hi):
@@ -858,9 +960,14 @@ class Zero1Optimizer:
             self._refresh_pending = world > 1
             self._configured, self._disk = True, None
 
+    def _state_arrays(self, prefix: str = "") -> List[Tuple[str, torch.Tensor]]:
+        """``(name, array)`` of the partitioned state: master, m, v and, when kept, the EMA."""
+        arrays = [("master", self.master), ("m", self.m), ("v", self.v)] + ([("ema", self.ema)] if self.ema is not None else [])
+        return [(prefix + n, a) for n, a in arrays]
+
     def _state_item(self) -> int:
-        """Bytes of (master, m, v) per element: 12 with fp32 moments, 8 with bf16."""
-        return self.master.element_size() + self.m.element_size() + self.v.element_size()
+        """Bytes of the partitioned state per element: 12 with fp32 moments, 8 with bf16, plus 4 or 2 with an EMA."""
+        return sum(a.element_size() for _, a in self._state_arrays())
 
     def _schedule_digest(self) -> Optional[str]:
         """What this rank publishes of its schedule and exemptions (``None`` without either: the record stays as it was)."""
@@ -948,12 +1055,15 @@ class Zero1Optimizer:
 
     @torch.no_grad()
     def _seed(self, ranges: Sequence[Range]) -> None:
-        """``master = float(param)``, ``m = v = 0`` on ``ranges`` (current stream)."""
+        """``master = float(param)``, ``m = v = 0`` and ``ema = master`` on ``ranges`` (current stream). bf16(master) is
+        ``param`` exactly, so a bf16 EMA starts equal to the master weights too."""
         for lo, hi in ranges:
             for a, b, at in self._pieces(self._table_host, lo, hi):
                 self.master[at:at + b - a].copy_(self.param[a:b])
                 self.m[at:at + b - a].zero_()
                 self.v[at:at + b - a].zero_()
+                if self.ema is not None:
+                    self.ema[at:at + b - a].copy_(self.param[a:b])
 
     # ------------------------------------------------------------------ per-step pipeline
     def unit_of(self, lo: int, hi: int) -> int:
@@ -1039,6 +1149,7 @@ class Zero1Optimizer:
     def update(self, events: Optional[Sequence[torch.cuda.Event]] = None) -> None:
         """Gated AdamW + weight all-gather for every unit, in forward order, on the commit stream; ``events[i]``
         fires when unit ``i``'s weights are current on THIS replica (all peers' pushes have landed)."""
+        self._not_in_ema("update")
         stream = self._commit_stream
         k = self.layout.replication
         lr = self.param_groups[0]["lr"]
@@ -1066,12 +1177,17 @@ class Zero1Optimizer:
         """The state arguments of ``zero1_update_`` for the unit that starts at element ``lo``. Full-size state passes
         the arrays at ``lo`` and no table, which selects the kernel without page lookups; paged state passes the pools
         and the page table, through which the kernel finds each element."""
+        ema = {} if self.ema is None else {"ema_c": self._ema_c}
         if self._table is None:
             # the global element index of the unit's start is what bf16 moments hash for their rounding bits
+            if self.ema is not None:
+                ema["ema"] = self.ema.data_ptr() + self._msize * lo
             return {"master": self.master.data_ptr() + 4 * lo, "m": self.m.data_ptr() + self._msize * lo,
-                    "v": self.v.data_ptr() + self._msize * lo, "state_off": lo}
+                    "v": self.v.data_ptr() + self._msize * lo, "state_off": lo, **ema}
+        if self.ema is not None:
+            ema["ema"] = self.ema.data_ptr()
         ptrs = {"master": self.master.data_ptr(), "m": self.m.data_ptr(), "v": self.v.data_ptr()}
-        return {**ptrs, "table": self._table.data_ptr(), "state_off": lo, "page_shift": self._page_shift}
+        return {**ptrs, "table": self._table.data_ptr(), "state_off": lo, "page_shift": self._page_shift, **ema}
 
     def resolved(self, verdict: bool) -> None:
         """The Manager learned the verdict of the last :meth:`commit` (lazily, on the quorum thread)."""
@@ -1101,6 +1217,7 @@ class Zero1Optimizer:
         ``manager_state`` is ``{"step", "batches_committed"}`` for the header. A save first waits for the previous
         write and re-raises its error; :meth:`wait_checkpoint` waits for this one. ``keep`` newest steps of the files
         this optimizer wrote are kept."""
+        self._not_in_ema("save")
         if not self._configured:
             raise RuntimeError("zero1: nothing to checkpoint before the first quorum")
         if self._commit_layout is not None:
@@ -1123,8 +1240,8 @@ class Zero1Optimizer:
         for lo, hi in ranges:
             written.append((lo, hi, e))
             e += hi - lo
-        sec = sections(e, self._msize)
-        stage = w.staging((6 + 2 * self._msize) * e)  # bf16 weights, fp32 master, m and v per primary element
+        sec = sections(e, self._msize, ema=self.ema is not None)
+        stage = w.staging((2 + self._state_item()) * e)  # bf16 weights, fp32 master, m, v (and the EMA) per element
         if self._snap_stream is None:
             self._snap_stream = torch.cuda.Stream(device=self.device)
         s = self._snap_stream
@@ -1138,7 +1255,7 @@ class Zero1Optimizer:
                     for a, b in intersect_ranges([(lo, hi)], [unit]):
                         x = off + a - lo
                         stage[2 * x:2 * (x + b - a)].copy_(self.param[a:b].view(u8), non_blocking=True)
-                        for name, arr in (("master", self.master), ("m", self.m), ("v", self.v)):
+                        for name, arr in self._state_arrays():
                             sz = arr.element_size()
                             base = sec[name] + sz * x
                             for c, d, at in self._pieces(self._table_host, a, b):  # maximal runs of consecutive slots
@@ -1155,6 +1272,8 @@ class Zero1Optimizer:
                               "weight_decay": self.weight_decay, "max_grad_norm": self.max_grad_norm}}
         if self._msize == 2:
             header["moments"] = "bf16"  # a header without the key describes fp32 moments
+        if self.ema is not None:
+            header["ema"] = {"decay": self.ema_decay}  # ... and one without this key has no EMA section
         w.submit(header, self._snap_done)
         return self.t
 
@@ -1177,6 +1296,7 @@ class Zero1Optimizer:
         or other units raise ``ValueError`` before any state changes."""
         from torchft_b200.checkpointing.sharded import check_compatible, scan
 
+        self._not_in_ema("restore")
         if self._configured:
             raise RuntimeError("zero1: restore must be called before the first quorum")
         headers = scan(directory)
@@ -1196,6 +1316,16 @@ class Zero1Optimizer:
 
     def _read_state(self, reads: Sequence[Tuple[Any, int, int, int]]) -> None:
         self._read_ranges(reads, ("master", "m", "v"))
+        if self.ema is not None:
+            have, seed = split_ema_reads(reads)
+            self._read_ranges(have, ("ema",))
+            if seed:
+                logger.warning("zero1: the checkpoint files of %s have no EMA of the weights: it starts from the "
+                               "master weights there", seed)
+                with torch.cuda.stream(self._reshard_stream):
+                    for lo, hi in seed:
+                        for a, b, at in self._pieces(self._table_host, lo, hi):
+                            self.ema[at:at + b - a].copy_(self.master[at:at + b - a])  # bf16: rounds to nearest
         self.disk_read_elements += total([(lo, hi) for _, _, lo, hi in reads])
 
     def _read_ranges(self, reads: Sequence[Tuple[Any, int, int, int]], arrays: Sequence[str]) -> None:
@@ -1203,7 +1333,7 @@ class Zero1Optimizer:
         stream (compact state: into the pool pages the table maps them to)."""
         from torchft_b200.checkpointing.sharded import RangedReader, file_dtype
 
-        dst = {"param": self.param, "master": self.master, "m": self.m, "v": self.v}
+        dst = {"param": self.param, **dict(self._state_arrays())}
         rd = RangedReader(self._reshard_stream)
         try:
             for h, off, lo, hi in reads:
@@ -1213,7 +1343,7 @@ class Zero1Optimizer:
                         if not convert:
                             rd.read(h, name, off + a - lo, dst[name][at:at + b - a])
                             continue
-                        # moments saved in the other type: fp32 -> bf16 rounds to nearest, bf16 -> fp32 is exact
+                        # moments (or EMA) saved in the other type: fp32 -> bf16 rounds to nearest, bf16 -> fp32 is exact
                         for c in range(a, b, CONVERT_CHUNK):
                             n = min(CONVERT_CHUNK, b - c)
                             with torch.cuda.stream(self._reshard_stream):
@@ -1237,7 +1367,7 @@ class Zero1Optimizer:
         return self._state_item() * total(self.layout.held(self.comm.rank, max(self.comm.world, 1)))
 
     def state_bytes_allocated(self) -> int:
-        """Device bytes of the master/m/v arrays (compact: the page pools)."""
+        """Device bytes of the master/m/v arrays and the EMA (compact: the page pools)."""
         return self._state_item() * self.master.numel()
 
     def held_state(self) -> Dict[Range, Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
@@ -1248,6 +1378,68 @@ class Zero1Optimizer:
             pieces = self._pieces(self._table_host, lo, hi)
             out[(lo, hi)] = tuple(torch.cat([x[at:at + b - a] for a, b, at in pieces]) for x in (self.master, self.m, self.v))
         return out
+
+    def held_ema(self) -> Dict[Range, torch.Tensor]:
+        """Copies of the EMA of the weights over each range this rank holds, keyed like :meth:`held_state`."""
+        if self.ema is None:
+            raise RuntimeError("zero1: this optimizer keeps no EMA of the weights (ema_decay)")
+        torch.cuda.synchronize(self.device)
+        return {(lo, hi): torch.cat([self.ema[at:at + b - a] for a, b, at in self._pieces(self._table_host, lo, hi)])
+                for lo, hi in self._holdings}
+
+    # ------------------------------------------------------------------ evaluating the EMA
+    @contextlib.contextmanager
+    def ema_weights(self) -> Iterator[None]:
+        """Inside the context ``param`` holds bf16(EMA) on every replica; on exit it holds bf16(master) again, bit for
+        bit. Every replica of the quorum enters after the same step (the swap pushes each primary slice to everybody).
+
+        Entry enqueues the EMA broadcast (update kernel mode 2) of every unit on the commit stream, behind the last
+        update, and makes the current stream wait for it; exit enqueues the refresh (mode 1) behind whatever the current
+        stream did inside, and makes the current stream wait for that. Both broadcasts start with a handshake, so no
+        replica's push overwrites a peer's ``param`` while that peer is still updating or evaluating it. Inside, :meth:`update`, :meth:`save` and
+        :meth:`restore` raise: training steps, checkpoints and the heal payload (:meth:`state_dict`, whose ``param``
+        a healing peer copies) must never see the EMA in place of the weights. A heal is served only from the Manager's
+        quorum task, which ``start_quorum`` starts at the beginning of a step and ``commit_on_device`` waits for (and
+        closes the checkpoint window after) before the step's update is enqueued; no step can start inside the context,
+        so no quorum task runs there either."""
+        if self.ema is None:
+            raise RuntimeError("zero1: this optimizer keeps no EMA of the weights (ema_decay)")
+        if not self._configured:
+            raise RuntimeError("zero1: there are no EMA weights to swap in before the first quorum")
+        self._not_in_ema("ema_weights")
+        self._broadcast(2)
+        self._ema_active = True
+        try:
+            yield
+        finally:
+            self._broadcast(1)
+            self._ema_active = False
+
+    def _broadcast(self, mode: int) -> None:
+        """Every unit's primary slice of bf16(EMA) (``mode`` 2) or bf16(master) (1) into every replica's ``param``, on
+        the commit stream between the current stream's work before and after.
+
+        The pushes land in the peers' ``param``, so they wait behind a handshake: no rank pushes before every peer's
+        commit stream has reached the same point, i.e. before every peer has finished its last update (at W = k that
+        update ends without a handshake of its own) and whatever its current stream read of ``param`` before it entered
+        or left the context (an evaluation)."""
+        stream, cur = self._commit_stream, torch.cuda.current_stream(self.device)
+        stream.wait_stream(cur)  # what the current stream reads of param (an evaluation) comes first
+        if self._snap_done is not None:
+            stream.wait_event(self._snap_done)  # the last save has copied param
+        self.comm.zero1_barrier_(stream)  # ... on every replica
+        hp = (self.param_groups[0]["lr"], self.betas[0], self.betas[1], self.eps, self.weight_decay)  # unused here
+        for lo, hi in self.layout.units:
+            self.comm.zero1_update_("z1_param", lo * 2, self.grad.data_ptr() + lo * 2, nelem=hi - lo, hyper=hp,
+                                    gate=self.gate, replication=self.layout.replication, mode=mode,
+                                    blocks=self._upd_blocks, stream=stream, moment_dtype=self.moment_dtype,
+                                    **self._update_state(lo))
+        cur.wait_stream(stream)
+
+    def _not_in_ema(self, what: str) -> None:
+        if self._ema_active:
+            raise RuntimeError(f"zero1: {what} inside ema_weights(): param holds the EMA weights, not the training "
+                               f"weights")
 
     def zero_grad(self, set_to_none: bool = False) -> None:  # gradients are overwritten by the wgrad GEMMs
         pass
