@@ -1,8 +1,8 @@
-"""Hardware tuning sweep for the fused P2P all-reduce: barrier recipe x algorithm x grid size.
+"""Hardware tuning sweep for the fused P2P all-reduce: algorithm x grid size.
 
     torchrun --nproc-per-node N bench/comm_tune.py --out gpurun_out/comm_tune.json
 
-For each message size prints the best (mode, algo, blocks) and the NCCL AVG time; the winning
+For each message size prints the best (algo, blocks) and the NCCL AVG time; the winning
 table is what ``SymmetricComm._plan`` encodes.
 """
 
@@ -41,7 +41,6 @@ def timed(fn, iters, warm=3):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default="gpurun_out/comm_tune.json")
-    ap.add_argument("--modes", default="2")
     ap.add_argument("--max-mb", type=int, default=256)
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ.get("LOCAL_RANK", 0))
@@ -52,7 +51,6 @@ def main():
     symm = comm.alloc("tune", args.max_mb << 20)
     comm.configure(dist.PrefixStore("tune", store), rank, world, 1)
     sizes = [1 << k for k in range(12, 31, 1) if (1 << k) <= (args.max_mb << 20)]
-    modes = [int(m) for m in args.modes.split(",")]
     rows = []
     for nbytes in sizes:
         buf = symm[:nbytes].view(torch.bfloat16)
@@ -71,16 +69,14 @@ def main():
                 else:
                     if nbytes // blocks < 2048 and blocks > 1:
                         continue
-                for mode in modes:
-                    comm._force_plan = (algo, blocks)
-                    comm._barrier_mode = mode
-                    ms = timed(lambda: comm.allreduce_(buf, scale=1.0 / world), iters)
-                    table[f"a{algo}_b{blocks}_m{mode}"] = round(ms * 1e3, 2)
-                    if best is None or ms < best[0]:
-                        best = (ms, algo, blocks, mode)
+                comm._force_plan = (algo, blocks)
+                ms = timed(lambda: comm.allreduce_(buf, scale=1.0 / world), iters)
+                table[f"a{algo}_b{blocks}"] = round(ms * 1e3, 2)
+                if best is None or ms < best[0]:
+                    best = (ms, algo, blocks)
         err = comm.errored()
         row = {"bytes": nbytes, "nccl_avg_us": round(nccl * 1e3, 2), "best_us": round(best[0] * 1e3, 2),
-               "best": {"algo": best[1], "blocks": best[2], "mode": best[3]}, "err": str(err) if err else None, "all_us": table}
+               "best": {"algo": best[1], "blocks": best[2]}, "err": str(err) if err else None, "all_us": table}
         rows.append(row)
         if rank == 0:
             top = sorted(table.items(), key=lambda kv: kv[1])[:6]

@@ -133,9 +133,7 @@ def main() -> None:
         a = torch.empty(n, dtype=torch.uint8, device=dev)
         b = torch.empty(n, dtype=torch.uint8, device=dev)
         for blocks in (32, 64, K.NUM_SMS):
-            record(f"heal_copy_local_b{blocks}", timeit(lambda: device_copy([(a.data_ptr(), b.data_ptr(), n)], blocks=blocks, bulk=False), args.iters, flush), 2 * n)
-        for blocks in (K.NUM_SMS, 2 * K.NUM_SMS, 3 * K.NUM_SMS):  # TMA variant: 64 KiB smem per CTA -> up to 3 CTAs per SM, 32 threads each
-            record(f"heal_copy_bulk_tma_b{blocks}", timeit(lambda: device_copy([(a.data_ptr(), b.data_ptr(), n)], blocks=blocks, bulk=True), args.iters, flush), 2 * n)
+            record(f"heal_copy_local_b{blocks}", timeit(lambda: device_copy([(a.data_ptr(), b.data_ptr(), n)], blocks=blocks), args.iters, flush), 2 * n)
         del a, b
     if want("diloco_outer"):
         n = 1 << 29

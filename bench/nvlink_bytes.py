@@ -134,8 +134,7 @@ def main() -> None:
                                  ((W - 1) + (k - 1)) / W * S, ((W - 1) + (k - 1)) / W * S),
         "zero1_update_allgather": (lambda: comm.zero1_update_("z1_param", 0, grad.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(),
                                                               nelem, hp, gate, k, 0, comm._K.NUM_SMS * 16), (W - k) / W * S, (W - k) / W * S),
-        "heal_copy_pull_lsu": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=128, bulk=False), S, S),
-        "heal_copy_pull_bulk_tma": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=comm._K.MAX_BLOCKS, bulk=True), S, S),
+        "heal_copy_pull_lsu": (lambda: device_copy([(peer_buf, local_dst.data_ptr(), S)], blocks=128), S, S),
     }
     if qb:
         q_total = n32 * (1 + 4.0 / 512)  # fp8 payload + one fp32 scale per 512 elements

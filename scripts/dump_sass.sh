@@ -21,7 +21,6 @@ dump p2p_send 'p2p_send_kernel'
 dump p2p_recv 'p2p_recv_kernel'
 dump diloco_outer_bf16 'diloco_outer_kernelI13__nv_bfloat16'
 dump heal_copy 'heal_copy_kernelE'
-dump heal_copy_bulk_tma 'heal_copy_bulk_kernel'
 dump q8_allreduce_bf16_w8 'q8_allreduce_kernelI13__nv_bfloat16Li8'
 dump allreduce_twoshot_bf16_w8_sum 'allreduce_twoshot_kernelI13__nv_bfloat16Li8ELi0'
 dump allreduce_oneshot_bf16_w2_sum 'allreduce_oneshot_kernelI13__nv_bfloat16Li2ELi0'

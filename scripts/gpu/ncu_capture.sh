@@ -17,8 +17,6 @@ $NCU -k regex:'diloco_outer_kernel' -s 3 -c 1 -o gpurun_out/ncu/diloco_outer -f 
   python bench/kernel_micro.py --only diloco_outer --iters 1 > gpurun_out/ncu/micro_b.log 2>&1
 $NCU -k regex:'heal_copy_kernel' -s 11 -c 1 -o gpurun_out/ncu/heal_copy_lsu -f \
   python bench/kernel_micro.py --only heal_copy --iters 1 > gpurun_out/ncu/micro_c.log 2>&1
-$NCU -k regex:'heal_copy_bulk_kernel' -s 3 -c 1 -o gpurun_out/ncu/heal_copy_bulk -f \
-  python bench/kernel_micro.py --only heal_copy --iters 1 > gpurun_out/ncu/micro_d.log 2>&1
 # the q8 large-message pipeline and the generic collectives (W=4 in-process, presignalled)
 $NCU -k regex:'q8_|reduce_scatter_kernel|push_exchange' -c 6 -o gpurun_out/ncu/collectives -f \
   python -c "import torch; torch.cuda.set_device(0); from torchft_b200.bench_utils import collectives_selfcheck as c; print(c(world=4, nelem=1<<22))" > gpurun_out/ncu/selfcheck.log 2>&1

@@ -218,30 +218,6 @@ def test_heal_copy(K):
         assert torch.equal(s, d)
 
 
-def test_heal_copy_bulk_tma_variant(K):
-    """cp.async.bulk ring (global -> shared -> global, mbarrier-tracked): same bytes as the LSU kernel, incl. odd tails."""
-    from torchft_b200.checkpointing.p2p_transport import device_copy
-
-    torch.manual_seed(8)
-    sizes = (16, 1000 * 4, (1 << 22) + 16, 12345 * 4, 48 * 1024, 7 << 20)
-    srcs = [torch.randint(0, 255, (n,), device="cuda", dtype=torch.uint8) for n in sizes]
-    srcs.append(torch.randint(0, 255, (100_003,), device="cuda", dtype=torch.uint8))  # 3-byte tail after the 16 B body
-    dsts = [torch.zeros_like(s) for s in srcs]
-    for chunk in (1 << 20, 4 << 20):
-        for d in dsts:
-            d.zero_()
-        device_copy([(s.data_ptr(), d.data_ptr(), s.numel()) for s, d in zip(srcs, dsts)], bulk=True, chunk_bytes=chunk)
-        torch.cuda.synchronize()
-        for s, d in zip(srcs, dsts):
-            assert torch.equal(s, d), (s.numel(), chunk)
-    # unaligned ranges silently use the LSU kernel
-    u = torch.randint(0, 255, (5000,), device="cuda", dtype=torch.uint8)[1:]
-    v = torch.zeros(4999, device="cuda", dtype=torch.uint8)
-    device_copy([(u.data_ptr(), v.data_ptr(), 4999)], bulk=True)
-    torch.cuda.synchronize()
-    assert torch.equal(u, v)
-
-
 def test_llama_tiny_fwd_bwd_matches_reference():
     from torchft_b200.models.llama import CONFIGS, Llama
     from torchft_b200.models.reference import reference_loss

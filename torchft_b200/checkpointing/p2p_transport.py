@@ -51,36 +51,24 @@ CHUNK_BYTES = 4 << 20
 
 
 def device_copy(entries: Sequence[Tuple[int, int, int]], stream: Optional[torch.cuda.Stream] = None,
-                blocks: int = 128, chunk_bytes: int = CHUNK_BYTES, bulk: Optional[bool] = None) -> None:
-    """Copy ``(src_ptr, dst_ptr, nbytes)`` ranges with one kernel launch. Either side may be a mapped peer pointer;
-    the kernel issues the NVLink traffic.
-
-    ``bulk`` selects the TMA variant (``heal_copy_bulk_kernel``: one thread per CTA drives a ring of ``cp.async.bulk``
-    global->shared->global transfers, no data in registers) instead of the LSU variant (``heal_copy_kernel``: 8 x 16-byte
-    loads in flight per thread). Default: env ``TORCHFT_B200_HEAL_BULK`` (off). Bulk needs 16-byte aligned ranges.
+                blocks: int = 128, chunk_bytes: int = CHUNK_BYTES) -> None:
+    """Copy ``(src_ptr, dst_ptr, nbytes)`` ranges with one kernel launch (``heal_copy_kernel``: 8 x 16-byte loads in
+    flight per thread). Either side may be a mapped peer pointer; the kernel issues the NVLink traffic.
     """
 
     K = _native.load()
-    if bulk is None:
-        bulk = os.environ.get("TORCHFT_B200_HEAL_BULK", "0") == "1"
     rows, chunk0 = [], 0
     for src, dst, n in entries:
         if n <= 0:
             continue
         rows.append((src, dst, n, chunk0))
         chunk0 += (n + chunk_bytes - 1) // chunk_bytes
-        if bulk and ((src | dst) & 15):
-            bulk = False
     if not rows:
         return
     table = torch.tensor(rows, dtype=torch.int64).cuda(non_blocking=False)
     s = stream if stream is not None else torch.cuda.current_stream()
     with torch.cuda.stream(s):
-        if bulk and chunk_bytes % 16 == 0:
-            # 64 KiB of shared memory per CTA -> 3 CTAs per SM; enough CTAs to put > 2 MB (NVLink) / > 8 MB (HBM) in flight
-            K.heal_copy_bulk(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(max(blocks, K.MAX_BLOCKS), chunk0)), int(s.cuda_stream))
-        else:
-            K.heal_copy(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(blocks, chunk0)), int(s.cuda_stream))
+        K.heal_copy(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(blocks, chunk0)), int(s.cuda_stream))
         table.record_stream(s)
 
 

@@ -48,7 +48,6 @@ struct ARArgs {
   uint64_t flag;         // barrier values flag+1, flag+2 are consumed
   int channel;
   int contribute;        // 0 => stage zeros (non-participant)
-  int barrier_mode;      // memory-ordering recipe of block_barrier
 };
 
 template <typename T>
@@ -92,7 +91,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_twoshot_kernel(ARArgs a) {
   const bool staged = (a.user_in != nullptr || !a.contribute);
   // peer data read below was produced before the peers' kernels started (or released by their
   // fence when staged) and is only touched with L1-bypassing loads: no acquire fence needed
-  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/staged, /*acquire=*/false, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/staged, /*acquire=*/false)) return;
 
   // ---- phase 1+2: reduce my slice from all peers, push result to all peers ----
   {
@@ -142,7 +141,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_twoshot_kernel(ARArgs a) {
       }
     }
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/a.user_out != nullptr, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/a.user_out != nullptr)) return;
 
   // ---- phase 3: symmetric segment -> user tensor ----
   if (a.user_out != nullptr) {
@@ -173,7 +172,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_oneshot_kernel(ARArgs a) {
       copy_region<T>(mine, reinterpret_cast<const T*>(a.user_in), lo, hi, a.nelem, !a.contribute);
   }
   if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/(a.user_in != nullptr || !a.contribute),
-                     /*acquire=*/false, a.barrier_mode))
+                     /*acquire=*/false))
     return;
 
   const T* src[W];
@@ -206,7 +205,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_oneshot_kernel(ARArgs a) {
         for (size_t k = e; k < a.nelem; ++k) out[k] = T(acc[k - e]);
       }
     }
-    block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false, a.barrier_mode);
+    block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
   } else {
     // In-place in staging: host guarantees chunk <= blockDim.x * kMaxRounds.
     constexpr int kMaxRounds = 8;
@@ -231,7 +230,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_oneshot_kernel(ARArgs a) {
         res[r] = Pack<T>::pack(acc);
       }
     }
-    if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false, a.barrier_mode)) return;
+    if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false)) return;
 #pragma unroll
     for (int r = 0; r < kMaxRounds; ++r) {
       const size_t v = lo + threadIdx.x + (size_t)r * blockDim.x;
@@ -296,7 +295,7 @@ static void launch_op(const ARArgs& a, int op, int algo, int blocks, int threads
 void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* user_in,
                       void* user_out, size_t nelem, int dtype, int op, float scale,
                       uint64_t flag, int channel, int contribute, int algo, int blocks,
-                      int threads, int barrier_mode, cudaStream_t stream) {
+                      int threads, cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("allreduce: bad grid");
   if (threads < 32 || threads > 512 || (threads & 31))
     throw std::runtime_error("allreduce: threads must be a multiple of 32 in [32, 512]");
@@ -312,7 +311,6 @@ void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const vo
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  a.barrier_mode = barrier_mode;
   if (pt.world == 1) {
     // Degenerate quorum: out = scale * in (or zeros).
     const void* src = user_in ? user_in : (const char*)pt.data[0] + off;

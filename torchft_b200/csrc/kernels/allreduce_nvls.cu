@@ -80,7 +80,6 @@ struct NvlsArgs {
   uint64_t flag;
   int channel;
   int contribute;
-  int barrier_mode;
 };
 
 template <typename T>
@@ -100,7 +99,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_nvls_kernel(NvlsArgs a) {
       for (size_t v = lo + threadIdx.x; v < hi; v += blockDim.x) st_stream(mine + v * N, Vec16{0, 0, 0, 0});
     }
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/!a.contribute, /*acquire=*/false, a.barrier_mode))
+  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/!a.contribute, /*acquire=*/false))
     return;
 
   {
@@ -132,12 +131,12 @@ __global__ void __launch_bounds__(512, 1) allreduce_nvls_kernel(NvlsArgs a) {
       }
     }
   }
-  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/false, a.barrier_mode);
+  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/false);
 }
 
 void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, size_t off, size_t nelem, int dtype,
                            float scale, uint64_t flag, int channel, int contribute, int blocks, int threads,
-                           int barrier_mode, cudaStream_t stream) {
+                           cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("allreduce_nvls: bad grid");
   if (off & 15) throw std::runtime_error("allreduce_nvls: offset must be 16 B aligned");
   if (pt.world < 2) throw std::runtime_error("allreduce_nvls: world must be >= 2");
@@ -151,7 +150,6 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  a.barrier_mode = barrier_mode;
   switch (dtype) {
     case kF32: allreduce_nvls_kernel<float><<<blocks, threads, 0, stream>>>(a); break;
     case kBF16: allreduce_nvls_kernel<__nv_bfloat16><<<blocks, threads, 0, stream>>>(a); break;

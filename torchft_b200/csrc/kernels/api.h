@@ -16,12 +16,12 @@ struct StatusBlock;
 void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* user_in,
                       void* user_out, size_t nelem, int dtype, int op, float scale,
                       uint64_t flag, int channel, int contribute, int algo, int blocks,
-                      int threads, int barrier_mode, cudaStream_t stream);
+                      int threads, cudaStream_t stream);
 
 // allreduce_nvls.cu ---------------------------------------------------------
 void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, size_t off, size_t nelem, int dtype,
                            float scale, uint64_t flag, int channel, int contribute, int blocks, int threads,
-                           int barrier_mode, cudaStream_t stream);
+                           cudaStream_t stream);
 
 // zero1.cu -------------------------------------------------------------------
 // FT-ZeRO-1: one-CTA handshake, sync-free reduce-scatter body (+ buddy push), device-side commit verdict, sync-free
@@ -42,9 +42,9 @@ void zero1_update_launch(zero1::UpdArgs a, int moment_dtype, int blocks, int thr
 // reduce-scatter; point-to-point pieces through per-pair mailboxes.
 void push_exchange_launch(const PeerTable& pt, StatusBlock* st, const void* in, void* out, const size_t* send_off,
                           const size_t* send_len, const size_t* recv_len, const size_t* out_off, size_t slot_stride,
-                          uint64_t flag, int channel, int blocks, int barrier_mode, cudaStream_t stream);
+                          uint64_t flag, int channel, int blocks, cudaStream_t stream);
 void reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* user_in, void* out, size_t n,
-                           int dtype, int op, float scale, uint64_t flag, int channel, int blocks, int barrier_mode,
+                           int dtype, int op, float scale, uint64_t flag, int channel, int blocks,
                            cudaStream_t stream);
 void p2p_launch(const PeerTable& pt, StatusBlock* st, int is_send, void* buf, size_t nbytes, int peer, size_t mailbox_off,
                 size_t mailbox_bytes, uint64_t seq0, int channel, cudaStream_t stream);
@@ -66,8 +66,7 @@ void q8_reduce_raw_launch(const void* const* srcs_dev, int nsrc, int first, size
                           size_t g_hi, float post_scale, void* dst, cudaStream_t stream);
 void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in_a,
                          const void* in_b, void* out, size_t nelem, int dtype, float post_scale,
-                         uint64_t flag, int channel, int contribute, int blocks, int barrier_mode,
-                         cudaStream_t stream);
+                         uint64_t flag, int channel, int contribute, int blocks, cudaStream_t stream);
 
 size_t q8_slice_buffer_bytes(size_t nelem, int world);
 void q8_slice_reduce_launch(const PeerTable& pt, const int* ok, size_t q_off, size_t r_off, size_t nelem, float post_scale,
@@ -77,7 +76,7 @@ void q8_gather_dequant_launch(const PeerTable& pt, const int* ok, size_t r_off, 
 size_t q8_rs_buffer_bytes(size_t slice_elems, int world);
 void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in, void* out, size_t nelem,
                               size_t slice_elems, int dtype, float post_scale, uint64_t flag, int channel,
-                              int contribute, int blocks, int barrier_mode, cudaStream_t stream);
+                              int contribute, int blocks, cudaStream_t stream);
 
 // model_ops.cu ---------------------------------------------------------------
 void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int rows, int H,
@@ -104,8 +103,5 @@ void diloco_outer_launch(void* param, void* original, const void* grad, float* m
 void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s);
 void heal_copy_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                       int blocks, cudaStream_t s);
-
-void heal_copy_bulk_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes, int blocks,
-                           cudaStream_t s);
 
 }  // namespace tft

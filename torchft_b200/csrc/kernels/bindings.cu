@@ -206,30 +206,30 @@ PYBIND11_MODULE(_K, m) {
       "allreduce",
       [](const PeerTableH& pt, const Status& st, size_t off, uintptr_t user_in, uintptr_t user_out,
          size_t nelem, int dtype, int op, float scale, uint64_t flag, int channel, bool contribute,
-         int algo, int blocks, int threads, int barrier_mode, uintptr_t stream) {
+         int algo, int blocks, int threads, uintptr_t stream) {
         allreduce_launch(pt.pt, st.dev(), off, P<void>(user_in), P<void>(user_out), nelem, dtype, op,
-                         scale, flag, channel, contribute ? 1 : 0, algo, blocks, threads, barrier_mode, S(stream));
+                         scale, flag, channel, contribute ? 1 : 0, algo, blocks, threads, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("off"), py::arg("user_in"), py::arg("user_out"),
       py::arg("nelem"), py::arg("dtype"), py::arg("op"), py::arg("scale"), py::arg("flag"),
       py::arg("channel"), py::arg("contribute"), py::arg("algo"), py::arg("blocks"),
-      py::arg("threads"), py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("threads"), py::arg("stream"));
 
   bind_vmm(m);
   m.def(
       "allreduce_nvls",
       [](const PeerTableH& pt, const Status& st, uintptr_t mc_base, size_t off, size_t nelem, int dtype, float scale,
-         uint64_t flag, int channel, bool contribute, int blocks, int threads, int barrier_mode, uintptr_t stream) {
+         uint64_t flag, int channel, bool contribute, int blocks, int threads, uintptr_t stream) {
         allreduce_nvls_launch(pt.pt, st.dev(), P<void>(mc_base), off, nelem, dtype, scale, flag, channel,
-                              contribute ? 1 : 0, blocks, threads, barrier_mode, S(stream));
+                              contribute ? 1 : 0, blocks, threads, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("mc_base"), py::arg("off"), py::arg("nelem"), py::arg("dtype"),
       py::arg("scale"), py::arg("flag"), py::arg("channel"), py::arg("contribute"), py::arg("blocks"),
-      py::arg("threads"), py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("threads"), py::arg("stream"));
 
   m.def(
       "zero1_handshake",
-      [](const PeerTableH& pt, const Status& st, uintptr_t ok_out, uint64_t flag, int channel, bool release, int barrier_mode,
+      [](const PeerTableH& pt, const Status& st, uintptr_t ok_out, uint64_t flag, int channel, bool release,
          uintptr_t stream) {
         zero1::HsArgs a{};
         a.pt = pt.pt;
@@ -238,11 +238,10 @@ PYBIND11_MODULE(_K, m) {
         a.flag = flag;
         a.channel = channel;
         a.release = release;
-        a.barrier_mode = barrier_mode;
         zero1_handshake_launch(a, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("ok_out"), py::arg("flag"), py::arg("channel"), py::arg("release"),
-      py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("stream"));
   m.def(
       "zero1_reduce",
       [](const PeerTableH& pt, uintptr_t ok, uintptr_t mc_base, size_t off, size_t nelem, float scale, int replication,
@@ -339,26 +338,25 @@ PYBIND11_MODULE(_K, m) {
       "push_exchange",
       [](const PeerTableH& pt, const Status& st, uintptr_t in, uintptr_t out, const std::vector<size_t>& send_off,
          const std::vector<size_t>& send_len, const std::vector<size_t>& recv_len, const std::vector<size_t>& out_off,
-         size_t slot_stride, uint64_t flag, int channel, int blocks, int barrier_mode, uintptr_t stream) {
+         size_t slot_stride, uint64_t flag, int channel, int blocks, uintptr_t stream) {
         const size_t w = (size_t)pt.pt.world;
         if (send_off.size() != w || send_len.size() != w || recv_len.size() != w || out_off.size() != w)
           throw std::runtime_error("push_exchange: need one entry per rank");
         push_exchange_launch(pt.pt, st.dev(), P<void>(in), P<void>(out), send_off.data(), send_len.data(), recv_len.data(),
-                             out_off.data(), slot_stride, flag, channel, blocks, barrier_mode, S(stream));
+                             out_off.data(), slot_stride, flag, channel, blocks, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("input"), py::arg("output"), py::arg("send_off"), py::arg("send_len"),
       py::arg("recv_len"), py::arg("out_off"), py::arg("slot_stride"), py::arg("flag"), py::arg("channel"),
-      py::arg("blocks"), py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("blocks"), py::arg("stream"));
   m.def(
       "reduce_scatter",
       [](const PeerTableH& pt, const Status& st, size_t off, uintptr_t user_in, uintptr_t out, size_t n, int dtype, int op,
-         float scale, uint64_t flag, int channel, int blocks, int barrier_mode, uintptr_t stream) {
+         float scale, uint64_t flag, int channel, int blocks, uintptr_t stream) {
         reduce_scatter_launch(pt.pt, st.dev(), off, P<void>(user_in), P<void>(out), n, dtype, op, scale, flag, channel,
-                              blocks, barrier_mode, S(stream));
+                              blocks, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("off"), py::arg("user_in"), py::arg("out"), py::arg("n"), py::arg("dtype"),
-      py::arg("op"), py::arg("scale"), py::arg("flag"), py::arg("channel"), py::arg("blocks"), py::arg("barrier_mode"),
-      py::arg("stream"));
+      py::arg("op"), py::arg("scale"), py::arg("flag"), py::arg("channel"), py::arg("blocks"), py::arg("stream"));
   m.def(
       "p2p",
       [](const PeerTableH& pt, const Status& st, bool is_send, uintptr_t buf, size_t nbytes, int peer, size_t mailbox_off,
@@ -401,13 +399,13 @@ PYBIND11_MODULE(_K, m) {
       "q8_allreduce",
       [](const PeerTableH& pt, const Status& st, size_t off, uintptr_t in_a, uintptr_t in_b,
          uintptr_t out, size_t nelem, int dtype, float post_scale, uint64_t flag, int channel,
-         bool contribute, int blocks, int barrier_mode, uintptr_t stream) {
+         bool contribute, int blocks, uintptr_t stream) {
         q8_allreduce_launch(pt.pt, st.dev(), off, P<void>(in_a), P<void>(in_b), P<void>(out), nelem,
-                            dtype, post_scale, flag, channel, contribute ? 1 : 0, blocks, barrier_mode, S(stream));
+                            dtype, post_scale, flag, channel, contribute ? 1 : 0, blocks, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("off"), py::arg("in_a"), py::arg("in_b"),
       py::arg("out"), py::arg("nelem"), py::arg("dtype"), py::arg("post_scale"), py::arg("flag"),
-      py::arg("channel"), py::arg("contribute"), py::arg("blocks"), py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("channel"), py::arg("contribute"), py::arg("blocks"), py::arg("stream"));
 
   m.def("q8_slice_buffer_bytes", &q8_slice_buffer_bytes);
   m.def("q8_slice_reduce", [](const PeerTableH& pt, uintptr_t ok, size_t q_off, size_t r_off, size_t nelem, float post_scale,
@@ -422,14 +420,13 @@ PYBIND11_MODULE(_K, m) {
   m.def(
       "q8_reduce_scatter",
       [](const PeerTableH& pt, const Status& st, size_t off, uintptr_t in, uintptr_t out, size_t nelem, size_t slice_elems,
-         int dtype, float post_scale, uint64_t flag, int channel, bool contribute, int blocks, int barrier_mode,
-         uintptr_t stream) {
+         int dtype, float post_scale, uint64_t flag, int channel, bool contribute, int blocks, uintptr_t stream) {
         q8_reduce_scatter_launch(pt.pt, st.dev(), off, P<void>(in), P<void>(out), nelem, slice_elems, dtype, post_scale, flag,
-                                 channel, contribute ? 1 : 0, blocks, barrier_mode, S(stream));
+                                 channel, contribute ? 1 : 0, blocks, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("off"), py::arg("input"), py::arg("out"), py::arg("nelem"),
       py::arg("slice_elems"), py::arg("dtype"), py::arg("post_scale"), py::arg("flag"), py::arg("channel"),
-      py::arg("contribute"), py::arg("blocks"), py::arg("barrier_mode"), py::arg("stream"));
+      py::arg("contribute"), py::arg("blocks"), py::arg("stream"));
 
   m.def("rmsnorm_fwd", [](uintptr_t x, uintptr_t w, uintptr_t y, uintptr_t rstd, int rows, int H,
                           float eps, uintptr_t s) {
@@ -482,9 +479,6 @@ PYBIND11_MODULE(_K, m) {
      py::arg("mu"), py::arg("nesterov"), py::arg("alpha"), py::arg("gate"), py::arg("stream"));
   m.def("sumsq", [](uintptr_t g, size_t n, uintptr_t out, uintptr_t s) {
     sumsq_launch(P<void>(g), n, P<float>(out), S(s));
-  });
-  m.def("heal_copy_bulk", [](uintptr_t table_dev, int nentries, size_t total_chunks, size_t chunk_bytes, int blocks, uintptr_t s) {
-    heal_copy_bulk_launch(P<void>(table_dev), nentries, total_chunks, chunk_bytes, blocks, S(s));
   });
   m.def("heal_copy", [](uintptr_t table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                         int blocks, uintptr_t s) {

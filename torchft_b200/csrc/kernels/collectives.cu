@@ -68,7 +68,6 @@ struct XArgs {
   size_t slot_stride;        // staging bytes per source rank
   uint64_t flag;             // consumes flag+1, flag+2
   int channel;
-  int barrier_mode;
 };
 
 __global__ void __launch_bounds__(512, 1) push_exchange_kernel(XArgs a) {
@@ -82,7 +81,7 @@ __global__ void __launch_bounds__(512, 1) push_exchange_kernel(XArgs a) {
     if (lo < hi)
       copy_bytes(reinterpret_cast<char*>(a.pt.data[p]) + (size_t)rank * a.slot_stride + lo, a.in + a.send_off[p] + lo, hi - lo);
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/true, /*acquire=*/true, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/true, /*acquire=*/true)) return;
   // ---- copy out: every source's slot of my staging ----
   const char* mine = reinterpret_cast<const char*>(a.pt.data[rank]);
   for (int p = 0; p < W; ++p) {
@@ -92,7 +91,7 @@ __global__ void __launch_bounds__(512, 1) push_exchange_kernel(XArgs a) {
     if (lo < hi) copy_bytes(a.out + a.out_off[p] + lo, mine + (size_t)p * a.slot_stride + lo, hi - lo);
   }
   // nobody may start overwriting my staging (next collective) before I have copied it out
-  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false, a.barrier_mode);
+  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
 }
 
 enum RedOp : int { kSum = 0, kMax = 1, kMin = 2 };
@@ -113,7 +112,6 @@ struct RSArgs {
   float scale;
   uint64_t flag;
   int channel;
-  int barrier_mode;
 };
 
 template <typename T, int W, int OP>
@@ -131,7 +129,7 @@ __global__ void __launch_bounds__(512, 1) reduce_scatter_kernel(RSArgs a) {
       copy_bytes(reinterpret_cast<char*>(mine + (size_t)s * a.n + lo), reinterpret_cast<const char*>(in + (size_t)s * a.n + lo),
                  (hi - lo) * sizeof(T));
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/a.user_in != nullptr, /*acquire=*/false, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/a.user_in != nullptr, /*acquire=*/false)) return;
   {
     const T* src[W];
 #pragma unroll
@@ -174,7 +172,7 @@ __global__ void __launch_bounds__(512, 1) reduce_scatter_kernel(RSArgs a) {
       }
     }
   }
-  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false, a.barrier_mode);
+  block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
 }
 
 // ---------------------------------------------------------------------------
@@ -284,7 +282,7 @@ void launch_rs_op(const RSArgs& a, int op, int blocks, cudaStream_t s) {
 
 void push_exchange_launch(const PeerTable& pt, StatusBlock* st, const void* in, void* out, const size_t* send_off,
                           const size_t* send_len, const size_t* recv_len, const size_t* out_off, size_t slot_stride,
-                          uint64_t flag, int channel, int blocks, int barrier_mode, cudaStream_t stream) {
+                          uint64_t flag, int channel, int blocks, cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("push_exchange: bad grid");
   if (slot_stride & 15) throw std::runtime_error("push_exchange: slot stride must be a multiple of 16 bytes");
   XArgs a;
@@ -304,17 +302,16 @@ void push_exchange_launch(const PeerTable& pt, StatusBlock* st, const void* in, 
   a.slot_stride = slot_stride;
   a.flag = flag;
   a.channel = channel;
-  a.barrier_mode = barrier_mode;
   push_exchange_kernel<<<blocks, 512, 0, stream>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
 void reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* user_in, void* out, size_t n,
-                           int dtype, int op, float scale, uint64_t flag, int channel, int blocks, int barrier_mode,
+                           int dtype, int op, float scale, uint64_t flag, int channel, int blocks,
                            cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("reduce_scatter: bad grid");
   if (off & 15) throw std::runtime_error("reduce_scatter: offset must be 16 B aligned");
-  RSArgs a{pt, st, off, user_in, out, n, scale, flag, channel, barrier_mode};
+  RSArgs a{pt, st, off, user_in, out, n, scale, flag, channel};
   switch (dtype) {
     case kF32: launch_rs_op<float>(a, op, blocks, stream); break;
     case kBF16: launch_rs_op<__nv_bfloat16>(a, op, blocks, stream); break;

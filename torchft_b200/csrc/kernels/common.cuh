@@ -74,11 +74,6 @@ struct PeerTable {
 __device__ __forceinline__ void st_release_sys(uint64_t* p, uint64_t v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) {
-  uint64_t v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ uint64_t ld_relaxed_sys(const uint64_t* p) {
   uint64_t v;
   asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
@@ -173,78 +168,24 @@ __device__ __forceinline__ bool wait_flag(const uint64_t* flag, uint64_t expecte
 //   acquire: this CTA reads peer-written data after the barrier within this
 //            kernel (all such loads bypass L1).
 //
-// `mode` selects the memory-ordering recipe (tuned on hardware, bench/comm_tune.py):
-//   0  per-peer thread: [fence.sc.sys if release] st.release.sys ; poll ld.acquire.sys
-//   1  per-peer thread: st.release.sys ; poll ld.relaxed.sys ; fence.acq_rel.sys
-//   2  per-peer thread (all in warp 0): [fence.acq_rel.sys if release] ; st.relaxed.sys ; poll relaxed ;
-//      [fence.acq_rel.sys if acquire]        (<= 2 warp-wide system fences per CTA, each in program order with its flag access)
-//   3  like 2 but the flag is published with red.release.sys (atomic max) so the
-//      store cannot linger in a write-combining path
-__device__ __forceinline__ bool wait_flag_acquire(const uint64_t* flag, uint64_t expected,
-                                                  StatusBlock* st, int peer, uint64_t budget) {
-  if (ld_acquire_sys(flag) >= expected) return true;
-  uint64_t t0 = 0;
-  uint32_t spins = 0;
-  while (true) {
-    if (ld_acquire_sys(flag) >= expected) return true;
-    if ((++spins & 0x3ff) == 0) {
-      if (st->abort || st->error != kOk) {
-        if (st->error == kOk) {
-          st->error_rank = peer;
-          st->error_seq = (uint32_t)expected;
-          st->error = kErrAborted;
-        }
-        return false;
-      }
-      if (t0 == 0) t0 = globaltimer_ns();
-      if (globaltimer_ns() - t0 > budget) {
-        st->error_rank = peer;
-        st->error_seq = (uint32_t)expected;
-        st->error = kErrTimeout;
-        __threadfence_system();
-        return false;
-      }
-    }
-    __nanosleep(32);
-  }
-}
-
-__device__ __forceinline__ void red_max_release_sys(uint64_t* p, uint64_t v) {
-  asm volatile("red.release.sys.global.max.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
+// Thread t < world (t != rank) signals peer t and waits for it: [fence.acq_rel.sys if release] ; st.relaxed.sys of
+// the flag into the peer's pad ; relaxed polling of our own pad (wait_flag) ; [fence.acq_rel.sys if acquire].
+// The signalling threads all sit in warp 0, so "every signalling thread fences" costs one warp-wide fence
+// instruction -- the same as thread 0 alone -- but gives each flag store / flag poll its own fence IN PROGRAM ORDER,
+// i.e. a well-formed release (fence; st.relaxed) and acquire (ld.relaxed; fence) pattern under the PTX memory model,
+// with at most two system fences per CTA and none per poll.
+// The CTA's data accesses are ordered around them by the __syncthreads() that opens this function (and the
+// __syncthreads_and() that closes it): bar.sync is morally strong at CTA scope and the fences are cumulative.
 __device__ __forceinline__ bool block_barrier(const PeerTable& pt, int ch, uint64_t flag,
-                                              StatusBlock* st, bool release, bool acquire, int mode) {
+                                              StatusBlock* st, bool release, bool acquire) {
   __syncthreads();
   const int t = threadIdx.x;
   int ok = 1;
-  if (mode <= 1) {
-    if (t < pt.world && t != pt.rank) {
-      if (mode == 0 && release) __threadfence_system();
-      st_release_sys(&pt.pads[t]->sig[ch][blockIdx.x][pt.rank], flag);
-      if (mode == 0) {
-        ok = wait_flag_acquire(&pt.pads[pt.rank]->sig[ch][blockIdx.x][t], flag, st, t, pt.timeout_ns) ? 1 : 0;
-      } else {
-        ok = wait_flag(&pt.pads[pt.rank]->sig[ch][blockIdx.x][t], flag, st, t, pt.timeout_ns) ? 1 : 0;
-        fence_acq_rel_sys();
-      }
-    }
-    return __syncthreads_and(ok) != 0;
-  }
-  // The signalling threads t < world all sit in warp 0, so "every signalling thread fences" costs one warp-wide fence
-  // instruction -- the same as thread 0 alone -- but gives each flag store / flag poll its own fence IN PROGRAM ORDER,
-  // i.e. a well-formed release (fence; st.relaxed) and acquire (ld.relaxed; fence) pattern under the PTX memory model.
-  // The CTA's data accesses are ordered around them by the __syncthreads() that opened this function (and the
-  // __syncthreads_and() below): bar.sync is morally strong at CTA scope and the fences are cumulative.
   const bool signaller = t < pt.world && t != pt.rank;
   if (t < 32) {
     if (signaller) {
       if (release) fence_acq_rel_sys();
-      uint64_t* remote = &pt.pads[t]->sig[ch][blockIdx.x][pt.rank];
-      if (mode == 3)
-        red_max_release_sys(remote, flag);
-      else
-        st_relaxed_sys(remote, flag);
+      st_relaxed_sys(&pt.pads[t]->sig[ch][blockIdx.x][pt.rank], flag);
       ok = wait_flag(&pt.pads[pt.rank]->sig[ch][blockIdx.x][t], flag, st, t, pt.timeout_ns) ? 1 : 0;
     }
     __syncwarp();  // reconverge the pollers so the acquire fence is ONE warp-wide instruction again

@@ -654,144 +654,6 @@ __global__ void __launch_bounds__(512) heal_copy_kernel(const CopyEntry* __restr
   }
 }
 
-// ------------------------------- heal copy, TMA bulk variant -------------------------------
-// Same job, driven by the copy engine instead of the LSU: ONE thread per CTA runs a 4-stage ring of 16 KiB shared-memory
-// buffers -- `cp.async.bulk` global->shared (completion on an mbarrier, transaction-byte counted) followed by
-// `cp.async.bulk` shared->global (bulk groups) -- so 64 KiB are in flight per CTA with 32 threads and ~30 registers, three
-// CTAs per SM. No data ever passes through registers. Source may be a mapped peer (NVLink) address. Needs 16-byte
-// aligned ranges; the host falls back to heal_copy_kernel otherwise. SASS: UBLKCP (bulk copy), SYNCS (mbarrier).
-constexpr int kBulkStages = 4;
-constexpr uint32_t kBulkBytes = 16 * 1024;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes)
-               : "memory");
-}
-
-// Cursor over the 16 KiB pieces of the chunks c = blockIdx.x, blockIdx.x + gridDim.x, ... owned by this CTA.
-struct PieceCursor {
-  const CopyEntry* table;
-  int nentries;
-  size_t total_chunks, chunk_bytes;
-  size_t c;        // current chunk
-  size_t off;      // byte offset of the next piece inside the chunk
-  const char* src;
-  char* dst;
-  size_t len;      // bytes of the current chunk (multiple of 16 except possibly the entry's last chunk)
-  __device__ void load_chunk() {
-    if (c >= total_chunks) return;
-    int lo = 0, hi = nentries - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (table[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
-    }
-    const CopyEntry e = table[lo];
-    const size_t start = (c - e.chunk0) * chunk_bytes;
-    src = e.src + start;
-    dst = e.dst + start;
-    len = min(chunk_bytes, e.bytes - start);
-    off = 0;
-  }
-  __device__ bool next(const char** s, char** d, uint32_t* n) {
-    while (c < total_chunks && off >= (len & ~size_t(15))) {
-      c += gridDim.x;
-      load_chunk();
-    }
-    if (c >= total_chunks) return false;
-    const size_t body = len & ~size_t(15);
-    *n = (uint32_t)min((size_t)kBulkBytes, body - off);
-    *s = src + off;
-    *d = dst + off;
-    off += *n;
-    return true;
-  }
-};
-
-__global__ void __launch_bounds__(32) heal_copy_bulk_kernel(const CopyEntry* __restrict__ table, int nentries,
-                                                            size_t total_chunks, size_t chunk_bytes) {
-  extern __shared__ __align__(128) unsigned char ring[];
-  __shared__ __align__(8) uint64_t full[kBulkStages];
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int i = 0; i < kBulkStages; ++i) mbar_init(&full[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-  // sub-16-byte tails of entries (at most one per entry) are copied by the lanes the pipeline does not need
-  if (threadIdx.x != 0) {
-    for (int e = blockIdx.x * 31 + (threadIdx.x - 1); e < nentries; e += gridDim.x * 31) {
-      const CopyEntry t = table[e];
-      for (size_t k = t.bytes & ~size_t(15); k < t.bytes; ++k) t.dst[k] = t.src[k];
-    }
-    return;
-  }
-  PieceCursor ld{table, nentries, total_chunks, chunk_bytes, blockIdx.x, 0, nullptr, nullptr, 0};
-  ld.load_chunk();
-  // the store side replays the same sequence of pieces: remember them in a small ring instead of a second cursor
-  char* sdst[kBulkStages];
-  uint32_t slen[kBulkStages];
-  size_t issued = 0, stored = 0;
-  const char* s;
-  char* d;
-  uint32_t n;
-  // prologue: fill the ring
-  while (issued < kBulkStages && ld.next(&s, &d, &n)) {
-    const int st = (int)(issued % kBulkStages);
-    mbar_expect_tx(&full[st], n);
-    bulk_g2s(ring + (size_t)st * kBulkBytes, s, n, &full[st]);
-    sdst[st] = d;
-    slen[st] = n;
-    ++issued;
-  }
-  while (stored < issued) {
-    const int st = (int)(stored % kBulkStages);
-    mbar_wait(&full[st], (uint32_t)((stored / kBulkStages) & 1));
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    bulk_s2g(sdst[st], ring + (size_t)st * kBulkBytes, slen[st]);
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    ++stored;
-    // refill the stage of the PREVIOUS piece: its store has finished reading shared memory once at most one group is pending
-    if (stored >= 2 && issued == stored - 2 + kBulkStages) {
-      asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      if (ld.next(&s, &d, &n)) {
-        const int rs = (int)(issued % kBulkStages);
-        mbar_expect_tx(&full[rs], n);
-        bulk_g2s(ring + (size_t)rs * kBulkBytes, s, n, &full[rs]);
-        sdst[rs] = d;
-        slen[rs] = n;
-        ++issued;
-      }
-    }
-  }
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
 // ------------------------------- launchers ----------------------------------
 static int grid_for(size_t work_items, int threads, int cap = kNumSMs * 8) {
   size_t g = (work_items + threads - 1) / threads;
@@ -973,21 +835,6 @@ void diloco_outer_launch(void* param, void* original, const void* grad, float* m
 
 void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s) {
   sumsq_kernel<<<grid_for(n / 8 + 1, 512, kNumSMs * 4), 512, 0, s>>>((const bf16*)g, n, out);
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void heal_copy_bulk_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes, int blocks,
-                           cudaStream_t s) {
-  if (total_chunks == 0) return;
-  if (chunk_bytes % 16) throw std::runtime_error("heal_copy_bulk: chunk size must be a multiple of 16 bytes");
-  static bool configured = false;
-  const int smem = kBulkStages * (int)kBulkBytes;
-  if (!configured) {
-    TFT_CUDA_CHECK(cudaFuncSetAttribute(heal_copy_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = true;
-  }
-  if (blocks < 1) blocks = 1;
-  heal_copy_bulk_kernel<<<blocks, 32, smem, s>>>((const CopyEntry*)table_dev, nentries, total_chunks, chunk_bytes);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -271,7 +271,6 @@ struct Q8Args {
   uint64_t flag;
   int channel;
   int contribute;
-  int barrier_mode;
   // mode 0: all-reduce (slices are contiguous runs of groups: slice_elems == groups_per_slice * 512).
   // mode 1: reduce-scatter (torchft/collectives.py:159-294): rank-slice s covers elements
   //         [s * slice_elems, (s+1) * slice_elems), quantised on its own group grid; `out` receives the
@@ -315,7 +314,7 @@ __global__ void __launch_bounds__(512, 1) q8_allreduce_kernel(Q8Args a) {
       st_stream(mine + poff + g * kGroup + lane * 16, q);
     }
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/true, /*acquire=*/false, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 1, a.st, /*release=*/true, /*acquire=*/false)) return;
 
   // ---- phase B: fp32 reduce of my slice from every peer, requantise, push ----
   {
@@ -361,10 +360,10 @@ __global__ void __launch_bounds__(512, 1) q8_allreduce_kernel(Q8Args a) {
   }
   if (a.mode == 1) {
     // peers must not requantise their next message over staging we are still reading
-    block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false, a.barrier_mode);
+    block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
     return;
   }
-  if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/true, a.barrier_mode)) return;
+  if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/true, /*acquire=*/true)) return;
 
   // ---- phase C: dequantise chunk b of every slice into the output tensor ----
   for (int s = 0; s < W; ++s) {
@@ -578,8 +577,7 @@ static void q8_ar_w(const Q8Args& a, int blocks, cudaStream_t stream) {
 
 void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in_a,
                          const void* in_b, void* out, size_t nelem, int dtype, float post_scale,
-                         uint64_t flag, int channel, int contribute, int blocks, int barrier_mode,
-                         cudaStream_t stream) {
+                         uint64_t flag, int channel, int contribute, int blocks, cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("q8_allreduce: bad grid");
   if (off & 15) throw std::runtime_error("q8_allreduce: offset must be 16 B aligned");
   Q8Args a;
@@ -595,7 +593,6 @@ void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  a.barrier_mode = barrier_mode;
   a.mode = 0;
   a.slice_elems = a.ngroups / pt.world * kGroup;
   if (pt.world < 2) throw std::runtime_error("q8_allreduce: world must be >= 2");
@@ -648,7 +645,7 @@ size_t q8_rs_buffer_bytes(size_t slice_elems, int world) {
 
 void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in, void* out, size_t nelem,
                               size_t slice_elems, int dtype, float post_scale, uint64_t flag, int channel,
-                              int contribute, int blocks, int barrier_mode, cudaStream_t stream) {
+                              int contribute, int blocks, cudaStream_t stream) {
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("q8_reduce_scatter: bad grid");
   if (off & 15) throw std::runtime_error("q8_reduce_scatter: offset must be 16 B aligned");
   if (pt.world < 2) throw std::runtime_error("q8_reduce_scatter: world must be >= 2");
@@ -667,7 +664,6 @@ void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, 
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  a.barrier_mode = barrier_mode;
   a.mode = 1;
   a.slice_elems = slice_elems;
   switch (dtype) {

@@ -103,7 +103,7 @@ struct Geo {
 // Handshake: one CTA, one flag exchange with every peer.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(32, 1) zero1_handshake_kernel(HsArgs a) {
-  const bool ok = block_barrier(a.pt, a.channel, a.flag + 1, a.st, a.release != 0, /*acquire=*/true, a.barrier_mode);
+  const bool ok = block_barrier(a.pt, a.channel, a.flag + 1, a.st, a.release != 0, /*acquire=*/true);
   if (threadIdx.x == 0) *a.ok_out = ok ? 1 : 0;
 }
 

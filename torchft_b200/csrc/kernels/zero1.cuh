@@ -17,8 +17,7 @@ struct HsArgs {
   int* ok_out;       // device word receiving 1/0, so the sync-free kernels behind it on the stream can turn into no-ops
   uint64_t flag;     // consumes flag+1
   int channel;
-  int release;       // this rank wrote peer-visible data in an earlier kernel of this stream
-  int barrier_mode;
+  int release;       // this rank wrote peer-visible data in an earlier kernel of this stream: fence before the flag store
 };
 
 // Reduce-scatter of one unit in place: rank r reduces slice r and stores it to itself and its k-1 buddies.

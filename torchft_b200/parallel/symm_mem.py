@@ -125,7 +125,6 @@ class SymmetricComm:
         self._peer_vmm: Dict[Tuple[str, int, str], Tuple[int, int, int]] = {}  # (host, pid, seg) -> (va, handle, size)
         self._mc: Dict[str, Tuple[int, int, int]] = {}  # segment -> (mc handle, multicast va, size)
         self._mc_gen, self._mc_members = "", ""  # creation the objects in _mc belong to / the member list they span
-        self._barrier_mode = int(os.environ.get("TORCHFT_B200_BARRIER_MODE", "2"))
         self._force_plan: Optional[Tuple[int, int]] = None  # (algo, blocks) override for tuning sweeps
         self.launches = 0  # native kernel launches issued (bench reports this)
         self._ptrs: Dict[str, List[int]] = {}  # segment -> mapped base pointer per quorum rank
@@ -501,12 +500,12 @@ class SymmetricComm:
                         and self._force_plan is None):
                     blocks = max(8, min(self._max_blocks, (n * es) // (64 << 10)))
                     K.allreduce_nvls(self._tables[seg.name], self._status, mc[1], off, n, dt, scale, self._next_flag(),
-                                     _CH_ALLREDUCE, contribute, blocks, self._threads, self._barrier_mode, sp)
+                                     _CH_ALLREDUCE, contribute, blocks, self._threads, sp)
                     self.launches += 1
                     return
                 algo, blocks = self._plan(n * es)
                 K.allreduce(self._tables[seg.name], self._status, off, 0, 0, n, dt, op, scale, self._next_flag(),
-                            _CH_ALLREDUCE, contribute, algo, blocks, self._threads, self._barrier_mode, sp)
+                            _CH_ALLREDUCE, contribute, algo, blocks, self._threads, sp)
                 self.launches += 1
                 return
             if t.data_ptr() % 16:
@@ -518,7 +517,7 @@ class SymmetricComm:
                 algo, blocks = self._plan(n * es)
                 ptr = flat.data_ptr() + lo * es
                 K.allreduce(self._tables["core"], self._status, 0, ptr, ptr, n, dt, op, scale, self._next_flag(),
-                            _CH_ALLREDUCE, contribute, algo, blocks, self._threads, self._barrier_mode, sp)
+                            _CH_ALLREDUCE, contribute, algo, blocks, self._threads, sp)
                 self.launches += 1
 
     def q8_bytes(self, numel: int) -> int:
@@ -582,7 +581,7 @@ class SymmetricComm:
                 blocks = max(4, min(self._q8_max_blocks, (n // 512) // 32 + 1))
                 K.q8_allreduce(self._tables["core"], self._status, 0, fa.data_ptr() + lo * es,
                                (fb.data_ptr() + lo * es) if fb is not None else 0, fo.data_ptr() + lo * es, n, dt,
-                               scale, self._next_flag(), _CH_Q8, contribute, blocks, self._barrier_mode, sp)
+                               scale, self._next_flag(), _CH_Q8, contribute, blocks, sp)
                 self.launches += 1
 
     def q8_reduce_scatter_(self, out: torch.Tensor, inp: torch.Tensor, slice_elems: int, scale: float = 1.0,
@@ -604,8 +603,7 @@ class SymmetricComm:
             groups = W * ((slice_elems + 511) // 512)
             blocks = max(4, min(self._q8_max_blocks, groups // 32 + 1))
             self._K.q8_reduce_scatter(self._tables["core"], self._status, 0, inp.data_ptr(), out.data_ptr(), inp.numel(), slice_elems,
-                                      dt, scale, self._next_flag(), _CH_Q8, contribute, blocks, self._barrier_mode,
-                                      _native.stream_ptr(stream))
+                                      dt, scale, self._next_flag(), _CH_Q8, contribute, blocks, _native.stream_ptr(stream))
             self.launches += 1
 
     # ------------------------------------------------------------------ the rest of the collective surface
@@ -632,7 +630,7 @@ class SymmetricComm:
             r_off = [o + min(lo, n) for o, n in recv]
             r_len = [max(0, min(stride, n - lo)) for _, n in recv]
             self._K.push_exchange(self._tables["core"], self._status, inp, out, s_off, s_len, r_len, r_off, stride,
-                                  self._next_flag(), _CH_ALLREDUCE, self._xblocks(max(s_len + r_len)), self._barrier_mode, sp)
+                                  self._next_flag(), _CH_ALLREDUCE, self._xblocks(max(s_len + r_len)), sp)
             self.launches += 1
 
     @staticmethod
@@ -738,13 +736,13 @@ class SymmetricComm:
             if hit is not None and hit[0].name != "core" and hit[1] % 16 == 0:
                 seg, off = hit  # zero-copy: peers read the input where it lives
                 self._K.reduce_scatter(self._tables[seg.name], self._status, off, 0, out.data_ptr(), n, dt, op, scale,
-                                       self._next_flag(), _CH_ALLREDUCE, self._xblocks(n * es), self._barrier_mode, sp)
+                                       self._next_flag(), _CH_ALLREDUCE, self._xblocks(n * es), sp)
                 self.launches += 1
                 return
             per = (self._staging_usable // (W * es)) // 8 * 8  # elements of every slot per round (16 B aligned slots)
             if n <= per:
                 self._K.reduce_scatter(self._tables["core"], self._status, 0, inp.data_ptr(), out.data_ptr(), n, dt, op, scale,
-                                       self._next_flag(), _CH_ALLREDUCE, self._xblocks(n * es), self._barrier_mode, sp)
+                                       self._next_flag(), _CH_ALLREDUCE, self._xblocks(n * es), sp)
                 self.launches += 1
                 return
             rows, flat_out = inp.view(W, n), out.view(-1)
@@ -752,7 +750,7 @@ class SymmetricComm:
                 hi = min(n, lo + per)
                 piece = rows[:, lo:hi].contiguous()
                 self._K.reduce_scatter(self._tables["core"], self._status, 0, piece.data_ptr(), flat_out[lo:hi].data_ptr(), hi - lo, dt,
-                                       op, scale, self._next_flag(), _CH_ALLREDUCE, self._xblocks((hi - lo) * es), self._barrier_mode, sp)
+                                       op, scale, self._next_flag(), _CH_ALLREDUCE, self._xblocks((hi - lo) * es), sp)
                 piece.record_stream(stream if stream is not None else torch.cuda.current_stream())
                 self.launches += 1
 
@@ -808,8 +806,7 @@ class SymmetricComm:
         return p, p + 8 * n
 
     def _handshake(self, slot: int, release: bool, channel: int, sp: int) -> None:
-        self._K.zero1_handshake(self._tables["core"], self._status, self._z1_ok(slot), self._next_flag(), channel, release,
-                                self._barrier_mode, sp)
+        self._K.zero1_handshake(self._tables["core"], self._status, self._z1_ok(slot), self._next_flag(), channel, release, sp)
         self.launches += 1
 
     def zero1_reduce_scatter_(self, segment: str, off: int, nelem: int, scale: float, contribute: bool,
