@@ -12,7 +12,7 @@ import pytest
 import torch
 
 import _q8_emulation as E
-from test_collectives_gpu import _ok, _run, _world
+from _collectives import _ok, _run, _world
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)

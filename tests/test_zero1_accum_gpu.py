@@ -9,51 +9,18 @@ Ranks are emulated in-process with ``SymmetricComm.virtual_world`` (see ``test_z
 
 from __future__ import annotations
 
-from datetime import timedelta
-
 import pytest
 import torch
 
-from _zero1_replicas import Replicas, ref_adamw
+from _zero1_replicas import NUMEL, UNITS, Replicas, kernel_world, raws, reduced, ref_adamw, trainer
 
 pytestmark = pytest.mark.gpu
 
-UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
-NUMEL = UNITS[-1][1]
 MAX_NORM = 50.0
-
-
-def _world(world, presignal=True):
-    from torchft_b200.parallel.symm_mem import SymmetricComm
-
-    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS)}
-    return SymmetricComm.virtual_world(world, seg, presignal=presignal, timeout=timedelta(seconds=20))
-
-
-def _raws(world, M, seed, scale=1.0):
-    """``raws[m][r]``: rank r's bf16 gradient of micro-batch m."""
-    dev = torch.device("cuda", 0)
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return [[(torch.randn(NUMEL, device=dev, generator=g) * (r + 1) * scale).bfloat16() for r in range(world)]
-            for _ in range(M)]
 
 
 def _scale(contributors, M):
     return 1.0 / (contributors * M)
-
-
-def _reduced(raws, quiet=None, contributors=None):
-    """The reference of the module doc; a quiet (healing / spare) rank contributes zeros in every micro-batch."""
-    world, M = len(raws[0]), len(raws)
-    contributors = contributors or world - (1 if quiet is not None else 0)
-    total = None
-    for raw in raws:
-        s = None
-        for r in range(world):
-            g = torch.zeros_like(raw[r], dtype=torch.float32) if r == quiet else raw[r].float()
-            s = g.clone() if s is None else s + g
-        total = s if total is None else total + s
-    return (total * torch.tensor(_scale(contributors, M), dtype=torch.float32, device=total.device)).bfloat16()
 
 
 def _accs(world, k):
@@ -68,17 +35,17 @@ def _accs(world, k):
     return out
 
 
-def _accum_reduce(world, k, raws, quiet=None, presignal=True, clip=False):
+def _accum_reduce(world, k, micro, quiet=None, presignal=True, clip=False):
     """All micro-batches of one step through ``zero1_reduce_scatter_`` with the accumulator. Returns every rank's
     gradient segment afterwards and (``clip``) its per-unit sum-of-squares partials."""
     from torchft_b200.parallel.zero1 import accum_mode
 
     dev = torch.device("cuda", 0)
-    comms = _world(world, presignal)
+    comms = kernel_world(world, presignal)
     grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     gnorm = [c.segment("z1_gnorm")[: 8 * len(UNITS)].view(torch.float64) for c in comms]
     accs = _accs(world, k)
-    M = len(raws)
+    M = len(micro)
     scale = _scale(world - (1 if quiet is not None else 0), M)
     order = ([quiet] if quiet is not None else []) + [r for r in range(world) if r != quiet]
 
@@ -91,7 +58,7 @@ def _accum_reduce(world, k, raws, quiet=None, presignal=True, clip=False):
                                            acc=acc.data_ptr() + 4 * offs[u], acc_mode=mode)
 
     if presignal:
-        for m, raw in enumerate(raws):
+        for m, raw in enumerate(micro):
             for r in range(world):  # backward of micro-batch m rewrites every rank's gradient buffer
                 grads[r].copy_(raw[r])
             if quiet is not None:
@@ -107,7 +74,7 @@ def _accum_reduce(world, k, raws, quiet=None, presignal=True, clip=False):
         comm = [torch.cuda.Stream(device=dev) for _ in comms]
         done = [torch.cuda.Event() for _ in comms]
         torch.cuda.synchronize()
-        for m, raw in enumerate(raws):
+        for m, raw in enumerate(micro):
             for r in range(world):
                 if m > 0:
                     compute[r].wait_event(done[r])
@@ -121,7 +88,7 @@ def _accum_reduce(world, k, raws, quiet=None, presignal=True, clip=False):
     return [g.clone() for g in grads], [x.clone() for x in gnorm]
 
 
-def _check_holders(world, k, grads, reduced):
+def _check_holders(world, k, grads, want):
     from torchft_b200.parallel.zero1 import ShardLayout
 
     L = ShardLayout(tuple(UNITS), k)
@@ -129,7 +96,7 @@ def _check_holders(world, k, grads, reduced):
         for s in range(world):
             lo, hi = L.slice_bounds(u, world, s)
             for h in L.holders(u, world, s):
-                assert torch.equal(grads[h][lo:hi], reduced[lo:hi]), f"holder {h} of unit {u} slice {s}"
+                assert torch.equal(grads[h][lo:hi], want[lo:hi]), f"holder {h} of unit {u} slice {s}"
 
 
 # ----------------------------------------------------------------------------- the kernel modes vs the reference
@@ -137,21 +104,21 @@ def _check_holders(world, k, grads, reduced):
 @pytest.mark.parametrize("world,k", [(1, 1), (2, 2), (3, 2), (4, 3), (8, 1), (8, 2)])
 def test_accumulated_reduce_matches_reference_bit_for_bit(world, k, M):
     quiet = 1 if world > 2 else None
-    raws = _raws(world, M, 10 * world + k + M)
-    grads, _ = _accum_reduce(world, k, raws, quiet=quiet)
-    _check_holders(world, k, grads, _reduced(raws, quiet))
+    micro = raws(world, 10 * world + k + M, (1.0,) * M)
+    grads, _ = _accum_reduce(world, k, micro, quiet=quiet)
+    _check_holders(world, k, grads, reduced(micro, quiet))
 
 
 def test_without_accumulator_the_launch_is_todays():
     """``acc = 0`` / ``acc_mode = 0`` is the plain launch: same number of launches, same bits."""
     world, k = 4, 2
-    raws = _raws(world, 1, 3)
+    micro = raws(world, 3)
     out = []
     for kw in ({}, {"acc": 0, "acc_mode": 0}):
-        comms = _world(world)
+        comms = kernel_world(world)
         grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
         for r in range(world):
-            grads[r].copy_(raws[0][r])
+            grads[r].copy_(micro[0][r])
         torch.cuda.synchronize()
         before = [c.launches for c in comms]
         for r in range(world):
@@ -161,19 +128,19 @@ def test_without_accumulator_the_launch_is_todays():
         out.append(([c.launches - b for c, b in zip(comms, before)], [g.clone() for g in grads]))
     assert out[0][0] == out[1][0]
     assert all(torch.equal(a, b) for a, b in zip(out[0][1], out[1][1]))
-    _check_holders(world, k, out[0][1], _reduced(raws))
+    _check_holders(world, k, out[0][1], reduced(micro))
 
 
 def test_real_signalling_between_micro_batches_gives_the_presignalled_bits():
     """W = 4 ranks in flight at once; each rank overwrites its gradient with the next micro-batch only behind the event
     its comm stream recorded after the previous micro-batch's trailing handshakes."""
     world, k, M = 4, 2, 3
-    raws = _raws(world, M, 44)
-    seq, _ = _accum_reduce(world, k, raws)
-    real, _ = _accum_reduce(world, k, raws, presignal=False)
+    micro = raws(world, 44, (1.0,) * M)
+    seq, _ = _accum_reduce(world, k, micro)
+    real, _ = _accum_reduce(world, k, micro, presignal=False)
     for r in range(world):
         assert torch.equal(seq[r], real[r]), f"rank {r}"
-    _check_holders(world, k, real, _reduced(raws))
+    _check_holders(world, k, real, reduced(micro))
 
 
 @pytest.mark.parametrize("world,k", [(1, 1), (4, 2)])
@@ -181,12 +148,12 @@ def test_norm_of_the_accumulated_gradient(world, k):
     """The last micro-batch's sum-of-squares partials are bit-identical to those the M = 1 clipping path produces from
     ``reduced`` itself (rank 0 holding ``reduced``, every other rank zeros, scale 1), and their total is its norm."""
     M = 3
-    raws = _raws(world, M, 60 + world)
-    reduced = _reduced(raws)
-    grads, parts = _accum_reduce(world, k, raws, clip=True)
-    _check_holders(world, k, grads, reduced)
-    plain = [[reduced] + [torch.zeros_like(reduced)] * (world - 1)]
-    comms = _world(world)
+    micro = raws(world, 60 + world, (1.0,) * M)
+    red = reduced(micro)
+    grads, parts = _accum_reduce(world, k, micro, clip=True)
+    _check_holders(world, k, grads, red)
+    plain = [[red] + [torch.zeros_like(red)] * (world - 1)]
+    comms = kernel_world(world)
     g = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     gn = [c.segment("z1_gnorm")[: 8 * len(UNITS)].view(torch.float64) for c in comms]
     for r in range(world):
@@ -198,23 +165,18 @@ def test_norm_of_the_accumulated_gradient(world, k):
     torch.cuda.synchronize()
     for r in range(world):
         assert torch.equal(parts[r], gn[r]), f"partials of rank {r}"
-    norm = float(reduced.double().norm())
+    norm = float(red.double().norm())
     dev = float(sum(float(p.sum()) for p in parts)) ** 0.5
     assert abs(dev - norm) <= 1e-5 * norm
 
 
 # ----------------------------------------------------------------------------- Zero1Optimizer
-def _replicas(n, M, compact=False, max_norm=None, min_world=3, k=2):
-    """``n`` replicas accumulating ``M`` micro-batches, driven through quorum changes."""
-    return Replicas(n, UNITS, k=k, compact=compact, min_world=min_world, max_norm=max_norm, M=M)
-
-
 @pytest.mark.parametrize("compact", [False, True])
 def test_optimizer_accumulates_through_a_change_of_world(compact):
     from torchft_b200.parallel.zero1 import ShardLayout, accum_elements, accum_offsets
 
     M, k = 3, 2
-    reps = _replicas(4, M, compact=compact)
+    reps = Replicas(4, compact=compact, min_world=3, grad_accum_steps=M)
     L = ShardLayout(tuple(UNITS), k)
     assert all(o.accum_bytes() == 4 * accum_elements(L, 3) for o in reps.opts)
     dev = torch.device("cuda", 0)
@@ -234,16 +196,16 @@ def test_optimizer_accumulates_through_a_change_of_world(compact):
             assert reps.opts[i]._acc_offsets == accum_offsets(L, rank, world)[0]
         for _ in range(2):
             seed += 1
-            raws = _raws(world, M, seed, scale=0.01)
-            reps.step(raws)
-            reduced = _reduced(raws)
+            micro = raws(world, seed, (0.01,) * M)
+            reps.step(micro)
+            red = reduced(micro)
             t += 1
-            ref_adamw(rm, rmm, rv, reduced.float(), t)
+            ref_adamw(rm, rmm, rv, red.float(), t)
             assert reps.verdicts() == {i: True for i in members}
             for rank, i in enumerate(members):
                 o = reps.opts[i]
                 for lo, hi in L.held(rank, world):  # the update read exactly the reference's reduced gradient
-                    assert torch.equal(o.grad[lo:hi], reduced[lo:hi]), f"member {i}, step {t}"
+                    assert torch.equal(o.grad[lo:hi], red[lo:hi]), f"member {i}, step {t}"
     reps.settle()
     for rank, i in enumerate(reps.members):
         o = reps.opts[i]
@@ -257,12 +219,12 @@ def test_optimizer_accumulates_through_a_change_of_world(compact):
 
 def test_a_unit_short_of_micro_batches_vetoes_the_step():
     M, world = 3, 4
-    reps = _replicas(world, M)
+    reps = Replicas(world, min_world=3, grad_accum_steps=M)
     reps.configure([0, 1, 2, 3], 1)
-    reps.step(_raws(world, M, 5))
+    reps.step(raws(world, 5, (1.0,) * M))
     reps.settle()
     before = [(o.param.clone(), {r: tuple(x.clone() for x in s) for r, s in o.held_state().items()}) for o in reps.opts]
-    reps.step(_raws(world, M, 6), skip=(1, M - 1))  # unit 1 never saw its last micro-batch
+    reps.step(raws(world, 6, (1.0,) * M), skip=(1, M - 1))  # unit 1 never saw its last micro-batch
     assert reps.verdicts() == {i: False for i in range(world)}
     reps.settle()
     for o, (p, st) in zip(reps.opts, before):
@@ -270,7 +232,7 @@ def test_a_unit_short_of_micro_batches_vetoes_the_step():
         assert torch.equal(o.param, p)
         for r, s in o.held_state().items():
             assert all(torch.equal(a, b) for a, b in zip(s, st[r]))
-    reps.step(_raws(world, M, 7))  # the counts start over: the next step commits
+    reps.step(raws(world, 7, (1.0,) * M))  # the counts start over: the next step commits
     assert reps.verdicts() == {i: True for i in range(world)}
     reps.settle()
     assert all(o.t == 2 for o in reps.opts)
@@ -278,7 +240,7 @@ def test_a_unit_short_of_micro_batches_vetoes_the_step():
 
 def test_clipped_accumulation_matches_adamw_and_an_inf_in_an_early_micro_batch_vetoes():
     M, world, k = 3, 4, 2
-    reps = _replicas(world, M, max_norm=MAX_NORM)
+    reps = Replicas(world, min_world=3, max_grad_norm=MAX_NORM, grad_accum_steps=M)
     reps.configure([0, 1, 2, 3], 1)
     dev = torch.device("cuda", 0)
     rm, rmm, rv = reps.init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)
@@ -287,12 +249,12 @@ def test_clipped_accumulation_matches_adamw_and_an_inf_in_an_early_micro_batch_v
     L = ShardLayout(tuple(UNITS), k)
     t, clipped = 0, []
     for step, scale in enumerate((1.0, 0.01, 1.0, 1.0)):
-        raws = _raws(world, M, 200 + step, scale=scale)
+        micro = raws(world, 200 + step, (scale,) * M)
         poisoned = step == 2
         if poisoned:
-            raws[0][3][UNITS[1][0] + 9] = float("inf")  # micro-batch 0 of 3, rank 3
-        reps.step(raws)
-        reduced = _reduced(raws)
+            micro[0][3][UNITS[1][0] + 9] = float("inf")  # micro-batch 0 of 3, rank 3
+        reps.step(micro)
+        red = reduced(micro)
         norms = [reps.opts[i].grad_norm.clone() for i in range(world)]
         assert all(torch.equal(n, norms[0]) for n in norms), "norm bits differ between ranks"
         if poisoned:
@@ -300,13 +262,13 @@ def test_clipped_accumulation_matches_adamw_and_an_inf_in_an_early_micro_batch_v
             assert reps.verdicts() == {i: False for i in range(world)}
             continue
         assert reps.verdicts() == {i: True for i in range(world)}
-        norm = float(reduced.double().norm())
+        norm = float(red.double().norm())
         assert abs(float(norms[0]) - norm) <= 1e-5 * norm
         coef = torch.clamp(MAX_NORM / (norms[0] + 1e-6), max=1.0)
         assert torch.equal(reps.opts[0]._clip[1], coef)
         clipped.append(bool(coef < 1))
         t += 1
-        ref_adamw(rm, rmm, rv, reduced.float() * coef, t)
+        ref_adamw(rm, rmm, rv, red.float() * coef, t)
     reps.settle()
     assert any(clipped) and not all(clipped), clipped
     for rank, o in enumerate(reps.opts):
@@ -321,7 +283,7 @@ def test_accumulator_too_small_for_the_quorum_raises():
 
     from torchft_b200.parallel.symm_mem import SymmetricComm
 
-    reps = _replicas(4, 2, min_world=3)
+    reps = Replicas(4, min_world=3, grad_accum_steps=2)
     SymmetricComm.virtual_quorum(reps.comms, [0, 1], 9)
     with pytest.raises(RuntimeError, match="accumulator bytes"):
         reps.opts[0]._on_configured(PrefixStore("q/9", reps.store), 0, 2, 9)
@@ -329,13 +291,7 @@ def test_accumulator_too_small_for_the_quorum_raises():
 
 # ----------------------------------------------------------------------------- trainer
 def _train(M, steps=3, tag="a", batch=4):
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
-    lh = local_lighthouse()
-    tr = FaultTolerantTrainer("llama3_debug", loopback(lh.address()), replica_id=f"z1acc_{tag}_0",
-                              timeout=timedelta(seconds=30), grad_accum_steps=M)
-    try:
+    with trainer("llama3_debug", f"z1acc_{tag}", grad_accum_steps=M) as tr:
         gen = torch.Generator().manual_seed(5)
         losses = []
         for _ in range(steps):
@@ -346,9 +302,6 @@ def _train(M, steps=3, tag="a", batch=4):
         tr.join()
         torch.cuda.synchronize()
         return losses, tr.state_dict()["param"].clone(), (tr.zopt.accum_bytes() if M > 1 else 0)
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
 
 def test_trainer_accumulating_two_micro_batches_matches_one_batch():

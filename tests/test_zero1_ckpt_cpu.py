@@ -10,7 +10,7 @@ import os
 import numpy as np
 import pytest
 
-from test_zero1_cpu import NUMEL, UNITS, _mask, _Sim
+from _zero1_sim import NUMEL, UNITS, _mask, _Sim
 from torchft_b200.checkpointing.sharded import (check_compatible, encode_header, file_name, read_header, scan,
                                                 sections)
 from torchft_b200.parallel.zero1 import (ShardLayout, ckpt_read_plan, intersect_ranges, merge_ranges,

@@ -8,12 +8,11 @@ rank launches on the current stream, the snapshot copies run on the optimizer's 
 from __future__ import annotations
 
 import os
-from datetime import timedelta
 
 import pytest
 import torch
 
-from _zero1_replicas import Replicas, seeded_weights
+from _zero1_replicas import Replicas, raws, seeded_weights, trainer
 
 pytestmark = pytest.mark.gpu
 
@@ -23,46 +22,24 @@ NUMEL = UNITS[-1][1]
 K = 2
 
 
-def _raws(world, seed):
-    dev = torch.device("cuda", 0)
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return [(torch.randn(NUMEL, device=dev, generator=g) * 0.01 * (r + 1)).bfloat16() for r in range(world)]
+def _step(reps, seed):
+    """Gradients, reduce-scatters, verdicts and updates of one step are enqueued; nothing waits for the device."""
+    reps.step(raws(len(reps.members), seed, (0.01,), NUMEL), sync=False)
 
 
-class _Reps(Replicas):
-    """``n`` replicas of ``K`` holders per slice, stepped without a host synchronisation."""
+def _state(reps):
+    """(master, m, v) over the whole vector, assembled from the holders, and the weights."""
+    return reps.full_state(), reps.opts[reps.members[0]].param.clone()
 
-    def __init__(self, n, compact=False, min_world=1, units=UNITS):
-        super().__init__(n, units, k=K, compact=compact, min_world=min_world)
 
-    def step(self, seed):
-        """Gradients, reduce-scatters, verdicts and updates of one step are enqueued; nothing waits for the device."""
-        super().step([_raws(len(self.members), seed)], sync=False)
-
-    def save(self, directory, keep=2):
-        self.settle()
-        t = {self.opts[i].save(directory, {"step": self.opts[i].t, "batches_committed": 0}, keep=keep) for i in self.members}
-        assert len(t) == 1
-        return t.pop()
-
-    def full_state(self):
-        """(master, m, v) over the whole vector, assembled from the holders, and the weights."""
-        self.settle()
-        out = [torch.full((NUMEL,), float("nan"), device="cuda") for _ in range(3)]
-        for i in self.members:
-            for (lo, hi), arrs in self.opts[i].held_state().items():
-                for o, a in zip(out, arrs):
-                    o[lo:hi] = a
-        return out, self.opts[self.members[0]].param.clone()
-
-    def check_against(self, ref, param):
-        self.settle()
-        for i in self.members:
-            o = self.opts[i]
-            assert torch.equal(o.param, param), f"weights of member {i}"
-            for (lo, hi), arrs in o.held_state().items():
-                for name, a, r in zip(("master", "m", "v"), arrs, ref):
-                    assert torch.equal(a, r[lo:hi]), f"{name} of member {i} over {(lo, hi)}"
+def _check_against(reps, ref, param):
+    reps.settle()
+    for i in reps.members:
+        o = reps.opts[i]
+        assert torch.equal(o.param, param), f"weights of member {i}"
+        for (lo, hi), arrs in o.held_state().items():
+            for name, a, r in zip(("master", "m", "v"), arrs, ref):
+                assert torch.equal(a, r[lo:hi]), f"{name} of member {i} over {(lo, hi)}"
 
 
 def _chain(world):
@@ -72,54 +49,54 @@ def _chain(world):
 
 @pytest.mark.parametrize("world,compact", [(4, False), (3, False), (1, False), (3, True)])
 def test_save_under_the_next_step_and_restore_at_another_world(tmp_path, world, compact):
-    live = _Reps(4)
+    live = Replicas(4, UNITS, k=K)
     live.configure([0, 1, 2, 3], 1)
-    live.step(11)
-    live.step(12)
-    ref, param = live.full_state()
+    _step(live, 11)
+    _step(live, 12)
+    ref, param = _state(live)
     assert not torch.isnan(ref[0]).any()
     assert live.save(str(tmp_path)) == 2
-    live.step(13)  # immediately: the update of each unit waits for that unit's snapshot copy, not for the host
+    _step(live, 13)  # immediately: the update of each unit waits for that unit's snapshot copy, not for the host
     for o in live.opts:
         o.wait_checkpoint()
     live.settle()
     assert all(o.t == 3 for o in live.opts)
     assert sorted(os.listdir(tmp_path)) == [f"z1_step_2.w4.r{r}.bin" for r in range(4)]
 
-    back = _Reps(world, compact=compact, min_world=3 if compact else 1)
+    back = Replicas(world, UNITS, k=K, compact=compact, min_world=3 if compact else 1)
     for o in back.opts:
         o.master.fill_(float("nan"))  # a re-shard must fill every held element
         assert o.restore(str(tmp_path)) == {"step": 2, "batches_committed": 0}
         assert torch.equal(o.param, param) and o.t == 2
     back.configure(list(range(world)), 1)
-    back.check_against(ref, param)
+    _check_against(back, ref, param)
     assert all(o.lost_elements == 0 for o in back.opts)
     assert sum(o.disk_read_elements for o in back.opts) == sum(
         sum(hi - lo for lo, hi in o.layout.held(r, world)) for r, o in enumerate(back.opts))
 
     # a live run that changed 4 -> world at T = 2 and the restored one agree bit for bit two steps later
-    ctl = _Reps(4)
+    ctl = Replicas(4, UNITS, k=K)
     ctl.configure([0, 1, 2, 3], 1)
-    ctl.step(11)
-    ctl.step(12)
+    _step(ctl, 11)
+    _step(ctl, 12)
     for e, members in enumerate(_chain(world)):
         ctl.configure(members, 2 + e)
     for seed in (21, 22):
-        ctl.step(seed)
-        back.step(seed)
-    st, p = ctl.full_state()
-    back.check_against(st, p)
+        _step(ctl, seed)
+        _step(back, seed)
+    st, p = _state(ctl)
+    _check_against(back, st, p)
     assert all(o.t == 4 for o in back.opts) and all(ctl.opts[i].lost_elements == 0 for i in ctl.members)
 
 
 def test_partial_restart_pulls_from_the_live_replica_and_reads_the_rest(tmp_path):
     from torchft_b200.parallel.zero1 import intersect_ranges, subtract_ranges, total
 
-    live = _Reps(4)
+    live = Replicas(4, UNITS, k=K)
     live.configure([0, 1, 2, 3], 1)
-    live.step(31)
-    live.step(32)
-    ref, param = live.full_state()
+    _step(live, 31)
+    _step(live, 32)
+    ref, param = _state(live)
     live.save(str(tmp_path))
     for o in live.opts:
         o.wait_checkpoint()
@@ -131,7 +108,7 @@ def test_partial_restart_pulls_from_the_live_replica_and_reads_the_rest(tmp_path
         assert o.restore(str(tmp_path))["step"] == 2
         live.opts[r] = o
     live.configure([0, 1, 2, 3], 2)
-    live.check_against(ref, param)
+    _check_against(live, ref, param)
     L = live.opts[0].layout
     for r in (1, 2, 3):
         o = live.opts[r]
@@ -142,21 +119,21 @@ def test_partial_restart_pulls_from_the_live_replica_and_reads_the_rest(tmp_path
 
 
 def test_missing_and_torn_files_fall_back_and_a_mismatch_refuses(tmp_path):
-    live = _Reps(2)
+    live = Replicas(2, UNITS, k=K)
     live.configure([0, 1], 1)
-    live.step(41)
+    _step(live, 41)
     live.save(str(tmp_path))
-    live.step(42)
+    _step(live, 42)
     live.save(str(tmp_path))
-    live.step(43)
+    _step(live, 43)
     live.save(str(tmp_path))  # keep = 2: step 1's files are pruned
     for o in live.opts:
         o.wait_checkpoint()
-    _, p2 = live.full_state()  # the weights of step 3
+    _, p2 = _state(live)  # the weights of step 3
     assert sorted(os.listdir(tmp_path)) == [f"z1_step_{t}.w2.r{r}.bin" for t in (2, 3) for r in (0, 1)]
 
     def restore_one():
-        o = _Reps(1).opts[0]
+        o = Replicas(1, UNITS, k=K).opts[0]
         return o.restore(str(tmp_path)), o
 
     sd, o = restore_one()
@@ -169,23 +146,13 @@ def test_missing_and_torn_files_fall_back_and_a_mismatch_refuses(tmp_path):
     sd, o = restore_one()
     assert sd is None and o.t == 0 and torch.equal(o.param, seeded_weights(NUMEL))
     # another unit split (as with another optimizer_blocks) refuses before touching anything
-    other = _Reps(1, units=[(0, UNITS[1][0]), (UNITS[1][0], NUMEL)]).opts[0]
+    other = Replicas(1, [(0, UNITS[1][0]), (UNITS[1][0], NUMEL)], k=K).opts[0]
     with pytest.raises(ValueError, match="units"):
         other.restore(str(tmp_path))
     assert other.t == 0 and torch.equal(other.param, seeded_weights(NUMEL))
 
 
 # ----------------------------------------------------------------------------- trainer
-def _trainer(tag, **kw):
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
-    lh = local_lighthouse()
-    tr = FaultTolerantTrainer("llama3_debug", loopback(lh.address()), replica_id=f"z1ckpt_{tag}_0",
-                              timeout=timedelta(seconds=30), **kw)
-    return tr, lh
-
-
 def _batches(cfg, n):
     gen = torch.Generator().manual_seed(9)
     return [(torch.randint(0, cfg.vocab_size, (2, 128), generator=gen).pin_memory(),
@@ -196,8 +163,7 @@ def test_trainer_resumes_bit_identically_where_the_durable_checkpointer_route_do
     from torchft_b200.checkpointing import DurableCheckpointer
 
     sharded, classic = str(tmp_path / "sharded"), str(tmp_path / "classic")
-    tr, lh = _trainer("a")
-    try:
+    with trainer("llama3_debug", "z1ckpt_a") as tr:
         data = _batches(tr.cfg, 5)
         for tok, tgt in data[:3]:
             tr.step(tok, tgt)
@@ -212,12 +178,8 @@ def test_trainer_resumes_bit_identically_where_the_durable_checkpointer_route_do
         tr.join()
         p_live = tr.zopt.param.clone()
         assert tr.manager.current_step() == 5
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
-    tr, lh = _trainer("b")
-    try:
+    with trainer("llama3_debug", "z1ckpt_b") as tr:
         assert tr.restore_checkpoint(sharded) == 3
         assert tr.manager.current_step() == 3
         resumed = [tr.step(tok, tgt) for tok, tgt in data[3:]]
@@ -225,37 +187,22 @@ def test_trainer_resumes_bit_identically_where_the_durable_checkpointer_route_do
         assert resumed == live
         assert torch.equal(tr.zopt.param, p_live)
         assert tr.manager.current_step() == 5 and tr.zopt.lost_elements == 0
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
     # the route this exists to replace: weights and t come back, master / m / v do not, so training continues from
     # the initial master weights with zero moments
-    tr, lh = _trainer("c")
-    try:
+    with trainer("llama3_debug", "z1ckpt_c") as tr:
         assert DurableCheckpointer(tr.manager, tr.state_dict, tr.load_state_dict, classic).restore() == 3
         for tok, tgt in data[3:]:
             tr.step(tok, tgt)
         tr.join()
         assert not torch.equal(tr.zopt.param, p_live)
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
 
 def test_trainer_refusals(tmp_path):
-    tr, lh = _trainer("classic", zero1=False)
-    try:
+    with trainer("llama3_debug", "z1ckpt_classic", zero1=False) as tr:
         with pytest.raises(ValueError, match="FT-ZeRO-1"):
             tr.save_checkpoint(str(tmp_path))
         with pytest.raises(ValueError, match="FT-ZeRO-1"):
             tr.restore_checkpoint(str(tmp_path))
-    finally:
-        tr.shutdown()
-        lh.shutdown()
-    tr, lh = _trainer("empty")
-    try:
+    with trainer("llama3_debug", "z1ckpt_empty") as tr:
         assert tr.restore_checkpoint(str(tmp_path / "nothing")) is None
-    finally:
-        tr.shutdown()
-        lh.shutdown()

@@ -8,26 +8,16 @@ norm in fp64 and ``coef = min(1, max_norm / (norm + 1e-6))`` in fp32, as ``torch
 
 from __future__ import annotations
 
-from datetime import timedelta
-
 import pytest
 import torch
 
-from _zero1_replicas import HP, SHIFT, Replicas, ref_adamw
+from _zero1_replicas import HP, NUMEL, SHIFT, UNITS, Replicas, kernel_world, raws, reduced, ref_adamw, trainer
+from _zero1_state import State
 
 pytestmark = pytest.mark.gpu
 
-UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
-NUMEL = UNITS[-1][1]
 MAX_NORM = 50.0
 STEP_SCALES = (1.0, 0.01, 1.0)  # norms of a few hundred, a few units, a few hundred: clipped, not clipped, clipped
-
-
-def _world(world, presignal=True):
-    from torchft_b200.parallel.symm_mem import SymmetricComm
-
-    seg = {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2, "z1_gnorm": 8 * len(UNITS)}
-    return SymmetricComm.virtual_world(world, seg, presignal=presignal, timeout=timedelta(seconds=20))
 
 
 def _coef(max_norm, norm):
@@ -35,48 +25,20 @@ def _coef(max_norm, norm):
     return torch.clamp(max_norm / (norm + 1e-6), max=1.0)
 
 
-def _raws(world, seed, scales=STEP_SCALES):
-    dev = torch.device("cuda", 0)
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return [[(torch.randn(NUMEL, device=dev, generator=g) * (r + 1) * s).bfloat16() for r in range(world)] for s in scales]
-
-
-def _reduced(raw, quiet):
-    acc = torch.zeros(NUMEL, device=raw[0].device)
-    contributors = len(raw) - (1 if quiet is not None else 0)
-    for r in range(len(raw)):  # fixed rank order, fp32 accumulate, then scale, then round to bf16
-        if r != quiet:
-            acc += raw[r].float()
-    return (acc * (1.0 / contributors)).bfloat16()
-
-
-def _pipeline(world, k, raws, max_norm, presignal=True, quiet=None, paged=False, seed=1):
-    """Reduce-scatter -> commit -> update for every step of ``raws`` (``raws[step][rank]``) on fresh ranks, with
+def _pipeline(world, k, steps, max_norm, presignal=True, quiet=None, paged=False, seed=1):
+    """Reduce-scatter -> commit -> update for every step of ``steps`` (``steps[step][rank]``) on fresh ranks, with
     clipping when ``max_norm`` is not None. Returns one record per step: verdicts, step counts, the [norm, coef] pair and
     the host-ring norm of every rank, and the weights and (full-size) state of every rank after the step."""
     dev = torch.device("cuda", 0)
-    comms = _world(world, presignal)
+    comms = kernel_world(world, presignal)
     g = torch.Generator(device=dev).manual_seed(seed)
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
     grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     params = [c.segment("z1_param")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     gnorm = [c.segment("z1_gnorm").data_ptr() for c in comms]
-    state = [[init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)] for _ in comms]
-    npages = (NUMEL + (1 << SHIFT) - 1) >> SHIFT
-    tables, idxs = [], []
-    for r in range(world):
-        params[r].copy_(init)
-        if paged:  # a pool with spare slots and the pages scattered over it in a random order
-            slots = torch.randperm(npages + 5, generator=torch.Generator().manual_seed(seed * 10 + r))[:npages].to(dev)
-            tables.append(slots.int())
-            idx = (slots.long()[:, None] * (1 << SHIFT) + torch.arange(1 << SHIFT, device=dev)).view(-1)[:NUMEL]
-            idxs.append(idx)
-            pools = []
-            for x in state[r]:
-                p = torch.full(((npages + 5) << SHIFT,), float("nan"), device=dev)
-                p[idx] = x
-                pools.append(p)
-            state[r] = pools
+    state = [State.seeded(init, SHIFT if paged else None, seed * 10 + r) for r in range(world)]
+    for p in params:
+        p.copy_(init)
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     clip = [torch.zeros(2, dtype=torch.float32, device=dev) for _ in comms]
     streams = [torch.cuda.Stream(device=dev) for _ in comms]
@@ -96,17 +58,12 @@ def _pipeline(world, k, raws, max_norm, presignal=True, quiet=None, paged=False,
     def upd(r, s):
         coef = clip[r].data_ptr() + 4 if max_norm is not None else 0
         for lo, hi in UNITS:
-            if paged:
-                comms[r].zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, state[r][0].data_ptr(),
-                                       state[r][1].data_ptr(), state[r][2].data_ptr(), hi - lo, HP, gates[r], k, 0, 4, s,
-                                       tables[r].data_ptr(), lo, SHIFT, coef=coef)
-            else:
-                comms[r].zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, state[r][0].data_ptr() + lo * 4,
-                                       state[r][1].data_ptr() + lo * 4, state[r][2].data_ptr() + lo * 4, hi - lo, HP,
-                                       gates[r], k, 0, 4, s, coef=coef)
+            comms[r].zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP,
+                                   gate=gates[r], replication=k, mode=0, blocks=4, stream=s, coef=coef,
+                                   **state[r].args(lo))
 
     out = []
-    for raw in raws:
+    for raw in steps:
         for r in range(world):
             grads[r].copy_(raw[r])
         if presignal and quiet is not None:
@@ -127,13 +84,12 @@ def _pipeline(world, k, raws, max_norm, presignal=True, quiet=None, paged=False,
                     upd(r, streams[r])
         torch.cuda.synchronize()
         assert all(c.errored() is None for c in comms)
-        st = [[x[idxs[r]] for x in state[r]] if paged else [x.clone() for x in state[r]] for r in range(world)]
         out.append({"verdict": [comms[r].verdict(seqs[r]) for r in range(world)],
                     "t": [int(gt[1]) for gt in gates],
                     "clip": [c.clone() for c in clip],
                     "host_norm": [comms[r].grad_norm(seqs[r]) if max_norm is not None else None for r in range(world)],
                     "params": [p.clone() for p in params],
-                    "state": st})
+                    "state": [st.get(0, NUMEL) for st in state]})
     return out
 
 
@@ -145,15 +101,15 @@ def test_clipped_pipeline_matches_reference(world, k):
     dev = torch.device("cuda", 0)
     L = ShardLayout(tuple(UNITS), k)
     quiet = 1 if world > 2 else None  # a healing / spare rank whose gradients count as zeros
-    raws = _raws(world, 100 + world * 3 + k)
-    recs = _pipeline(world, k, raws, MAX_NORM, quiet=quiet)
+    steps = raws(world, 100 + world * 3 + k, STEP_SCALES)
+    recs = _pipeline(world, k, steps, MAX_NORM, quiet=quiet)
     g = torch.Generator(device=dev).manual_seed(1)  # the seeded initial weights of _pipeline
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
     rm, rmm, rv = init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)
     clipped = []
-    for step, (raw, rec) in enumerate(zip(raws, recs), start=1):
-        reduced = _reduced(raw, quiet)
-        norm = float(reduced.double().norm())
+    for step, (raw, rec) in enumerate(zip(steps, recs), start=1):
+        red = reduced([raw], quiet)
+        norm = float(red.double().norm())
         for r in range(world):
             assert torch.equal(rec["clip"][r], rec["clip"][0]), f"norm / coef bits of rank {r}, step {step}"
             assert rec["host_norm"][r] == float(rec["clip"][0][0])
@@ -163,7 +119,7 @@ def test_clipped_pipeline_matches_reference(world, k):
         coef = _coef(MAX_NORM, torch.tensor(norm, dtype=torch.float32, device=dev))
         clipped.append(bool(coef < 1))
         assert rec["verdict"] == [True] * world and rec["t"] == [step] * world
-        ref_adamw(rm, rmm, rv, reduced.float() * coef, step)
+        ref_adamw(rm, rmm, rv, red.float() * coef, step)
     assert any(clipped) and not all(clipped), clipped
     last = recs[-1]
     for r in range(1, world):
@@ -192,9 +148,9 @@ def test_infinite_max_norm_changes_nothing(world, k):
 
     L = ShardLayout(tuple(UNITS), k)
     quiet = 1 if world > 2 else None
-    raws = _raws(world, 7 + world)
-    off = _pipeline(world, k, raws, None, quiet=quiet)
-    inf = _pipeline(world, k, raws, float("inf"), quiet=quiet)
+    steps = raws(world, 7 + world, STEP_SCALES)
+    off = _pipeline(world, k, steps, None, quiet=quiet)
+    inf = _pipeline(world, k, steps, float("inf"), quiet=quiet)
     for a, b in zip(off, inf):
         assert all(float(c[1]) == 1.0 for c in b["clip"])
         for r in range(world):
@@ -207,9 +163,9 @@ def test_infinite_max_norm_changes_nothing(world, k):
 def test_real_signalling_gives_the_same_norm_bits_and_weights():
     """W = 4 ranks in flight at once on four streams against the pre-signalled sequential run."""
     world, k = 4, 2
-    raws = _raws(world, 21)
-    seq = _pipeline(world, k, raws, MAX_NORM)
-    real = _pipeline(world, k, raws, MAX_NORM, presignal=False)
+    steps = raws(world, 21, STEP_SCALES)
+    seq = _pipeline(world, k, steps, MAX_NORM)
+    real = _pipeline(world, k, steps, MAX_NORM, presignal=False)
     for a, b in zip(seq, real):
         assert b["verdict"] == [True] * world
         for r in range(world):
@@ -220,10 +176,10 @@ def test_real_signalling_gives_the_same_norm_bits_and_weights():
 @pytest.mark.parametrize("poison", ["inf", "nan"])
 def test_nonfinite_gradient_vetoes_the_step_on_every_rank(poison):
     world, k = 4, 2
-    raws = _raws(world, 33, scales=(1.0, 1.0, 1.0))
+    steps = raws(world, 33, scales=(1.0, 1.0, 1.0))
     lo, hi = UNITS[1]
-    raws[1][2][lo + 100] = float(poison)  # one element of one unit of one rank's raw gradient, step 2
-    recs = _pipeline(world, k, raws, MAX_NORM, presignal=False)
+    steps[1][2][lo + 100] = float(poison)  # one element of one unit of one rank's raw gradient, step 2
+    recs = _pipeline(world, k, steps, MAX_NORM, presignal=False)
     before, bad, after = recs
     assert before["verdict"] == [True] * world and before["t"] == [1] * world
     assert bad["verdict"] == [False] * world, "the veto must reach every rank"
@@ -240,9 +196,9 @@ def test_nonfinite_gradient_vetoes_the_step_on_every_rank(poison):
 @pytest.mark.parametrize("world", [2, 4, 8])
 def test_paged_update_with_clipping_matches_flat(world):
     k = 2
-    raws = _raws(world, 50 + world)
-    flat = _pipeline(world, k, raws, MAX_NORM, seed=4)
-    paged = _pipeline(world, k, raws, MAX_NORM, paged=True, seed=4)
+    steps = raws(world, 50 + world, STEP_SCALES)
+    flat = _pipeline(world, k, steps, MAX_NORM, seed=4)
+    paged = _pipeline(world, k, steps, MAX_NORM, paged=True, seed=4)
     _check_paged_vs_flat(world, k, flat, paged)
 
 
@@ -260,19 +216,15 @@ def _check_paged_vs_flat(world, k, flat, paged):
 
 
 # ----------------------------------------------------------------------------- Zero1Optimizer
-def _optimizers(world, max_norm):
-    return Replicas(world, UNITS, max_norm=max_norm).opts
-
-
 def test_optimizer_reports_norms_one_step_late_and_counts_nonfinite_steps():
     """Through enqueue / update / wait / resolved in the Manager's order: a step's verdict (and norm) is settled when
     the next step starts."""
     world = 4
-    opts = _optimizers(world, MAX_NORM)
-    raws = _raws(world, 77, scales=(1.0, 0.01, 1.0, 1.0, 1.0))
-    raws[2][3][UNITS[0][0] + 5] = float("inf")  # step 3 is poisoned
+    opts = Replicas(world, max_grad_norm=MAX_NORM).opts
+    steps = raws(world, 77, scales=(1.0, 0.01, 1.0, 1.0, 1.0))
+    steps[2][3][UNITS[0][0] + 5] = float("inf")  # step 3 is poisoned
     norms, pending = [], None
-    for step, raw in enumerate(raws):
+    for step, raw in enumerate(steps):
         if pending is not None:  # the Manager books the previous step at the start of this one
             for o, s in zip(opts, pending):
                 o.resolved(o.wait(s))
@@ -288,7 +240,7 @@ def test_optimizer_reports_norms_one_step_late_and_counts_nonfinite_steps():
         for o in opts:
             o.update()
         torch.cuda.synchronize()
-        ref = float(_reduced(raw, None).double().norm())
+        ref = float(reduced([raw]).double().norm())
         dev_norm = float(opts[0].grad_norm)
         assert dev_norm == ref == float("inf") if step == 2 else abs(dev_norm - ref) <= 1e-5 * ref, (step, dev_norm, ref)
         norms.append(dev_norm)
@@ -298,12 +250,12 @@ def test_optimizer_reports_norms_one_step_late_and_counts_nonfinite_steps():
     for o in opts:
         assert o.last_grad_norm == norms[-1]
         assert o.nonfinite_steps == 1
-        assert o.t == len(raws) - 1  # the poisoned step was not applied
+        assert o.t == len(steps) - 1  # the poisoned step was not applied
     assert all(torch.equal(o.param, opts[0].param) for o in opts)
 
 
 def test_optimizer_at_world_one_scales_in_place_and_norms_the_whole_buffer():
-    opts = _optimizers(1, 1.0)
+    opts = Replicas(1, max_grad_norm=1.0).opts
     o = opts[0]
     dev = torch.device("cuda", 0)
     raw = torch.randn(NUMEL, device=dev, generator=torch.Generator(device=dev).manual_seed(9)).bfloat16()
@@ -323,13 +275,7 @@ def test_optimizer_at_world_one_scales_in_place_and_norms_the_whole_buffer():
 
 # ----------------------------------------------------------------------------- trainer
 def _train(max_grad_norm, steps=4, tag="a", read_grad=False):
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
-    lh = local_lighthouse()
-    tr = FaultTolerantTrainer("llama3_debug", loopback(lh.address()), replica_id=f"z1clip_{tag}_0",
-                              timeout=timedelta(seconds=30), max_grad_norm=max_grad_norm)
-    try:
+    with trainer("llama3_debug", f"z1clip_{tag}", max_grad_norm=max_grad_norm) as tr:
         gen = torch.Generator().manual_seed(5)
         losses, reported, grad_norms = [], [], []
         for _ in range(steps):
@@ -343,9 +289,6 @@ def _train(max_grad_norm, steps=4, tag="a", read_grad=False):
         tr.join()
         torch.cuda.synchronize()
         return losses, tr.state_dict()["param"].clone(), reported, grad_norms
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
 
 def test_trainer_with_infinite_max_norm_reproduces_the_trainer_without_clipping():

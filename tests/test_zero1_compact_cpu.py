@@ -6,7 +6,7 @@ from __future__ import annotations
 import numpy as np
 import pytest
 
-from test_zero1_cpu import NUMEL, UNITS, _Sim
+from _zero1_sim import NUMEL, UNITS, _mask, _Sim
 from torchft_b200.models.llama import CONFIGS
 from torchft_b200.parallel.zero1 import (ShardLayout, intersect_ranges, merge_ranges, page_ranges, plan_quorum,
                                          pool_pages, total)
@@ -104,13 +104,6 @@ class _CompactSim:
                 self.pool[m][self._idx(m, lo, hi)] += 1
             self.hold[m] = self.L.held(i, world)
             self.t[m] += 1
-
-
-def _mask(rs, n):
-    m = np.zeros(n, bool)
-    for lo, hi in rs:
-        m[lo:hi] = True
-    return m
 
 
 @pytest.mark.parametrize("seed", range(6))

@@ -10,45 +10,24 @@ from datetime import timedelta
 import pytest
 import torch
 
-from _zero1_replicas import HP, SHIFT, Replicas
+from _zero1_replicas import HP, NUMEL, SHIFT, UNITS, Replicas, kernel_world
+from _zero1_state import State
 
 pytestmark = pytest.mark.gpu
-
-UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
-NUMEL = UNITS[-1][1]
-
-
-def _world(world, segments, presignal=True):
-    from torchft_b200.parallel.symm_mem import SymmetricComm
-
-    return SymmetricComm.virtual_world(world, segments, presignal=presignal, timeout=timedelta(seconds=20))
 
 
 def _run_update_kernels(world, k, presignal, paged, seed):
     """Several gated steps (one vetoed), then a refresh, on fresh ranks; returns the weights and the state of every rank
     as full-size tensors (paged state gathered back through its page table)."""
     dev = torch.device("cuda", 0)
-    comms = _world(world, {"z1_param": NUMEL * 2}, presignal)
+    comms = kernel_world(world, presignal)
     g = torch.Generator(device=dev).manual_seed(seed)
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
-    npages = (NUMEL + (1 << SHIFT) - 1) >> SHIFT
     params = [c.segment("z1_param")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     grads = [torch.empty(NUMEL, dtype=torch.bfloat16, device=dev) for _ in comms]
-    state = [[init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)] for _ in comms]
-    tables = []
-    for r in range(world):
-        params[r].copy_(init)
-        if paged:
-            # a pool with spare slots and the pages scattered over it in a random order
-            slots = torch.randperm(npages + 5, generator=torch.Generator().manual_seed(seed * 10 + r))[:npages].to(dev)
-            tables.append(slots.int())
-            idx = (slots.long()[:, None] * (1 << SHIFT) + torch.arange(1 << SHIFT, device=dev)).view(-1)[:NUMEL]
-            pools = []
-            for x in state[r]:
-                p = torch.full(((npages + 5) << SHIFT,), float("nan"), device=dev)
-                p[idx] = x
-                pools.append(p)
-            state[r] = pools
+    state = [State.seeded(init, SHIFT if paged else None, seed * 10 + r) for r in range(world)]
+    for p in params:
+        p.copy_(init)
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     streams = [torch.cuda.Stream(device=dev) for _ in comms]
 
@@ -58,14 +37,8 @@ def _run_update_kernels(world, k, presignal, paged, seed):
             if mode == 0:
                 c.zero1_commit_(gates[r], host_ok, True, s)
             for lo, hi in UNITS:
-                if paged:
-                    c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, state[r][0].data_ptr(),
-                                    state[r][1].data_ptr(), state[r][2].data_ptr(), hi - lo, HP, gates[r], k, mode, 4, s,
-                                    tables[r].data_ptr(), lo, SHIFT)
-                else:
-                    c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, state[r][0].data_ptr() + lo * 4,
-                                    state[r][1].data_ptr() + lo * 4, state[r][2].data_ptr() + lo * 4, hi - lo, HP, gates[r],
-                                    k, mode, 4, s)
+                c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP, gate=gates[r],
+                                replication=k, mode=mode, blocks=4, stream=s, **state[r].args(lo))
 
     for step, (mode, veto) in enumerate([(0, False), (0, False), (0, True), (0, False), (1, False), (0, False)]):
         gstep = torch.randn(NUMEL, device=dev, generator=g).bfloat16()
@@ -76,14 +49,7 @@ def _run_update_kernels(world, k, presignal, paged, seed):
             launch(r, mode, not (veto and r == world - 1))
         torch.cuda.synchronize()
         assert all(c.errored() is None for c in comms)
-    out_state = []
-    for r in range(world):
-        if paged:
-            idx = (tables[r].long()[:, None] * (1 << SHIFT) + torch.arange(1 << SHIFT, device=dev)).view(-1)[:NUMEL]
-            out_state.append([x[idx] for x in state[r]])
-        else:
-            out_state.append(state[r])
-    return [p.clone() for p in params], out_state, [gt.clone() for gt in gates]
+    return [p.clone() for p in params], [st.get(0, NUMEL) for st in state], [gt.clone() for gt in gates]
 
 
 @pytest.mark.parametrize("world", [2, 3, 4, 8])
@@ -128,7 +94,7 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
     assert cap < NUMEL >> SHIFT  # the pools really are smaller than the vector
     g = torch.Generator(device=dev).manual_seed(3)
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
-    reps = {kind: Replicas(n, UNITS, k=k, compact=kind == "compact", min_world=min_world, init=init)
+    reps = {kind: Replicas(n, k=k, compact=kind == "compact", min_world=min_world, init=init)
             for kind in ("flat", "compact")}
     opts = {kind: r.opts for kind, r in reps.items()}
     assert opts["compact"][0].state_bytes_allocated() == 12 * (cap << SHIFT)
@@ -138,7 +104,7 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
         for r in reps.values():
             r.configure(members, epoch)
 
-    def step(members, veto=None):
+    def step(members, veto=()):
         gstep = torch.randn(NUMEL, device=dev, generator=g).bfloat16()  # the reduced gradient, identical everywhere
         for r in reps.values():
             r.step([[gstep] * len(members)], veto=veto, reduce=False)
@@ -165,7 +131,7 @@ def test_compact_optimizer_tracks_full_size_optimizer_through_kill_rejoin_and_sp
         r.opts[2] = o
     configure([0, 1, 2, 3], 3)
     step([0, 1, 2, 3])
-    step([0, 1, 2, 3], veto=1)                     # split commit: member 1 misses the update the others apply
+    step([0, 1, 2, 3], veto=[1])                   # split commit: member 1 misses the update the others apply
     assert opts["compact"][1].t + 1 == opts["compact"][0].t
     configure([0, 1, 2, 3], 4)
     step([0, 1, 2, 3])

@@ -10,15 +10,9 @@ import numpy as np
 import pytest
 from torch.distributed import TCPStore
 
+from _zero1_sim import NUMEL, UNITS, _mask, _Sim
 from torchft_b200.parallel.zero1 import (ShardLayout, intersect_ranges, merge_ranges, page_ranges, plan_quorum,
                                          subtract_ranges, total)
-
-
-def _mask(rs, n):
-    m = np.zeros(n, bool)
-    for lo, hi in rs:
-        m[lo:hi] = True
-    return m
 
 
 def test_interval_arithmetic_matches_bitmaps():
@@ -33,10 +27,6 @@ def test_interval_arithmetic_matches_bitmaps():
         assert (_mask(subtract_ranges(a, b), n) == (ma & ~mb)).all()
         m = merge_ranges(a)
         assert all(x[1] < y[0] for x, y in zip(m, m[1:])) and all(lo < hi for lo, hi in m)
-
-
-UNITS = ((0, 4096), (4096, 4096 + 8 * 1001), (4096 + 8 * 1001, 4096 + 8 * 1001 + 64))
-NUMEL = UNITS[-1][1]
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
@@ -56,54 +46,6 @@ def test_layout_every_element_has_exactly_k_holders_and_one_primary(world, k):
         for s in range(world):
             lo, hi = L.slice_bounds(u, world, s)
             assert lo % 8 == 0 and hi % 8 == 0 and UNITS[u][0] <= lo <= hi <= UNITS[u][1]
-
-
-class _Sim:
-    """Numpy emulation of N replicas running the FT-ZeRO-1 state protocol (update = +1 on held ranges), re-sharded by
-    the optimizer's own planner (``plan_quorum``); only the state arrays and the counters are the emulation's."""
-
-    def __init__(self, n, k):
-        self.L = ShardLayout(UNITS, k)
-        self.state = {r: np.zeros(NUMEL) for r in range(n)}      # every replica seeds identically
-        self.hold = {r: [(0, NUMEL)] for r in range(n)}
-        self.t = {r: 0 for r in range(n)}
-        self.members = list(range(n))
-        self.lost = 0
-        self.read = 0
-
-    def configure(self, members, ckpt=None):
-        """``ckpt``: checkpoint files for ``plan_quorum``, whose file objects are the arrays of values they store."""
-        self.members = list(members)
-        published = {i: {"t": self.t[m], "hold": self.hold[m]} for i, m in enumerate(members)}
-        plans = plan_quorum(self.L, len(members), published, ckpt=ckpt)
-        for i, m in enumerate(members):  # a source never writes the ranges it is read from: they are current there
-            p = plans[i]
-            for src, lo, hi in p.pulls:
-                self.state[m][lo:hi] = self.state[members[src]][lo:hi]
-            for vals, off, lo, hi in p.reads:
-                self.state[m][lo:hi] = vals[off:off + hi - lo]
-                self.read += hi - lo
-            for lo, hi in p.lost:
-                self.state[m][lo:hi] = -1000.0 if p.counted else 0.0
-                self.lost += (hi - lo) if p.counted else 0
-            self.hold[m], self.t[m] = p.hold, p.tmax
-
-    def step(self, commit_on=None):
-        world = len(self.members)
-        for i, m in enumerate(self.members):
-            if commit_on is not None and m not in commit_on:
-                continue
-            for lo, hi in self.L.held(i, world):
-                self.state[m][lo:hi] += 1
-            self.hold[m] = self.L.held(i, world)
-            self.t[m] += 1
-
-    def check(self):
-        world = len(self.members)
-        tmax = max(self.t[m] for m in self.members)
-        for i, m in enumerate(self.members):
-            for lo, hi in self.L.held(i, world):
-                assert (self.state[m][lo:hi] == tmax).all(), (m, lo, hi)
 
 
 def test_reshard_survives_any_single_loss_join_and_split_commit():

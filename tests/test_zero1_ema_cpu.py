@@ -7,14 +7,11 @@ from __future__ import annotations
 import numpy as np
 import pytest
 
+from _zero1_replicas import widen
 from torchft_b200.checkpointing.sharded import file_dtype, payload_bytes, sections
 from torchft_b200.parallel.zero1 import (SR_SEED, SR_SEED_EMA, bf16_sr, bf16_sr_ema, check_ema_agreement, ckpt_read_plan,
                                          ema_coefficient, ema_decay_value, ema_record, ema_step, merge_ranges,
                                          split_ema_reads, sr_bits, sr_bits_ema)
-
-
-def _widen(bits):
-    return (bits.astype(np.uint32) << np.uint32(16)).view(np.float32)
 
 
 # ----------------------------------------------------------------------------- the step
@@ -97,7 +94,7 @@ def test_a_bf16_ema_stalls_with_round_to_nearest_and_tracks_with_stochastic_roun
     e = np.arange(n, dtype=np.uint64)
     rng = np.random.default_rng(3)
     start = (1.0 + rng.random(n) * 0.5).astype(np.float32)
-    start = _widen((start.view(np.uint32) >> np.uint32(16)).astype(np.uint16))  # bf16 values
+    start = widen((start.view(np.uint32) >> np.uint32(16)).astype(np.uint16))  # bf16 values
     target = (start + np.float32(0.5)).astype(np.float32)  # the weights sit half a unit above, ~32 bf16 ulps
     rn_bits = (start.view(np.uint32) >> np.uint32(16)).astype(np.uint16)
     sr = rn_bits.copy()
@@ -106,16 +103,16 @@ def test_a_bf16_ema_stalls_with_round_to_nearest_and_tracks_with_stochastic_roun
 
     for t in range(1, steps + 1):
         f32 = ema_step(f32, target, c)
-        rn = torch.from_numpy(ema_step(_widen(rn_bits), target, c)).bfloat16().view(torch.int16).numpy().view(np.uint16)
+        rn = torch.from_numpy(ema_step(widen(rn_bits), target, c)).bfloat16().view(torch.int16).numpy().view(np.uint16)
         assert (rn == rn_bits).all(), "round-to-nearest moved"
-        sr = bf16_sr_ema(ema_step(_widen(sr), target, c), e, t)
+        sr = bf16_sr_ema(ema_step(widen(sr), target, c), e, t)
     expect = 0.5 * (1 - d ** steps)  # of the gap, ~0.432
-    moved_sr = float((_widen(sr) - start).mean())
+    moved_sr = float((widen(sr) - start).mean())
     assert abs(moved_sr - expect) < 0.01 * expect, (moved_sr, expect)
     assert abs(float((f32 - start).mean()) - expect) < 1e-3
     # element by element the rounding noise adds up like a random walk that the decay pulls back: a stationary spread of
     # about sqrt(p (1 - p) / 2c) bf16 ulps (2^-7 at [1, 2)) around the fp32 EMA, p the fraction a step moves (~0.06 here)
-    dev = (_widen(sr) - f32) / 2.0 ** -7
+    dev = (widen(sr) - f32) / 2.0 ** -7
     assert float(np.sqrt((dev ** 2).mean())) < 8, float(np.sqrt((dev ** 2).mean()))
     assert abs(float(dev.mean())) < 0.5
 

@@ -11,71 +11,17 @@ import contextlib
 import os
 import threading
 from datetime import timedelta
-from unittest import mock
 
 import numpy as np
 import pytest
 import torch
 
-from _zero1_replicas import PG
-from test_zero1_moments_gpu import MReplicas, _bits, _widen
-from test_zero1_sched_gpu import UNITS, _configure_errors, _raws, _step_vetoed_by_all, warmup_cosine
+from _zero1_replicas import PG, UNITS, Replicas, bits, raws, trainer, warmup_cosine, widen
 
 pytestmark = pytest.mark.gpu
 
 BF16, FP32 = torch.bfloat16, torch.float32
 DECAY = 0.9
-
-
-class EReplicas(MReplicas):
-    """:class:`MReplicas` whose optimizers keep an EMA with ``decay`` (a float, ``None``, or one per member); the
-    virtual world gets a ``z1_ema`` segment the size of ``z1_master``. Moments (and so the EMA) are fp32 by default."""
-
-    def __init__(self, n, decay=DECAY, moments=FP32, **kw):
-        from torchft_b200.parallel.symm_mem import SymmetricComm
-
-        self.decay = decay
-        kw["moments"] = moments
-        real = SymmetricComm.virtual_world
-
-        def with_ema(world, segments, **kws):
-            return real(world, {**segments, "z1_ema": segments["z1_master"]}, **kws)
-
-        with mock.patch.object(SymmetricComm, "virtual_world", staticmethod(with_ema)):
-            super().__init__(n, **kw)
-
-    def make(self, comm):
-        from torchft_b200.parallel.zero1 import Zero1Optimizer
-
-        i = self.comms.index(comm)
-        md = self.moments[i] if isinstance(self.moments, list) else self.moments
-        d = self.decay[i] if isinstance(self.decay, list) else self.decay
-        return Zero1Optimizer(PG(comm), self.numel, units=self.units, lr=1e-2, betas=(0.9, 0.95), eps=1e-8,
-                              weight_decay=0.1, replication=self.k, blocks=self.blocks, compact=self.compact,
-                              min_world=self.min_world, page_shift=8, max_grad_norm=self.max_norm,
-                              grad_accum_steps=self.M, lr_lambda=self.lam, lr_steps=self.lr_steps, moment_dtype=md,
-                              ema_decay=d)
-
-    def get_ema(self, i, lo, hi):
-        o = self.opts[i]
-        torch.cuda.synchronize()
-        return torch.cat([o.ema[at:at + b - a] for a, b, at in o._pieces(o._table_host, lo, hi)])
-
-    def full_ema(self):
-        """The EMA over the whole vector assembled from the holders, which must agree bit for bit."""
-        self.settle()
-        out = torch.zeros(self.numel, dtype=self.opts[self.members[0]].ema.dtype, device="cuda")
-        seen = torch.zeros(self.numel, dtype=torch.bool, device="cuda")
-        for i, lo, hi in self.held():
-            got = self.get_ema(i, lo, hi)
-            had = seen[lo:hi]
-            assert torch.equal(out[lo:hi][had].view(torch.uint8 if got.dtype == FP32 else torch.int16),
-                               got[had].view(torch.uint8 if got.dtype == FP32 else torch.int16)), \
-                f"holders disagree on the EMA over {(lo, hi)} (member {i})"
-            out[lo:hi] = got
-            seen[lo:hi] = True
-        assert bool(seen.all())
-        return out
 
 
 def _c(decay=DECAY):
@@ -95,13 +41,13 @@ def test_kernel_ema_equals_the_numpy_specification(moments, paged):
     from torchft_b200.parallel.zero1 import bf16_sr_ema, ema_step
 
     world = 4
-    reps = EReplicas(world, moments=moments, k=2, compact=paged)
+    reps = Replicas(world, k=2, compact=paged, moment_dtype=moments, ema_decay=DECAY)
     reps.configure(list(range(world)), 1)
     first = reps.full_ema()
     assert torch.equal(first.float(), reps.init.float()), "seeded with the master weights"
     for step in range(4):
         before = {(i, lo, hi): reps.get_ema(i, lo, hi) for i, lo, hi in reps.held()}
-        reps.step([_raws(world, 500 + step)])
+        reps.step(raws(world, 500 + step))
         reps.settle()
         t = reps.opts[0].t
         assert t == step + 1
@@ -112,8 +58,8 @@ def test_kernel_ema_equals_the_numpy_specification(moments, paged):
                 want = ema_step(_np(e0), w, _c())
                 assert (_np(e1).view(np.uint32) == want.view(np.uint32)).all(), f"member {i} {(lo, hi)} t={t}"
             else:
-                want = bf16_sr_ema(ema_step(_widen(_bits(e0)), w, _c()), np.arange(lo, hi, dtype=np.uint64), t)
-                assert (_bits(e1) == want).all(), f"member {i} {(lo, hi)} t={t}"
+                want = bf16_sr_ema(ema_step(widen(bits(e0)), w, _c()), np.arange(lo, hi, dtype=np.uint64), t)
+                assert (bits(e1) == want).all(), f"member {i} {(lo, hi)} t={t}"
             assert not torch.equal(e0, e1)
 
 
@@ -127,15 +73,15 @@ def test_kernel_ema_follows_an_fp64_ema_of_the_device_masters(world, k, paged):
     times, and the error contracts by d per step). Clipping and a schedule in some cases: they change ``w'`` only."""
     extras = {}
     if world == 4:
-        extras = dict(max_norm=5.0)
+        extras = dict(max_grad_norm=5.0)
     if world == 8:
-        extras = dict(lam=warmup_cosine, lr_steps=6)
-    reps = EReplicas(world, k=k, compact=paged, **extras)
+        extras = dict(lr_lambda=warmup_cosine, lr_steps=6)
+    reps = Replicas(world, k=k, compact=paged, moment_dtype=FP32, ema_decay=DECAY, **extras)
     reps.configure(list(range(world)), 1)
     c = float(np.float32(1 - DECAY))
     ref = reps.init.double()
     for step in range(6):
-        reps.step([_raws(world, 40 * world + 7 * k + step)])
+        reps.step(raws(world, 40 * world + 7 * k + step))
         master = reps.full_state()[0]
         ref = ref + c * (master.double() - ref)
     got = reps.full_ema()
@@ -148,13 +94,13 @@ def test_kernel_ema_follows_an_fp64_ema_of_the_device_masters(world, k, paged):
 
 def test_bf16_ema_follows_the_fp64_ema_within_its_rounding_noise():
     world, steps = 2, 12
-    reps = EReplicas(world, moments=BF16, k=2)
+    reps = Replicas(world, k=2, moment_dtype=BF16, ema_decay=DECAY)
     reps.configure(list(range(world)), 1)
     c = float(np.float32(1 - DECAY))
     ref = reps.init.double()
     mag = ref.abs()  # each step rounds at the EMA's magnitude then: the noise is in ulps of the largest one it passed
     for step in range(steps):
-        reps.step([_raws(world, 900 + step)])
+        reps.step(raws(world, 900 + step))
         ref = ref + c * (reps.full_state()[0].double() - ref)
         mag = torch.maximum(mag, ref.abs())
     got = reps.full_ema().double()
@@ -170,19 +116,19 @@ def test_holders_agree_a_vetoed_step_leaves_the_ema_and_paged_equals_flat():
     runs = {}
     for moments in (FP32, BF16):
         for paged, blocks in ((False, 1), (False, 8), (True, 8)):
-            reps = EReplicas(world, moments=moments, k=2, compact=paged, blocks=blocks)
+            reps = Replicas(world, k=2, blocks=blocks, compact=paged, moment_dtype=moments, ema_decay=DECAY)
             reps.configure(list(range(world)), 1)
             for step in range(4):
-                raw = _raws(world, 60 + step)
+                rs = raws(world, 60 + step)
                 if step == 2:
                     reps.settle()
                     before = [o.ema.clone() for o in reps.opts]
-                    _step_vetoed_by_all(reps, raw)
+                    reps.step_vetoed_by_all(rs)
                     reps.settle()
                     for o, b in zip(reps.opts, before):
                         assert torch.equal(o.ema.view(torch.uint8), b.view(torch.uint8)), "a vetoed step moved the EMA"
                 else:
-                    reps.step([raw])
+                    reps.step(rs)
             runs[(moments, paged, blocks)] = (reps.full_ema(), reps.full_state()[0])
             assert all(o.t == 3 for o in reps.opts)
     for (moments, paged, blocks), (ema, master) in runs.items():
@@ -191,7 +137,7 @@ def test_holders_agree_a_vetoed_step_leaves_the_ema_and_paged_equals_flat():
 
 
 def test_without_an_ema_nothing_is_allocated_and_the_context_refuses():
-    reps = EReplicas(2, decay=None)
+    reps = Replicas(2, moment_dtype=FP32, ema_decay=None)
     reps.configure([0, 1], 1)
     o = reps.opts[0]
     assert o.ema is None and o._state_item() == 12 and o.state_bytes_allocated() == 12 * o.numel
@@ -206,14 +152,14 @@ def test_without_an_ema_nothing_is_allocated_and_the_context_refuses():
 @pytest.mark.parametrize("compact", [False, True])
 def test_kill_rejoin_and_split_commit_keep_the_ema_on_every_holder(compact):
     world = 4
-    reps = EReplicas(world, moments=BF16 if compact else FP32, k=2, compact=compact, min_world=3)
+    reps = Replicas(world, k=2, compact=compact, min_world=3, moment_dtype=BF16 if compact else FP32, ema_decay=DECAY)
     reps.configure([0, 1, 2, 3], 1)
     for step in range(2):
-        reps.step([_raws(4, 70 + step)])
+        reps.step(raws(4, 70 + step))
     src = reps.full_ema()
     reps.configure([0, 1, 3], 2)  # member 2 dies: its slices, EMA included, move to the survivors
     assert torch.equal(reps.full_ema(), src)
-    reps.step([_raws(3, 80)])
+    reps.step(raws(3, 80))
     reps.settle()
     src = reps.full_ema()
     o = reps.make(reps.comms[2])  # ... and restarts with nothing but the weights
@@ -226,7 +172,7 @@ def test_kill_rejoin_and_split_commit_keep_the_ema_on_every_holder(compact):
     held = sum(hi - lo for lo, hi in reps.layout().held(2, 4))
     assert o.pulled_bytes == o._state_item() * held == (10 if compact else 16) * held  # master + m + v + EMA
     # a split commit: member 1 misses an update the others apply, then pulls their state at the next quorum
-    reps.step([_raws(4, 81)], veto=1)
+    reps.step(raws(4, 81), veto=[1])
     reps.settle()
     assert reps.opts[1].t + 1 == reps.opts[0].t
     others = {(lo, hi): reps.get_ema(i, lo, hi) for i, lo, hi in reps.held() if i != 1}
@@ -235,16 +181,16 @@ def test_kill_rejoin_and_split_commit_keep_the_ema_on_every_holder(compact):
         for rank, i in enumerate(reps.members):
             if any(a <= lo and hi <= b for a, b in reps.opts[i]._holdings):
                 assert torch.equal(reps.get_ema(i, lo, hi), e)
-    reps.step([_raws(4, 82)])
+    reps.step(raws(4, 82))
     reps.full_ema()
 
 
 def test_a_slice_lost_with_all_its_holders_is_reseeded_from_the_weights_and_counted():
     world = 3
-    reps = EReplicas(world, k=1)
+    reps = Replicas(world, k=1, moment_dtype=FP32, ema_decay=DECAY)
     reps.configure([0, 1, 2], 1)
     for step in range(3):
-        reps.step([_raws(3, 110 + step)])
+        reps.step(raws(3, 110 + step))
     reps.settle()
     L = reps.layout()
     lost = L.held(2, 3)
@@ -260,9 +206,9 @@ def test_a_slice_lost_with_all_its_holders_is_reseeded_from_the_weights_and_coun
 
 def test_mismatched_decays_raise_on_every_rank_before_anything_moves():
     for decay in ([DECAY, DECAY, 0.99], [DECAY, None, DECAY]):
-        reps = EReplicas(3, decay=decay, compact=True)
+        reps = Replicas(3, compact=True, moment_dtype=FP32, ema_decay=decay)
         before = [(o.t, list(o._holdings)) for o in reps.opts]
-        errs = _configure_errors(reps, [0, 1, 2], 1)
+        errs = reps.configure_errors([0, 1, 2], 1)
         assert sorted(errs) == [0, 1, 2]
         for e in errs.values():
             assert isinstance(e, RuntimeError) and "disagree on the EMA" in str(e)
@@ -272,10 +218,10 @@ def test_mismatched_decays_raise_on_every_rank_before_anything_moves():
 
 # ----------------------------------------------------------------------------- checkpoints
 def _saved(tmp_path, moments, decay=DECAY, world=4):
-    live = EReplicas(world, moments=moments, k=2, decay=decay)
+    live = Replicas(world, k=2, moment_dtype=moments, ema_decay=decay)
     live.configure(list(range(world)), 1)
     for step in range(2):
-        live.step([_raws(world, 90 + step)])
+        live.step(raws(world, 90 + step))
     state = live.full_state()
     ema = live.full_ema() if decay is not None else None
     for o in live.opts:
@@ -295,14 +241,14 @@ def test_restore_at_another_world_keeps_or_converts_the_ema(tmp_path, saved, res
     ms = 2 if saved == BF16 else 4
     assert h["ema"] == {"decay": DECAY} and h["sections"] == sections(h["elements"], ms, ema=True)
     assert os.path.getsize(h["path"]) == h["data"] + (6 + 3 * ms) * h["elements"]
-    back = EReplicas(3, moments=restored, k=2, compact=compact, min_world=3)
+    back = Replicas(3, k=2, compact=compact, min_world=3, moment_dtype=restored, ema_decay=DECAY)
     for o in back.opts:
         assert o.restore(str(tmp_path))["step"] == 2
     back.configure([0, 1, 2], 1)
     assert torch.equal(back.full_state()[0], master)
     assert torch.equal(back.full_ema(), ema.to(restored))  # same type: the file's bits; otherwise converted
     assert all(o.lost_elements == 0 for o in back.opts)
-    back.step([_raws(3, 95)])
+    back.step(raws(3, 95))
     back.full_ema()
 
 
@@ -311,7 +257,7 @@ def test_restore_from_files_without_an_ema_seeds_it_from_the_master_weights(tmp_
     from torchft_b200.checkpointing.sharded import read_header
 
     assert "ema" not in read_header(os.path.join(tmp_path, "z1_step_2.w4.r0.bin"))
-    back = EReplicas(2, k=2, compact=True, min_world=2)
+    back = Replicas(2, k=2, compact=True, min_world=2, moment_dtype=FP32, ema_decay=DECAY)
     for o in back.opts:
         o.restore(str(tmp_path))
     with caplog.at_level("WARNING"):
@@ -321,18 +267,18 @@ def test_restore_from_files_without_an_ema_seeds_it_from_the_master_weights(tmp_
     # and a run without an EMA ignores a file's EMA section
     d2 = tmp_path / "with"
     _saved(d2, FP32)
-    plain = EReplicas(2, k=2, decay=None)
+    plain = Replicas(2, k=2, moment_dtype=FP32, ema_decay=None)
     for o in plain.opts:
         o.restore(str(d2))
     plain.configure([0, 1], 1)
-    plain.step([_raws(2, 97)])
+    plain.step(raws(2, 97))
     plain.full_state()
 
 
 def test_save_update_and_restore_raise_inside_ema_weights(tmp_path):
-    reps = EReplicas(2, k=2)
+    reps = Replicas(2, k=2, moment_dtype=FP32, ema_decay=DECAY)
     reps.configure([0, 1], 1)
-    reps.step([_raws(2, 5)])
+    reps.step(raws(2, 5))
     reps.settle()
     o = reps.opts[0]
     with o.ema_weights():
@@ -346,11 +292,11 @@ def test_save_update_and_restore_raise_inside_ema_weights(tmp_path):
 @pytest.mark.parametrize("moments,world,k,paged", [(FP32, 4, 2, False), (BF16, 4, 2, True), (FP32, 1, 1, False),
                                                     (BF16, 3, 3, False)])
 def test_ema_weights_puts_bf16_ema_in_every_param_and_restores_the_weights_bit_for_bit(moments, world, k, paged):
-    reps = EReplicas(world, moments=moments, k=k, compact=paged)
+    reps = Replicas(world, k=k, compact=paged, moment_dtype=moments, ema_decay=DECAY)
     reps.configure(list(range(world)), 1)
     for step in range(3):
-        reps.step([_raws(world, 130 + step)])
-    reps.step([_raws(world, 133)], sync=False)  # the last update may still be queued when the context is entered
+        reps.step(raws(world, 130 + step))
+    reps.step(raws(world, 133), sync=False)  # the last update may still be queued when the context is entered
     reps.settle()
     params = [o.param.clone() for o in reps.opts]
     assert all(torch.equal(p, params[0]) for p in params)
@@ -366,7 +312,7 @@ def test_ema_weights_puts_bf16_ema_in_every_param_and_restores_the_weights_bit_f
     torch.cuda.synchronize()
     for o, p in zip(reps.opts, params):
         assert torch.equal(o.param.view(torch.int16), p.view(torch.int16))
-    reps.step([_raws(world, 134)])  # training goes on from the same weights
+    reps.step(raws(world, 134))  # training goes on from the same weights
     reps.full_ema()
 
 
@@ -427,21 +373,10 @@ def test_ema_weights_waits_for_every_peer_before_it_pushes_with_real_signalling(
 
 
 # ----------------------------------------------------------------------------- trainer
-def _trainer(tag, **kw):
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
-    lh = local_lighthouse()
-    tr = FaultTolerantTrainer("llama3_tiny", loopback(lh.address()), replica_id=f"z1ema_{tag}_0",
-                              timeout=timedelta(seconds=30), lr=1e-3, **kw)
-    return lh, tr
-
-
 def test_trainer_ema_matches_an_fp64_ema_of_its_masters_and_evaluates_it(monkeypatch, tmp_path):
     monkeypatch.delenv("TORCHFT_B200_Z1_EMA_DECAY", raising=False)
     decay = 0.8
-    lh, tr = _trainer("ema", ema_decay=decay)
-    try:
+    with trainer("llama3_tiny", "z1ema_ema", lr=1e-3, ema_decay=decay) as tr:
         gen = torch.Generator().manual_seed(5)
         tok = torch.randint(0, tr.cfg.vocab_size, (2, 64), generator=gen).pin_memory()
         tgt = torch.randint(0, tr.cfg.vocab_size, (2, 64), generator=gen).pin_memory()
@@ -478,21 +413,14 @@ def test_trainer_ema_matches_an_fp64_ema_of_its_masters_and_evaluates_it(monkeyp
         tr.step(tok, tgt)  # training continues from the same weights
         tr.manager.state_dict()
         assert zo.t == 6
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
 
 def test_trainer_takes_the_decay_from_the_environment_and_refuses_the_classic_pipeline(monkeypatch):
     from torchft_b200.parallel.trainer import FaultTolerantTrainer
 
     monkeypatch.setenv("TORCHFT_B200_Z1_EMA_DECAY", "0.99")
-    lh, tr = _trainer("env")
-    try:
+    with trainer("llama3_tiny", "z1ema_env", lr=1e-3) as tr:
         assert tr.zopt.ema_decay == 0.99 and tr.zopt.ema is not None and tr.zopt.ema.dtype == FP32
-    finally:
-        tr.shutdown()
-        lh.shutdown()
     for pipe in (dict(zero1=False), dict(backend="nccl")):
         with pytest.raises(ValueError, match="ema_decay"):
             FaultTolerantTrainer("llama3_tiny", "unused:0", ema_decay=0.99, **pipe)

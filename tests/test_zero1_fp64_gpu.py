@@ -27,17 +27,15 @@ import pytest
 import torch
 
 from _fp64 import FTZ, U, _adamw_ref, _f32, _report_margins, assert_close_elementwise  # noqa: F401
+from _zero1_state import BF16, FP32, S16, State, chunks
 
 pytestmark = pytest.mark.gpu
 
-BF16, FP32 = torch.bfloat16, torch.float32
 B1B, B8B = 60_821_504, 218_112_000  # llama3_1b and llama3_8b transformer blocks, in elements
 PAD = 4096  # elements of each neighbouring unit around the unit under test (sentinel-filled)
-S16, S32 = 0x7FA5, 0x7FA5A5A5  # sentinel bit patterns (NaNs no kernel produces)
 LR, B1, EPS, WD = 1e-3, 0.9, 1e-8, 0.1
 TS = (1, 2, 10, 100, 1000, 3000, 10 ** 4, 10 ** 6)
 LR_STEPS = 50  # t = 1, 2, 10 read the table, later t its last entry
-CHUNK = 1 << 24
 MAX_NORM = 1.0
 NSM = 132
 CAP = NSM * 32  # grid cap of both kernels
@@ -110,11 +108,6 @@ def _held(r, W, k):
 
 def _gen(seed):
     return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _chunks(lo, hi):
-    for a in range(lo, hi, CHUNK):
-        yield a, min(hi, a + CHUNK)
 
 
 def _random_grad(n, seed):
@@ -261,68 +254,11 @@ def test_reduce_edge_units(W):
 
 
 # ----------------------------------------------------------------------------- update
-class State:
-    """One rank's optimizer state of the unit: full-size (``shift`` None; element e at e) or a pool of pages in a
-    shuffled slot order with spare slots (element e of the unit, flat index soff + e, at
-    ``table[(soff + e) >> shift] << shift | ((soff + e) & mask)``). Everything outside the held ranges is a sentinel."""
-
-    def __init__(self, n, held, shift, soff, md, seed):
-        self.n, self.held, self.shift, self.soff, self.md = n, held, shift, soff, md
-        self.table = None
-        if shift is None:
-            size = n
-        else:
-            page = 1 << shift
-            pages = sorted({p for lo, hi in held for p in range((soff + lo) >> shift, ((soff + hi - 1) >> shift) + 1)})
-            nslots = len(pages) + 3
-            slots = torch.randperm(nslots, generator=torch.Generator().manual_seed(seed))[:len(pages)]
-            tab = torch.full((((soff + n) >> shift) + 1,), -1, dtype=torch.int32)
-            if pages:
-                tab[torch.tensor(pages)] = slots.int()
-            self.table = tab.cuda()
-            size = nslots * page
-        self.master = torch.empty(max(size, 8), device="cuda")
-        self.master.view(torch.int32).fill_(S32)
-        mdt = FP32 if md == "f32" else BF16
-        self.m = torch.empty(max(size, 8), dtype=mdt, device="cuda")
-        self.v = torch.empty(max(size, 8), dtype=mdt, device="cuda")
-        for x in (self.m, self.v):
-            x.view(torch.int32 if mdt == FP32 else torch.int16).fill_(S32 if mdt == FP32 else S16)
-        self.mask = torch.zeros(max(size, 8), dtype=torch.bool, device="cuda")
-        for lo, hi in held:
-            for a, b in _chunks(lo, hi):
-                self.mask[self.pos(a, b)] = True
-
-    def pos(self, lo, hi):
-        if self.table is None:
-            return slice(lo, hi)
-        e = torch.arange(self.soff + lo, self.soff + hi, device="cuda")
-        return (self.table[e >> self.shift].long() << self.shift) | (e & ((1 << self.shift) - 1))
-
-    def get(self, lo, hi):
-        """Copies of (master, m, v) over unit elements [lo, hi)."""
-        p = self.pos(lo, hi)
-        return self.master[p].clone(), self.m[p].clone(), self.v[p].clone()
-
-    def put(self, lo, hi, w, m, v):
-        p = self.pos(lo, hi)
-        self.master[p], self.m[p], self.v[p] = w, m, v
-
-    def untouched(self):
-        out = ~self.mask
-        ok = bool((self.master.view(torch.int32)[out] == S32).all())
-        if self.m.dtype == FP32:
-            ok &= bool((self.m.view(torch.int32)[out] == S32).all()) and bool((self.v.view(torch.int32)[out] == S32).all())
-        else:
-            ok &= bool((self.m.view(torch.int16)[out] == S16).all()) and bool((self.v.view(torch.int16)[out] == S16).all())
-        return ok
-
-
 def _init_state(n, sl, W, k, shift, soff, md, seed):
     """Every holder of slice s starts from the same seeded master / m / v."""
     states = [State(n, [sl[s] for s in _held(r, W, k) if sl[s][0] < sl[s][1]], shift, soff, md, seed + r) for r in range(W)]
     for s, (lo, hi) in enumerate(sl):
-        for a, b in _chunks(lo, hi):
+        for a, b in chunks(lo, hi):
             g = _gen(seed * 31 + s * 7 + a)
             w = torch.randn(b - a, device="cuda", generator=g) * 0.05
             m = torch.randn(b - a, device="cuda", generator=g) * 1e-3
@@ -380,17 +316,15 @@ def _update_case(comms, n, k, shift, md, coef, lr_tab, nd, steps, grid, seed, re
             x[PAD:PAD + n].copy_(g)
         for p in params:
             p.view(torch.int16).fill_(S16)
-        before = [[states[s].get(a, b) for a, b in _chunks(*sl[s])] for s in range(W)]  # primary holder s of slice s
+        before = [[states[s].get(a, b) for a, b in chunks(*sl[s])] for s in range(W)]  # primary holder s of slice s
         gates = [torch.tensor([1, t], dtype=torch.int32, device="cuda") for _ in comms]
         for r, c in enumerate(comms):
             st = states[r]
-            c.zero1_update_("z1_param", PAD * 2, grads[r].data_ptr() + PAD * 2, st.master.data_ptr(), st.m.data_ptr(),
-                            st.v.data_ptr(), n, (LR, B1, b2, EPS, WD), gates[r], k, 0, grid, None,
-                            table=st.table.data_ptr() if shift is not None else 0, state_off=soff,
-                            page_shift=shift or 0, coef=coef_t.data_ptr() if coef is not None else 0,
+            c.zero1_update_("z1_param", PAD * 2, grads[r].data_ptr() + PAD * 2, nelem=n, hyper=(LR, B1, b2, EPS, WD),
+                            gate=gates[r], replication=k, mode=0, blocks=grid,
+                            coef=coef_t.data_ptr() if coef is not None else 0,
                             lr_table=lr_tab.data_ptr() if lr_tab is not None else 0,
-                            lr_steps=LR_STEPS if lr_tab is not None else 0, no_decay=nd,
-                            moment_dtype=FP32 if md == "f32" else BF16)
+                            lr_steps=LR_STEPS if lr_tab is not None else 0, no_decay=nd, **st.args())
             if record:
                 RAN.add(("update", W, shift is not None, coef is not None, md))
         torch.cuda.synchronize()
@@ -399,7 +333,7 @@ def _update_case(comms, n, k, shift, md, coef, lr_tab, nd, steps, grid, seed, re
         what = f"{'bf16' if md == 'bf16' else 'f32'} b2={b2}"
         full_master = torch.empty(n, device="cuda")
         for s, (lo, hi) in enumerate(sl):
-            for (a, b), (w0, m0, v0) in zip(_chunks(lo, hi), before[s]):
+            for (a, b), (w0, m0, v0) in zip(chunks(lo, hi), before[s]):
                 w1, m1, v1 = states[s].get(a, b)
                 full_master[a:b] = w1
                 for r in range(W):  # every holder stores the primary's bits
@@ -447,10 +381,9 @@ def _update_case(comms, n, k, shift, md, coef, lr_tab, nd, steps, grid, seed, re
         gates = [torch.tensor([0, steps[-1][0]], dtype=torch.int32, device="cuda") for _ in comms]
         for r, c in enumerate(comms):
             st = states[r]
-            c.zero1_update_("z1_param", PAD * 2, grads[r].data_ptr() + PAD * 2, st.master.data_ptr(), st.m.data_ptr(),
-                            st.v.data_ptr(), n, (LR, B1, steps[-1][1], EPS, WD), gates[r], k, 1, grid, None,
-                            table=st.table.data_ptr() if shift is not None else 0, state_off=soff,
-                            page_shift=shift or 0, moment_dtype=FP32 if md == "f32" else BF16)
+            c.zero1_update_("z1_param", PAD * 2, grads[r].data_ptr() + PAD * 2, nelem=n,
+                            hyper=(LR, B1, steps[-1][1], EPS, WD), gate=gates[r], replication=k, mode=1, blocks=grid,
+                            **st.args())
         torch.cuda.synchronize()
         for r in range(W):
             assert torch.equal(params[r].view(torch.int16)[PAD:PAD + n], want.view(torch.int16)), f"refresh of rank {r} ({tag})"
@@ -581,10 +514,9 @@ def test_bits_do_not_depend_on_the_grid_or_on_real_signalling():
         for r, c in enumerate(live):
             st = states[r]
             with torch.cuda.stream(streams[r]):
-                c.zero1_update_("z1_param", PAD * 2, _seg(c, "z1_grad", n).data_ptr() + PAD * 2, st.master.data_ptr(),
-                                st.m.data_ptr(), st.v.data_ptr(), n, (LR, B1, 0.999, EPS, WD), gates[r], k, 0, UPD_DEFAULT,
-                                streams[r], table=st.table.data_ptr(), state_off=soff, page_shift=16,
-                                coef=coef.data_ptr(), moment_dtype=BF16)
+                c.zero1_update_("z1_param", PAD * 2, _seg(c, "z1_grad", n).data_ptr() + PAD * 2, nelem=n,
+                                hyper=(LR, B1, 0.999, EPS, WD), gate=gates[r], replication=k, mode=0,
+                                blocks=UPD_DEFAULT, stream=streams[r], coef=coef.data_ptr(), **st.args())
         torch.cuda.synchronize()
         assert all(c.errored() is None for c in live)
         for r, c in enumerate(live):
@@ -618,8 +550,8 @@ def test_world_one_update_stores_the_bits_of_the_flat_optimizer():
             st.put(0, n, w, m, v)
             grad[PAD:PAD + n].copy_(g)
             gate = torch.tensor([1, t], dtype=torch.int32, device="cuda")
-            c.zero1_update_("z1_param", PAD * 2, grad.data_ptr() + PAD * 2, st.master.data_ptr(), st.m.data_ptr(),
-                            st.v.data_ptr(), n, (LR, B1, b2, EPS, WD), gate, 1, 0, UPD_DEFAULT)
+            c.zero1_update_("z1_param", PAD * 2, grad.data_ptr() + PAD * 2, nelem=n, hyper=(LR, B1, b2, EPS, WD),
+                            gate=gate, replication=1, mode=0, blocks=UPD_DEFAULT, **st.args())
             opt = fused.FlatAdamW(torch.empty(n, dtype=BF16, device="cuda"), g.clone(), lr=LR, betas=(B1, b2), eps=EPS,
                                   weight_decay=WD)
             opt.master.copy_(w)

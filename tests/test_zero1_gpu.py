@@ -7,32 +7,13 @@ Reference for the numerics: plain PyTorch fp32 AdamW on the fp32-accumulated, bf
 
 from __future__ import annotations
 
-from datetime import timedelta
-
 import pytest
 import torch
 
+from _zero1_replicas import HP, NUMEL, UNITS, kernel_world, reduced, ref_adamw, trainer
+from _zero1_state import State
+
 pytestmark = pytest.mark.gpu
-
-UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
-NUMEL = UNITS[-1][1]
-HP = (1e-2, 0.9, 0.95, 1e-8, 0.1)  # lr, b1, b2, eps, wd
-
-
-def _world(world, presignal=True):
-    from torchft_b200.parallel.symm_mem import SymmetricComm
-
-    return SymmetricComm.virtual_world(world, {"z1_grad": NUMEL * 2, "z1_param": NUMEL * 2}, presignal=presignal,
-                                       timeout=timedelta(seconds=20))
-
-
-def _ref_adamw(master, m, v, g, t):
-    lr, b1, b2, eps, wd = HP
-    m.mul_(b1).add_(g, alpha=1 - b1)
-    v.mul_(b2).addcmul_(g, g, value=1 - b2)
-    bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t
-    denom = v.sqrt() / (bc2 ** 0.5) + eps
-    master.mul_(1 - lr * wd).addcdiv_(m, denom, value=-lr / bc1)
 
 
 @pytest.mark.parametrize("world,k", [(2, 2), (3, 2), (8, 2), (8, 1), (4, 3)])
@@ -40,7 +21,7 @@ def test_reduce_scatter_commit_update_match_reference(world, k):
     from torchft_b200.parallel.zero1 import ShardLayout
 
     dev = torch.device("cuda", 0)
-    comms = _world(world)
+    comms = kernel_world(world)
     L = ShardLayout(tuple(UNITS), k)
     g = torch.Generator(device=dev).manual_seed(11)
     grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
@@ -48,9 +29,7 @@ def test_reduce_scatter_commit_update_match_reference(world, k):
     init = (torch.randn(NUMEL, device=dev, generator=g) * 0.05).bfloat16()
     for p in params:
         p.copy_(init)
-    master = [init.float() for _ in comms]
-    m = [torch.zeros(NUMEL, device=dev) for _ in comms]
-    v = [torch.zeros(NUMEL, device=dev) for _ in comms]
+    state = [State.seeded(init) for _ in comms]
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     rm, rmm, rv = init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)
     quiet = 1 if world > 2 else None  # a healing / spare rank whose gradients must count as zeros
@@ -62,11 +41,7 @@ def test_reduce_scatter_commit_update_match_reference(world, k):
             grads[r].copy_(raw[r])
         if quiet is not None:
             grads[quiet].zero_()  # sequential emulation: the quiet rank's in-kernel zeroing must precede rank 0's reads
-        acc = torch.zeros(NUMEL, device=dev)
-        for r in range(world):  # fixed rank order, fp32 accumulate, then scale, then round to bf16
-            if r != quiet:
-                acc += raw[r].float()
-        reduced = (acc * (1.0 / contributors)).bfloat16()
+        red = reduced([raw], quiet)
 
         # one-kernel-at-a-time emulation: the quiet rank zeroes its buffer inside its kernel, which on real hardware
         # happens before anybody's push (barrier 1) -- so its kernel goes first here
@@ -77,29 +52,30 @@ def test_reduce_scatter_commit_update_match_reference(world, k):
         torch.cuda.synchronize()
         for r in range(world):
             for lo, hi in L.held(r, world):
-                assert torch.equal(grads[r][lo:hi], reduced[lo:hi]), f"rank {r} held range [{lo},{hi}) step {step}"
+                assert torch.equal(grads[r][lo:hi], red[lo:hi]), f"rank {r} held range [{lo},{hi}) step {step}"
 
         seqs = [c.zero1_commit_(gates[r], True, True) for r, c in enumerate(comms)]
         for r, c in enumerate(comms):
             for lo, hi in UNITS:
-                c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, master[r].data_ptr() + lo * 4,
-                                m[r].data_ptr() + lo * 4, v[r].data_ptr() + lo * 4, hi - lo, HP, gates[r], k, 0, 4)
+                c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP,
+                                gate=gates[r], replication=k, mode=0, blocks=4, **state[r].args(lo))
         torch.cuda.synchronize()
         assert all(c.errored() is None for c in comms)
         assert all(c.verdict(s) is True for c, s in zip(comms, seqs))
         assert all(int(gt[0]) == 1 and int(gt[1]) == step for gt in gates)
 
-        _ref_adamw(rm, rmm, rv, reduced.float(), step)
+        ref_adamw(rm, rmm, rv, red.float(), step)
         for r in range(1, world):
             assert torch.equal(params[0], params[r]), "weights must be bit-identical across replicas"
         # the bf16 weights are the rounded masters of their primary holders
+        master = [st.master for st in state]
         for r in range(world):
             for lo, hi in L.primary(r, world):
                 assert torch.equal(params[0][lo:hi], master[r][lo:hi].bfloat16())
             for lo, hi in L.held(r, world):
                 torch.testing.assert_close(master[r][lo:hi], rm[lo:hi], rtol=2e-5, atol=1e-7)
-                torch.testing.assert_close(m[r][lo:hi], rmm[lo:hi], rtol=1e-5, atol=1e-7)
-                torch.testing.assert_close(v[r][lo:hi], rv[lo:hi], rtol=1e-5, atol=1e-9)
+                torch.testing.assert_close(state[r].m[lo:hi], rmm[lo:hi], rtol=1e-5, atol=1e-7)
+                torch.testing.assert_close(state[r].v[lo:hi], rv[lo:hi], rtol=1e-5, atol=1e-9)
         # holders of the same slice computed bit-identical state
         for u in range(len(UNITS)):
             for s in range(world):
@@ -112,12 +88,10 @@ def test_reduce_scatter_commit_update_match_reference(world, k):
 def test_gate_zero_skips_update_and_refresh_rebroadcasts_masters():
     dev = torch.device("cuda", 0)
     world, k = 4, 2
-    comms = _world(world)
+    comms = kernel_world(world)
     params = [c.segment("z1_param")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
-    master = [torch.full((NUMEL,), 1.5, device=dev) for _ in comms]
-    m = [torch.zeros(NUMEL, device=dev) for _ in comms]
-    v = [torch.zeros(NUMEL, device=dev) for _ in comms]
+    state = [State.seeded(torch.full((NUMEL,), 1.5, device=dev)) for _ in comms]
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     for p, gr in zip(params, grads):
         p.fill_(9.0)
@@ -126,26 +100,26 @@ def test_gate_zero_skips_update_and_refresh_rebroadcasts_masters():
     for r, c in enumerate(comms):
         seq = c.zero1_commit_(gates[r], False, True)
         for lo, hi in UNITS:
-            c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, master[r].data_ptr() + lo * 4,
-                            m[r].data_ptr() + lo * 4, v[r].data_ptr() + lo * 4, hi - lo, HP, gates[r], k, 0, 4)
+            c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP, gate=gates[r],
+                            replication=k, mode=0, blocks=4, **state[r].args(lo))
         torch.cuda.synchronize()
         assert c.verdict(seq) is False
     assert all(int(gt[0]) == 0 and int(gt[1]) == 0 for gt in gates)
-    assert all(bool((p == 9.0).all()) for p in params) and all(bool((x == 1.5).all()) for x in master)
+    assert all(bool((p == 9.0).all()) for p in params) and all(bool((st.master == 1.5).all()) for st in state)
     # refresh (mode 1): ungated re-broadcast of bf16(master) of the primary slices, state untouched
     for r, c in enumerate(comms):
         for lo, hi in UNITS:
-            c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, master[r].data_ptr() + lo * 4,
-                            m[r].data_ptr() + lo * 4, v[r].data_ptr() + lo * 4, hi - lo, HP, gates[r], k, 1, 4)
+            c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP, gate=gates[r],
+                            replication=k, mode=1, blocks=4, **state[r].args(lo))
     torch.cuda.synchronize()
-    assert all(bool((p == 1.5).all()) for p in params) and all(bool((x == 0).all()) for x in m)
+    assert all(bool((p == 1.5).all()) for p in params) and all(bool((st.m == 0).all()) for st in state)
 
 
 @pytest.mark.parametrize("world", [2, 8])
 def test_commit_verdict_is_unanimous_with_real_signalling(world):
     """Concurrent launch on W streams (presignal off): one rank's veto must reach every rank's gate."""
     dev = torch.device("cuda", 0)
-    comms = _world(world, presignal=False)
+    comms = kernel_world(world, presignal=False)
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     streams = [torch.cuda.Stream(device=dev) for _ in comms]
     for veto in (None, world - 1, None):
@@ -165,15 +139,13 @@ def test_concurrent_ranks_full_pipeline_in_one_process():
     """All W ranks' kernels in flight at once on W streams: real barriers, same result as the reference."""
     dev = torch.device("cuda", 0)
     world, k = 4, 2
-    comms = _world(world, presignal=False)
+    comms = kernel_world(world, presignal=False)
     g = torch.Generator(device=dev).manual_seed(5)
     grads = [c.segment("z1_grad")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     params = [c.segment("z1_param")[: NUMEL * 2].view(torch.bfloat16) for c in comms]
     raw = [torch.randn(NUMEL, device=dev, generator=g).bfloat16() for _ in comms]
     init = torch.randn(NUMEL, device=dev, generator=g).bfloat16()
-    master = [init.float() for _ in comms]
-    m = [torch.zeros(NUMEL, device=dev) for _ in comms]
-    v = [torch.zeros(NUMEL, device=dev) for _ in comms]
+    state = [State.seeded(init) for _ in comms]
     gates = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in comms]
     for r in range(world):
         grads[r].copy_(raw[r])
@@ -187,15 +159,12 @@ def test_concurrent_ranks_full_pipeline_in_one_process():
                 c.zero1_reduce_scatter_("z1_grad", lo * 2, hi - lo, 1.0 / world, True, k, 2, s)
             c.zero1_commit_(gates[r], True, True, s)
             for lo, hi in UNITS:
-                c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, master[r].data_ptr() + lo * 4,
-                                m[r].data_ptr() + lo * 4, v[r].data_ptr() + lo * 4, hi - lo, HP, gates[r], k, 0, 2, s)
+                c.zero1_update_("z1_param", lo * 2, grads[r].data_ptr() + lo * 2, nelem=hi - lo, hyper=HP,
+                                gate=gates[r], replication=k, mode=0, blocks=2, stream=s, **state[r].args(lo))
     torch.cuda.synchronize()
     assert all(c.errored() is None for c in comms)
-    acc = torch.zeros(NUMEL, device=dev)
-    for r in range(world):
-        acc += raw[r].float()
     rm, rmm, rv = init.float(), torch.zeros(NUMEL, device=dev), torch.zeros(NUMEL, device=dev)
-    _ref_adamw(rm, rmm, rv, (acc / world).bfloat16().float(), 1)
+    ref_adamw(rm, rmm, rv, reduced([raw]).float(), 1)
     for r in range(world):
         assert torch.equal(params[0], params[r])
     torch.testing.assert_close(params[0].float(), rm.bfloat16().float(), rtol=0, atol=2e-2)
@@ -203,15 +172,9 @@ def test_concurrent_ranks_full_pipeline_in_one_process():
 
 
 def test_trainer_zero1_matches_classic_adamw_at_world_one():
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
     out = []
     for zero1 in (False, True):
-        lh = local_lighthouse()
-        tr = FaultTolerantTrainer("llama3_debug", loopback(lh.address()), replica_id=f"z1eq_{int(zero1)}_0",
-                                  timeout=timedelta(seconds=30), bucket_mb=1.0, zero1=zero1)
-        try:
+        with trainer("llama3_debug", f"z1eq_{int(zero1)}", bucket_mb=1.0, zero1=zero1) as tr:
             gen = torch.Generator().manual_seed(5)
             losses = []
             for _ in range(4):
@@ -222,9 +185,6 @@ def test_trainer_zero1_matches_classic_adamw_at_world_one():
             sd = tr.state_dict()
             torch.cuda.synchronize()
             out.append((losses, sd["param"].clone()))
-        finally:
-            tr.shutdown()
-            lh.shutdown()
     (l0, p0), (l1, p1) = out
     # the same update rule with the same fp32 bias corrections (1 - b^t of the fp32 betas, rounded once) on both sides
     diff = (p0.float() - p1.float()).abs()

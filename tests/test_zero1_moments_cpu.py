@@ -9,14 +9,11 @@ import numpy as np
 import pytest
 import torch
 
-from test_zero1_cpu import UNITS
+from _zero1_replicas import widen
+from _zero1_sim import UNITS
 from torchft_b200.checkpointing.sharded import encode_header, file_dtype, moment_size, payload_bytes, sections
 from torchft_b200.parallel.zero1 import (PAGE_SHIFT, ShardLayout, bf16_sr, check_moment_agreement, moment_type,
                                          newest_complete_step, pool_pages, sr_bits)
-
-
-def _widen(bits):
-    return (np.asarray(bits, dtype=np.uint16).astype(np.uint32) << np.uint32(16)).view(np.float32)
 
 
 def _down(x):
@@ -26,7 +23,7 @@ def _down(x):
 
 # ----------------------------------------------------------------------------- the rounding
 def test_exact_bf16_values_come_back_unchanged_for_every_r():
-    exact = _widen(np.array([0x0000, 0x8000, 0x3F80, 0xBF80, 0x0001, 0x8001, 0x7F7F, 0xFF7F, 0x4049, 0x0080], np.uint16))
+    exact = widen(np.array([0x0000, 0x8000, 0x3F80, 0xBF80, 0x0001, 0x8001, 0x7F7F, 0xFF7F, 0x4049, 0x0080], np.uint16))
     r = np.arange(1 << 16, dtype=np.uint32)
     for x in exact:
         out = bf16_sr(np.full(r.shape, x, np.float32), None, None, 0, r=r)
@@ -42,7 +39,7 @@ def test_result_is_one_of_the_two_neighbours_and_rounds_away_from_zero_with_the_
         out = bf16_sr(x, e, t, which)
         lo = _down(x)
         assert ((out == lo) | (out == lo + 1)).all()
-        assert (np.abs(_widen(out)) >= np.abs(_widen(lo))).all()
+        assert (np.abs(widen(out)) >= np.abs(widen(lo))).all()
     # every r: the value goes up exactly when r reaches 2**16 - (discarded bits)
     r = np.arange(1 << 16, dtype=np.uint32)
     for v in (np.float32(1.2345678), np.float32(-7.000123e-12)):
@@ -60,7 +57,7 @@ def test_inf_and_nan_pass_through():
     nans = np.array([0x7FC00000, 0xFFC00000, 0x7F800001, 0xFF80FFFF, 0x7FFFFFFF], np.uint32).view(np.float32)
     for which in (0, 1):
         out = bf16_sr(nans, np.arange(5), 3, which)
-        assert np.isnan(_widen(out)).all()
+        assert np.isnan(widen(out)).all()
         assert ((out & 0x8000) == (nans.view(np.uint32) >> 16 & 0x8000)).all()  # the sign is kept
 
 
@@ -68,14 +65,14 @@ def test_mean_is_unbiased_over_elements_and_over_updates():
     """N draws of a fixed x: the error of the mean has standard deviation <= ulp / (2 sqrt(N)); 5 of those is the bound."""
     n = 1 << 16
     for x in (np.float32(1.2345678), np.float32(-0.00317), np.float32(1.0 + 2.0 ** -15)):
-        ulp = float(np.abs(_widen(_down(x) + 1) - _widen(_down(x))))
+        ulp = float(np.abs(widen(_down(x) + 1) - widen(_down(x))))
         bound = 5 * ulp / (2 * np.sqrt(n))
         streams = {"elements": (np.arange(n, dtype=np.uint64) + np.uint64(1 << 33), 7),
                    "updates": (np.uint64(123456789), np.arange(1, n + 1)),
                    "both": (np.arange(n, dtype=np.uint64) * np.uint64(8), np.arange(n) % 251)}
         for name, (e, t) in streams.items():
             for which in (0, 1):
-                got = _widen(bf16_sr(np.full(n, x, np.float32), e, t, which)).astype(np.float64).mean()
+                got = widen(bf16_sr(np.full(n, x, np.float32), e, t, which)).astype(np.float64).mean()
                 assert abs(got - float(x)) < bound, (x, name, which, got - float(x), bound)
 
 
@@ -135,7 +132,7 @@ def test_second_moment_with_beta2_999_stalls_under_round_to_nearest_and_converge
     sr = np.zeros(n, np.float32)
     for t in range(1, steps + 1):
         rn = (rn.float() * float(b2) + float(np.float32(1) - b2) * float(g2)).bfloat16()
-        sr = _widen(bf16_sr(b2 * sr + (np.float32(1) - b2) * g2, e, t, 1))
+        sr = widen(bf16_sr(b2 * sr + (np.float32(1) - b2) * g2, e, t, 1))
     rn = rn.float().numpy()
     assert (rn == rn[0]).all() and rn[0] < 0.3, f"round-to-nearest stalls far below g^2: {rn[0]}"
     # 1 - 0.999**6000 = 0.9975; one element's stationary noise is ulp / sqrt(6 * 2 * 0.001) = 3.6 % (1 sigma)

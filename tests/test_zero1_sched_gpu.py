@@ -8,31 +8,18 @@ its scheduler once per committed step, on the same reduced gradients, in fp32.
 
 from __future__ import annotations
 
-import math
-import threading
-from datetime import timedelta
-
 import numpy as np
 import pytest
 import torch
 
-from _zero1_replicas import HP, PG, Replicas
+from _zero1_replicas import HP, NUMEL, STEPS, UNITS, Replicas, raws, reduced, trainer, warmup_cosine
 
 pytestmark = pytest.mark.gpu
 
 LR, B1, B2, EPS, WD = HP
-UNITS = [(0, 8 * 4096), (8 * 4096, 8 * 4096 + 8 * 1001), (8 * 4096 + 8 * 1001, 8 * 4096 + 8 * 1001 + 8 * 7)]
-NUMEL = UNITS[-1][1]
 # exempt ranges in every unit: short and long ones, across slice and page bounds, one ending at a unit's end
-NO_DECAY = [(8, 64), (4096, 20000), (UNITS[1][0] + 800, UNITS[1][0] + 1600), (UNITS[2][0] + 16, UNITS[2][1])]
-STEPS = 4
-
-
-def warmup_cosine(i):
-    """Two warmup steps, then a cosine to 0.1 over the rest of the table."""
-    if i < 2:
-        return (i + 1) / 2
-    return 0.1 + 0.9 * 0.5 * (1 + math.cos(math.pi * (i - 2) / (STEPS - 2)))
+NO_DECAY = ((8, 64), (4096, 20000), (UNITS[1][0] + 800, UNITS[1][0] + 1600), (UNITS[2][0] + 16, UNITS[2][1]))
+SCHED = dict(lr_lambda=warmup_cosine, lr_steps=STEPS, no_decay=NO_DECAY)  # the schedule and exemptions of most tests
 
 
 def _mask(ranges):
@@ -69,38 +56,6 @@ class Ref:
             x[self.mask] = get(self.pn)
             out.append(x)
         return out
-
-
-class SchedReplicas(Replicas):
-    """:class:`Replicas` whose optimizers take a schedule and exemptions (``lam`` and ``no_decay`` may be per-member
-    lists, to build replicas that disagree)."""
-
-    def __init__(self, n, units=UNITS, lam=warmup_cosine, lr_steps=STEPS, no_decay=NO_DECAY, **kw):
-        self.lam, self.lr_steps, self.no_decay = lam, lr_steps, no_decay
-        super().__init__(n, units, **kw)
-
-    def make(self, comm):
-        from torchft_b200.parallel.zero1 import Zero1Optimizer
-
-        i = self.comms.index(comm)
-        lam = self.lam[i] if isinstance(self.lam, list) else self.lam
-        nd = self.no_decay[i] if self.no_decay and isinstance(self.no_decay[0], list) else self.no_decay
-        return Zero1Optimizer(PG(comm), self.numel, units=self.units, lr=LR, betas=(B1, B2), eps=EPS, weight_decay=WD,
-                              replication=self.k, blocks=4, compact=self.compact, min_world=self.min_world,
-                              page_shift=8, max_grad_norm=self.max_norm, grad_accum_steps=self.M,
-                              lr_lambda=lam, lr_steps=self.lr_steps if lam is not None else 0, no_decay=nd)
-
-
-def _raws(world, seed, scale=1.0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    return [(torch.randn(NUMEL, device="cuda", generator=g) * (r + 1) * scale).bfloat16() for r in range(world)]
-
-
-def _reduced(raw):
-    acc = torch.zeros(NUMEL, device="cuda")
-    for x in raw:  # fixed rank order, fp32 accumulate, then scale, then round to bf16
-        acc += x.float()
-    return (acc * (1.0 / len(raw))).bfloat16()
 
 
 def _check(reps, ref, weights=True):
@@ -153,14 +108,14 @@ CASES = [(w, k, paged) for w in (1, 2, 4, 8) for k in (1, 2) if k <= w for paged
 @pytest.mark.parametrize("world,k,paged", CASES)
 def test_scheduled_update_with_exemptions_matches_adamw_with_lambda_lr(world, k, paged):
     clip = world == 4 or (world == 8 and paged)
-    reps = SchedReplicas(world, k=k, compact=paged, max_norm=5.0 if clip else None)
+    reps = Replicas(world, k=k, compact=paged, max_grad_norm=5.0 if clip else None, **SCHED)
     reps.configure(list(range(world)), 1)
     ref = Ref(reps.init, warmup_cosine, STEPS, NO_DECAY)
     clipped = []
     for step in range(STEPS + 2):  # two updates past the end of the table
-        raw = _raws(world, 100 * world + 10 * k + step, scale=1.0 if step % 2 else 0.01)
-        reps.step([raw])
-        g = _reduced(raw).float()
+        rs = raws(world, 100 * world + 10 * k + step, (1.0 if step % 2 else 0.01,))
+        reps.step(rs)
+        g = reduced(rs).float()
         if clip:
             coef = reps.opts[0]._clip[1].clone()
             clipped.append(float(coef) < 1)
@@ -179,10 +134,10 @@ def test_neutral_schedule_and_no_exemptions_change_nothing(world, paged):
     """A lambda that is always 1.0 and no exempt ranges: the same bits as the launch without either."""
     runs = []
     for lam in (None, lambda i: 1.0):
-        reps = SchedReplicas(world, lam=lam, lr_steps=3, no_decay=[], compact=paged)
+        reps = Replicas(world, compact=paged, lr_lambda=lam, lr_steps=3)
         reps.configure(list(range(world)), 1)
         for step in range(5):
-            reps.step([_raws(world, 7 + step)])
+            reps.step(raws(world, 7 + step))
         reps.settle()
         runs.append([(o.param.clone(), o.held_state()) for o in reps.opts])
     assert runs[1][0][1], "something is held"
@@ -194,41 +149,26 @@ def test_neutral_schedule_and_no_exemptions_change_nothing(world, paged):
                 assert torch.equal(x, y)
 
 
-def _step_vetoed_by_all(reps, raw):
-    """``Replicas.step`` in which every member votes no: the verdict one rank's veto gives every rank once the commit
-    kernel has exchanged it (the pre-signalled virtual world does not exchange verdicts)."""
-    reps.settle()
-    for rank, i in enumerate(reps.members):
-        reps.opts[i].grad.copy_(raw[rank])
-    for i in reps.members:
-        for u in range(len(reps.units)):
-            reps.opts[i].reduce_scatter(u, 1.0 / len(reps.members), True)
-    reps.pending = {i: reps.opts[i].enqueue(False) for i in reps.members}
-    for i in reps.members:
-        reps.opts[i].update()
-    torch.cuda.synchronize()
-
-
 def test_vetoed_steps_do_not_advance_the_schedule():
     world = 4
     lam = [1.0, 0.25, 2.0, 0.5, 1.5, 0.75].__getitem__  # a wrong rate anywhere shows in the state
-    reps = SchedReplicas(world, lam=lam, lr_steps=6, max_norm=float("inf"))
+    reps = Replicas(world, max_grad_norm=float("inf"), **{**SCHED, "lr_lambda": lam, "lr_steps": 6})
     reps.configure(list(range(world)), 1)
     ref = Ref(reps.init, lam, 6, NO_DECAY)
     plan = [None, "veto", None, "nonfinite", None]
     committed = 0
     for step, what in enumerate(plan):
-        raw = _raws(world, 60 + step)
+        rs = raws(world, 60 + step)
         if what == "nonfinite":
-            raw[2][UNITS[1][0] + 100] = float("inf")
+            rs[0][2][UNITS[1][0] + 100] = float("inf")
         if what == "veto":
-            _step_vetoed_by_all(reps, raw)
+            reps.step_vetoed_by_all(rs)
         else:
-            reps.step([raw])
+            reps.step(rs)
         reps.settle()
         if what is None:
             committed += 1
-            ref.step(_reduced(raw).float())
+            ref.step(reduced(rs).float())
         for o in reps.opts:
             assert o.t == committed, (step, what)
             assert o.lr_at(o.t + 1) == float(np.float32(LR * lam(committed)))
@@ -236,17 +176,17 @@ def test_vetoed_steps_do_not_advance_the_schedule():
     _check(reps, ref)
 
     # a split commit: member 1 misses an update the others apply, then adopts their count at the next quorum
-    raw = _raws(world, 70)
-    reps.step([raw], veto=1)
+    rs = raws(world, 70)
+    reps.step(rs, veto=[1])
     reps.settle()
-    ref.step(_reduced(raw).float())
+    ref.step(reduced(rs).float())
     assert reps.opts[1].t == committed and all(reps.opts[i].t == committed + 1 for i in (0, 2, 3))
     reps.configure(list(range(world)), 2)
     assert all(o.t == committed + 1 for o in reps.opts)
     for seed in (71, 72):
-        raw = _raws(world, seed)
-        reps.step([raw])
-        ref.step(_reduced(raw).float())
+        rs = raws(world, seed)
+        reps.step(rs)
+        ref.step(reduced(rs).float())
         _check(reps, ref, weights=seed == 72)
     assert all(o.t == committed + 3 for o in reps.opts)
 
@@ -254,7 +194,7 @@ def test_vetoed_steps_do_not_advance_the_schedule():
 def test_kill_and_rejoin_keep_every_holder_on_the_schedule():
     world = 4
     lam = [1.0, 0.5, 2.0, 0.25, 1.5, 0.75, 1.25, 0.6].__getitem__  # a distinct rate per update
-    reps = SchedReplicas(world, k=2, lam=lam, lr_steps=8)
+    reps = Replicas(world, k=2, **{**SCHED, "lr_lambda": lam, "lr_steps": 8})
     ref = Ref(reps.init, lam, 8, NO_DECAY)
     g = torch.Generator(device="cuda").manual_seed(3)
 
@@ -291,7 +231,7 @@ def test_kill_and_rejoin_keep_every_holder_on_the_schedule():
 def test_restore_continues_the_schedule(tmp_path, world):
     g = torch.Generator(device="cuda").manual_seed(8)
     grads = [torch.randn(NUMEL, device="cuda", generator=g).bfloat16() for _ in range(4)]
-    live = SchedReplicas(4)
+    live = Replicas(4, **SCHED)
     ref = Ref(live.init, warmup_cosine, STEPS, NO_DECAY)
     live.configure([0, 1, 2, 3], 1)
     for gs in grads[:2]:
@@ -307,7 +247,7 @@ def test_restore_continues_the_schedule(tmp_path, world):
         ref.step(gs.float())
     live.settle()
 
-    back = SchedReplicas(world)
+    back = Replicas(world, **SCHED)
     for o in back.opts:
         assert o.restore(str(tmp_path))["step"] == 2 and o.t == 2
     back.configure(list(range(world)), 1)
@@ -326,37 +266,15 @@ def test_restore_continues_the_schedule(tmp_path, world):
     _check(back, ref)
 
 
-def _configure_errors(reps, members, epoch):
-    """``Replicas.configure`` that returns each member's exception instead of asserting there is none."""
-    from torch.distributed import PrefixStore
-
-    from torchft_b200.parallel.symm_mem import SymmetricComm
-
-    SymmetricComm.virtual_quorum(reps.comms, members, epoch)
-    errs = {}
-
-    def run(rank, m):
-        try:
-            reps.opts[m]._on_configured(PrefixStore(f"q/{epoch}", reps.store), rank, len(members), epoch)
-        except Exception as e:  # noqa: BLE001
-            errs[m] = e
-
-    ts = [threading.Thread(target=run, args=(rank, m)) for rank, m in enumerate(members)]
-    [t.start() for t in ts]
-    [t.join() for t in ts]
-    torch.cuda.synchronize()
-    return errs
-
-
 @pytest.mark.parametrize("what", ["lambda", "no_decay", "schedule_on_one_rank"])
 def test_mismatched_schedules_raise_on_every_rank_before_anything_moves(what):
     world = 3
-    kw = {"lambda": dict(lam=[warmup_cosine, warmup_cosine, lambda i: 1.0]),
+    kw = {"lambda": dict(lr_lambda=[warmup_cosine, warmup_cosine, lambda i: 1.0]),
           "no_decay": dict(no_decay=[NO_DECAY, NO_DECAY, NO_DECAY[:2]]),
-          "schedule_on_one_rank": dict(lam=[warmup_cosine, None, warmup_cosine])}[what]
-    reps = SchedReplicas(world, compact=what == "no_decay", **kw)
+          "schedule_on_one_rank": dict(lr_lambda=[warmup_cosine, None, warmup_cosine])}[what]
+    reps = Replicas(world, compact=what == "no_decay", **{**SCHED, **kw})
     before = [(o.t, list(o._holdings)) for o in reps.opts]
-    errs = _configure_errors(reps, [0, 1, 2], 1)
+    errs = reps.configure_errors([0, 1, 2], 1)
     assert sorted(errs) == [0, 1, 2]
     for e in errs.values():
         assert isinstance(e, RuntimeError) and "disagree" in str(e)
@@ -366,13 +284,7 @@ def test_mismatched_schedules_raise_on_every_rank_before_anything_moves(what):
 
 # ----------------------------------------------------------------------------- trainer
 def _train(tag, steps=3, lr=3e-4, **kw):
-    from torchft_b200.bench_utils import local_lighthouse, loopback
-    from torchft_b200.parallel.trainer import FaultTolerantTrainer
-
-    lh = local_lighthouse()
-    tr = FaultTolerantTrainer("llama3_tiny", loopback(lh.address()), replica_id=f"z1sched_{tag}_0",
-                              timeout=timedelta(seconds=30), lr=lr, **kw)
-    try:
+    with trainer("llama3_tiny", f"z1sched_{tag}", lr=lr, **kw) as tr:
         torch.cuda.synchronize()
         start = (tr.zopt.param.clone(), tr.zopt.master.clone())
         gen = torch.Generator().manual_seed(5)
@@ -392,9 +304,6 @@ def _train(tag, steps=3, lr=3e-4, **kw):
                  for q, o in zip(tr.flat.params, tr.flat.offsets) if q is p}
         return {"loss": losses, "lr": lrs, "t": ts, "start": start, "param": tr.zopt.param.clone(),
                 "master": tr.zopt.master.clone(), "where": where}
-    finally:
-        tr.shutdown()
-        lh.shutdown()
 
 
 def test_trainer_with_a_constant_schedule_reproduces_the_trainer_without_one():
