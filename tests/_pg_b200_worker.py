@@ -111,6 +111,19 @@ def main() -> None:
     pg.alltoall_base(v_out, v_in, out_rows, in_rows, AllToAllOptions()).wait()
     torch.cuda.synchronize()
     check("alltoall_base_unequal_splits", torch.equal(v_out, torch.cat([torch.full((out_rows[p], 3), 1000 * p + rank, device=dev, dtype=torch.int64) for p in range(world)])))
+    # skewed splits: rank 0 keeps 1 MiB rows for itself and sends one row to each peer, so its own row and column of
+    # the split matrix call for a larger grid than any peer's; every rank must still launch the same one
+    row = 1 << 18  # fp32 elements: 1 MiB per row
+    in_rows = [1] * world
+    out_rows = [1] * world
+    if rank == 0:
+        in_rows[0] = out_rows[0] = 2
+    v_in = torch.cat([torch.full((in_rows[p], row), float(1000 * rank + p), device=dev) for p in range(world)])
+    v_out = torch.full((sum(out_rows), row), -1.0, device=dev)
+    pg.alltoall_base(v_out, v_in, out_rows, in_rows, AllToAllOptions()).wait()
+    torch.cuda.synchronize()
+    check("alltoall_base_skewed_splits", pg.errored() is None and torch.equal(v_out, torch.cat(
+        [torch.full((out_rows[p], row), float(1000 * p + rank), device=dev) for p in range(world)])), err=str(pg.errored()))
 
     # ring send/recv (both posted before either is waited on: sends and receives run on separate streams)
     msg = torch.full((200_000,), float(rank), device=dev)

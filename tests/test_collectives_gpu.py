@@ -1,8 +1,10 @@
-"""Every peer-memory collective kernel, W ranks of one quorum emulated in ONE process on ONE GPU
+"""Peer-memory collectives, W ranks of one quorum emulated in ONE process on ONE GPU
 (``SymmetricComm.virtual_world(presignal=False)``: the ranks' kernels run concurrently on W streams and
-synchronise through the real signal-pad protocol). Exact values per collective, as the reference's
-process_group_test.py:143-492 does with rank threads, plus the resiliency contract of :890-949: when a rank
-never shows up the survivors' collective fails within the timeout and ``errored()`` is latched.
+synchronise through the real signal-pad protocol): staging rounds, multi-piece send/recv, the fp8 collectives
+against their emulation, the pre-signalled mode, and the resiliency contract of the reference's
+process_group_test.py:890-949: when a rank never shows up the survivors' collective fails within the timeout and
+``errored()`` is latched. The plain all-reduce, reduce-scatter and push-exchange results are checked byte for byte in
+``test_collectives_exact_gpu.py``.
 """
 
 from __future__ import annotations
@@ -16,93 +18,6 @@ from _collectives import DEV, _ok, _run, _world
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("world", [2, 3, 8])
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_allreduce_paths_exact(world, dtype):
-    comms = _world(world)
-    g = torch.Generator(device=DEV).manual_seed(world)
-    for n, plan in ((5, None), (4096, (0, 4)), (100_003, (1, 8)), (1 << 19, (1, 16)), (70_000, None)):
-        xs = [torch.randint(-8, 8, (n,), device=DEV, generator=g).to(dtype) for _ in range(world)]  # exactly summable
-        want = sum(x.float() for x in xs)
-        # symmetric (zero-copy) path
-        es = xs[0].element_size()
-        views = [c.segment("buf")[: n * es].view(dtype) for c in comms]
-        for v, x in zip(views, xs):
-            v.copy_(x)
-
-        def symm(r, c, s):
-            c._force_plan = plan
-            c.allreduce_(views[r], scale=0.5, stream=s)
-            c._force_plan = None
-
-        _run(comms, symm)
-        _ok(comms)
-        for v in views:
-            assert torch.equal(v.float(), want * 0.5)
-        # staged path (tensor outside symmetric memory), MAX, and a non-contributing rank
-        ys = [x.clone() for x in xs]
-        _run(comms, lambda r, c, s: c.allreduce_(ys[r], op=1, stream=s))
-        for y in ys:
-            assert torch.equal(y.float(), torch.stack([x.float() for x in xs]).max(0).values)
-        zs = [x.clone() for x in xs]
-        _run(comms, lambda r, c, s: c.allreduce_(zs[r], contribute=(r != 0), stream=s))
-        _ok(comms)
-        for z in zs:
-            assert torch.equal(z.float(), want - xs[0].float())
-    # random normal values: the sum is exact only in the kernels' order, rank 0 first, in fp32, then the scale and one
-    # round-to-nearest-even cast, on every rank and for both plans
-    n = 100_003
-    xs = [torch.randn(n, device=DEV, generator=g).to(dtype) for _ in range(world)]
-    want = _rank_order_sum(xs, 0.5).to(dtype)
-    for plan in ((0, 16), (1, 8)):
-        views = [c.segment("buf")[: n * xs[0].element_size()].view(dtype) for c in comms]
-        for v, x in zip(views, xs):
-            v.copy_(x)
-        ys = [x.clone() for x in xs]
-
-        def both(r, c, s):
-            c._force_plan = plan
-            c.allreduce_(views[r], scale=0.5, stream=s)
-            c.allreduce_(ys[r], scale=0.5, stream=s)
-            c._force_plan = None
-
-        _run(comms, both)
-        _ok(comms)
-        for v, y in zip(views, ys):
-            assert torch.equal(v, want) and torch.equal(y, want), plan
-
-
-def _rank_order_sum(xs, scale):
-    acc = xs[0].float()
-    for x in xs[1:]:
-        acc = acc + x.float()
-    return acc * scale
-
-
-@pytest.mark.parametrize("world", [2, 3, 8])
-def test_allgather_broadcast_alltoall_exact(world):
-    comms = _world(world)
-    for n, dtype in ((7, torch.int64), (4096, torch.float32), (33_333, torch.bfloat16), (1 << 20, torch.uint8)):
-        xs = [(torch.arange(n, device=DEV) * (r + 1) % 251).to(dtype) for r in range(world)]
-        outs = [torch.empty(world * n, dtype=dtype, device=DEV) for _ in range(world)]
-        _run(comms, lambda r, c, s: c.allgather_(outs[r], xs[r], stream=s))
-        _ok(comms)
-        want = torch.cat(xs)
-        assert all(torch.equal(o, want) for o in outs)
-        for root in (0, world - 1):
-            bs = [x.clone() for x in xs]
-            _run(comms, lambda r, c, s: c.broadcast_(bs[r], root, stream=s))
-            assert all(torch.equal(b, xs[root]) for b in bs)
-        m = n - n % world or world
-        ins = [(torch.arange(m, device=DEV) + 1000 * r).to(torch.int32) for r in range(world)]
-        a2a = [torch.empty(m, dtype=torch.int32, device=DEV) for _ in range(world)]
-        _run(comms, lambda r, c, s: c.alltoall_(a2a[r], ins[r], stream=s))
-        _ok(comms)
-        c_ = m // world
-        for r in range(world):
-            assert torch.equal(a2a[r], torch.cat([ins[p][r * c_:(r + 1) * c_] for p in range(world)]))
-
-
 def test_exchange_larger_than_staging_runs_in_rounds():
     comms = _world(4, staging=2 << 20)  # usable staging 1.5 MiB -> 384 KiB slots
     n = 1_000_003
@@ -111,38 +26,6 @@ def test_exchange_larger_than_staging_runs_in_rounds():
     _run(comms, lambda r, c, s: c.allgather_(outs[r], xs[r], stream=s))
     _ok(comms)
     assert all(torch.equal(o, torch.cat(xs)) for o in outs)
-
-
-@pytest.mark.parametrize("world", [2, 3, 8])
-def test_reduce_scatter_exact(world):
-    comms = _world(world, segs={"buf": 8 << 20})
-    g = torch.Generator(device=DEV).manual_seed(3)
-    for n, dtype in ((8, torch.float32), (1001, torch.float32), (65_536, torch.bfloat16)):
-        ins = [torch.randint(-8, 8, (world * n,), device=DEV, generator=g).to(dtype) for _ in range(world)]
-        outs = [torch.empty(n, dtype=dtype, device=DEV) for _ in range(world)]
-        _run(comms, lambda r, c, s: c.reduce_scatter_(outs[r], ins[r], scale=0.25, stream=s))
-        _ok(comms)
-        tot = sum(x.float() for x in ins)
-        for r in range(world):
-            assert torch.equal(outs[r].float(), tot[r * n:(r + 1) * n] * 0.25)
-        # zero-copy: input already in symmetric memory
-        es = ins[0].element_size()
-        views = [c.segment("buf")[: world * n * es].view(dtype) for c in comms]
-        for v, x in zip(views, ins):
-            v.copy_(x)
-        _run(comms, lambda r, c, s: c.reduce_scatter_(outs[r], views[r], op=2, stream=s))
-        _ok(comms)
-        mn = torch.stack([x.float() for x in ins]).min(0).values
-        for r in range(world):
-            assert torch.equal(outs[r].float(), mn[r * n:(r + 1) * n])
-    for n, dtype in ((1001, torch.float32), (65_536, torch.bfloat16), (4104, torch.float16)):
-        ins = [torch.randn(world * n, device=DEV, generator=g).to(dtype) for _ in range(world)]
-        outs = [torch.empty(n, dtype=dtype, device=DEV) for _ in range(world)]
-        _run(comms, lambda r, c, s: c.reduce_scatter_(outs[r], ins[r], scale=0.25, stream=s))
-        _ok(comms)
-        want = _rank_order_sum(ins, 0.25).to(dtype)
-        for r in range(world):
-            assert torch.equal(outs[r], want[r * n:(r + 1) * n]), (n, dtype, r)
 
 
 def test_send_recv_multi_piece_fifo():

@@ -108,14 +108,27 @@ __global__ void __launch_bounds__(512, 1) allreduce_twoshot_kernel(ARArgs a) {
     }
     const size_t lo = rank * slice + blockIdx.x * chunk;
     const size_t hi = min(min(lo + chunk, (size_t)(rank + 1) * slice), nvec);
+    // a message that is not a whole number of vectors ends in one partial vector: it is reduced element by element,
+    // because in a user segment the bytes after the message belong to someone else
+    const size_t nfull = a.nelem / N;
+    const size_t e = nfull * N + threadIdx.x;
+    if (lo <= nfull && nfull < hi && e < a.nelem) {
+      float acc = float(__ldcg(src[0] + e));
+#pragma unroll
+      for (int p = 1; p < W; ++p) acc = red<OP>(acc, float(__ldcg(src[p] + e)));
+      const T out = T(acc * a.scale);
+#pragma unroll
+      for (int p = 0; p < W; ++p) dst[p][e] = out;
+    }
+    const size_t vhi = min(hi, nfull);
     // vectors in flight per thread: peer loads have microseconds of latency, so keep U*W >= 16 outstanding
     constexpr int U = (W >= 8) ? 2 : (W >= 3 ? 4 : 8);
-    for (size_t base = lo; base < hi; base += (size_t)blockDim.x * U) {
+    for (size_t base = lo; base < vhi; base += (size_t)blockDim.x * U) {
       Vec16 in[U][W];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const size_t v = base + threadIdx.x + (size_t)u * blockDim.x;
-        if (v < hi) {
+        if (v < vhi) {
 #pragma unroll
           for (int p = 0; p < W; ++p) in[u][p] = ld_stream(src[p] + v * N);
         }
@@ -123,7 +136,7 @@ __global__ void __launch_bounds__(512, 1) allreduce_twoshot_kernel(ARArgs a) {
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const size_t v = base + threadIdx.x + (size_t)u * blockDim.x;
-        if (v < hi) {
+        if (v < vhi) {
           float acc[N], f[N];
           Pack<T>::unpack(in[u][0], acc);
 #pragma unroll
@@ -207,13 +220,16 @@ __global__ void __launch_bounds__(512, 1) allreduce_oneshot_kernel(ARArgs a) {
     }
     block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
   } else {
-    // In-place in staging: host guarantees chunk <= blockDim.x * kMaxRounds.
+    // In-place in staging: host guarantees chunk <= blockDim.x * kMaxRounds. A partial last vector is reduced and
+    // stored element by element (one element per thread), so nothing after the message is written.
     constexpr int kMaxRounds = 8;
+    const size_t nfull = a.nelem / N;
+    const size_t vhi = min(hi, nfull);
     Vec16 res[kMaxRounds];
 #pragma unroll
     for (int r = 0; r < kMaxRounds; ++r) {
       const size_t v = lo + threadIdx.x + (size_t)r * blockDim.x;
-      if (v < hi) {
+      if (v < vhi) {
         float acc[N], f[N];
         Vec16 in[W];
 #pragma unroll
@@ -230,12 +246,22 @@ __global__ void __launch_bounds__(512, 1) allreduce_oneshot_kernel(ARArgs a) {
         res[r] = Pack<T>::pack(acc);
       }
     }
+    const size_t e = nfull * N + threadIdx.x;
+    const bool tail = lo <= nfull && nfull < hi && e < a.nelem;
+    T tail_res = T(0.f);
+    if (tail) {
+      float acc = float(__ldcg(src[0] + e));
+#pragma unroll
+      for (int p = 1; p < W; ++p) acc = red<OP>(acc, float(__ldcg(src[p] + e)));
+      tail_res = T(acc * a.scale);
+    }
     if (!block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false)) return;
 #pragma unroll
     for (int r = 0; r < kMaxRounds; ++r) {
       const size_t v = lo + threadIdx.x + (size_t)r * blockDim.x;
-      if (v < hi) st_stream(mine + v * N, res[r]);
+      if (v < vhi) st_stream(mine + v * N, res[r]);
     }
+    if (tail) mine[e] = tail_res;
   }
 }
 

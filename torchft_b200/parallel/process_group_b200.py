@@ -372,8 +372,9 @@ class ProcessGroupB200(ProcessGroup):
     def alltoall_base(self, output_buffer: torch.Tensor, input_buffer: torch.Tensor, output_split_sizes: List[int],
                       input_split_sizes: List[int], opts: Any) -> Work:
         w = self._world
-        equal = ((not output_split_sizes or len(set(output_split_sizes)) == 1) and (not input_split_sizes or len(set(input_split_sizes)) == 1)
-                 and input_buffer.numel() % max(w, 1) == 0
+        # given splits may be equal here and ragged on another rank, which must run the same collective: only a call
+        # without splits (equal on every rank by definition) takes the equal-split kernel path
+        equal = (not output_split_sizes and not input_split_sizes and input_buffer.numel() % max(w, 1) == 0
                  and input_buffer.numel() * input_buffer.element_size() == output_buffer.numel() * output_buffer.element_size())
         if equal and self._raw_ok(output_buffer) and self._raw_ok(input_buffer):
             return self._launch(lambda s: self._comm.alltoall_(output_buffer, input_buffer, stream=s), output_buffer)

@@ -496,8 +496,9 @@ class SymmetricComm:
                 seg, off = hit
                 n = t.numel()
                 mc = self._mc.get(seg.name)
+                # multimem stores write whole 16-byte vectors: a message that ends inside one goes to the P2P kernels
                 if (mc is not None and op == _native.OP_SUM and n * es >= self._nvls_min and self._world > 1
-                        and self._force_plan is None):
+                        and (n * es) % 16 == 0 and self._force_plan is None):
                     blocks = max(8, min(self._max_blocks, (n * es) // (64 << 10)))
                     K.allreduce_nvls(self._tables[seg.name], self._status, mc[1], off, n, dt, scale, self._next_flag(),
                                      _CH_ALLREDUCE, contribute, blocks, self._threads, sp)
@@ -611,13 +612,13 @@ class SymmetricComm:
         return max(1, min(self._max_blocks, self._K.MAX_BLOCKS, nbytes // (64 << 10)))
 
     def _exchange(self, inp: int, out: int, send: List[Tuple[int, int]], recv: List[Tuple[int, int]], stream: Any,
-                  rounds: Optional[int] = None) -> None:
+                  blocks: int, rounds: Optional[int] = None) -> None:
         """One push-exchange launch per staging round. ``send[p] = (offset, bytes)`` into ``inp`` owed to rank p,
         ``recv[p] = (offset, bytes)`` into ``out`` expected from rank p. Every rank must run the same number of
-        rounds: either the message lengths are known quorum-wide (default: derived from them) or the caller agreed on
-        ``rounds`` beforehand (:meth:`alltoallv_`)."""
-        W = self._world
-        stride = (self._staging_usable // W) & ~15
+        rounds on the same grid ``blocks``: CTA b cuts each message by the grid size and meets only CTA b of every
+        peer. Either the message lengths are known quorum-wide (rounds derived from them) or the caller agreed on
+        ``rounds`` and ``blocks`` beforehand (:meth:`alltoallv_`)."""
+        stride = self._slot_stride()
         longest = max([n for _, n in send] + [n for _, n in recv] + [0])
         if rounds is not None:
             longest = rounds * stride
@@ -630,8 +631,17 @@ class SymmetricComm:
             r_off = [o + min(lo, n) for o, n in recv]
             r_len = [max(0, min(stride, n - lo)) for _, n in recv]
             self._K.push_exchange(self._tables["core"], self._status, inp, out, s_off, s_len, r_len, r_off, stride,
-                                  self._next_flag(), _CH_ALLREDUCE, self._xblocks(max(s_len + r_len)), sp)
+                                  self._next_flag(), _CH_ALLREDUCE, blocks, sp)
             self.launches += 1
+
+    def _slot_stride(self) -> int:
+        """Staging bytes per source rank of one push-exchange round."""
+        return (self._staging_usable // self._world) & ~15
+
+    def _xgrid(self, longest: int) -> int:
+        """Grid of every push-exchange round of a collective whose longest per-peer message, over the whole quorum,
+        is ``longest`` bytes."""
+        return self._xblocks(min(self._slot_stride(), longest))
 
     @staticmethod
     def _check_raw(*ts: torch.Tensor) -> None:
@@ -652,7 +662,8 @@ class SymmetricComm:
                     out.view(-1).view(torch.uint8)[:n].copy_(inp.view(-1).view(torch.uint8))
                 return
             W = self._world
-            self._exchange(inp.data_ptr(), out.data_ptr(), [(0, n)] * W, [(p * n, n) for p in range(W)], stream)
+            self._exchange(inp.data_ptr(), out.data_ptr(), [(0, n)] * W, [(p * n, n) for p in range(W)], stream,
+                           self._xgrid(n))
 
     def broadcast_(self, t: torch.Tensor, root: int, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Root's ``t`` lands in everybody's ``t`` (root stores into the peers' staging slots; n bytes per peer link)."""
@@ -666,7 +677,7 @@ class SymmetricComm:
             W, me = self._world, self._rank
             send = [(0, n if (me == root and p != me) else 0) for p in range(W)]
             recv = [(0, n if (p == root and me != root) else 0) for p in range(W)]
-            self._exchange(t.data_ptr(), t.data_ptr(), send, recv, stream)
+            self._exchange(t.data_ptr(), t.data_ptr(), send, recv, stream, self._xgrid(n))
 
     def alltoall_(self, out: torch.Tensor, inp: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Equal-split all-to-all: chunk p of ``inp`` goes to rank p, where it becomes chunk ``rank`` of ``out``."""
@@ -683,14 +694,16 @@ class SymmetricComm:
                     out.view(-1).view(torch.uint8).copy_(inp.view(-1).view(torch.uint8))
                 return
             c = nb // W
-            self._exchange(inp.data_ptr(), out.data_ptr(), [(p * c, c) for p in range(W)], [(p * c, c) for p in range(W)], stream)
+            self._exchange(inp.data_ptr(), out.data_ptr(), [(p * c, c) for p in range(W)], [(p * c, c) for p in range(W)], stream,
+                           self._xgrid(c))
 
     def alltoallv_(self, out: torch.Tensor, inp: torch.Tensor, out_bytes: List[int], in_bytes: List[int],
                    stream: Optional[torch.cuda.Stream] = None) -> None:
         """All-to-all with per-peer lengths: the first ``in_bytes[p]`` ... bytes of ``inp`` (consecutive chunks) go to rank
         p, which stores what it gets from rank q as its q-th consecutive chunk of ``out_bytes[q]`` bytes. A rank only
-        knows its own row and column of the split matrix, so the ranks first agree on the number of staging rounds with
-        one 16-byte MAX all-reduce that is read back on the host (a synchronisation: this is not a hot-path collective)."""
+        knows its own row and column of the split matrix, so the ranks first agree on the number of staging rounds and
+        on the longest per-peer message (which sets the grid: it must be the same on every rank) with one 16-byte MAX
+        all-reduce that is read back on the host (a synchronisation: this is not a hot-path collective)."""
         self._check_raw(out, inp)
         with self._lock:
             if not self._configured:
@@ -703,19 +716,21 @@ class SymmetricComm:
             if W == 1:
                 out.view(-1).view(torch.uint8)[: in_bytes[0]].copy_(inp.view(-1).view(torch.uint8)[: in_bytes[0]])
                 return
-            stride = (self._staging_usable // W) & ~15
-            mine = (max(list(in_bytes) + list(out_bytes)) + stride - 1) // stride
+            stride = self._slot_stride()
+            longest = max(int(x) for x in list(in_bytes) + list(out_bytes))
+            # both in fp32 exactly: a round count and a length in 64 KiB units (the grid's granularity) are far below 2^24
             with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
-                agree = torch.tensor([float(mine), 0.0, 0.0, 0.0], dtype=torch.float32, device=self.device)
-            self.allreduce_(agree, op=_native.OP_MAX, stream=stream)
-            rounds = int(agree[0].item())  # exact: a round count is far below 2^24
+                agree = torch.tensor([float((longest + stride - 1) // stride), float(longest >> 16), 0.0, 0.0],
+                                     dtype=torch.float32, device=self.device)
+                self.allreduce_(agree, op=_native.OP_MAX, stream=stream)
+                rounds, units = int(agree[0].item()), int(agree[1].item())
             send, recv, so, ro = [], [], 0, 0
             for p in range(W):
                 send.append((so, int(in_bytes[p])))
                 recv.append((ro, int(out_bytes[p])))
                 so += int(in_bytes[p])
                 ro += int(out_bytes[p])
-            self._exchange(inp.data_ptr(), out.data_ptr(), send, recv, stream, rounds=rounds)
+            self._exchange(inp.data_ptr(), out.data_ptr(), send, recv, stream, self._xgrid(units << 16), rounds=rounds)
 
     def reduce_scatter_(self, out: torch.Tensor, inp: torch.Tensor, op: int = _native.OP_SUM, scale: float = 1.0,
                         stream: Optional[torch.cuda.Stream] = None) -> None:
