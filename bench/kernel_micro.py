@@ -123,9 +123,10 @@ def main() -> None:
         n = 1 << 28
         x = torch.randn(n, device=dev).bfloat16()
         buf = torch.empty(Q.q8_bytes(n, 8), dtype=torch.uint8, device=dev)
-        record("q8_quantize_bf16", timeit(lambda: K.q8_quantize(x.data_ptr(), 0, n, 1, 8, buf.data_ptr(), sp()), args.iters, flush), n * 3)
+        ng = K.q8_ngroups(n, 8)
+        record("q8_quantize_bf16", timeit(lambda: K.q8_quantize(x.data_ptr(), 0, n, ng, 1, buf.data_ptr(), sp()), args.iters, flush), n * 3)
         out = torch.empty_like(x)
-        record("q8_dequantize_bf16", timeit(lambda: K.q8_dequantize(buf.data_ptr(), n, 1, 8, out.data_ptr(), sp()), args.iters, flush), n * 3)
+        record("q8_dequantize_bf16", timeit(lambda: K.q8_dequantize(buf.data_ptr(), ng, out.data_ptr(), n, 1, sp()), args.iters, flush), n * 3)
     if want("heal_copy"):
         from torchft_b200.checkpointing.p2p_transport import device_copy
 

@@ -338,7 +338,7 @@ def slice_plan(numels: Sequence[int], world: int, slice_elems: Optional[Sequence
 
 
 def _plan_reduce(xs: Sequence[torch.Tensor], se: int, g: int, post: float, v: Variant) -> List[Q8]:
-    """Every rank's reduced, requantised slice of one tensor of the generic path (``q8_reduce_raw`` over what the
+    """Every rank's reduced, requantised slice of one tensor of the generic path (``q8_reduce`` over what the
     all-to-all delivered: slice r of every peer, summed from rank r on an accumulator that starts at +0)."""
     W, n = len(xs), xs[0].numel()
     reds = []

@@ -106,9 +106,9 @@ def test_fused_quantize_reduce_dequantize_exact(world):
             _assert_bits(t, E.cast(E.dequant(got).reshape(-1)[: t.numel()], t.dtype), f"fused dequantize tensor {i}")
 
 
-def test_raw_launchers_exact():
-    """``q8_quantize_raw`` with more groups than the data needs, ``q8_reduce_raw`` over a sub-range of groups with
-    ``first`` != 0, ``q8_dequantize_raw`` of fewer elements than the groups hold."""
+def test_standalone_launchers_exact():
+    """``q8_quantize`` with more groups than the data needs, ``q8_reduce`` over a sub-range of groups with
+    ``first`` != 0, ``q8_dequantize`` of fewer elements than the groups hold."""
     from torchft_b200.ops import _native
 
     K, sp = _native.load(), _native.stream_ptr()
@@ -117,20 +117,20 @@ def test_raw_launchers_exact():
     bufs = [torch.zeros(E.payload_off(ng) + ng * E.GROUP, dtype=torch.uint8, device=DEV) for _ in range(W)]
     xd = _dev(xs)
     for x, b in zip(xd, bufs):
-        K.q8_quantize_raw(x.data_ptr(), 0, n, ng, _native.dtype_code(x), b.data_ptr(), sp)
+        K.q8_quantize(x.data_ptr(), 0, n, ng, _native.dtype_code(x), b.data_ptr(), sp)
     qs = [E.quantize(E.load(x), ng) for x in xs]
     for r in range(W):
-        _assert_q8(E.Q8.from_bytes(bufs[r], ng), qs[r], f"raw quantize rank {r}")
+        _assert_q8(E.Q8.from_bytes(bufs[r], ng), qs[r], f"quantize rank {r}")
     dst = torch.zeros_like(bufs[0])
     ptrs = torch.tensor([b.data_ptr() for b in bufs], dtype=torch.int64, device=DEV)
-    K.q8_reduce_raw(ptrs.data_ptr(), W, 2, ng, 2, 7, 0.25, dst.data_ptr(), sp)
+    K.q8_reduce(ptrs.data_ptr(), W, 2, ng, 2, 7, 0.25, dst.data_ptr(), sp)
     red = E.group_quant(E.reduce([q[2:7] for q in qs], torch.full((5,), 2), 0.25, start_zero=True))
     got = E.Q8.from_bytes(dst, ng)
-    _assert_q8(got[2:7], red, "raw reduce")
+    _assert_q8(got[2:7], red, "reduce")
     assert torch.equal(got.scales[:2], torch.zeros(2)) and torch.equal(got.scales[7:], torch.zeros(2))
     out = torch.zeros(1500, dtype=torch.float16, device=DEV)
-    K.q8_dequantize_raw(dst.data_ptr(), ng, out.data_ptr(), 1500, _native.dtype_code(out), sp)
-    _assert_bits(out, E.cast(E.dequant(got).reshape(-1)[:1500], torch.float16), "raw dequantize")
+    K.q8_dequantize(dst.data_ptr(), ng, out.data_ptr(), 1500, _native.dtype_code(out), sp)
+    _assert_bits(out, E.cast(E.dequant(got).reshape(-1)[:1500], torch.float16), "dequantize")
 
 
 # ------------------------------------------------------------------------------------------------ fused all-reduce

@@ -121,7 +121,7 @@ def _quantize_slices(tensors: List[torch.Tensor], plan: _SlicePlan, send: torch.
         for r in range(plan.world):
             valid = max(0, min(se, n - r * se))
             src = t.data_ptr() + r * se * es if valid > 0 else t.data_ptr()
-            K.q8_quantize_raw(src, 0, valid, g, _native.dtype_code(t), send[r].data_ptr() + off, sp)
+            K.q8_quantize(src, 0, valid, g, _native.dtype_code(t), send[r].data_ptr() + off, sp)
 
 
 def _reduce_slices(tensors: List[torch.Tensor], plan: _SlicePlan, recv: torch.Tensor, out_chunk: torch.Tensor,
@@ -130,7 +130,7 @@ def _reduce_slices(tensors: List[torch.Tensor], plan: _SlicePlan, recv: torch.Te
     sp = _native.stream_ptr()
     for g, off in zip(plan.groups, plan.offsets):
         ptrs = torch.tensor([recv[p].data_ptr() + off for p in range(plan.world)], dtype=torch.int64, device=recv.device)
-        K.q8_reduce_raw(ptrs.data_ptr(), plan.world, rank, g, 0, g, post_scale, out_chunk.data_ptr() + off, sp)
+        K.q8_reduce(ptrs.data_ptr(), plan.world, rank, g, 0, g, post_scale, out_chunk.data_ptr() + off, sp)
 
 
 def allreduce_quantized(tensors: List[torch.Tensor], opts: AllreduceOptions | ReduceOp, process_group: dist.ProcessGroup,
@@ -174,8 +174,8 @@ def allreduce_quantized(tensors: List[torch.Tensor], opts: AllreduceOptions | Re
             for r in range(world):
                 valid = max(0, min(se, n - r * se))
                 if valid > 0:
-                    K.q8_dequantize_raw(gathered[r].data_ptr() + off, g, t.data_ptr() + r * se * es, valid,
-                                        _native.dtype_code(t), sp)
+                    K.q8_dequantize(gathered[r].data_ptr() + off, g, t.data_ptr() + r * se * es, valid,
+                                    _native.dtype_code(t), sp)
         for t, c in zip(tensors, contig):
             if t.data_ptr() != c.data_ptr():
                 t.copy_(c)
@@ -238,10 +238,10 @@ def reduce_scatter_quantized(output: torch.Tensor, inputs: List[torch.Tensor], o
             for p, s, g, coff in zip(work_tensors, plan.slice_elems, plan.groups, plan.offsets):
                 dst = output[off : off + s]
                 if aligned_out and (off * es) % 16 == 0:
-                    K.q8_dequantize_raw(mine.data_ptr() + coff, g, dst.data_ptr(), s, _native.dtype_code(p), sp)
+                    K.q8_dequantize(mine.data_ptr() + coff, g, dst.data_ptr(), s, _native.dtype_code(p), sp)
                 else:
                     tmp = torch.empty(s, dtype=p.dtype, device=dev)
-                    K.q8_dequantize_raw(mine.data_ptr() + coff, g, tmp.data_ptr(), s, _native.dtype_code(p), sp)
+                    K.q8_dequantize(mine.data_ptr() + coff, g, tmp.data_ptr(), s, _native.dtype_code(p), sp)
                     dst.copy_(tmp)
                 off += s
         output.record_stream(stream)

@@ -28,15 +28,6 @@
 
 namespace tft {
 
-enum RedOp : int { kSum = 0, kMax = 1, kMin = 2 };
-
-template <int OP>
-__device__ __forceinline__ float red(float a, float b) {
-  if (OP == kSum) return a + b;
-  if (OP == kMax) return fmaxf(a, b);
-  return fminf(a, b);
-}
-
 struct ARArgs {
   PeerTable pt;
   StatusBlock* st;
@@ -285,39 +276,6 @@ __global__ void scale_copy_kernel(T* dst, const T* src, size_t nelem, float scal
   }
 }
 
-template <typename T, int W, int OP>
-static void launch_w(const ARArgs& a, int algo, int blocks, int threads, cudaStream_t stream) {
-  if (algo == 0)
-    allreduce_oneshot_kernel<T, W, OP><<<blocks, threads, 0, stream>>>(a);
-  else
-    allreduce_twoshot_kernel<T, W, OP><<<blocks, threads, 0, stream>>>(a);
-}
-
-template <typename T, int OP>
-static void launch_t(const ARArgs& a, int algo, int blocks, int threads, cudaStream_t stream) {
-  switch (a.pt.world) {
-    case 2: launch_w<T, 2, OP>(a, algo, blocks, threads, stream); break;
-    case 3: launch_w<T, 3, OP>(a, algo, blocks, threads, stream); break;
-    case 4: launch_w<T, 4, OP>(a, algo, blocks, threads, stream); break;
-    case 5: launch_w<T, 5, OP>(a, algo, blocks, threads, stream); break;
-    case 6: launch_w<T, 6, OP>(a, algo, blocks, threads, stream); break;
-    case 7: launch_w<T, 7, OP>(a, algo, blocks, threads, stream); break;
-    case 8: launch_w<T, 8, OP>(a, algo, blocks, threads, stream); break;
-    default: throw std::runtime_error("allreduce: world size must be in [2, 8]");
-  }
-}
-
-template <typename T>
-static void launch_op(const ARArgs& a, int op, int algo, int blocks, int threads,
-                      cudaStream_t stream) {
-  switch (op) {
-    case kSum: launch_t<T, kSum>(a, algo, blocks, threads, stream); break;
-    case kMax: launch_t<T, kMax>(a, algo, blocks, threads, stream); break;
-    case kMin: launch_t<T, kMin>(a, algo, blocks, threads, stream); break;
-    default: throw std::runtime_error("allreduce: unsupported reduce op");
-  }
-}
-
 void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* user_in,
                       void* user_out, size_t nelem, int dtype, int op, float scale,
                       uint64_t flag, int channel, int contribute, int algo, int blocks,
@@ -337,41 +295,34 @@ void allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const vo
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  if (pt.world == 1) {
-    // Degenerate quorum: out = scale * in (or zeros).
-    const void* src = user_in ? user_in : (const char*)pt.data[0] + off;
-    void* dst = user_out ? user_out : (char*)pt.data[0] + off;
-    const int g = (int)std::min<size_t>(kNumSMs * 8, (nelem + 4095) / 4096 + 1);
-    switch (dtype) {
-      case kF32:
-        scale_copy_kernel<float><<<g, 512, 0, stream>>>((float*)dst, (const float*)src, nelem,
-                                                        scale, !contribute);
-        break;
-      case kBF16:
-        scale_copy_kernel<__nv_bfloat16><<<g, 512, 0, stream>>>(
-            (__nv_bfloat16*)dst, (const __nv_bfloat16*)src, nelem, scale, !contribute);
-        break;
-      case kF16:
-        scale_copy_kernel<__half><<<g, 512, 0, stream>>>((__half*)dst, (const __half*)src, nelem,
-                                                         scale, !contribute);
-        break;
-      default: throw std::runtime_error("allreduce: unsupported dtype");
-    }
-    TFT_CUDA_CHECK(cudaGetLastError());
-    return;
-  }
   if (algo == 0 && user_out == nullptr) {
     // in-place one-shot keeps results in registers: bound the per-block chunk
     const size_t vecs = (nelem * (dtype == kF32 ? 4 : 2) + 15) / 16;
     const size_t chunk = (vecs + blocks - 1) / blocks;
     if (chunk > (size_t)threads * 8) algo = 1;
   }
-  switch (dtype) {
-    case kF32: launch_op<float>(a, op, algo, blocks, threads, stream); break;
-    case kBF16: launch_op<__nv_bfloat16>(a, op, algo, blocks, threads, stream); break;
-    case kF16: launch_op<__half>(a, op, algo, blocks, threads, stream); break;
-    default: throw std::runtime_error("allreduce: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    using T = Elem<D>;
+    if (pt.world == 1) {
+      // Degenerate quorum: out = scale * in (or zeros). The reduce op plays no part.
+      const void* src = user_in ? user_in : (const char*)pt.data[0] + off;
+      void* dst = user_out ? user_out : (char*)pt.data[0] + off;
+      const int g = (int)std::min<size_t>(kNumSMs * 8, (nelem + 4095) / 4096 + 1);
+      scale_copy_kernel<T><<<g, 512, 0, stream>>>((T*)dst, (const T*)src, nelem, scale, !contribute);
+      return;
+    }
+    const bool known_op = dispatch<kSum, kMax, kMin>(op, [&](auto OP) {
+      const bool known_world = dispatch<2, 3, 4, 5, 6, 7, 8>(pt.world, [&](auto W) {
+        if (algo == 0)
+          allreduce_oneshot_kernel<T, W, OP><<<blocks, threads, 0, stream>>>(a);
+        else
+          allreduce_twoshot_kernel<T, W, OP><<<blocks, threads, 0, stream>>>(a);
+      });
+      if (!known_world) throw std::runtime_error("allreduce: world size must be in [2, 8]");
+    });
+    if (!known_op) throw std::runtime_error("allreduce: unsupported reduce op");
+  });
+  if (!known_dtype) throw std::runtime_error("allreduce: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

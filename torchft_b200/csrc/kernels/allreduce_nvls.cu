@@ -150,12 +150,10 @@ void allreduce_nvls_launch(const PeerTable& pt, StatusBlock* st, void* mc_base, 
   a.flag = flag;
   a.channel = channel;
   a.contribute = contribute;
-  switch (dtype) {
-    case kF32: allreduce_nvls_kernel<float><<<blocks, threads, 0, stream>>>(a); break;
-    case kBF16: allreduce_nvls_kernel<__nv_bfloat16><<<blocks, threads, 0, stream>>>(a); break;
-    case kF16: allreduce_nvls_kernel<__half><<<blocks, threads, 0, stream>>>(a); break;
-    default: throw std::runtime_error("allreduce_nvls: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    allreduce_nvls_kernel<Elem<D>><<<blocks, threads, 0, stream>>>(a);
+  });
+  if (!known_dtype) throw std::runtime_error("allreduce_nvls: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

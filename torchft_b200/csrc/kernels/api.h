@@ -52,18 +52,11 @@ void p2p_launch(const PeerTable& pt, StatusBlock* st, int is_send, void* buf, si
 // quant.cu -------------------------------------------------------------------
 size_t q8_ngroups(size_t nelem, int world);
 size_t q8_buffer_bytes(size_t nelem, int world);
-void q8_quantize_launch(const void* a, const void* b, size_t nelem, int dtype, int world,
-                        void* qbuf, cudaStream_t stream);
-void q8_dequantize_launch(const void* qbuf, size_t nelem, int dtype, int world, void* out,
-                          cudaStream_t stream);
-void q8_reduce_launch(const void* const* srcs_dev, int world, int rank, size_t nelem,
+void q8_quantize_launch(const void* a, const void* b, size_t nelem, size_t ngroups, int dtype, void* qbuf,
+                        cudaStream_t stream);
+void q8_dequantize_launch(const void* qbuf, size_t ngroups, void* out, size_t nelem, int dtype, cudaStream_t stream);
+void q8_reduce_launch(const void* const* srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo, size_t g_hi,
                       float post_scale, void* dst, cudaStream_t stream);
-void q8_quantize_raw_launch(const void* a, const void* b, size_t nelem, size_t ngroups, int dtype, void* qbuf,
-                            cudaStream_t stream);
-void q8_dequantize_raw_launch(const void* qbuf, size_t ngroups, void* out, size_t nelem, int dtype,
-                              cudaStream_t stream);
-void q8_reduce_raw_launch(const void* const* srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo,
-                          size_t g_hi, float post_scale, void* dst, cudaStream_t stream);
 void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in_a,
                          const void* in_b, void* out, size_t nelem, int dtype, float post_scale,
                          uint64_t flag, int channel, int contribute, int blocks, cudaStream_t stream);

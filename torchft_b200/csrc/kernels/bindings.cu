@@ -369,31 +369,18 @@ PYBIND11_MODULE(_K, m) {
 
   m.def("q8_ngroups", &q8_ngroups);
   m.def("q8_buffer_bytes", &q8_buffer_bytes);
-  m.def("q8_quantize", [](uintptr_t a, uintptr_t b, size_t nelem, int dtype, int world, uintptr_t qbuf,
+  m.def("q8_quantize", [](uintptr_t a, uintptr_t b, size_t nelem, size_t ngroups, int dtype, uintptr_t qbuf,
                           uintptr_t stream) {
-    q8_quantize_launch(P<void>(a), P<void>(b), nelem, dtype, world, P<void>(qbuf), S(stream));
+    q8_quantize_launch(P<void>(a), P<void>(b), nelem, ngroups, dtype, P<void>(qbuf), S(stream));
   });
-  m.def("q8_dequantize", [](uintptr_t qbuf, size_t nelem, int dtype, int world, uintptr_t out,
+  m.def("q8_dequantize", [](uintptr_t qbuf, size_t ngroups, uintptr_t out, size_t nelem, int dtype,
                             uintptr_t stream) {
-    q8_dequantize_launch(P<void>(qbuf), nelem, dtype, world, P<void>(out), S(stream));
+    q8_dequantize_launch(P<void>(qbuf), ngroups, P<void>(out), nelem, dtype, S(stream));
   });
-  m.def("q8_reduce", [](uintptr_t srcs_dev, int world, int rank, size_t nelem, float post_scale,
-                        uintptr_t dst, uintptr_t stream) {
-    q8_reduce_launch(P<const void* const>(srcs_dev), world, rank, nelem, post_scale, P<void>(dst),
+  m.def("q8_reduce", [](uintptr_t srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo, size_t g_hi,
+                        float post_scale, uintptr_t dst, uintptr_t stream) {
+    q8_reduce_launch(P<const void* const>(srcs_dev), nsrc, first, ngroups, g_lo, g_hi, post_scale, P<void>(dst),
                      S(stream));
-  });
-  m.def("q8_quantize_raw", [](uintptr_t a, uintptr_t b, size_t nelem, size_t ngroups, int dtype, uintptr_t qbuf,
-                              uintptr_t stream) {
-    q8_quantize_raw_launch(P<void>(a), P<void>(b), nelem, ngroups, dtype, P<void>(qbuf), S(stream));
-  });
-  m.def("q8_dequantize_raw", [](uintptr_t qbuf, size_t ngroups, uintptr_t out, size_t nelem, int dtype,
-                                uintptr_t stream) {
-    q8_dequantize_raw_launch(P<void>(qbuf), ngroups, P<void>(out), nelem, dtype, S(stream));
-  });
-  m.def("q8_reduce_raw", [](uintptr_t srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo, size_t g_hi,
-                            float post_scale, uintptr_t dst, uintptr_t stream) {
-    q8_reduce_raw_launch(P<const void* const>(srcs_dev), nsrc, first, ngroups, g_lo, g_hi, post_scale, P<void>(dst),
-                         S(stream));
   });
   m.def(
       "q8_allreduce",

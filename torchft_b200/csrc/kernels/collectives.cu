@@ -94,14 +94,6 @@ __global__ void __launch_bounds__(512, 1) push_exchange_kernel(XArgs a) {
   block_barrier(a.pt, a.channel, a.flag + 2, a.st, /*release=*/false, /*acquire=*/false);
 }
 
-enum RedOp : int { kSum = 0, kMax = 1, kMin = 2 };
-template <int OP>
-__device__ __forceinline__ float red(float x, float y) {
-  if (OP == kSum) return x + y;
-  if (OP == kMax) return fmaxf(x, y);
-  return fminf(x, y);
-}
-
 struct RSArgs {
   PeerTable pt;          // data[] = the buffer holding every rank's W*n input (staging or a user segment)
   StatusBlock* st;
@@ -255,29 +247,6 @@ __global__ void __launch_bounds__(512, 1) p2p_recv_kernel(P2PArgs a) {
   }
 }
 
-template <typename T, int OP>
-void launch_rs_w(const RSArgs& a, int blocks, cudaStream_t s) {
-  switch (a.pt.world) {
-    case 2: reduce_scatter_kernel<T, 2, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 3: reduce_scatter_kernel<T, 3, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 4: reduce_scatter_kernel<T, 4, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 5: reduce_scatter_kernel<T, 5, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 6: reduce_scatter_kernel<T, 6, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 7: reduce_scatter_kernel<T, 7, OP><<<blocks, 512, 0, s>>>(a); break;
-    case 8: reduce_scatter_kernel<T, 8, OP><<<blocks, 512, 0, s>>>(a); break;
-    default: throw std::runtime_error("reduce_scatter: world size must be in [2, 8]");
-  }
-}
-template <typename T>
-void launch_rs_op(const RSArgs& a, int op, int blocks, cudaStream_t s) {
-  switch (op) {
-    case kSum: launch_rs_w<T, kSum>(a, blocks, s); break;
-    case kMax: launch_rs_w<T, kMax>(a, blocks, s); break;
-    case kMin: launch_rs_w<T, kMin>(a, blocks, s); break;
-    default: throw std::runtime_error("reduce_scatter: unsupported reduce op");
-  }
-}
-
 }  // namespace
 
 void push_exchange_launch(const PeerTable& pt, StatusBlock* st, const void* in, void* out, const size_t* send_off,
@@ -312,12 +281,16 @@ void reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, con
   if (blocks < 1 || blocks > kMaxBlocks) throw std::runtime_error("reduce_scatter: bad grid");
   if (off & 15) throw std::runtime_error("reduce_scatter: offset must be 16 B aligned");
   RSArgs a{pt, st, off, user_in, out, n, scale, flag, channel};
-  switch (dtype) {
-    case kF32: launch_rs_op<float>(a, op, blocks, stream); break;
-    case kBF16: launch_rs_op<__nv_bfloat16>(a, op, blocks, stream); break;
-    case kF16: launch_rs_op<__half>(a, op, blocks, stream); break;
-    default: throw std::runtime_error("reduce_scatter: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    const bool known_op = dispatch<kSum, kMax, kMin>(op, [&](auto OP) {
+      const bool known_world = dispatch<2, 3, 4, 5, 6, 7, 8>(pt.world, [&](auto W) {
+        reduce_scatter_kernel<Elem<D>, W, OP><<<blocks, 512, 0, stream>>>(a);
+      });
+      if (!known_world) throw std::runtime_error("reduce_scatter: world size must be in [2, 8]");
+    });
+    if (!known_op) throw std::runtime_error("reduce_scatter: unsupported reduce op");
+  });
+  if (!known_dtype) throw std::runtime_error("reduce_scatter: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

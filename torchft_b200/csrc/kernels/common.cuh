@@ -12,6 +12,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace tft {
 
 constexpr int kMaxRanks = 8;          // one NVSwitch domain (HGX H100)
@@ -21,6 +23,41 @@ constexpr int kSignalChannels = 4;    // independent flag arrays (allreduce / q8
 
 // dtype codes shared with Python (torchft_b200/ops/_dtypes.py)
 enum DType : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
+
+// Element type of a dtype code: Elem<kF32> = float, Elem<kBF16> = __nv_bfloat16, Elem<kF16> = __half.
+template <int D>
+struct ElemOf;
+template <>
+struct ElemOf<kF32> {
+  using type = float;
+};
+template <>
+struct ElemOf<kBF16> {
+  using type = __nv_bfloat16;
+};
+template <>
+struct ElemOf<kF16> {
+  using type = __half;
+};
+template <int D>
+using Elem = typename ElemOf<D>::type;
+
+// reduce op codes shared with Python (torchft_b200/ops/_native.py); the kernels take the op as an int template parameter
+enum RedOp : int { kSum = 0, kMax = 1, kMin = 2 };
+
+template <int OP>
+__device__ __forceinline__ float red(float a, float b) {
+  if (OP == kSum) return a + b;
+  if (OP == kMax) return fmaxf(a, b);
+  return fminf(a, b);
+}
+
+// Calls f(std::integral_constant<decltype(V), V>{}) for the V of Vs equal to the runtime value v: the one place where a
+// launcher's runtime selector becomes a template argument. Returns false when v is none of Vs.
+template <auto... Vs, typename T, typename F>
+bool dispatch(T v, F&& f) {
+  return ((v == Vs && (f(std::integral_constant<decltype(Vs), Vs>{}), true)) || ...);
+}
 
 // ---------------------------------------------------------------------------
 // Status block: lives in host-pinned, device-mapped memory. The host can flip

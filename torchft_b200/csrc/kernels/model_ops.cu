@@ -815,21 +815,12 @@ void adamw_launch(void* p, float* master, float* m, float* v, const void* g, siz
 void diloco_outer_launch(void* param, void* original, const void* grad, float* mom, size_t n, int dtype, float lr,
                          float mu, int nesterov, float alpha, const int* gate, cudaStream_t s) {
   const int grid = grid_for(n / 4 + 1, 512, kNumSMs * 16);
-  switch (dtype) {
-    case kF32:
-      diloco_outer_kernel<float><<<grid, 512, 0, s>>>((float*)param, (float*)original, (const float*)grad, mom, n, lr, mu,
-                                                      nesterov, alpha, gate);
-      break;
-    case kBF16:
-      diloco_outer_kernel<bf16><<<grid, 512, 0, s>>>((bf16*)param, (bf16*)original, (const bf16*)grad, mom, n, lr, mu,
-                                                     nesterov, alpha, gate);
-      break;
-    case kF16:
-      diloco_outer_kernel<__half><<<grid, 512, 0, s>>>((__half*)param, (__half*)original, (const __half*)grad, mom, n, lr,
-                                                       mu, nesterov, alpha, gate);
-      break;
-    default: throw std::runtime_error("diloco_outer: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    using T = Elem<D>;
+    diloco_outer_kernel<T><<<grid, 512, 0, s>>>((T*)param, (T*)original, (const T*)grad, mom, n, lr, mu, nesterov, alpha,
+                                                gate);
+  });
+  if (!known_dtype) throw std::runtime_error("diloco_outer: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

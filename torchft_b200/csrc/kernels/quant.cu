@@ -25,77 +25,29 @@ namespace tft {
 constexpr int kGroup = 512;
 constexpr float kFp8Max = 448.f;
 
+// 16 elements of p starting at e <-> 16 floats; elements at or past nelem load as 0 and are not stored.
 template <typename T>
-__device__ __forceinline__ void load16(const T* p, size_t e, size_t nelem, float* f);
-
-template <>
-__device__ __forceinline__ void load16<float>(const float* p, size_t e, size_t nelem, float* f) {
+__device__ __forceinline__ void load16(const T* p, size_t e, size_t nelem, float* f) {
+  constexpr int N = Pack<T>::N;
   if (e + 16 <= nelem) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) Pack<float>::unpack(ld_stream(p + e + 4 * i), f + 4 * i);
+    for (int i = 0; i < 16 / N; ++i) Pack<T>::unpack(ld_stream(p + e + N * i), f + N * i);
   } else {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = (e + i < nelem) ? p[e + i] : 0.f;
-  }
-}
-template <>
-__device__ __forceinline__ void load16<__nv_bfloat16>(const __nv_bfloat16* p, size_t e,
-                                                      size_t nelem, float* f) {
-  if (e + 16 <= nelem) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) Pack<__nv_bfloat16>::unpack(ld_stream(p + e + 8 * i), f + 8 * i);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = (e + i < nelem) ? __bfloat162float(p[e + i]) : 0.f;
-  }
-}
-template <>
-__device__ __forceinline__ void load16<__half>(const __half* p, size_t e, size_t nelem, float* f) {
-  if (e + 16 <= nelem) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) Pack<__half>::unpack(ld_stream(p + e + 8 * i), f + 8 * i);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = (e + i < nelem) ? __half2float(p[e + i]) : 0.f;
+    for (int i = 0; i < 16; ++i) f[i] = (e + i < nelem) ? float(p[e + i]) : 0.f;
   }
 }
 
 template <typename T>
-__device__ __forceinline__ void store16(T* p, size_t e, size_t nelem, const float* f);
-
-template <>
-__device__ __forceinline__ void store16<float>(float* p, size_t e, size_t nelem, const float* f) {
+__device__ __forceinline__ void store16(T* p, size_t e, size_t nelem, const float* f) {
+  constexpr int N = Pack<T>::N;
   if (e + 16 <= nelem) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) st_stream(p + e + 4 * i, Pack<float>::pack(f + 4 * i));
+    for (int i = 0; i < 16 / N; ++i) st_stream(p + e + N * i, Pack<T>::pack(f + N * i));
   } else {
 #pragma unroll
     for (int i = 0; i < 16; ++i)
-      if (e + i < nelem) p[e + i] = f[i];
-  }
-}
-template <>
-__device__ __forceinline__ void store16<__nv_bfloat16>(__nv_bfloat16* p, size_t e, size_t nelem,
-                                                       const float* f) {
-  if (e + 16 <= nelem) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) st_stream(p + e + 8 * i, Pack<__nv_bfloat16>::pack(f + 8 * i));
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (e + i < nelem) p[e + i] = __float2bfloat16(f[i]);
-  }
-}
-template <>
-__device__ __forceinline__ void store16<__half>(__half* p, size_t e, size_t nelem,
-                                                const float* f) {
-  if (e + 16 <= nelem) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) st_stream(p + e + 8 * i, Pack<__half>::pack(f + 8 * i));
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (e + i < nelem) p[e + i] = __float2half(f[i]);
+      if (e + i < nelem) p[e + i] = T(f[i]);
   }
 }
 
@@ -464,115 +416,36 @@ static int q8_grid(size_t ngroups, int max_blocks) {
   return (int)b;
 }
 
-void q8_quantize_launch(const void* a, const void* b, size_t nelem, int dtype, int world,
-                        void* qbuf, cudaStream_t stream) {
-  const size_t ng = q8_ngroups(nelem, world);
-  const int grid = q8_grid(ng, kNumSMs * 8);
-  switch (dtype) {
-    case kF32:
-      q8_quantize_kernel<float><<<grid, 512, 0, stream>>>((const float*)a, (const float*)b, nelem,
-                                                          ng, (char*)qbuf);
-      break;
-    case kBF16:
-      q8_quantize_kernel<__nv_bfloat16><<<grid, 512, 0, stream>>>(
-          (const __nv_bfloat16*)a, (const __nv_bfloat16*)b, nelem, ng, (char*)qbuf);
-      break;
-    case kF16:
-      q8_quantize_kernel<__half><<<grid, 512, 0, stream>>>((const __half*)a, (const __half*)b,
-                                                           nelem, ng, (char*)qbuf);
-      break;
-    default: throw std::runtime_error("q8_quantize: unsupported dtype");
-  }
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void q8_dequantize_launch(const void* qbuf, size_t nelem, int dtype, int world, void* out,
-                          cudaStream_t stream) {
-  const size_t ng = q8_ngroups(nelem, world);
-  const int grid = q8_grid(ng, kNumSMs * 8);
-  switch (dtype) {
-    case kF32:
-      q8_dequantize_kernel<float><<<grid, 512, 0, stream>>>((const char*)qbuf, ng, (float*)out, nelem);
-      break;
-    case kBF16:
-      q8_dequantize_kernel<__nv_bfloat16><<<grid, 512, 0, stream>>>((const char*)qbuf, ng,
-                                                                    (__nv_bfloat16*)out, nelem);
-      break;
-    case kF16:
-      q8_dequantize_kernel<__half><<<grid, 512, 0, stream>>>((const char*)qbuf, ng, (__half*)out, nelem);
-      break;
-    default: throw std::runtime_error("q8_dequantize: unsupported dtype");
-  }
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void q8_quantize_raw_launch(const void* a, const void* b, size_t nelem, size_t ngroups, int dtype, void* qbuf,
-                            cudaStream_t stream) {
+void q8_quantize_launch(const void* a, const void* b, size_t nelem, size_t ngroups, int dtype, void* qbuf,
+                        cudaStream_t stream) {
   if (ngroups == 0) return;
   const int grid = q8_grid(ngroups, kNumSMs * 8);
-  switch (dtype) {
-    case kF32:
-      q8_quantize_kernel<float><<<grid, 512, 0, stream>>>((const float*)a, (const float*)b, nelem, ngroups, (char*)qbuf);
-      break;
-    case kBF16:
-      q8_quantize_kernel<__nv_bfloat16><<<grid, 512, 0, stream>>>((const __nv_bfloat16*)a, (const __nv_bfloat16*)b,
-                                                                  nelem, ngroups, (char*)qbuf);
-      break;
-    case kF16:
-      q8_quantize_kernel<__half><<<grid, 512, 0, stream>>>((const __half*)a, (const __half*)b, nelem, ngroups, (char*)qbuf);
-      break;
-    default: throw std::runtime_error("q8_quantize: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    using T = Elem<D>;
+    q8_quantize_kernel<T><<<grid, 512, 0, stream>>>((const T*)a, (const T*)b, nelem, ngroups, (char*)qbuf);
+  });
+  if (!known_dtype) throw std::runtime_error("q8_quantize: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-void q8_dequantize_raw_launch(const void* qbuf, size_t ngroups, void* out, size_t nelem, int dtype,
-                              cudaStream_t stream) {
+void q8_dequantize_launch(const void* qbuf, size_t ngroups, void* out, size_t nelem, int dtype, cudaStream_t stream) {
   if (ngroups == 0 || nelem == 0) return;
   const int grid = q8_grid(ngroups, kNumSMs * 8);
-  switch (dtype) {
-    case kF32: q8_dequantize_kernel<float><<<grid, 512, 0, stream>>>((const char*)qbuf, ngroups, (float*)out, nelem); break;
-    case kBF16:
-      q8_dequantize_kernel<__nv_bfloat16><<<grid, 512, 0, stream>>>((const char*)qbuf, ngroups, (__nv_bfloat16*)out, nelem);
-      break;
-    case kF16: q8_dequantize_kernel<__half><<<grid, 512, 0, stream>>>((const char*)qbuf, ngroups, (__half*)out, nelem); break;
-    default: throw std::runtime_error("q8_dequantize: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    using T = Elem<D>;
+    q8_dequantize_kernel<T><<<grid, 512, 0, stream>>>((const char*)qbuf, ngroups, (T*)out, nelem);
+  });
+  if (!known_dtype) throw std::runtime_error("q8_dequantize: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-void q8_reduce_raw_launch(const void* const* srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo,
-                          size_t g_hi, float post_scale, void* dst, cudaStream_t stream) {
+void q8_reduce_launch(const void* const* srcs_dev, int nsrc, int first, size_t ngroups, size_t g_lo, size_t g_hi,
+                      float post_scale, void* dst, cudaStream_t stream) {
   if (g_hi <= g_lo) return;
   const int grid = q8_grid(g_hi - g_lo, kNumSMs * 8);
   q8_reduce_kernel<<<grid, 512, 0, stream>>>((const char* const*)srcs_dev, nsrc, first, ngroups, g_lo, g_hi,
                                              post_scale, (char*)dst);
   TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void q8_reduce_launch(const void* const* srcs_dev, int world, int rank, size_t nelem,
-                      float post_scale, void* dst, cudaStream_t stream) {
-  const size_t ng = q8_ngroups(nelem, world);
-  const size_t slice = ng / world;
-  const int grid = q8_grid(slice, kNumSMs * 8);
-  q8_reduce_kernel<<<grid, 512, 0, stream>>>((const char* const*)srcs_dev, world, rank, ng,
-                                             rank * slice, (rank + 1) * slice, post_scale,
-                                             (char*)dst);
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-template <typename T>
-static void q8_ar_w(const Q8Args& a, int blocks, cudaStream_t stream) {
-  switch (a.pt.world) {
-    case 2: q8_allreduce_kernel<T, 2><<<blocks, 512, 0, stream>>>(a); break;
-    case 3: q8_allreduce_kernel<T, 3><<<blocks, 512, 0, stream>>>(a); break;
-    case 4: q8_allreduce_kernel<T, 4><<<blocks, 512, 0, stream>>>(a); break;
-    case 5: q8_allreduce_kernel<T, 5><<<blocks, 512, 0, stream>>>(a); break;
-    case 6: q8_allreduce_kernel<T, 6><<<blocks, 512, 0, stream>>>(a); break;
-    case 7: q8_allreduce_kernel<T, 7><<<blocks, 512, 0, stream>>>(a); break;
-    case 8: q8_allreduce_kernel<T, 8><<<blocks, 512, 0, stream>>>(a); break;
-    default: throw std::runtime_error("q8_allreduce: world size must be in [2, 8]");
-  }
 }
 
 void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const void* in_a,
@@ -596,12 +469,13 @@ void q8_allreduce_launch(const PeerTable& pt, StatusBlock* st, size_t off, const
   a.mode = 0;
   a.slice_elems = a.ngroups / pt.world * kGroup;
   if (pt.world < 2) throw std::runtime_error("q8_allreduce: world must be >= 2");
-  switch (dtype) {
-    case kF32: q8_ar_w<float>(a, blocks, stream); break;
-    case kBF16: q8_ar_w<__nv_bfloat16>(a, blocks, stream); break;
-    case kF16: q8_ar_w<__half>(a, blocks, stream); break;
-    default: throw std::runtime_error("q8_allreduce: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    const bool known_world = dispatch<2, 3, 4, 5, 6, 7, 8>(pt.world, [&](auto W) {
+      q8_allreduce_kernel<Elem<D>, W><<<blocks, 512, 0, stream>>>(a);
+    });
+    if (!known_world) throw std::runtime_error("q8_allreduce: world size must be in [2, 8]");
+  });
+  if (!known_dtype) throw std::runtime_error("q8_allreduce: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -627,14 +501,11 @@ void q8_gather_dequant_launch(const PeerTable& pt, const int* ok, size_t r_off, 
   Q8Ptrs r;
   for (int p = 0; p < kMaxRanks; ++p) r.p[p] = p < pt.world ? reinterpret_cast<const char*>(pt.data[p]) + r_off : nullptr;
   if (blocks < 1) blocks = 1;
-  switch (dtype) {
-    case kF32: q8_gather_dequant_kernel<float><<<blocks, 512, 0, stream>>>(r, ng, slice, (float*)out, nelem, ok); break;
-    case kBF16:
-      q8_gather_dequant_kernel<__nv_bfloat16><<<blocks, 512, 0, stream>>>(r, ng, slice, (__nv_bfloat16*)out, nelem, ok);
-      break;
-    case kF16: q8_gather_dequant_kernel<__half><<<blocks, 512, 0, stream>>>(r, ng, slice, (__half*)out, nelem, ok); break;
-    default: throw std::runtime_error("q8_gather_dequant: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    using T = Elem<D>;
+    q8_gather_dequant_kernel<T><<<blocks, 512, 0, stream>>>(r, ng, slice, (T*)out, nelem, ok);
+  });
+  if (!known_dtype) throw std::runtime_error("q8_gather_dequant: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -666,12 +537,13 @@ void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, 
   a.contribute = contribute;
   a.mode = 1;
   a.slice_elems = slice_elems;
-  switch (dtype) {
-    case kF32: q8_ar_w<float>(a, blocks, stream); break;
-    case kBF16: q8_ar_w<__nv_bfloat16>(a, blocks, stream); break;
-    case kF16: q8_ar_w<__half>(a, blocks, stream); break;
-    default: throw std::runtime_error("q8_reduce_scatter: unsupported dtype");
-  }
+  const bool known_dtype = dispatch<kF32, kBF16, kF16>(dtype, [&](auto D) {
+    const bool known_world = dispatch<2, 3, 4, 5, 6, 7, 8>(pt.world, [&](auto W) {
+      q8_allreduce_kernel<Elem<D>, W><<<blocks, 512, 0, stream>>>(a);
+    });
+    if (!known_world) throw std::runtime_error("q8_reduce_scatter: world size must be in [2, 8]");
+  });
+  if (!known_dtype) throw std::runtime_error("q8_reduce_scatter: unsupported dtype");
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

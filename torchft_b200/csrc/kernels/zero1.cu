@@ -57,7 +57,6 @@
 #include <algorithm>
 #include <stdexcept>
 #include <string>
-#include <type_traits>
 
 #include "api.h"
 #include "common.cuh"
@@ -584,13 +583,6 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
   }
 }
 
-// Calls f(std::integral_constant<decltype(V), V>{}) for the V of Vs equal to the runtime value v: the one place where a
-// launcher's runtime selector becomes a template argument. Returns false when v is none of Vs.
-template <auto... Vs, typename T, typename F>
-bool dispatch(T v, F&& f) {
-  return ((v == Vs && (f(std::integral_constant<decltype(Vs), Vs>{}), true)) || ...);
-}
-
 void check_grid(int blocks, int threads, const char* who) {
   if (blocks < 1 || blocks > kNumSMs * 32) throw std::runtime_error(std::string(who) + ": bad grid");
   if (threads < 32 || threads > 512 || (threads & 31)) throw std::runtime_error(std::string(who) + ": bad block size");
@@ -677,8 +669,7 @@ void zero1_update_launch(UpdArgs a, int moment_dtype, int blocks, int threads, c
           dispatch<kF32, kBF16>(moment_dtype, [&](auto MD) {
             dispatch<false, true>(a.ema != nullptr, [&](auto EMA) {
               // one rank pushes to nobody: never multicast
-              using MT = std::conditional_t<MD == kBF16, bf16, float>;
-              zero1_update_kernel<W, (W > 1 && NVLS), PAGED, CLIP, MT, EMA><<<blocks, threads, 0, stream>>>(a);
+              zero1_update_kernel<W, (W > 1 && NVLS), PAGED, CLIP, Elem<MD>, EMA><<<blocks, threads, 0, stream>>>(a);
             });
           });
         });

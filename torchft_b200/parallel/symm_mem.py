@@ -564,7 +564,7 @@ class SymmetricComm:
                     ngroups = self._K.q8_ngroups(n, self._world)
                     big = max(1, min(self._K.NUM_SMS * 16, ngroups // 16 + 1))
                     if contribute:
-                        K.q8_quantize_raw(a.data_ptr(), b.data_ptr() if b is not None else 0, n, ngroups, dt, seg.ptr, sp)
+                        K.q8_quantize(a.data_ptr(), b.data_ptr() if b is not None else 0, n, ngroups, dt, seg.ptr, sp)
                     else:
                         K.memset_async(seg.ptr, 0, q_bytes, sp)  # zero scales: this replica adds nothing
                     self._handshake(2, True, _CH_Q8, sp)

@@ -44,7 +44,7 @@ def quantize_q8(x: torch.Tensor, world_size: int = 1, subtract: torch.Tensor | N
     _check(x)
     buf = torch.empty(K.q8_buffer_bytes(x.numel(), world_size), dtype=torch.uint8, device=x.device)
     K.q8_quantize(x.data_ptr(), subtract.data_ptr() if subtract is not None else 0, x.numel(),
-                  _native.dtype_code(x), world_size, buf.data_ptr(), _native.stream_ptr())
+                  K.q8_ngroups(x.numel(), world_size), _native.dtype_code(x), buf.data_ptr(), _native.stream_ptr())
     return buf
 
 
@@ -54,7 +54,8 @@ def dequantize_q8(buf: torch.Tensor, numel: int, dtype: torch.dtype, world_size:
     if out is None:
         out = torch.empty(numel, dtype=dtype, device=buf.device)
     _check(out)
-    K.q8_dequantize(buf.data_ptr(), numel, _native.DTYPE_CODE[dtype], world_size, out.data_ptr(), _native.stream_ptr())
+    K.q8_dequantize(buf.data_ptr(), K.q8_ngroups(numel, world_size), out.data_ptr(), numel, _native.DTYPE_CODE[dtype],
+                    _native.stream_ptr())
     return out
 
 
@@ -76,7 +77,8 @@ def fused_quantize_into_fp8(inputs: List[torch.Tensor], world_size: int) -> torc
     for t, o in zip(inputs, offs):
         t = t.contiguous()
         _check(t)
-        K.q8_quantize(t.data_ptr(), 0, t.numel(), _native.dtype_code(t), world_size, buf.data_ptr() + o, sp)
+        K.q8_quantize(t.data_ptr(), 0, t.numel(), K.q8_ngroups(t.numel(), world_size), _native.dtype_code(t),
+                      buf.data_ptr() + o, sp)
     return buf
 
 
@@ -88,13 +90,14 @@ def fused_dequantize_from_fp8(inputs: List[torch.Tensor], quantized: torch.Tenso
     assert quantized.numel() >= total
     sp = _native.stream_ptr()
     for t, o in zip(inputs, offs):
+        g = K.q8_ngroups(t.numel(), world_size)
         if not t.is_contiguous():
             tmp = torch.empty_like(t, memory_format=torch.contiguous_format)
-            K.q8_dequantize(quantized.data_ptr() + o, t.numel(), _native.dtype_code(t), world_size, tmp.data_ptr(), sp)
+            K.q8_dequantize(quantized.data_ptr() + o, g, tmp.data_ptr(), t.numel(), _native.dtype_code(t), sp)
             t.copy_(tmp)
         else:
             _check(t)
-            K.q8_dequantize(quantized.data_ptr() + o, t.numel(), _native.dtype_code(t), world_size, t.data_ptr(), sp)
+            K.q8_dequantize(quantized.data_ptr() + o, g, t.data_ptr(), t.numel(), _native.dtype_code(t), sp)
 
 
 def fused_reduce_fp8(inputs: List[torch.Tensor], all_buffers: List[torch.Tensor], world_size: int, rank: int,
@@ -117,7 +120,11 @@ def fused_reduce_fp8(inputs: List[torch.Tensor], all_buffers: List[torch.Tensor]
     dev = inputs[0].device
     for t, o in zip(inputs, offs):
         ptrs = torch.tensor([b.data_ptr() + o for b in all_buffers], dtype=torch.int64, device=dev)
-        K.q8_reduce(ptrs.data_ptr(), world_size, rank, t.numel(), post, all_buffers[rank].data_ptr() + o, sp)
+        g = K.q8_ngroups(t.numel(), world_size)
+        sl = g // world_size
+        # the sum starts at this rank's own buffer and wraps, over the groups of this rank's slice
+        K.q8_reduce(ptrs.data_ptr(), world_size, rank, g, rank * sl, (rank + 1) * sl, post,
+                    all_buffers[rank].data_ptr() + o, sp)
 
 
 
