@@ -15,6 +15,6 @@ ASAN_OPTIONS="detect_leaks=1" UBSAN_OPTIONS="print_stacktrace=1:halt_on_error=1"
 if python -c "import torch,sys; sys.exit(0 if torch.cuda.is_available() else 1)"; then
   for tool in memcheck racecheck synccheck; do
     compute-sanitizer --tool $tool --error-exitcode 1 --launch-timeout 120 \
-      python -m pytest tests/test_kernels_gpu.py -x -q -m gpu -k "rmsnorm or swiglu or rope or cross_entropy or adamw or q8_roundtrip or heal_copy"
+      python -m pytest tests/test_kernels_gpu.py tests/test_heal_exact_gpu.py::test_heal_copy -x -q -m gpu -k "rmsnorm or swiglu or rope or cross_entropy or adamw or q8_roundtrip or heal_copy"
   done
 fi

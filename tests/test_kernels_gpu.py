@@ -205,19 +205,6 @@ def test_q8_roundtrip(K, dtype, n):
     assert rel < 0.04
 
 
-def test_heal_copy(K):
-    from torchft_b200.checkpointing.p2p_transport import device_copy
-
-    torch.manual_seed(7)
-    srcs = [torch.randn(n, device="cuda") for n in (1, 1000, 1 << 20, 12345)]
-    srcs.append(torch.randint(0, 255, (777,), device="cuda", dtype=torch.uint8)[1:])  # unaligned
-    dsts = [torch.empty_like(s) for s in srcs]
-    device_copy([(s.data_ptr(), d.data_ptr(), s.numel() * s.element_size()) for s, d in zip(srcs, dsts)])
-    torch.cuda.synchronize()
-    for s, d in zip(srcs, dsts):
-        assert torch.equal(s, d)
-
-
 def test_llama_tiny_fwd_bwd_matches_reference():
     from torchft_b200.models.llama import CONFIGS, Llama
     from torchft_b200.models.reference import reference_loss

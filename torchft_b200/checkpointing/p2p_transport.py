@@ -50,6 +50,21 @@ T = TypeVar("T")
 CHUNK_BYTES = 4 << 20
 
 
+def copy_table(entries: Sequence[Tuple[int, int, int]], chunk_bytes: int) -> Tuple[List[Tuple[int, int, int, int]], int]:
+    """The rows ``(src, dst, nbytes, chunk0)`` of ``heal_copy_kernel``'s table and the number of chunks they span.
+
+    Entry ``i`` owns chunks ``[chunk0, chunk0 + ceil(nbytes / chunk_bytes))``. Empty entries are dropped, so every row owns
+    a chunk: the kernel maps a chunk to the LAST row whose ``chunk0`` is not above it, and an empty row sharing the
+    ``chunk0`` of a non-empty row before it would take that row's first chunk and leave it uncopied."""
+    rows, chunk0 = [], 0
+    for src, dst, n in entries:
+        if n <= 0:
+            continue
+        rows.append((src, dst, n, chunk0))
+        chunk0 += (n + chunk_bytes - 1) // chunk_bytes
+    return rows, chunk0
+
+
 def device_copy(entries: Sequence[Tuple[int, int, int]], stream: Optional[torch.cuda.Stream] = None,
                 blocks: int = 128, chunk_bytes: int = CHUNK_BYTES) -> None:
     """Copy ``(src_ptr, dst_ptr, nbytes)`` ranges with one kernel launch (``heal_copy_kernel``: 8 x 16-byte loads in
@@ -57,18 +72,13 @@ def device_copy(entries: Sequence[Tuple[int, int, int]], stream: Optional[torch.
     """
 
     K = _native.load()
-    rows, chunk0 = [], 0
-    for src, dst, n in entries:
-        if n <= 0:
-            continue
-        rows.append((src, dst, n, chunk0))
-        chunk0 += (n + chunk_bytes - 1) // chunk_bytes
+    rows, chunks = copy_table(entries, chunk_bytes)
     if not rows:
         return
     table = torch.tensor(rows, dtype=torch.int64).cuda(non_blocking=False)
     s = stream if stream is not None else torch.cuda.current_stream()
     with torch.cuda.stream(s):
-        K.heal_copy(table.data_ptr(), len(rows), chunk0, chunk_bytes, max(1, min(blocks, chunk0)), int(s.cuda_stream))
+        K.heal_copy(table.data_ptr(), len(rows), chunks, chunk_bytes, max(1, min(blocks, chunks)), int(s.cuda_stream))
         table.record_stream(s)
 
 
@@ -99,6 +109,8 @@ class P2PTransport(CheckpointTransport[T], Generic[T]):
         self._step = -1
         self._manifest: Optional[bytes] = None
         self._keepalive: Any = None
+        self._staged: List[int] = []  # cudaMalloc copies of leaves that CUDA IPC cannot export, freed with the manifest
+        self._staged_logged: set = set()
         self._sessions: Dict[str, Any] = {}  # session id -> its open connection (closing it releases its read lock)
         self._sess_lock = threading.Lock()
         self._lease_s = max(1.0, timeout.total_seconds())
@@ -169,35 +181,44 @@ class P2PTransport(CheckpointTransport[T], Generic[T]):
         items: List[Dict[str, Any]] = []
         handles: Dict[int, str] = {}
         keep = []
+        staged: List[int] = []
         # make sure everything the state_dict views has been produced
         if torch.cuda.is_available():
             torch.cuda.current_stream().synchronize()
-        for leaf in leaves:
-            host = isinstance(leaf, torch.Tensor) and not leaf.is_cuda and leaf.numel() * leaf.element_size() >= 4096
-            if (isinstance(leaf, torch.Tensor) and leaf.is_cuda) or host:
-                t = leaf.detach()
-                if isinstance(t, torch.distributed.tensor.DTensor):  # type: ignore[attr-defined]
-                    t = t.to_local()
-                if host:
-                    # CPU tensors (e.g. DiLoCo's pinned backup weights) ride the same NVLink pull: stage them on the GPU
-                    # once instead of embedding them in the manifest (ADVICE r1: that doubled them as hex in memory)
-                    t = t.to(torch.device("cuda", torch.cuda.current_device()), non_blocking=True)
-                # bytes actually backing this view
-                if not t.is_contiguous():
-                    t = t.contiguous()
-                keep.append(t)
-                ptr = t.data_ptr()
-                nbytes = t.numel() * t.element_size()
-                base, size = K.address_range(ptr) if nbytes else (0, 0)
-                if nbytes and base not in handles:
-                    handles[base] = K.ipc_get_handle(base).hex()
-                items.append({"k": "cuda", "base": base, "off": ptr - base, "nbytes": nbytes,
-                              "dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape),
-                              "device": t.device.index, "host": host})
-            else:
-                items.append({"k": "obj", "data": pickle.dumps(leaf)})
-        if torch.cuda.is_available():
-            torch.cuda.current_stream().synchronize()  # staged host tensors have landed
+        try:
+            for leaf in leaves:
+                host = isinstance(leaf, torch.Tensor) and not leaf.is_cuda and leaf.numel() * leaf.element_size() >= 4096
+                if (isinstance(leaf, torch.Tensor) and leaf.is_cuda) or host:
+                    t = leaf.detach()
+                    if isinstance(t, torch.distributed.tensor.DTensor):  # type: ignore[attr-defined]
+                        t = t.to_local()
+                    if host:
+                        # CPU tensors (e.g. DiLoCo's pinned backup weights) ride the same NVLink pull: stage them on the
+                        # GPU once instead of embedding them in the manifest (ADVICE r1: that doubled them as hex in memory)
+                        t = t.to(torch.device("cuda", torch.cuda.current_device()), non_blocking=True)
+                    # bytes actually backing this view
+                    if not t.is_contiguous():
+                        t = t.contiguous()
+                    nbytes = t.numel() * t.element_size()
+                    if nbytes and not K.ipc_capable(t.data_ptr()):
+                        t = self._stage(K, t, nbytes, staged)
+                    keep.append(t)
+                    ptr = t.data_ptr()
+                    base, size = K.address_range(ptr) if nbytes else (0, 0)
+                    if nbytes and base not in handles:
+                        handles[base] = K.ipc_get_handle(base).hex()
+                    items.append({"k": "cuda", "base": base, "off": ptr - base, "nbytes": nbytes,
+                                  "dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape),
+                                  "device": t.device.index, "host": host})
+                else:
+                    items.append({"k": "obj", "data": pickle.dumps(leaf)})
+            if torch.cuda.is_available():
+                torch.cuda.current_stream().synchronize()  # staged host tensors have landed
+        except BaseException:
+            _free(staged)  # no manifest names them yet
+            raise
+        _free(self._staged)
+        self._staged = staged
         self._keepalive = keep
         self._manifest = pickle.dumps({"spec": spec, "items": items, "handles": handles, "pid": _pid(),
                                        "host": socket.gethostname()})
@@ -230,6 +251,30 @@ class P2PTransport(CheckpointTransport[T], Generic[T]):
         self._allowed = False  # flipped only once the write lock is really held, so the two can never disagree
         self._manifest = None
         self._keepalive = None
+        _free(self._staged)
+        self._staged = []
+
+    def _stage(self, K: Any, t: torch.Tensor, nbytes: int, staged: List[int]) -> torch.Tensor:
+        """A copy of ``t`` in a ``cudaMalloc`` allocation, which CUDA IPC can export. Legacy IPC refuses ``cuMemCreate``
+        memory: the symmetric segments in vmm mode (the FT-ZeRO-1 weights) and PyTorch's expandable segments."""
+        from torchft_b200.parallel.symm_mem import tensor_from_ptr
+
+        base = K.address_range(t.data_ptr())[0]
+        if base not in self._staged_logged:
+            self._staged_logged.add(base)
+            logger.warning("p2p_transport: CUDA IPC cannot export the allocation at %#x (cuMemCreate memory); its tensors "
+                           "are copied into cudaMalloc memory for every heal they serve", base)
+        with torch.cuda.device(t.device):
+            ptr = K.symm_alloc(nbytes)
+            staged.append(ptr)
+            # symm_alloc zero-fills on the legacy default stream, which the current stream (the Manager's recovery stream
+            # is a non-blocking one) does not wait for: the fill must be done before the copy starts, and the copy before
+            # the manifest names it
+            torch.cuda.synchronize()
+            out = tensor_from_ptr(ptr, nbytes, t.device)
+            out.copy_(t.reshape(-1).view(torch.uint8))
+            torch.cuda.current_stream().synchronize()
+        return out.view(t.dtype).view(t.shape)
 
     # ---------------------------------------------------------------- receiver
     def recv_checkpoint(self, src_rank: int, metadata: str, step: int, timeout: timedelta) -> T:
@@ -336,10 +381,24 @@ class P2PTransport(CheckpointTransport[T], Generic[T]):
             conn.close()
 
     def shutdown(self, wait: bool = True) -> None:
+        try:
+            self.disallow_checkpoint()  # a receiver may still be pulling the tensors and staged copies we serve
+        except TimeoutError:
+            logger.warning("p2p_transport: a heal session outlived shutdown; its staged copies are not freed")
+            self._staged = []
         self._server.shutdown()
         self._server.server_close()
         if wait:
             self._thread.join(timeout=5)
+
+
+def _free(staged: List[int]) -> None:
+    """``cudaFree`` the staged copies ``staged`` once the device has finished with them."""
+    if staged:
+        torch.cuda.synchronize()
+        K = _native.load()
+        for ptr in staged:
+            K.symm_free(ptr)
 
 
 def _pid() -> int:

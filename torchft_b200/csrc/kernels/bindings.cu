@@ -139,6 +139,25 @@ py::tuple address_range(uintptr_t ptr) {
   return py::make_tuple((uintptr_t)base, size);
 }
 
+// Whether cudaIpcGetMemHandle can export the allocation containing `ptr`. It cannot for cuMemCreate memory (vmm-mode
+// symmetric segments, PyTorch's expandable segments); asking the driver first keeps a refused export from leaving an
+// error behind for the next launch check.
+bool ipc_capable(uintptr_t ptr) {
+  typedef CUresult (*fn_t)(void*, CUpointer_attribute, CUdeviceptr);
+  static fn_t fn = nullptr;
+  if (!fn) {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    TFT_CUDA_CHECK(cudaGetDriverEntryPoint("cuPointerGetAttribute", &f, cudaEnableDefault, &q));
+    if (!f) throw std::runtime_error("cuPointerGetAttribute unavailable");
+    fn = reinterpret_cast<fn_t>(f);
+  }
+  int v = 0;
+  CUresult r = fn(&v, CU_POINTER_ATTRIBUTE_IS_LEGACY_CUDA_IPC_CAPABLE, (CUdeviceptr)ptr);
+  if (r != CUDA_SUCCESS) throw std::runtime_error("cuPointerGetAttribute failed: " + std::to_string((int)r));
+  return v != 0;
+}
+
 void memset_async(uintptr_t p, int value, size_t nbytes, uintptr_t stream) {
   TFT_CUDA_CHECK(cudaMemsetAsync(P<void>(p), value, nbytes, S(stream)));
 }
@@ -197,6 +216,7 @@ PYBIND11_MODULE(_K, m) {
   m.def("ipc_open_handle", &ipc_open_handle);
   m.def("ipc_close_handle", &ipc_close_handle);
   m.def("address_range", &address_range);
+  m.def("ipc_capable", &ipc_capable);
   m.def("memset_async", &memset_async);
   m.def("memcpy_async", &memcpy_async);
   m.def("memcpy_h2d", &memcpy_h2d);

@@ -829,6 +829,8 @@ void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s) {
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
+// The table's chunk0 must not decrease and no row may be empty: a chunk goes to the last row whose chunk0 is <= it, so
+// an empty row after a non-empty one with the same chunk0 would take that row's first chunk (copy_table drops them).
 void heal_copy_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                       int blocks, cudaStream_t s) {
   if (total_chunks == 0) return;
