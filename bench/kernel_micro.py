@@ -77,18 +77,6 @@ def main() -> None:
         part = torch.empty(grid, H, device=dev)
         dw = torch.empty_like(w)
         record("rmsnorm_bwd", timeit(lambda: K.rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), rstd.data_ptr(), dx.data_ptr(), part.data_ptr(), dw.data_ptr(), False, T, H, sp()), args.iters, flush), 3 * x.numel() * 2)
-        if args.only == "rmsnorm_sweep":  # CTA shape x prefetch x CTAs/SM (the default is set in model_ops.cu)
-            part = torch.empty(K.NUM_SMS * 8, H, device=dev)
-            for tpb in (128, 256, 512):
-                for pf in (0, 1):
-                    for cps in (2, 3, 4, 6, 8):
-                        K.rmsnorm_tune(0, tpb, pf, cps)
-                        K.rmsnorm_tune(1, tpb, pf, cps)
-                        tag = f"t{tpb}_pf{pf}_c{cps}"
-                        record("rmsnorm_sweep_fwd_" + tag, timeit(lambda: K.rmsnorm_fwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), rstd.data_ptr(), T, H, 1e-5, sp()), args.iters, flush), 2 * x.numel() * 2)
-                        record("rmsnorm_sweep_bwd_" + tag, timeit(lambda: K.rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), rstd.data_ptr(), dx.data_ptr(), part.data_ptr(), dw.data_ptr(), False, T, H, sp()), args.iters, flush), 3 * x.numel() * 2)
-            K.rmsnorm_tune(0, 128, 1, 6)
-            K.rmsnorm_tune(1, 256, 1, 4)
     if want("swiglu"):
         gu = torch.randn(T, 2 * F, device=dev).bfloat16()
         y = torch.empty(T, F, device=dev, dtype=torch.bfloat16)
@@ -100,8 +88,11 @@ def main() -> None:
         Hq, Hkv, D = 32, 8, 128
         qkv = torch.randn(T, (Hq + 2 * Hkv) * D, device=dev).bfloat16()
         cs = fused.rope_table(T, D, 500000.0, dev)
-        q = torch.empty(T, Hq * D, device=dev, dtype=torch.bfloat16)
-        record("rope_q", timeit(lambda: K.rope(qkv.data_ptr(), q.data_ptr(), cs.data_ptr(), T, T, Hq, D, qkv.shape[1], Hq * D, 1.0, sp()), args.iters, flush), 2 * T * Hq * D * 2)
+        q = torch.empty(1, T, Hq, D, device=dev, dtype=torch.bfloat16)
+        k = torch.empty(1, T, Hkv, D, device=dev, dtype=torch.bfloat16)
+        # forward (dir 0, no v output): q and k rotated out of the packed rows, each element read once and written once
+        strides = [*q.stride()[:3], *k.stride()[:3], 0, 0, 0]
+        record("rope_qkv_fwd", timeit(lambda: K.rope_qkv(qkv.data_ptr(), qkv.shape[1], q.data_ptr(), k.data_ptr(), 0, strides, cs.data_ptr(), T, T, D, Hq, Hkv, 0, sp()), args.iters, flush), 2 * T * (Hq + Hkv) * D * 2)
     if want("xent"):
         rows = 2048
         logits = torch.randn(rows, V, device=dev).bfloat16()

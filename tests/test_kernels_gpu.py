@@ -100,37 +100,6 @@ def test_rope_qkv_backward_takes_sdpa_ordered_gradients(D, Hq, Hkv):
         torch.autograd.backward([q, k, v], gs)
         grads.append(qkv.grad)
     assert torch.equal(grads[0], grads[1])
-    # and the raw single-tensor kernel (generic API) agrees with the fused split on q
-    K = fused._native.load()
-    q2 = torch.empty(B * S, Hq * D, device="cuda", dtype=torch.bfloat16)
-    K.rope(base.data_ptr(), q2.data_ptr(), cs.data_ptr(), B * S, S, Hq, D, base.shape[1], Hq * D, 1.0, fused._native.stream_ptr())
-    q, _, _ = fused.rope_qkv(base, cs, B, S, Hq, Hkv, D)
-    assert torch.equal(q.reshape(B * S, Hq * D), q2)
-
-
-@pytest.mark.parametrize("tpb,pf,cps", [(128, 0, 4), (128, 1, 2), (256, 1, 3), (512, 0, 8), (512, 1, 1)])
-@pytest.mark.parametrize("H", [256, 4096, 5120])
-def test_rmsnorm_every_cta_shape_matches_reference(tpb, pf, cps, H):
-    from torchft_b200.ops import fused
-
-    K = fused._native.load()
-    try:
-        K.rmsnorm_tune(0, tpb, pf, cps)
-        K.rmsnorm_tune(1, tpb, pf, cps)
-        torch.manual_seed(5)
-        rows = 777
-        x = torch.randn(rows, H, device="cuda").bfloat16().requires_grad_()
-        w = (1 + 0.1 * torch.randn(H, device="cuda")).bfloat16().requires_grad_()
-        y = fused.rmsnorm(x, w, 1e-5)
-        dy = torch.randn_like(y)
-        y.backward(dy)
-        xf, wf = x.detach().float().requires_grad_(), w.detach().float().requires_grad_()
-        yf = xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + 1e-5) * wf
-        yf.backward(dy.float())
-        assert _rel(y, yf) < 1e-2 and _rel(x.grad, xf.grad) < 1e-2 and _rel(w.grad, wf.grad) < 2e-2
-    finally:
-        K.rmsnorm_tune(0, 128, 1, 6)
-        K.rmsnorm_tune(1, 256, 1, 4)
 
 
 @pytest.mark.parametrize("T,V", [(64, 1000), (33, 4104), (16, 128256)])
@@ -188,8 +157,6 @@ def test_flat_adamw_matches_torch():
     gate.zero_()
     opt.step(gate=gate)  # gated off: must be a no-op
     assert torch.equal(before, opt.master)
-    ss = opt.grad_sumsq()
-    assert abs(ss.item() - g.float().pow(2).sum().item()) < 1e-2 * ss.item()
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16])
@@ -356,7 +323,7 @@ def _rms(x, g, eps):
 
 @pytest.mark.parametrize("with_res", [False, True])
 def test_fused_block_ops_match_fp32_reference(with_res):
-    """norm_linear(_res) / linear(res=) / swiglu_linear(res=): forward and every gradient (input, residual stream,
+    """norm_linear_res / linear(res=) / swiglu_linear(res=): forward and every gradient (input, residual stream,
     norm weight, projection weights) against a plain fp32 PyTorch graph of the same sub-block."""
     from torchft_b200.ops import fused
 
@@ -372,7 +339,7 @@ def test_fused_block_ops_match_fp32_reference(with_res):
         h = fused.swiglu_linear(gu, W2, res=xs)
         out = fused.linear(h, Wo, res=h)
     else:
-        gu = fused.norm_linear(x, g, W13, eps)
+        _, gu = fused.norm_linear_res(x, g, W13, eps)
         h = x + fused.swiglu_linear(gu, W2)
         out = h + fused.linear(h, Wo)
     dout = torch.randn_like(out)

@@ -67,7 +67,6 @@ def _rows_with_scales(rows, H, gen, scales=(1.0, 1e3, 1e-3, 0.0)):
 # -> 53 U; the fast-math division by H adds 2 ulp (4 U) and + eps U; the square root halves all that, and rsqrtf adds
 # 2 ulp (4 U): (53 + 4 + 1) / 2 + 4 = 33 U, rounded up to 34 U for the reference's own rounding.
 R_RSTD = 34 * U
-RMS_FWD_DEFAULT, RMS_BWD_DEFAULT = (128, 1, 6), (256, 1, 4)
 
 
 def _check_rmsnorm(K, x, w, dy, dres, eps, tag, y, rstd, dx, dw):
@@ -118,26 +117,13 @@ def _run_rmsnorm(K, rows, H, seed, with_dres=False, tag=""):
 
 
 @gpu
-@pytest.mark.parametrize("H", [8, 2048, 2056, 4096, 16384])
+@pytest.mark.parametrize("H", [8, 2048, 2056, 4096, 8192, 16384])
 @pytest.mark.parametrize("rows", [1, 263, 264, 265, 791, 792, 793, 8192])
 def test_rmsnorm_raw_launchers(K, rows, H):
-    """Rows below, at and above the default CTA caps (792 forward, 264 backward): one row or many per CTA."""
+    """Rows below, at and above the CTA caps (792 forward, 264 backward): one row or many per CTA. The H set reaches
+    every launch shape: forward (NV, TPB) (1,128) (2,128) (4,128) (4,256) (4,512), backward (1,256) (2,256) (4,256)
+    (4,512)."""
     _run_rmsnorm(K, rows, H, seed=rows * 7 + H, with_dres=(rows % 2 == 1))
-
-
-@gpu
-@pytest.mark.parametrize("tpb", [128, 256, 512])
-@pytest.mark.parametrize("pf", [0, 1])
-@pytest.mark.parametrize("cps", [1, 4, 8])
-def test_rmsnorm_every_tuning(K, tpb, pf, cps):
-    try:
-        K.rmsnorm_tune(0, tpb, pf, cps)
-        K.rmsnorm_tune(1, tpb, pf, cps)
-        for rows, H in ((793, 2056), (2000, 16384), (265, 4096)):
-            _run_rmsnorm(K, rows, H, seed=tpb + pf + cps + H, with_dres=True, tag="tuned ")
-    finally:
-        K.rmsnorm_tune(0, *RMS_FWD_DEFAULT)
-        K.rmsnorm_tune(1, *RMS_BWD_DEFAULT)
 
 
 @gpu
@@ -657,29 +643,6 @@ def test_diloco_outer(K, dtype, n):
                    True, 0.3, gate.data_ptr(), _sp())
     for a, b in zip(before, (param, orig, mom)):
         assert torch.equal(a, b)  # gate 0 changes nothing
-
-
-# ------------------------------------------------------------------ sum of squares
-@gpu
-@pytest.mark.parametrize("n", [1, 8, (1 << 28) + 5])
-def test_grad_sumsq(K, n):
-    from torchft_b200.ops import fused
-
-    gen = torch.Generator(device="cuda").manual_seed(n % 97)
-    g = torch.randn(n, device="cuda", generator=gen).bfloat16()
-    if n <= 8:
-        got = fused.FlatAdamW(torch.zeros_like(g), g).grad_sumsq()
-    else:
-        got = torch.zeros(1, device="cuda")
-        K.sumsq(g.data_ptr(), n, got.data_ptr(), _sp())
-    ref = sum(float(c.double().pow(2).sum()) for c in g.split(1 << 26))
-    # all terms >= 0: relative error <= (chain length) U, the chain being a thread's partial (8 squares per vector, one
-    # vector per pass of a grid of <= 132 * 4 CTAs of 512 threads, + the <= 7 tail elements), 10 shuffle levels, one
-    # atomic add per CTA, and the rounding of each square
-    grid = min(max(1, math.ceil((n // 8 + 1) / 512)), 132 * 4)
-    chain = 8 * math.ceil(n // 8 / (grid * 512)) + 7 + 10 + grid + 1
-    ref_t = torch.tensor([ref], dtype=torch.float64, device="cuda")
-    assert_close_elementwise(got, ref_t, ulps=0, abs_slack=chain * U * ref_t, what=f"sumsq n={n}")
 
 
 # ------------------------------------------------------------------ the whole model

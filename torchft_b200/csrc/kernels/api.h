@@ -75,7 +75,6 @@ void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, 
 void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int rows, int H,
                         float eps, cudaStream_t s);
 int rmsnorm_bwd_grid(int rows);
-void rmsnorm_tune(int bwd, int tpb, int prefetch, int ctas_per_sm_at_128);
 void rmsnorm_bwd_launch(const void* dy, const void* x, const void* w, const float* rstd, void* dx,
                         float* dw_partial, void* dw, int accumulate, int rows, int H,
                         cudaStream_t s, const void* dres = nullptr);
@@ -83,8 +82,6 @@ void swiglu_fwd_launch(const void* gu, void* y, size_t T, int F, cudaStream_t s)
 void swiglu_bwd_launch(const void* dy, const void* gu, void* dgu, size_t T, int F, cudaStream_t s);
 void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const int64_t* strides9, const void* cs,
                      size_t T, int S, int D, int Hq, int Hkv, int dir, cudaStream_t s);
-void rope_launch(const void* in, void* out, const void* cs, size_t T, int S, int heads, int D,
-                 size_t in_stride, size_t out_stride, float sign, cudaStream_t s);
 void xent_launch(void* logits, const void* target, float* loss, size_t rows, int V,
                  size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s,
                  const float* scale = nullptr);
@@ -93,7 +90,6 @@ void adamw_launch(void* p, float* master, float* m, float* v, const void* g, siz
                   const int* gate, int max_blocks, cudaStream_t s);
 void diloco_outer_launch(void* param, void* original, const void* grad, float* mom, size_t n, int dtype, float lr,
                          float mu, int nesterov, float alpha, const int* gate, cudaStream_t s);
-void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s);
 void heal_copy_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                       int blocks, cudaStream_t s);
 

@@ -440,7 +440,6 @@ PYBIND11_MODULE(_K, m) {
     rmsnorm_fwd_launch(P<void>(x), P<void>(w), P<void>(y), P<float>(rstd), rows, H, eps, S(s));
   });
   m.def("rmsnorm_bwd_grid", &rmsnorm_bwd_grid);
-  m.def("rmsnorm_tune", &rmsnorm_tune, "(0 forward | 1 backward, CTA size 128/256/512, prefetch next row, CTAs/SM at 128 threads)");
   m.def("rmsnorm_bwd", [](uintptr_t dy, uintptr_t x, uintptr_t w, uintptr_t rstd, uintptr_t dx,
                           uintptr_t dw_partial, uintptr_t dw, bool accumulate, int rows, int H,
                           uintptr_t s, uintptr_t dres) {
@@ -453,10 +452,6 @@ PYBIND11_MODULE(_K, m) {
   });
   m.def("swiglu_bwd", [](uintptr_t dy, uintptr_t gu, uintptr_t dgu, size_t T, int F, uintptr_t s) {
     swiglu_bwd_launch(P<void>(dy), P<void>(gu), P<void>(dgu), T, F, S(s));
-  });
-  m.def("rope", [](uintptr_t in, uintptr_t out, uintptr_t cs, size_t T, int S_, int heads, int D,
-                   size_t in_stride, size_t out_stride, float sign, uintptr_t s) {
-    rope_launch(P<void>(in), P<void>(out), P<void>(cs), T, S_, heads, D, in_stride, out_stride, sign, S(s));
   });
   m.def("rope_qkv", [](uintptr_t packed, size_t row, uintptr_t q, uintptr_t k, uintptr_t v, std::vector<int64_t> strides,
                        uintptr_t cs, size_t T, int S_, int D, int Hq, int Hkv, int dir, uintptr_t s) {
@@ -484,9 +479,6 @@ PYBIND11_MODULE(_K, m) {
                         alpha, P<const int>(gate), S(s));
   }, py::arg("param"), py::arg("original"), py::arg("grad"), py::arg("mom"), py::arg("n"), py::arg("dtype"), py::arg("lr"),
      py::arg("mu"), py::arg("nesterov"), py::arg("alpha"), py::arg("gate"), py::arg("stream"));
-  m.def("sumsq", [](uintptr_t g, size_t n, uintptr_t out, uintptr_t s) {
-    sumsq_launch(P<void>(g), n, P<float>(out), S(s));
-  });
   m.def("heal_copy", [](uintptr_t table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                         int blocks, uintptr_t s) {
     heal_copy_launch(P<void>(table_dev), nentries, total_chunks, chunk_bytes, blocks, S(s));

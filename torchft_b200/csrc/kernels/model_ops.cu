@@ -26,10 +26,17 @@ using P8 = Pack<bf16>;
 // thread adds the <= 16 partials itself), and with PF the next row's loads are issued before the current row's reduction so
 // a CTA always has a full row of 16 B loads in flight. Small CTAs (128 threads x 4 vectors) with 4 per SM keep ~64 KB per
 // SM in flight, more than HBM bandwidth times latency per SM (Little's law) asks for.
+//
+// The launch shape is a fixed function of H and direction. The CTA starts at kRms{Fwd,Bwd}Threads and doubles until
+// kRmsMaxVec vectors per thread cover the row; the CTAs per SM are kRms{Fwd,Bwd}CtasPerSM at 128 threads, scaled by
+// 128 / TPB (at least 1). (NV, TPB) is forward (1,128) (2,128) (4,128) up to H = 4096, then (4,256) up to 8192 and (4,512)
+// up to 16384; backward (1,256) (2,256) (4,256) up to 8192, then (4,512). Prefetch is off at 4 x 512: there the backward's
+// second row does not fit in the 128 registers a 512-thread CTA leaves each thread, and it spills 172 B.
 constexpr int kRmsMaxVec = 4;
-// {forward, backward}: CTA threads, prefetch, CTAs per SM at 128 threads (rmsnorm_tune() overrides; bench/kernel_micro.py
-// sweeps them): forward 128 x 4 vectors at 6 CTAs/SM, backward 256 x 2 vectors at 4 CTAs/SM.
-static int g_rms_tpb[2] = {128, 256}, g_rms_pf[2] = {1, 1}, g_rms_cps[2] = {6, 4};
+constexpr int kRmsFwdThreads = 128, kRmsFwdCtasPerSM = 6;
+constexpr int kRmsBwdThreads = 256, kRmsBwdCtasPerSM = 4;
+template <int NV, int TPB>
+constexpr bool kRmsPrefetch = !(NV == 4 && TPB == 512);
 
 template <int TPB>
 __device__ __forceinline__ float row_sum(float v, float (*red)[TPB / 32], int& parity) {
@@ -44,10 +51,11 @@ __device__ __forceinline__ float row_sum(float v, float (*red)[TPB / 32], int& p
   return r;
 }
 
-template <int NV, int TPB, bool PF>
+template <int NV, int TPB>
 __global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
                                                           bf16* __restrict__ y, float* __restrict__ rstd, int rows,
                                                           int H, float eps) {
+  constexpr bool PF = kRmsPrefetch<NV, TPB>;
   __shared__ float red[2][TPB / 32];
   const int nvec = H / 8;
   int parity = 0;
@@ -107,11 +115,12 @@ __global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict
 // dx = rstd * (dy*w - xhat * mean(dy*w*xhat)) (+ dres); dw_partial[block] += dy * xhat
 // dres (optional) is the gradient arriving over the residual connection that bypasses the norm:
 // adding it here saves the separate elementwise accumulation pass autograd would run.
-template <int NV, int TPB, bool PF>
+template <int NV, int TPB>
 __global__ void __launch_bounds__(TPB) rmsnorm_bwd_kernel(
     const bf16* __restrict__ dy, const bf16* __restrict__ x, const bf16* __restrict__ w,
     const float* __restrict__ rstd, bf16* __restrict__ dx, float* __restrict__ dw_partial,
     const bf16* __restrict__ dres, int rows, int H) {
+  constexpr bool PF = kRmsPrefetch<NV, TPB>;
   __shared__ float red[2][TPB / 32];
   const int nvec = H / 8;
   int parity = 0;
@@ -284,51 +293,11 @@ __global__ void __launch_bounds__(512) swiglu_bwd_kernel(const bf16* __restrict_
 }
 
 // ------------------------------- RoPE ---------------------------------------
-// Interleaved-pair rotation (x[2i], x[2i+1]) by angle pos * theta_i; cs holds
-// (cos, sin) pairs: cs[pos][i] = float2. sign = +1 forward, -1 backward.
-// in/out row strides in elements so q/k can be read straight out of the packed
-// qkv projection and written contiguous.
+// Interleaved-pair rotation (x[2i], x[2i+1]) by angle pos * theta_i; cs holds (cos, sin) pairs: cs[pos][i] = float2.
 // A thread keeps its vector-in-head index for the whole kernel and walks (token, head) "slots" two at a time (both 16 B
 // loads issued before either is used); all index math is 32-bit (64-bit divisions per vector and a single load in flight
 // per thread leave the kernel latency-bound).
-__global__ void __launch_bounds__(256) rope_kernel(const bf16* __restrict__ in, bf16* __restrict__ out,
-                                                   const float2* __restrict__ cs, unsigned nslots, unsigned S,
-                                                   unsigned heads, unsigned D, size_t in_stride, size_t out_stride,
-                                                   float sign) {
-  const unsigned vph = D / 8;
-  const unsigned vh = threadIdx.x % vph, s0 = threadIdx.x / vph, per = blockDim.x / vph;
-  for (unsigned base = blockIdx.x * 2 * per; base < nslots; base += gridDim.x * 2 * per) {
-    Vec16 v[2];
-    unsigned t[2], h[2];
-    bool ok[2];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const unsigned g = base + s0 + j * per;
-      ok[j] = g < nslots;
-      t[j] = g / heads;
-      h[j] = g - t[j] * heads;
-      if (ok[j]) v[j] = ld_stream(in + (size_t)t[j] * in_stride + h[j] * D + vh * 8);
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      if (!ok[j]) continue;
-      const unsigned pos = t[j] % S;
-      const float4* c = reinterpret_cast<const float4*>(cs + (size_t)pos * (D / 2) + vh * 4);
-      const float4 c0 = c[0], c1 = c[1];
-      const float cx[4] = {c0.x, c0.z, c1.x, c1.z}, sy[4] = {c0.y, c0.w, c1.y, c1.w};
-      float f[8], o[8];
-      P8::unpack(v[j], f);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float sn = sy[k] * sign;
-        o[2 * k] = f[2 * k] * cx[k] - f[2 * k + 1] * sn;
-        o[2 * k + 1] = f[2 * k] * sn + f[2 * k + 1] * cx[k];
-      }
-      st_stream(out + (size_t)t[j] * out_stride + h[j] * D + vh * 8, P8::pack(o));
-    }
-  }
-}
-
+//
 // RoPE + q/k/v split (dir 0: packed qkv projection -> rotated q, rotated k, v) and its backward (dir 1: dq, dk, dv in ANY
 // [B, S, H, D] stride order -> inverse-rotated packed d_qkv) as ONE launch: every (token, head) slot of the packed row is
 // read once and written once; the v heads are a plain copy. Replaces two rope launches plus the library's strided copy of
@@ -581,29 +550,6 @@ __global__ void __launch_bounds__(512, 2) diloco_outer_kernel(T* __restrict__ pa
   }
 }
 
-// sum of squares of a bf16 buffer -> out[0] (+=), for grad-norm clipping
-__global__ void __launch_bounds__(512) sumsq_kernel(const bf16* __restrict__ g, size_t n,
-                                                    float* __restrict__ out) {
-  __shared__ float red[32];
-  const size_t nvec = n / 8;
-  float s = 0.f;
-  for (size_t v = blockIdx.x * (size_t)blockDim.x + threadIdx.x; v < nvec;
-       v += (size_t)gridDim.x * blockDim.x) {
-    float f[8];
-    P8::unpack(ld_stream(g + v * 8), f);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) s += f[k] * f[k];
-  }
-  if (blockIdx.x == 0) {
-    for (size_t k = nvec * 8 + threadIdx.x; k < n; k += blockDim.x) {
-      const float x = __bfloat162float(g[k]);
-      s += x * x;
-    }
-  }
-  s = block_sum(s, red);
-  if (threadIdx.x == 0) atomicAdd(out, s);
-}
-
 // ------------------------------- heal copy ----------------------------------
 // Live-recovery transport: stream state_dict shards GPU->GPU over NVLink from
 // inside a kernel (reference moves them GPU->CPU->TCP->CPU->GPU,
@@ -662,73 +608,49 @@ static int grid_for(size_t work_items, int threads, int cap = kNumSMs * 8) {
   return (int)g;
 }
 
-// (TPB, NV) for a row of nvec 16 B vectors: the tuned CTA size if NV <= 4 covers the row, else the next larger CTA.
-static void rms_shape(int nvec, int bwd, int& tpb, int& nv) {
-  for (tpb = g_rms_tpb[bwd]; tpb <= 512; tpb *= 2) {
-    const int need = (nvec + tpb - 1) / tpb;
-    nv = need <= 1 ? 1 : need <= 2 ? 2 : 4;
-    if (need <= kRmsMaxVec) return;
-  }
-  tpb = 512;
-  nv = kRmsMaxVec;
+// Calls f(NV, TPB) with the launch shape of a row of H elements whose CTA starts at TPB0 threads: V, the 16 B vectors per
+// thread the row needs at TPB0 rounded up to a power of two, selects NV = min(V, kRmsMaxVec) and TPB = TPB0 * V / NV.
+// Vs lists every V a row of up to 16384 elements reaches, so exactly the shapes that run are instantiated.
+template <int TPB0, int... Vs, typename F>
+static void rms_shape(int H, F&& f) {
+  int v = 1;
+  while (v * TPB0 < H / 8) v *= 2;
+  dispatch<Vs...>(v, [&](auto V) {
+    constexpr int NV = V < kRmsMaxVec ? V : kRmsMaxVec;
+    f(std::integral_constant<int, NV>{}, std::integral_constant<int, TPB0 * V / NV>{});
+  });
 }
-static int rms_grid(int rows, int bwd, int tpb) {
-  const int cap = kNumSMs * std::max(1, g_rms_cps[bwd] * 128 / tpb);
-  return rows < cap ? rows : cap;
+static int rms_grid(int rows, int ctas_per_sm_at_128, int tpb) {
+  return std::min(rows, kNumSMs * std::max(1, ctas_per_sm_at_128 * 128 / tpb));
 }
-
-void rmsnorm_tune(int bwd, int tpb, int prefetch, int ctas_per_sm_at_128) {
-  if (tpb != 128 && tpb != 256 && tpb != 512) throw std::runtime_error("rmsnorm_tune: tpb must be 128, 256 or 512");
-  bwd = bwd ? 1 : 0;
-  g_rms_tpb[bwd] = tpb;
-  g_rms_pf[bwd] = prefetch ? 1 : 0;
-  g_rms_cps[bwd] = std::max(1, ctas_per_sm_at_128);
-}
-
-#define RMS_DISPATCH(KERNEL, BWD, ...)                                                                         \
-  do {                                                                                                     \
-    auto go = [&](auto nvc, auto tpbc, auto pfc) {                                                         \
-      KERNEL<decltype(nvc)::value, decltype(tpbc)::value, decltype(pfc)::value><<<grid, tpb, 0, s>>>(__VA_ARGS__); \
-    };                                                                                                     \
-    auto by_pf = [&](auto nvc, auto tpbc) {                                                                \
-      if (g_rms_pf[BWD] && !(nv == 4 && tpb == 512)) go(nvc, tpbc, std::true_type{}); else go(nvc, tpbc, std::false_type{}); \
-    };                                                                                                     \
-    auto by_tpb = [&](auto nvc) {                                                                          \
-      if (tpb == 128) by_pf(nvc, std::integral_constant<int, 128>{});                                      \
-      else if (tpb == 256) by_pf(nvc, std::integral_constant<int, 256>{});                                 \
-      else by_pf(nvc, std::integral_constant<int, 512>{});                                                 \
-    };                                                                                                     \
-    if (nv == 1) by_tpb(std::integral_constant<int, 1>{});                                                 \
-    else if (nv == 2) by_tpb(std::integral_constant<int, 2>{});                                            \
-    else by_tpb(std::integral_constant<int, 4>{});                                                         \
-  } while (0)
 
 void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int rows, int H,
                         float eps, cudaStream_t s) {
   if (H % 8 || H > 8 * kRmsMaxVec * 512) throw std::runtime_error("rmsnorm: H must be %8 and <= 16384");
   if (rows == 0) return;  // a zero-CTA grid is an invalid launch
-  int tpb, nv;
-  rms_shape(H / 8, 0, tpb, nv);
-  const int grid = rms_grid(rows, 0, tpb);
-  RMS_DISPATCH(rmsnorm_fwd_kernel, 0, (const bf16*)x, (const bf16*)w, (bf16*)y, rstd, rows, H, eps);
+  rms_shape<kRmsFwdThreads, 1, 2, 4, 8, 16>(H, [&](auto NV, auto TPB) {
+    rmsnorm_fwd_kernel<NV, TPB><<<rms_grid(rows, kRmsFwdCtasPerSM, TPB), TPB.value, 0, s>>>(
+        (const bf16*)x, (const bf16*)w, (bf16*)y, rstd, rows, H, eps);
+  });
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
-// rows of the fp32 partial-dw buffer the caller must provide (an upper bound on the grid for any H)
-int rmsnorm_bwd_grid(int rows) { return rms_grid(rows, 1, 128); }
+// rows of the fp32 partial-dw buffer the caller must provide: the backward grid at its smallest CTA, the largest for any H
+int rmsnorm_bwd_grid(int rows) { return rms_grid(rows, kRmsBwdCtasPerSM, kRmsBwdThreads); }
 
 void rmsnorm_bwd_launch(const void* dy, const void* x, const void* w, const float* rstd, void* dx,
                         float* dw_partial, void* dw, int accumulate, int rows, int H,
                         cudaStream_t s, const void* dres) {
   if (H % 8 || H > 8 * kRmsMaxVec * 512) throw std::runtime_error("rmsnorm: H must be %8 and <= 16384");
-  int tpb, nv;
-  rms_shape(H / 8, 1, tpb, nv);
-  const int grid = rms_grid(rows, 1, tpb);
-  // no rows: skip the (zero-CTA, invalid) row launch; the column sum over zero partials still writes dw = 0 (or leaves
-  // it unchanged when accumulating), the gradient of an empty batch
-  if (rows > 0)
-    RMS_DISPATCH(rmsnorm_bwd_kernel, 1, (const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd, (bf16*)dx, dw_partial,
-                 (const bf16*)dres, rows, H);
+  int grid = 0;
+  rms_shape<kRmsBwdThreads, 1, 2, 4, 8>(H, [&](auto NV, auto TPB) {
+    grid = rms_grid(rows, kRmsBwdCtasPerSM, TPB);
+    // no rows: skip the (zero-CTA, invalid) row launch; the column sum over zero partials still writes dw = 0 (or
+    // leaves it unchanged when accumulating), the gradient of an empty batch
+    if (rows > 0)
+      rmsnorm_bwd_kernel<NV, TPB><<<grid, TPB.value, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd,
+                                                             (bf16*)dx, dw_partial, (const bf16*)dres, rows, H);
+  });
   colsum_kernel<<<(H + 31) / 32, 1024, 0, s>>>(dw_partial, grid, H, (bf16*)dw, accumulate);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
@@ -742,19 +664,6 @@ void swiglu_bwd_launch(const void* dy, const void* gu, void* dgu, size_t T, int 
   if (F % 8) throw std::runtime_error("swiglu: F must be a multiple of 8");
   swiglu_bwd_kernel<<<grid_for(T * (F / 8), 512), 512, 0, s>>>((const bf16*)dy, (const bf16*)gu,
                                                                (bf16*)dgu, T, F);
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void rope_launch(const void* in, void* out, const void* cs, size_t T, int S, int heads, int D,
-                 size_t in_stride, size_t out_stride, float sign, cudaStream_t s) {
-  if (D % 8 || D > 2048) throw std::runtime_error("rope: head_dim must be a multiple of 8 and <= 2048");
-  if (T * (size_t)heads >= (1ull << 31)) throw std::runtime_error("rope: tokens * heads must be < 2^31");
-  if (T == 0) return;
-  const unsigned vph = D / 8, per = 256 / vph, threads = per * vph;  // whole (token, head) slots per CTA pass
-  const unsigned nslots = (unsigned)(T * heads);
-  const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), kNumSMs * 8);
-  rope_kernel<<<grid, threads, 0, s>>>((const bf16*)in, (bf16*)out, (const float2*)cs, nslots, (unsigned)S,
-                                       (unsigned)heads, (unsigned)D, in_stride, out_stride, sign);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -821,11 +730,6 @@ void diloco_outer_launch(void* param, void* original, const void* grad, float* m
                                                 gate);
   });
   if (!known_dtype) throw std::runtime_error("diloco_outer: unsupported dtype");
-  TFT_CUDA_CHECK(cudaGetLastError());
-}
-
-void sumsq_launch(const void* g, size_t n, float* out, cudaStream_t s) {
-  sumsq_kernel<<<grid_for(n / 8 + 1, 512, kNumSMs * 4), 512, 0, s>>>((const bf16*)g, n, out);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -12,7 +12,7 @@ laid out for one-GPU-per-replica training in the 80 GB of an H100:
 * RMSNorm, RoPE(+qkv split), SwiGLU, softmax-cross-entropy and AdamW are
   hand-written sm_90a kernels (``torchft_b200/csrc/kernels/model_ops.cu``);
 * normalised activations and the SwiGLU product are recomputed in backward
-  instead of stored (see ``ops.fused.norm_linear`` / ``swiglu_linear``);
+  instead of stored (see ``ops.fused.norm_linear_res`` / ``swiglu_linear``);
 * attention is the SDPA library kernel (flash / cuDNN), causal, GQA.
 """
 

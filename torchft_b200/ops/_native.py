@@ -20,8 +20,8 @@ _err: Optional[BaseException] = None
 # kernels launched per wrapper call (for the benchmark's `gpu_launches` claim)
 _LAUNCHES_PER_CALL = {
     "allreduce": 1, "allreduce_nvls": 1, "q8_allreduce": 1, "q8_quantize": 1, "q8_dequantize": 1, "q8_reduce": 1,
-    "rmsnorm_fwd": 1, "rmsnorm_bwd": 2, "swiglu_fwd": 1, "swiglu_bwd": 1, "rope": 1, "rope_qkv": 1, "xent": 1,
-    "adamw": 1, "diloco_outer": 1, "sumsq": 1, "heal_copy": 1,
+    "rmsnorm_fwd": 1, "rmsnorm_bwd": 2, "swiglu_fwd": 1, "swiglu_bwd": 1, "rope_qkv": 1, "xent": 1,
+    "adamw": 1, "diloco_outer": 1, "heal_copy": 1,
     "q8_reduce_scatter": 1, "q8_slice_reduce": 1, "q8_gather_dequant": 1, "push_exchange": 1, "reduce_scatter": 1, "p2p": 1,
     "zero1_handshake": 1, "zero1_reduce": 1, "zero1_commit": 1, "zero1_update": 1,
 }

@@ -309,12 +309,6 @@ class FlatAdamW:
                     self.weight_decay, bc1, bc2, grad_scale, gp, stream.cuda_stream, max_blocks)
             ev.record(stream)
 
-    def grad_sumsq(self) -> torch.Tensor:
-        K = _native.load()
-        out = torch.zeros(1, dtype=torch.float32, device=self.g.device)
-        K.sumsq(self.g.data_ptr(), self.g.numel(), out.data_ptr(), _native.stream_ptr())
-        return out
-
     def state_dict(self) -> dict:
         return {"t": self.t, "master": self.master, "m": self.m, "v": self.v}
 
@@ -326,51 +320,6 @@ class FlatAdamW:
         self.p.copy_(self.master)
 
 
-class _NormLinear(torch.autograd.Function):
-    """y = rmsnorm(x, g) @ W^T, saving only (x, rstd): the normalised activation
-    is recomputed in backward by one extra RMSNorm pass instead of living in HBM
-    for the whole forward/backward (64 MB per call at 8k x 4096 bf16)."""
-
-    @staticmethod
-    def forward(ctx, x: torch.Tensor, g: torch.Tensor, W: torch.Tensor, eps: float) -> torch.Tensor:  # type: ignore[override]
-        K = _native.load()
-        x = x.contiguous()
-        H = x.shape[-1]
-        rows = x.numel() // H
-        n = torch.empty_like(x)
-        rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
-        K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, eps, _native.stream_ptr())
-        y = n.view(rows, H) @ W.t()
-        ctx.save_for_backward(x, g, W, rstd)
-        ctx.eps = eps
-        return y.view(x.shape[:-1] + (W.shape[0],))
-
-    @staticmethod
-    def backward(ctx, dy: torch.Tensor):  # type: ignore[override]
-        K = _native.load()
-        x, g, W, rstd = ctx.saved_tensors
-        H = x.shape[-1]
-        rows = x.numel() // H
-        sp = _native.stream_ptr()
-        dy2 = dy.reshape(rows, W.shape[0])
-        n = torch.empty_like(x)
-        K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, ctx.eps, sp)
-        dW = _wgrad(dy2, n.view(rows, H), W)
-        dn = dy2 @ W
-        dx = n  # reuse the recompute buffer for dx
-        grid = K.rmsnorm_bwd_grid(rows)
-        partial = torch.empty((grid, H), dtype=torch.float32, device=x.device)
-        dg = torch.empty_like(g)
-        K.rmsnorm_bwd(dn.data_ptr(), x.data_ptr(), g.data_ptr(), rstd.data_ptr(), dx.data_ptr(),
-                      partial.data_ptr(), dg.data_ptr(), False, rows, H, sp)
-        return dx, dg, dW, None
-
-
-def norm_linear(x: torch.Tensor, norm_weight: torch.Tensor, W: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
-    """``rmsnorm(x, norm_weight) @ W.T`` with the normalised activation recomputed in backward."""
-    return _NormLinear.apply(x, norm_weight, W, eps)
-
-
 class _NormLinearRes(torch.autograd.Function):
     """Pre-norm residual branch point: returns ``(x, rmsnorm(x, g) @ W^T)``.
 
@@ -379,6 +328,9 @@ class _NormLinearRes(torch.autograd.Function):
     gradient arrives here together with the branch gradient, and the RMSNorm backward kernel adds
     it while writing ``dx`` — autograd's separate ``dres + dbranch`` accumulation pass
     (3 x 64 MB of HBM traffic per norm at 8k x 4096) disappears.
+
+    Of the activations only ``(x, rstd)`` is saved: the normalised activation is recomputed in backward by one extra
+    RMSNorm pass instead of living in HBM for the whole forward/backward (64 MB per call at 8k x 4096).
     """
 
     @staticmethod
@@ -420,8 +372,8 @@ class _NormLinearRes(torch.autograd.Function):
 
 
 def norm_linear_res(x: torch.Tensor, norm_weight: torch.Tensor, W: torch.Tensor, eps: float = 1e-5) -> Tuple[torch.Tensor, torch.Tensor]:
-    """``(x, rmsnorm(x, norm_weight) @ W.T)``: like :func:`norm_linear` but also hands back the residual
-    stream so that its gradient is accumulated inside the RMSNorm backward kernel."""
+    """``(x, rmsnorm(x, norm_weight) @ W.T)`` with the normalised activation recomputed in backward. The first output
+    is the residual stream, handed back so that its gradient is accumulated inside the RMSNorm backward kernel."""
     return _NormLinearRes.apply(x, norm_weight, W, eps)
 
 
