@@ -5,6 +5,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <utility>
+
 namespace tft {
 
 struct PeerTable;
@@ -74,6 +76,9 @@ void q8_reduce_scatter_launch(const PeerTable& pt, StatusBlock* st, size_t off, 
 // model_ops.cu ---------------------------------------------------------------
 void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int rows, int H,
                         float eps, cudaStream_t s);
+// the same normalisation written as e4m3 y8 [rows, H] with one scale per row (fp8.cuh): fp8_rows(rmsnorm_fwd(x))
+void rmsnorm_fwd_fp8_launch(const void* x, const void* w, void* y8, float* yscale, float* rstd, int rows, int H,
+                            float eps, cudaStream_t s);
 int rmsnorm_bwd_grid(int rows);
 void rmsnorm_bwd_launch(const void* dy, const void* x, const void* w, const float* rstd, void* dx,
                         float* dw_partial, void* dw, int accumulate, int rows, int H,
@@ -92,5 +97,15 @@ void diloco_outer_launch(void* param, void* original, const void* grad, float* m
                          float mu, int nesterov, float alpha, const int* gate, cudaStream_t s);
 void heal_copy_launch(const void* table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                       int blocks, cudaStream_t s);
+
+// fp8.cu ---------------------------------------------------------------------
+// Row-scaled e4m3 operands of the fp8 block linears (format in fp8.cuh). fp8_rows: bf16 [rows, C] with row stride ld
+// (elements) -> e4m3 [rows, C] + fp32 scale per row. fp8_swiglu: packed gate|up [T, 2F] -> e4m3 silu(g) * u [T, F] +
+// scale per row. fp8_cols_t: W [N, K] -> e4m3 W^T [K, N] + scale per column of W; amax_ws is a u32 [K] workspace.
+void fp8_rows_launch(const void* x, size_t ld, void* q, float* scale, int rows, int C, cudaStream_t s);
+// (chunks of 16 per thread, threads) of the fp8_rows / fp8_swiglu CTA for a row of C elements
+std::pair<int, int> fp8_rows_shape(int C);
+void fp8_swiglu_launch(const void* gu, void* q, float* scale, int T, int F, cudaStream_t s);
+void fp8_cols_t_launch(const void* w, int N, int K, void* q, float* scale, uint32_t* amax_ws, cudaStream_t s);
 
 }  // namespace tft

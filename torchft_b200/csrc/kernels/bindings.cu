@@ -439,6 +439,11 @@ PYBIND11_MODULE(_K, m) {
                           float eps, uintptr_t s) {
     rmsnorm_fwd_launch(P<void>(x), P<void>(w), P<void>(y), P<float>(rstd), rows, H, eps, S(s));
   });
+  m.def("rmsnorm_fwd_fp8", [](uintptr_t x, uintptr_t w, uintptr_t y8, uintptr_t yscale, uintptr_t rstd, int rows, int H,
+                              float eps, uintptr_t s) {
+    rmsnorm_fwd_fp8_launch(P<void>(x), P<void>(w), P<void>(y8), P<float>(yscale), P<float>(rstd), rows, H, eps, S(s));
+  }, py::arg("x"), py::arg("w"), py::arg("y8"), py::arg("yscale"), py::arg("rstd"), py::arg("rows"), py::arg("H"),
+     py::arg("eps"), py::arg("stream"));
   m.def("rmsnorm_bwd_grid", &rmsnorm_bwd_grid);
   m.def("rmsnorm_bwd", [](uintptr_t dy, uintptr_t x, uintptr_t w, uintptr_t rstd, uintptr_t dx,
                           uintptr_t dw_partial, uintptr_t dw, bool accumulate, int rows, int H,
@@ -479,6 +484,16 @@ PYBIND11_MODULE(_K, m) {
                         alpha, P<const int>(gate), S(s));
   }, py::arg("param"), py::arg("original"), py::arg("grad"), py::arg("mom"), py::arg("n"), py::arg("dtype"), py::arg("lr"),
      py::arg("mu"), py::arg("nesterov"), py::arg("alpha"), py::arg("gate"), py::arg("stream"));
+  m.def("fp8_rows", [](uintptr_t x, size_t ld, uintptr_t q, uintptr_t scale, int rows, int C, uintptr_t s) {
+    fp8_rows_launch(P<void>(x), ld, P<void>(q), P<float>(scale), rows, C, S(s));
+  }, py::arg("x"), py::arg("ld"), py::arg("q"), py::arg("scale"), py::arg("rows"), py::arg("C"), py::arg("stream"));
+  m.def("fp8_rows_shape", &fp8_rows_shape, "(chunks per thread, threads) of the fp8_rows / fp8_swiglu CTA for a row of C");
+  m.def("fp8_swiglu", [](uintptr_t gu, uintptr_t q, uintptr_t scale, int T, int F, uintptr_t s) {
+    fp8_swiglu_launch(P<void>(gu), P<void>(q), P<float>(scale), T, F, S(s));
+  }, py::arg("gu"), py::arg("q"), py::arg("scale"), py::arg("T"), py::arg("F"), py::arg("stream"));
+  m.def("fp8_cols_t", [](uintptr_t w, int N, int K, uintptr_t q, uintptr_t scale, uintptr_t amax_ws, uintptr_t s) {
+    fp8_cols_t_launch(P<void>(w), N, K, P<void>(q), P<float>(scale), P<uint32_t>(amax_ws), S(s));
+  }, py::arg("w"), py::arg("N"), py::arg("K"), py::arg("q"), py::arg("scale"), py::arg("amax_ws"), py::arg("stream"));
   m.def("heal_copy", [](uintptr_t table_dev, int nentries, size_t total_chunks, size_t chunk_bytes,
                         int blocks, uintptr_t s) {
     heal_copy_launch(P<void>(table_dev), nentries, total_chunks, chunk_bytes, blocks, S(s));

@@ -14,6 +14,7 @@
 
 #include "api.h"
 #include "common.cuh"
+#include "fp8.cuh"
 
 namespace tft {
 
@@ -51,10 +52,13 @@ __device__ __forceinline__ float row_sum(float v, float (*red)[TPB / 32], int& p
   return r;
 }
 
-template <int NV, int TPB>
-__global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
-                                                          bf16* __restrict__ y, float* __restrict__ rstd, int rows,
-                                                          int H, float eps) {
+// FP8: instead of the bf16 y, the row's bf16-rounded values (the bytes the bf16 kernel stores) are quantised to e4m3 with
+// one scale per row (fp8.cuh): one more CTA-wide reduction, a max over the values already in registers. Its bytes equal
+// fp8_rows(rmsnorm_fwd(x)); rstd is written as by the bf16 kernel.
+template <int NV, int TPB, bool FP8>
+__device__ __forceinline__ void rmsnorm_fwd_rows(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                 void* __restrict__ y, float* __restrict__ yscale,
+                                                 float* __restrict__ rstd, int rows, int H, float eps) {
   constexpr bool PF = kRmsPrefetch<NV, TPB>;
   __shared__ float red[2][TPB / 32];
   const int nvec = H / 8;
@@ -91,16 +95,43 @@ __global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict
     ss = row_sum<TPB>(ss, red, parity);
     const float r = rsqrtf(ss / H + eps);
     if (threadIdx.x == 0) rstd[row] = r;
+    if constexpr (FP8) {
+      __shared__ uint32_t redm[2][TPB / 32];
+      Vec16 ov[NV];
+      uint32_t m = 0;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int v = threadIdx.x + i * TPB;
-      if (v < nvec) {
-        float f[8], wf[8], o[8];
-        P8::unpack(xv[i], f);
-        P8::unpack(wv[i], wf);
+      for (int i = 0; i < NV; ++i) {
+        if (threadIdx.x + i * TPB < nvec) {
+          float f[8], wf[8], o[8];
+          P8::unpack(xv[i], f);
+          P8::unpack(wv[i], wf);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) o[k] = f[k] * r * wf[k];
-        st_stream(y + (size_t)row * H + v * 8, P8::pack(o));
+          for (int k = 0; k < 8; ++k) o[k] = f[k] * r * wf[k];
+          ov[i] = P8::pack(o);
+          m = absmax_bits(ov[i], m);
+        }
+      }
+      m = row_max_bits<TPB>(m, redm, parity);
+      float inv;
+      const float sc = fp8_scale(m, inv);
+      if (threadIdx.x == 0) yscale[row] = sc;
+#pragma unroll
+      for (int i = 0; i < NV; ++i) {
+        const int v = threadIdx.x + i * TPB;
+        if (v < nvec) *reinterpret_cast<uint2*>((uint8_t*)y + (size_t)row * H + v * 8) = quant8(ov[i], inv, m >= kBf16Inf);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < NV; ++i) {
+        const int v = threadIdx.x + i * TPB;
+        if (v < nvec) {
+          float f[8], wf[8], o[8];
+          P8::unpack(xv[i], f);
+          P8::unpack(wv[i], wf);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) o[k] = f[k] * r * wf[k];
+          st_stream((bf16*)y + (size_t)row * H + v * 8, P8::pack(o));
+        }
       }
     }
     if (PF) {
@@ -110,6 +141,21 @@ __global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict
       load_row(next, xv);
     }
   }
+}
+
+template <int NV, int TPB>
+__global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                          bf16* __restrict__ y, float* __restrict__ rstd, int rows,
+                                                          int H, float eps) {
+  rmsnorm_fwd_rows<NV, TPB, false>(x, w, y, nullptr, rstd, rows, H, eps);
+}
+
+// the fp8-output instance: e4m3 y8 [rows, H] and its scale per row
+template <int NV, int TPB>
+__global__ void __launch_bounds__(TPB) rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                          uint8_t* __restrict__ y8, float* __restrict__ yscale,
+                                                          float* __restrict__ rstd, int rows, int H, float eps) {
+  rmsnorm_fwd_rows<NV, TPB, true>(x, w, y8, yscale, rstd, rows, H, eps);
 }
 
 // dx = rstd * (dy*w - xhat * mean(dy*w*xhat)) (+ dres); dw_partial[block] += dy * xhat
@@ -631,6 +677,18 @@ void rmsnorm_fwd_launch(const void* x, const void* w, void* y, float* rstd, int 
   rms_shape<kRmsFwdThreads, 1, 2, 4, 8, 16>(H, [&](auto NV, auto TPB) {
     rmsnorm_fwd_kernel<NV, TPB><<<rms_grid(rows, kRmsFwdCtasPerSM, TPB), TPB.value, 0, s>>>(
         (const bf16*)x, (const bf16*)w, (bf16*)y, rstd, rows, H, eps);
+  });
+  TFT_CUDA_CHECK(cudaGetLastError());
+}
+
+void rmsnorm_fwd_fp8_launch(const void* x, const void* w, void* y8, float* yscale, float* rstd, int rows, int H,
+                            float eps, cudaStream_t s) {
+  if (H % 16 || H > 8 * kRmsMaxVec * 512) throw std::runtime_error("rmsnorm_fwd_fp8: H must be %16 and <= 16384");
+  if ((uintptr_t)y8 % 16) throw std::runtime_error("rmsnorm_fwd_fp8: the e4m3 output must be 16-byte aligned");
+  if (rows == 0) return;
+  rms_shape<kRmsFwdThreads, 1, 2, 4, 8, 16>(H, [&](auto NV, auto TPB) {
+    rmsnorm_fwd_kernel<NV, TPB><<<rms_grid(rows, kRmsFwdCtasPerSM, TPB), TPB.value, 0, s>>>(
+        (const bf16*)x, (const bf16*)w, (uint8_t*)y8, yscale, rstd, rows, H, eps);
   });
   TFT_CUDA_CHECK(cudaGetLastError());
 }

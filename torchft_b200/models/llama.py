@@ -45,6 +45,9 @@ class LlamaConfig:
     # "none": keep activations (fused recompute only); "full": checkpoint every block
     activation_checkpoint: str = "none"
     loss_chunk: int = 2048
+    # the forward and input-gradient GEMMs of the four block linears (wqkv, wo, w13, w2) on fp8 tensor cores with
+    # row-scaled e4m3 operands; weight gradients, the LM head, the embedding and attention stay bf16
+    fp8_linears: bool = False
 
     @property
     def head_dim(self) -> int:
@@ -94,16 +97,17 @@ class Block(nn.Module):
         B, S, d = x.shape
         # residual stream is threaded through the norm nodes (norm_linear_res) and added in the
         # projection GEMMs' epilogues: no standalone elementwise add in forward or backward
-        x, qkv = fused.norm_linear_res(x, self.attention_norm, self.wqkv, cfg.norm_eps)
+        fp8 = cfg.fp8_linears
+        x, qkv = fused.norm_linear_res(x, self.attention_norm, self.wqkv, cfg.norm_eps, fp8=fp8)
         q, k, v = fused.rope_qkv(qkv.view(B * S, -1), cs, B, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
         o = F.scaled_dot_product_attention(
             q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True,
             enable_gqa=cfg.n_kv_heads != cfg.n_heads,
         )
         o = o.transpose(1, 2).reshape(B, S, d)
-        h = fused.linear(o, self.wo, res=x)
-        h, gu = fused.norm_linear_res(h, self.ffn_norm, self.w13, cfg.norm_eps)
-        return fused.swiglu_linear(gu, self.w2, res=h)
+        h = fused.linear(o, self.wo, res=x, fp8=fp8)
+        h, gu = fused.norm_linear_res(h, self.ffn_norm, self.w13, cfg.norm_eps, fp8=fp8)
+        return fused.swiglu_linear(gu, self.w2, res=h, fp8=fp8)
 
 
 class Llama(nn.Module):

@@ -35,6 +35,64 @@ def _chk(t: torch.Tensor, name: str) -> None:
         raise ValueError(f"{name} must be 16-byte aligned")
 
 
+# ------------------------------------------------------------------------------------------------- fp8 operands
+# The fp8 block linears run rowwise torch._scaled_mm: a e4m3 row-major with one fp32 scale per row ([M, 1]), b e4m3
+# column-major with one scale per column ([1, N]), fp32 accumulation (use_fast_accum=False), bf16 output. Scales are
+# powers of two computed from the tensor at hand on every call (csrc/kernels/fp8.cuh), so there is no scaling state.
+E4M3 = torch.float8_e4m3fn
+
+
+def fp8_rows(x2: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """bf16 ``[R, C]`` (any row stride, unit column stride) -> (e4m3 ``[R, C]``, fp32 scale ``[R, 1]``), one scale per
+    row. ``C`` must be a multiple of 16 and the rows 16-byte aligned."""
+    K = _native.load()
+    _chk(x2, "x")
+    if x2.dim() != 2 or x2.stride(1) != 1:
+        raise ValueError(f"fp8_rows takes a 2-D tensor with unit column stride, got shape {tuple(x2.shape)} strides {x2.stride()}")
+    R, C = x2.shape
+    q = torch.empty((R, C), dtype=E4M3, device=x2.device)
+    scale = torch.empty((R, 1), dtype=torch.float32, device=x2.device)
+    K.fp8_rows(x2.data_ptr(), x2.stride(0), q.data_ptr(), scale.data_ptr(), R, C, _native.stream_ptr())
+    return q, scale
+
+
+def fp8_cols_t(W: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """bf16 ``W [N, K]`` -> (e4m3 ``W^T [K, N]``, fp32 scale ``[1, K]``), one scale per column of ``W``: ``q.t()`` is the
+    column-major ``[N, K]`` operand of the input-gradient GEMM ``dy @ W``."""
+    K_ = _native.load()
+    W = W.contiguous()
+    _chk(W, "W")
+    N, Kd = W.shape
+    q = torch.empty((Kd, N), dtype=E4M3, device=W.device)
+    scale = torch.empty((1, Kd), dtype=torch.float32, device=W.device)
+    ws = torch.empty(Kd, dtype=torch.int32, device=W.device)
+    K_.fp8_cols_t(W.data_ptr(), N, Kd, q.data_ptr(), scale.data_ptr(), ws.data_ptr(), _native.stream_ptr())
+    return q, scale
+
+
+def _mm_fp8(a: Tuple[torch.Tensor, torch.Tensor], b: Tuple[torch.Tensor, torch.Tensor]) -> torch.Tensor:
+    """``a @ b`` of a quantised ``(e4m3 [M, K], scale [M, 1])`` and ``(e4m3 [K, N] column-major, scale [1, N])``."""
+    return torch._scaled_mm(a[0], b[0], scale_a=a[1], scale_b=b[1], out_dtype=torch.bfloat16, use_fast_accum=False)
+
+
+def _fwd_fp8(a: Tuple[torch.Tensor, torch.Tensor], W: torch.Tensor) -> torch.Tensor:
+    """Forward GEMM ``a @ W^T``: W quantised per output channel (per row), its row-major copy seen as W^T."""
+    qw, sw = fp8_rows(W)
+    return _mm_fp8(a, (qw.t(), sw.view(1, -1)))
+
+
+def _dgrad_fp8(dy2: torch.Tensor, W: torch.Tensor) -> torch.Tensor:
+    """Input-gradient GEMM ``dy @ W``: dy per token row, W per input channel (per column) from its transposed copy."""
+    qt, st = fp8_cols_t(W)
+    return _mm_fp8(fp8_rows(_rows_ok(dy2)), (qt.t(), st))
+
+
+def _rows_ok(t: torch.Tensor) -> torch.Tensor:
+    """``t`` itself when fp8_rows can read it in place (unit column stride, 16-byte aligned rows), else a copy."""
+    ok = t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0
+    return t if ok else t.contiguous()
+
+
 class _RMSNorm(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:  # type: ignore[override]
@@ -331,20 +389,31 @@ class _NormLinearRes(torch.autograd.Function):
 
     Of the activations only ``(x, rstd)`` is saved: the normalised activation is recomputed in backward by one extra
     RMSNorm pass instead of living in HBM for the whole forward/backward (64 MB per call at 8k x 4096).
+
+    With ``fp8`` the RMSNorm kernel writes the normalised activation as e4m3 with a scale per row (never as bf16), and
+    the forward and input-gradient GEMMs run on fp8 tensor cores; the weight gradient stays the bf16 GEMM.
     """
 
     @staticmethod
-    def forward(ctx, x: torch.Tensor, g: torch.Tensor, W: torch.Tensor, eps: float):  # type: ignore[override]
+    def forward(ctx, x: torch.Tensor, g: torch.Tensor, W: torch.Tensor, eps: float, fp8: bool = False):  # type: ignore[override]
         K = _native.load()
         x = x.contiguous()
         H = x.shape[-1]
         rows = x.numel() // H
-        n = torch.empty_like(x)
         rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
-        K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, eps, _native.stream_ptr())
-        y = n.view(rows, H) @ W.t()
+        if fp8:
+            q = torch.empty((rows, H), dtype=E4M3, device=x.device)
+            qs = torch.empty((rows, 1), dtype=torch.float32, device=x.device)
+            K.rmsnorm_fwd_fp8(x.data_ptr(), g.data_ptr(), q.data_ptr(), qs.data_ptr(), rstd.data_ptr(), rows, H, eps,
+                              _native.stream_ptr())
+            y = _fwd_fp8((q, qs), W)
+        else:
+            n = torch.empty_like(x)
+            K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, eps, _native.stream_ptr())
+            y = n.view(rows, H) @ W.t()
         ctx.save_for_backward(x, g, W, rstd)
         ctx.eps = eps
+        ctx.fp8 = fp8
         return x, y.view(x.shape[:-1] + (W.shape[0],))  # autograd re-wraps the returned input as a new node output
 
     @staticmethod
@@ -358,7 +427,7 @@ class _NormLinearRes(torch.autograd.Function):
         n = torch.empty_like(x)
         K.rmsnorm_fwd(x.data_ptr(), g.data_ptr(), n.data_ptr(), rstd.data_ptr(), rows, H, ctx.eps, sp)
         dW = _wgrad(dy2, n.view(rows, H), W)
-        dn = dy2 @ W
+        dn = _dgrad_fp8(dy2, W) if ctx.fp8 else dy2 @ W
         dx = n  # reuse the recompute buffer for dx
         grid = K.rmsnorm_bwd_grid(rows)
         partial = torch.empty((grid, H), dtype=torch.float32, device=x.device)
@@ -368,31 +437,45 @@ class _NormLinearRes(torch.autograd.Function):
             assert dres.dtype == x.dtype and dres.numel() == x.numel()
         K.rmsnorm_bwd(dn.data_ptr(), x.data_ptr(), g.data_ptr(), rstd.data_ptr(), dx.data_ptr(),
                       partial.data_ptr(), dg.data_ptr(), False, rows, H, sp, dres.data_ptr() if dres is not None else 0)
-        return dx, dg, dW, None
+        return dx, dg, dW, None, None
 
 
-def norm_linear_res(x: torch.Tensor, norm_weight: torch.Tensor, W: torch.Tensor, eps: float = 1e-5) -> Tuple[torch.Tensor, torch.Tensor]:
+def norm_linear_res(x: torch.Tensor, norm_weight: torch.Tensor, W: torch.Tensor, eps: float = 1e-5,
+                    fp8: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
     """``(x, rmsnorm(x, norm_weight) @ W.T)`` with the normalised activation recomputed in backward. The first output
-    is the residual stream, handed back so that its gradient is accumulated inside the RMSNorm backward kernel."""
-    return _NormLinearRes.apply(x, norm_weight, W, eps)
+    is the residual stream, handed back so that its gradient is accumulated inside the RMSNorm backward kernel.
+    ``fp8``: the forward and input-gradient GEMMs take row-scaled e4m3 operands (the weight gradient stays bf16)."""
+    return _NormLinearRes.apply(x, norm_weight, W, eps, fp8)
 
 
 class _SwiGLULinear(torch.autograd.Function):
-    """out = swiglu(gu) @ W2^T saving only gu (the [T, F] product is recomputed)."""
+    """out = swiglu(gu) @ W2^T saving only gu (the [T, F] product is recomputed). With ``fp8`` the SwiGLU kernel writes
+    the product as e4m3 with a scale per row (never as bf16) for the fp8 forward GEMM."""
 
     @staticmethod
-    def forward(ctx, gu: torch.Tensor, W2: torch.Tensor, res: Optional[torch.Tensor]) -> torch.Tensor:  # type: ignore[override]
+    def forward(ctx, gu: torch.Tensor, W2: torch.Tensor, res: Optional[torch.Tensor], fp8: bool = False) -> torch.Tensor:  # type: ignore[override]
         K = _native.load()
         gu = gu.contiguous()
         F2 = gu.shape[-1]
         F = F2 // 2
         T = gu.numel() // F2
-        a = torch.empty((T, F), dtype=gu.dtype, device=gu.device)
-        K.swiglu_fwd(gu.data_ptr(), a.data_ptr(), T, F, _native.stream_ptr())
-        # residual add rides in the GEMM epilogue (beta = 1) instead of a separate elementwise pass
-        out = a @ W2.t() if res is None else torch.addmm(res.reshape(T, W2.shape[0]), a, W2.t())
+        if fp8:
+            _chk(gu, "gate_up")
+            q = torch.empty((T, F), dtype=E4M3, device=gu.device)
+            qs = torch.empty((T, 1), dtype=torch.float32, device=gu.device)
+            K.fp8_swiglu(gu.data_ptr(), q.data_ptr(), qs.data_ptr(), T, F, _native.stream_ptr())
+            out = _fwd_fp8((q, qs), W2)
+            if res is not None:
+                # _scaled_mm has no beta epilogue: the residual costs one elementwise pass here
+                out.add_(res.reshape(T, W2.shape[0]))
+        else:
+            a = torch.empty((T, F), dtype=gu.dtype, device=gu.device)
+            K.swiglu_fwd(gu.data_ptr(), a.data_ptr(), T, F, _native.stream_ptr())
+            # residual add rides in the GEMM epilogue (beta = 1) instead of a separate elementwise pass
+            out = a @ W2.t() if res is None else torch.addmm(res.reshape(T, W2.shape[0]), a, W2.t())
         ctx.save_for_backward(gu, W2)
         ctx.has_res = res is not None
+        ctx.fp8 = fp8
         return out.view(gu.shape[:-1] + (W2.shape[0],))
 
     @staticmethod
@@ -407,24 +490,34 @@ class _SwiGLULinear(torch.autograd.Function):
         a = torch.empty((T, F), dtype=gu.dtype, device=gu.device)
         K.swiglu_fwd(gu.data_ptr(), a.data_ptr(), T, F, sp)
         dW2 = _wgrad(d2, a, W2)
-        da = torch.mm(d2, W2, out=a)  # reuse buffer
+        da = _dgrad_fp8(d2, W2) if ctx.fp8 else torch.mm(d2, W2, out=a)  # bf16: reuse buffer
         dgu = torch.empty_like(gu)
         K.swiglu_bwd(da.data_ptr(), gu.data_ptr(), dgu.data_ptr(), T, F, sp)
-        return dgu, dW2, (dout if ctx.has_res else None)
+        return dgu, dW2, (dout if ctx.has_res else None), None
 
 
-def swiglu_linear(gate_up: torch.Tensor, W2: torch.Tensor, res: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``(silu(gate) * up) @ W2.T (+ res)`` with the activation product recomputed in backward."""
-    return _SwiGLULinear.apply(gate_up, W2, res)
+def swiglu_linear(gate_up: torch.Tensor, W2: torch.Tensor, res: Optional[torch.Tensor] = None,
+                  fp8: bool = False) -> torch.Tensor:
+    """``(silu(gate) * up) @ W2.T (+ res)`` with the activation product recomputed in backward. ``fp8``: the forward and
+    input-gradient GEMMs take row-scaled e4m3 operands (the weight gradient stays bf16)."""
+    return _SwiGLULinear.apply(gate_up, W2, res, fp8)
 
 
 class _Linear(torch.autograd.Function):
     """y = x @ W^T whose weight gradient is written straight into the flat gradient buffer."""
 
     @staticmethod
-    def forward(ctx, x: torch.Tensor, W: torch.Tensor, res: Optional[torch.Tensor]) -> torch.Tensor:  # type: ignore[override]
+    def forward(ctx, x: torch.Tensor, W: torch.Tensor, res: Optional[torch.Tensor], fp8: bool = False) -> torch.Tensor:  # type: ignore[override]
         ctx.save_for_backward(x, W)
         ctx.has_res = res is not None
+        ctx.fp8 = fp8
+        if fp8:
+            x2 = x.reshape(-1, x.shape[-1])
+            y = _fwd_fp8(fp8_rows(_rows_ok(x2)), W)
+            if res is not None:
+                # _scaled_mm has no beta epilogue: the residual costs one elementwise pass here
+                y.add_(res.reshape(x2.shape[0], W.shape[0]))
+            return y.view(x.shape[:-1] + (W.shape[0],))
         if res is None:
             return x @ W.t()
         x2 = x.reshape(-1, x.shape[-1])
@@ -435,10 +528,12 @@ class _Linear(torch.autograd.Function):
         x, W = ctx.saved_tensors
         dy2 = dy.reshape(-1, dy.shape[-1])
         dW = _wgrad(dy2, x.reshape(-1, x.shape[-1]), W)
-        return (dy2 @ W).view(x.shape), dW, (dy if ctx.has_res else None)
+        dx = _dgrad_fp8(dy2, W) if ctx.fp8 else dy2 @ W
+        return dx.view(x.shape), dW, (dy if ctx.has_res else None), None
 
 
-def linear(x: torch.Tensor, W: torch.Tensor, res: Optional[torch.Tensor] = None) -> torch.Tensor:
+def linear(x: torch.Tensor, W: torch.Tensor, res: Optional[torch.Tensor] = None, fp8: bool = False) -> torch.Tensor:
     """``x @ W.T (+ res)`` with the wgrad GEMM writing directly into the flat gradient bucket; the
-    residual add, when given, is the GEMM's beta=1 epilogue."""
-    return _Linear.apply(x, W, res)
+    residual add, when given, is the GEMM's beta=1 epilogue. ``fp8``: the forward and input-gradient GEMMs take
+    row-scaled e4m3 operands (the weight gradient stays bf16) and the residual is a separate add."""
+    return _Linear.apply(x, W, res, fp8)

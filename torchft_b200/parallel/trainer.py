@@ -55,6 +55,17 @@ def no_decay_ranges(flat: FlatParams, module: nn.Module, select: Callable[[str, 
     return merge_ranges(out)
 
 
+def fp8_linears_from_env(default: bool = False) -> bool:
+    """``TORCHFT_B200_FP8``: ``"1"`` turns the fp8 block linears on, ``"0"`` turns them off, unset gives ``default``
+    (the model config's setting, off unless the config asks for it); any other value raises."""
+    v = os.environ.get("TORCHFT_B200_FP8")
+    if v is None:
+        return default
+    if v not in ("0", "1"):
+        raise ValueError(f"TORCHFT_B200_FP8 must be 0 or 1, got {v!r}")
+    return v == "1"
+
+
 class FaultTolerantTrainer:
     """Llama trainer over one replica group per GPU.
 
@@ -89,6 +100,11 @@ class FaultTolerantTrainer:
             partitioned optimizer state of the moments' type, advanced by every committed update (``None``: env
             ``TORCHFT_B200_Z1_EMA_DECAY``, unset = no EMA). :meth:`ema_weights` evaluates it. Not available on the
             classic all-reduce pipeline.
+        fp8_linears: run the forward and input-gradient GEMMs of the four block linears on fp8 tensor cores with
+            row-scaled e4m3 operands (``LlamaConfig.fp8_linears``); weight gradients, the LM head and attention stay
+            bf16, so the gradient buffer and the optimizer see bf16 exactly as without it. A model property: it applies
+            to every pipeline. ``None``: env ``TORCHFT_B200_FP8`` (``1`` on, ``0`` off, anything else raises; unset: the
+            config's ``fp8_linears``, off by default)
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
         overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
@@ -105,12 +121,17 @@ class FaultTolerantTrainer:
                  grad_accum_steps: int = 1, lr_lambda: Optional[Callable[[int], float]] = None,
                  lr_steps: Optional[int] = None,
                  no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None,
-                 moment_dtype: Optional[torch.dtype] = None, ema_decay: Optional[float] = None) -> None:
+                 moment_dtype: Optional[torch.dtype] = None, ema_decay: Optional[float] = None,
+                 fp8_linears: Optional[bool] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
         if activation_checkpoint is not None:
             cfg = dataclasses.replace(cfg, activation_checkpoint=activation_checkpoint)
+        if fp8_linears is None:
+            fp8_linears = fp8_linears_from_env(cfg.fp8_linears)
+        if bool(fp8_linears) != cfg.fp8_linears:
+            cfg = dataclasses.replace(cfg, fp8_linears=bool(fp8_linears))
         self.cfg = cfg
         self.backend = backend
         if zero1 is None:
