@@ -39,6 +39,16 @@ void zero1_reduce_launch(zero1::RSArgs a, int acc_mode, int blocks, int threads,
 void zero1_commit_launch(const zero1::CommitArgs& a, cudaStream_t stream);
 void zero1_update_launch(zero1::UpdArgs a, int moment_dtype, int blocks, int threads, cudaStream_t stream);
 
+// audit.cu -------------------------------------------------------------------
+// FT-ZeRO-1 replica audit: digests of the weights and the held state into each rank's z1_audit slots (table rows:
+// audit::DigestEntry), and the one-CTA comparison of every rank's slots that latches kErrDiverged (audit.cuh).
+namespace audit {
+struct CompareArgs;
+}  // namespace audit
+void z1_digest_launch(const void* table_dev, int nentries, size_t total_chunks, unsigned long long* slots, int blocks,
+                      cudaStream_t stream);
+void z1_audit_compare_launch(const audit::CompareArgs& a, cudaStream_t stream);
+
 // collectives.cu --------------------------------------------------------------
 // push exchange = all-gather / broadcast / all-to-all over staging slots (arrays have pt.world entries);
 // reduce-scatter; point-to-point pieces through per-pair mailboxes.

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "api.h"
+#include "audit.cuh"
 #include "common.cuh"
 #include "zero1.cuh"
 
@@ -64,6 +65,32 @@ class Status {
  private:
   StatusBlock* host_ = nullptr;
   StatusBlock* dev_ = nullptr;
+};
+
+// Host-pinned, device-mapped words a kernel writes and the host reads without a copy (the audit report).
+class MappedWords {
+ public:
+  explicit MappedWords(size_t n) : n_(n) {
+    TFT_CUDA_CHECK(cudaHostAlloc(&host_, n * 8, cudaHostAllocMapped | cudaHostAllocPortable));
+    std::memset((void*)host_, 0, n * 8);
+    void* d = nullptr;
+    TFT_CUDA_CHECK(cudaHostGetDevicePointer(&d, (void*)host_, 0));
+    dev_ = reinterpret_cast<unsigned long long*>(d);
+  }
+  ~MappedWords() {
+    if (host_) cudaFreeHost((void*)host_);
+  }
+  MappedWords(const MappedWords&) = delete;
+  MappedWords& operator=(const MappedWords&) = delete;
+  uintptr_t dev_ptr() const { return reinterpret_cast<uintptr_t>(dev_); }
+  size_t size() const { return n_; }
+  // the words as little-endian bytes (a snapshot; the caller orders it after the kernel that wrote them)
+  py::bytes read() const { return py::bytes(reinterpret_cast<const char*>(const_cast<unsigned long long*>(host_)), n_ * 8); }
+
+ private:
+  size_t n_;
+  volatile unsigned long long* host_ = nullptr;
+  unsigned long long* dev_ = nullptr;
 };
 
 class PeerTableH {
@@ -201,6 +228,12 @@ PYBIND11_MODULE(_K, m) {
       .def("grad_norm", &Status::grad_norm)
       .def("set_timeout_ms", &Status::set_timeout_ms)
       .def("timeout_ms", &Status::timeout_ms);
+
+  py::class_<MappedWords>(m, "MappedWords")
+      .def(py::init<size_t>())
+      .def("dev_ptr", &MappedWords::dev_ptr)
+      .def("size", &MappedWords::size)
+      .def("read", &MappedWords::read);
 
   py::class_<PeerTableH>(m, "PeerTable")
       .def(py::init<const std::vector<uintptr_t>&, const std::vector<uintptr_t>&, int, int>(),
@@ -353,6 +386,36 @@ PYBIND11_MODULE(_K, m) {
       py::arg("wd"), py::arg("replication"), py::arg("mode"), py::arg("table"), py::arg("soff"), py::arg("page_shift"),
       py::arg("coef"), py::arg("lr_tab"), py::arg("lr_steps"), py::arg("no_decay"), py::arg("moment_dtype"),
       py::arg("ema"), py::arg("ema_c"), py::arg("blocks"), py::arg("threads"), py::arg("stream"));
+
+  m.attr("Z1_DIGEST_CHUNK_WORDS") = audit::kDigestChunkWords;
+  m.attr("Z1_AUDIT_REPORT_HEADER") = audit::kReportHeader;
+  m.def(
+      "z1_digest",
+      [](uintptr_t table_dev, int nentries, size_t total_chunks, uintptr_t slots, int blocks, uintptr_t stream) {
+        z1_digest_launch(P<void>(table_dev), nentries, total_chunks, P<unsigned long long>(slots), blocks, S(stream));
+      },
+      py::arg("table"), py::arg("nentries"), py::arg("total_chunks"), py::arg("slots"), py::arg("blocks"),
+      py::arg("stream"));
+  m.def(
+      "z1_audit_compare",
+      [](const PeerTableH& pt, const Status& st, uintptr_t ok, const MappedWords& report, uint64_t seq, int nunits,
+         int stride, int k, int narrays, uintptr_t stream) {
+        audit::CompareArgs a{};
+        a.pt = pt.pt;
+        a.st = st.dev();
+        a.ok = P<const int>(ok);
+        a.report = P<unsigned long long>(report.dev_ptr());
+        a.seq = seq;
+        a.nunits = nunits;
+        a.stride = stride;
+        a.k = k;
+        a.narrays = narrays;
+        if (report.size() < (size_t)audit::kReportHeader + (size_t)pt.pt.world * ((size_t)nunits * stride + 1))
+          throw std::runtime_error("z1_audit_compare: the report is too small for this quorum's slots");
+        z1_audit_compare_launch(a, S(stream));
+      },
+      py::arg("pt"), py::arg("status"), py::arg("ok"), py::arg("report"), py::arg("seq"), py::arg("nunits"),
+      py::arg("stride"), py::arg("k"), py::arg("narrays"), py::arg("stream"));
 
   m.def(
       "push_exchange",

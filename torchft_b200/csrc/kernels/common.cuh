@@ -68,7 +68,7 @@ bool dispatch(T v, F&& f) {
 // ---------------------------------------------------------------------------
 struct StatusBlock {
   volatile uint32_t abort;        // host -> device: bail out of all spins
-  volatile uint32_t error;        // device -> host: 0 ok, 1 timeout, 2 aborted
+  volatile uint32_t error;        // device -> host: 0 ok, 1 timeout, 2 aborted, 3 replicas diverged (audit.cu)
   volatile uint32_t error_rank;   // peer we were waiting for when we gave up
   volatile uint32_t error_seq;    // low 32 bits of the flag we waited for
   volatile uint64_t timeout_ns;   // host -> device: spin budget per wait
@@ -82,7 +82,7 @@ struct StatusBlock {
 };
 constexpr uint32_t kVerdictRing = 64;
 
-enum ErrCode : uint32_t { kOk = 0, kErrTimeout = 1, kErrAborted = 2 };
+enum ErrCode : uint32_t { kOk = 0, kErrTimeout = 1, kErrAborted = 2, kErrDiverged = 3 };
 
 // One per rank, allocated inside the symmetric segment so peers can write it.
 // sig[channel][block][src_rank]; 64-bit epoch-tagged sequence numbers:

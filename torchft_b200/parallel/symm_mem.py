@@ -942,6 +942,22 @@ class SymmetricComm:
             if self._world > 1:
                 self._handshake(1, True, _CH_HEAL, _native.stream_ptr(stream))
 
+    def z1_audit_compare_(self, segment: str, report: Any, seq: int, nunits: int, stride: int, k: int, narrays: int,
+                          stream: Optional[torch.cuda.Stream] = None) -> None:
+        """The FT-ZeRO-1 audit's comparison: one handshake on the channel of :meth:`zero1_barrier_` (every rank's digests
+        into ``segment`` are complete), then one CTA that copies every rank's slots and update count into the
+        host-mapped ``report`` (``_K.MappedWords``) with ``seq``, compares the weights digests of the ranks at the highest
+        update count and the state digests of each slice's holders (``k > 1``), and latches ``kErrDiverged`` on any
+        disagreement. Every rank calls it at the same point of its FT-ZeRO-1 launches; never at world 1."""
+        with self._lock:
+            if not self._configured:
+                raise RuntimeError("SymmetricComm is not configured")
+            sp = _native.stream_ptr(stream)
+            self._handshake(1, True, _CH_HEAL, sp)
+            self._K.z1_audit_compare(self._tables[segment], self._status, self._z1_ok(1), report, int(seq), int(nunits),
+                                     int(stride), int(k), int(narrays), sp)
+            self.launches += 1
+
     # ------------------------------------------------------------------ status
     def abort(self) -> None:
         """Make every in-flight / future kernel wait bail out immediately."""
@@ -954,6 +970,9 @@ class SymmetricComm:
         code, peer, seq = self._status.error()
         if code == 0:
             return None
+        if code == 3:
+            return RuntimeError(f"FT-ZeRO-1 audit: replicas or holders of a slice diverged (lowest quorum rank "
+                                f"involved: {peer}, audit {seq})")
         what = {1: "timeout", 2: "aborted"}.get(code, f"error {code}")
         return RuntimeError(f"peer-memory collective {what} waiting for replica rank {peer} (seq {seq})")
 

@@ -100,6 +100,10 @@ class FaultTolerantTrainer:
             partitioned optimizer state of the moments' type, advanced by every committed update (``None``: env
             ``TORCHFT_B200_Z1_EMA_DECAY``, unset = no EMA). :meth:`ema_weights` evaluates it. Not available on the
             classic all-reduce pipeline.
+        audit_every: FT-ZeRO-1: every ``N``-th update since the last quorum change, check on the device that every
+            replica holds the same bf16 weights and the holders of each slice the same optimizer state; a disagreement
+            fails the next step on every replica, and the next quorum repairs it (``Zero1Optimizer``). ``None``: env
+            ``TORCHFT_B200_Z1_AUDIT_EVERY``, unset = 0, off. Not available on the classic all-reduce pipeline.
         fp8_linears: run the forward and input-gradient GEMMs of the four block linears on fp8 tensor cores with
             row-scaled e4m3 operands (``LlamaConfig.fp8_linears``); weight gradients, the LM head and attention stay
             bf16, so the gradient buffer and the optimizer see bf16 exactly as without it. A model property: it applies
@@ -122,7 +126,7 @@ class FaultTolerantTrainer:
                  lr_steps: Optional[int] = None,
                  no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None,
                  moment_dtype: Optional[torch.dtype] = None, ema_decay: Optional[float] = None,
-                 fp8_linears: Optional[bool] = None) -> None:
+                 fp8_linears: Optional[bool] = None, audit_every: Optional[int] = None) -> None:
         self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)
         cfg = CONFIGS[model] if isinstance(model, str) else model
@@ -152,6 +156,8 @@ class FaultTolerantTrainer:
             raise ValueError("moment_dtype needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         if ema_decay is not None and not self.zero1:
             raise ValueError("ema_decay needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if audit_every is not None and audit_every and not self.zero1:
+            raise ValueError("audit_every needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         self._in_ema = False  # inside ema_weights(): the model holds the EMA weights
         if lr_lambda is not None and lr_steps is None:
             raise ValueError("lr_lambda needs lr_steps, the length of the schedule")
@@ -184,7 +190,8 @@ class FaultTolerantTrainer:
             self.zopt = Zero1Optimizer(self.pg, numel, lr=lr, replication=replication, blocks=optimizer_blocks or None,
                                        compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
                                        grad_accum_steps=self.grad_accum_steps, lr_lambda=lr_lambda,
-                                       lr_steps=lr_steps or 0, moment_dtype=moment_dtype, ema_decay=ema_decay)
+                                       lr_steps=lr_steps or 0, moment_dtype=moment_dtype, ema_decay=ema_decay,
+                                       audit_every=audit_every)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:

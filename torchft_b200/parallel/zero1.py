@@ -47,7 +47,8 @@ __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "
            "clip_threshold", "accum_offsets", "accum_elements", "accum_mode", "newest_complete_step", "ckpt_read_plan",
            "lr_schedule_table", "split_no_decay", "schedule_digest", "check_moment_agreement", "moment_type", "sr_bits", "bf16_sr",
            "sr_bits_ema", "bf16_sr_ema", "ema_decay_value", "ema_coefficient", "ema_step", "ema_record", "check_ema_agreement",
-           "split_ema_reads"]
+           "split_ema_reads", "z1_digest", "audit_every_value", "audit_stride", "decode_audit_report", "audit_findings",
+           "audit_seed_source"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 CONVERT_CHUNK = 1 << 24  # restore into the other moment type: elements converted per device temporary
@@ -251,6 +252,148 @@ def split_ema_reads(reads: Sequence[Tuple[Any, int, int, int]]) -> Tuple[List[Tu
     have = [r for r in reads if "ema" in r[0]]
     seed = merge_ranges([(lo, hi) for h, _, lo, hi in reads if "ema" not in h])
     return have, seed
+
+
+# --------------------------------------------------------------------------- replica audit
+AUDIT_SEEDS = {"weights": 0x5851F42D4C957F2D, "master": 0x14057B7EF767814F, "m": 0x2545F4914F6CDD1D,
+               "v": 0x27BB2EE687B0B0FD, "ema": 0x369DEA0F31A53F85}  # seed_A of z1_digest per array
+AUDIT_ARRAYS = ("master", "m", "v", "ema")  # the state arrays in slot order (the EMA only when kept)
+AUDIT_GOLDEN = 0x9E3779B97F4A7C15
+
+
+def _fmix64(x: Any) -> Any:
+    import numpy as np
+
+    with np.errstate(over="ignore"):
+        x = x ^ (x >> np.uint64(33))
+        x = x * np.uint64(0xFF51AFD7ED558CCD)
+        x = x ^ (x >> np.uint64(33))
+        x = x * np.uint64(0xC4CEB9FE1A85EC53)
+        return x ^ (x >> np.uint64(33))
+
+
+def z1_digest(data: Any, word0: int, seed: int) -> int:
+    """The audit digest of a range of one partitioned array: ``data`` is the byte image of the range (any numpy array,
+    read as its bytes, a multiple of 8 bytes) and ``word0`` the GLOBAL index of its first 8-byte word (word ``i`` is bytes
+    ``[8 i, 8 i + 8)`` of the flat vector's image). The result is ``sum fmix64(w ^ (i * 0x9E3779B97F4A7C15 + seed))``
+    over the little-endian words ``w`` at global index ``i``, mod 2**64, with murmur3's 64-bit finaliser ``fmix64``.
+    This is the specification of ``z1_digest_kernel`` (``csrc/kernels/audit.cu``), which returns the same bits:
+
+    * It does not depend on grid, order or thread: wraparound integer addition is associative and commutative.
+    * Flat and paged state give the same digest: the index is global, and a page is a multiple of 8 elements, so no
+      word straddles a page.
+    * Any change confined to one word changes the digest, since ``fmix64`` (and the xor with a fixed value) is a
+      bijection. Changes of two or more words collide with probability about 2**-64.
+    * Every quantity is an exact integer, so the device reproduces it bit for bit."""
+    import numpy as np
+
+    w = np.ascontiguousarray(data).view(np.uint8).view("<u8").astype(np.uint64)
+    i = np.arange(int(word0), int(word0) + w.size, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        x = _fmix64(w ^ (i * np.uint64(AUDIT_GOLDEN) + np.uint64(seed)))
+    return int(x.sum(dtype=np.uint64)) if x.size else 0
+
+
+def audit_every_value(audit_every: Optional[int]) -> int:
+    """The audit period :class:`Zero1Optimizer` uses: ``audit_every``, or env ``TORCHFT_B200_Z1_AUDIT_EVERY`` when it is
+    ``None`` (unset or empty: 0, no audit). Negative values raise ``ValueError``."""
+    if audit_every is None:
+        env = os.environ.get("TORCHFT_B200_Z1_AUDIT_EVERY", "").strip()
+        audit_every = int(env) if env else 0
+    if int(audit_every) != audit_every or audit_every < 0:
+        raise ValueError(f"audit_every must be an integer >= 0 (0: no audit), got {audit_every}")
+    return int(audit_every)
+
+
+def audit_stride(replication: int) -> int:
+    """Slots per unit in the ``z1_audit`` segment: the weights digest, then one per (held slice ``j < k``, array)."""
+    return 1 + min(int(replication), 8) * len(AUDIT_ARRAYS)
+
+
+def decode_audit_report(raw: bytes, nunits: int, stride: int, narrays: int, k: int) -> Dict[str, Any]:
+    """The compare kernel's host-mapped report as ``{seq, mismatches, world, t, weights, state}``: ``t[r]`` is rank
+    ``r``'s update count, ``weights[r][u]`` its weights digest of unit ``u`` and ``state[r][u][j][a]`` its digest of
+    array ``a`` (``AUDIT_ARRAYS`` order) of its ``j``-th held slice, slice ``r - j``."""
+    import numpy as np
+
+    w = np.frombuffer(raw, dtype="<u8")
+    seq, mismatches, world, n = (int(x) for x in w[:4])
+    rep: Dict[str, Any] = {"seq": seq, "mismatches": mismatches, "world": world, "t": [], "weights": [], "state": []}
+    if world == 0:
+        return rep
+    assert n == nunits * stride + 1, "the report was written for another slot layout"
+    slots = w[4:4 + world * n].reshape(world, n)
+    for r in range(world):
+        rep["t"].append(int(slots[r, -1]))
+        rep["weights"].append([int(slots[r, u * stride]) for u in range(nunits)])
+        rep["state"].append([[[int(slots[r, u * stride + 1 + j * narrays + a]) for a in range(narrays)] for j in range(k)]
+                             for u in range(nunits)])
+    return rep
+
+
+def _outside_majority(digests: Dict[int, Any]) -> List[int]:
+    """The ranks whose digest is not that of a strict majority (all of them when there is none)."""
+    counts: Dict[Any, int] = {}
+    for d in digests.values():
+        counts[d] = counts.get(d, 0) + 1
+    top = max(counts, key=lambda d: counts[d])
+    if 2 * counts[top] <= len(digests):
+        return sorted(digests)
+    return sorted(r for r, d in digests.items() if d != top)
+
+
+def audit_seed_source(published: Dict[int, Dict[str, Any]]) -> int:
+    """The rank whose bf16 weights the holders of a slice that a diverged audit condemned re-seed it from: the lowest
+    rank of the new quorum at its highest update count. Every rank reads the same published records, so every rank picks
+    the same one; a joiner (behind, and about to be healed) is never picked."""
+    tmax = max(int(p["t"]) for p in published.values())
+    return min(r for r, p in published.items() if int(p["t"]) == tmax)
+
+
+def audit_findings(report: Dict[str, Any], layout: ShardLayout, world: int) -> Tuple[List[Dict[str, Any]], Dict[int, List[Range]]]:
+    """What a decoded audit report (:func:`decode_audit_report`) of a quorum of ``world`` ranks says: the findings, one
+    per group whose digests disagree, as ``{unit, array, slice, ranks, t}`` (``slice`` is ``None`` for the weights), and
+    per rank the ranges it must stop claiming. Only ranks at the quorum's highest update count are compared.
+
+    For each (unit, slice, array) whose holders disagree, the holders outside a strict majority drop the slice; with no
+    strict majority (e.g. ``k = 2``) every holder drops it, and the next re-shard re-seeds it. Weights mismatches drop
+    nothing: the first update of the next quorum re-broadcasts every unit from the master weights.
+
+    A rank whose row is all zeros (its next audit's memset ran before this rank's compare read it, which a rank whose
+    error is already latched can do) is compared as a holder whose digests match nobody, not left out: so a report with
+    zeroed rows makes every other rank drop at least what the complete report would, never less."""
+    t = report["t"]
+    drops: Dict[int, List[Range]] = {r: [] for r in range(world)}
+    findings: List[Dict[str, Any]] = []
+    if not t:
+        return findings, drops
+    tmax = max(t)
+    zeroed = {r for r in range(world) if not any(report["weights"][r])}  # a unit's digest is 0 with probability 2**-64
+    part = [r for r in range(world) if t[r] == tmax or r in zeroed]
+
+    def digest(x: int, r: int) -> Any:
+        return ("zeroed", r) if r in zeroed else x
+
+    k = layout.k(world)
+    narrays = len(report["state"][0][0][0]) if k > 1 else 0
+    for u in range(len(layout.units)):
+        w = {r: digest(report["weights"][r][u], r) for r in part}
+        if len(set(w.values())) > 1:
+            findings.append({"unit": u, "array": "weights", "slice": None, "ranks": _outside_majority(w), "t": tmax})
+        if k < 2:
+            continue
+        for s in range(world):
+            lo, hi = layout.slice_bounds(u, world, s)
+            holders = [h for h in layout.holders(u, world, s) if h in part]
+            for a in range(narrays):
+                d = {h: digest(report["state"][h][u][(h - s) % world][a], h) for h in holders}
+                if len(set(d.values())) > 1:
+                    out = _outside_majority(d)
+                    findings.append({"unit": u, "array": AUDIT_ARRAYS[a], "slice": s, "ranks": out, "t": tmax})
+                    for h in out:
+                        if hi > lo:
+                            drops[h].append((lo, hi))
+    return findings, {r: merge_ranges(x) for r, x in drops.items()}
 
 
 # --------------------------------------------------------------------------- interval arithmetic
@@ -651,6 +794,17 @@ class Zero1Optimizer:
             the update kernel after every committed update, ``ema + fp32(1 - d) * (w' - ema)``; re-shards, heals and
             checkpoints carry it; it is seeded from the weights wherever the master weights are. :meth:`ema_weights`
             swaps it into ``param`` for evaluation. Every replica of a quorum must use the same decay.
+        audit_every: every ``N``-th :meth:`update` since the last quorum change, audit replica consistency on the device
+            (``None``: env ``TORCHFT_B200_Z1_AUDIT_EVERY``, unset = 0, no audit). Behind the last unit's update, on the
+            commit stream, a kernel digests this rank's bf16 weights of every unit and each held slice of every state
+            array (:func:`z1_digest`) into its ``z1_audit`` slots; behind a handshake, a one-CTA kernel compares every
+            rank's slots: the weights of all ranks at the quorum's update count, and the state of each slice's holders.
+            A disagreement latches an error (``kErrDiverged``) that fails the next commit on every rank; at the next
+            quorum the holders outside a strict majority of a diverged slice stop claiming it (:func:`audit_findings`),
+            so it is pulled from the majority or re-seeded, and the weights are re-broadcast from the masters. With
+            ``k = 1`` only the weights are compared; at world 1 nothing is audited. ``audits``, ``divergences`` and
+            ``last_audit`` (the decoded report, :meth:`audit_report`) tell what it found. Every replica of a quorum must
+            use the same period.
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
@@ -660,7 +814,7 @@ class Zero1Optimizer:
                  max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1,
                  lr_lambda: Optional[Callable[[int], float]] = None, lr_steps: int = 0,
                  no_decay: Sequence[Range] = (), moment_dtype: Optional[torch.dtype] = None,
-                 ema_decay: Optional[float] = None) -> None:
+                 ema_decay: Optional[float] = None, audit_every: Optional[int] = None) -> None:
         from torchft_b200.ops import _native
 
         self.moment_dtype = moment_type(moment_dtype)
@@ -670,6 +824,18 @@ class Zero1Optimizer:
         self.ema: Optional[torch.Tensor] = None  # EMA of the weights, of the moment type, indexed like master
         self._ema_active = False                 # inside ema_weights(): param holds bf16(EMA)
         self.max_grad_norm = clip_threshold(max_grad_norm)
+        self.audit_every = audit_every_value(audit_every)
+        self.audits = 0                  # audits enqueued
+        self.divergences = 0             # audits whose report showed replicas or holders that disagree
+        self.last_audit: Optional[Dict[str, Any]] = None  # the last decoded report (audit_report)
+        self._audit_report: Any = None   # host-mapped words the compare kernel writes (allocated at the first audit)
+        self._audit_event: Optional[torch.cuda.Event] = None  # the last audit's compare has run
+        self._audit_seq = 0              # sequence number of the last audit enqueued
+        self._audit_seen = 0             # ... and of the last report a re-shard acted on
+        self._audit_quorums: Dict[int, Tuple[int, int]] = {}  # audit seq -> (rank, world) it ran at
+        self._audit_table: Optional[Tuple[Tuple[int, int], torch.Tensor, int, int]] = None  # digest table of (rank, world)
+        self._audit_dropped: List[Range] = []  # ranges the last re-shard stopped claiming after a diverged audit
+        self._updates_since_config = 0   # update() calls since the last quorum change: the same count on every rank
         # learning-rate schedule: fp32 rate of committed update i + 1 at index i (host copy and device table)
         self._lr_host = lr_schedule_table(lr, lr_lambda, lr_steps) if lr_lambda is not None else None
         self.no_decay: List[Range] = [(int(a), int(b)) for a, b in no_decay]  # split by unit in set_units
@@ -708,6 +874,10 @@ class Zero1Optimizer:
         self.grad_norm: Optional[torch.Tensor] = None  # clipping: device fp32 norm of the last commit
         self.last_grad_norm: Optional[float] = None    # clipping: host norm of the last resolved step
         self.nonfinite_steps = 0                       # clipping: steps vetoed because the norm was inf / nan
+        if self.audit_every:
+            # one u64 slot per (unit, weights | held slice x array), and the update count; peers read them in the compare
+            self._audit_stride = audit_stride(self._replication)
+            self._audit_slots = pg.alloc_symmetric("z1_audit", (GNORM_UNITS * self._audit_stride + 1) * 8)
         if self.max_grad_norm is not None:
             # symmetric segments are zero-filled at allocation, so the FlatParams.ALIGN padding of z1_grad, which no
             # wgrad GEMM writes, adds nothing to the norm. One fp64 partial per unit; peers read them in the commit.
@@ -773,6 +943,8 @@ class Zero1Optimizer:
         assert merge_ranges(units) == [(0, self.numel)] and total(units) == self.numel, "units must tile the flat buffer exactly"
         if self.max_grad_norm is not None and len(units) > GNORM_UNITS:
             raise ValueError(f"gradient clipping supports at most {GNORM_UNITS} units, got {len(units)}")
+        if self.audit_every and len(units) > GNORM_UNITS:
+            raise ValueError(f"the replica audit supports at most {GNORM_UNITS} units, got {len(units)}")
         if self.compact and self.capacity:
             raise RuntimeError("compact state: the units are fixed once the page pools are allocated")
         units = tuple((int(a), int(b)) for a, b in units)
@@ -869,7 +1041,7 @@ class Zero1Optimizer:
                 # a snapshot copy may still read the state that pulls, seeds, page reuse and heal are about to rewrite
                 self._snap_done.synchronize()
             names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ()) \
-                + (("z1_ema",) if self.ema is not None else ())
+                + (("z1_ema",) if self.ema is not None else ()) + (("z1_audit",) if self.audit_every else ())
             missing = [n for n in names if not self.comm.is_symmetric(n)]
             if missing:
                 # the kernels dereference peer pointers: every replica must construct its Zero1Optimizer before its first
@@ -877,7 +1049,10 @@ class Zero1Optimizer:
                 raise RuntimeError(f"FT-ZeRO-1 segments {missing} are not mapped on every replica of this quorum")
             if self.grad_accum_steps > 1:
                 self._accum_for(rank, world)
+            self._apply_audit()  # before publishing: the ranges a diverged audit condemned are not claimed
             me = {"t": self.t, "hold": self._holdings}
+            if self.audit_every:
+                me["audit"] = self.audit_every  # no audit publishes no key
             sched = self._schedule_digest()
             if sched is not None:
                 me["sched"] = sched
@@ -905,6 +1080,10 @@ class Zero1Optimizer:
                                    f"weight-decay exemptions (digest per rank: {digests})")
             check_moment_agreement(peers)
             check_ema_agreement(peers)
+            periods = {r: p.get("audit", 0) for r, p in peers.items()}
+            if len(set(periods.values())) > 1:
+                # the audit's handshake would pair with another kernel of a peer that does not audit at the same step
+                raise RuntimeError(f"zero1: the replicas of this quorum disagree on audit_every (per rank: {periods})")
             ckpt = self._ckpt_files(rank, peers)
             plans = plan_quorum(self.layout, world, peers, self._page_shift if self.compact else None, ckpt)
             plan = plans[rank]
@@ -939,6 +1118,14 @@ class Zero1Optimizer:
                     device_copy(entries, s, chunk_bytes=1 << 20)
                 if plan.reads:
                     self._read_state(plan.reads)  # nobody live holds these at T: the restored checkpoint does
+                seed_src = audit_seed_source(peers)
+                same_w = intersect_ranges(plan.lost, self._audit_dropped) if rank != seed_src else []
+                if same_w:
+                    # the holders of a diverged slice may hold different weights: every holder seeds it from the same
+                    # rank's copy, so their masters agree. That rank is at tmax, so no heal writes its param, and its
+                    # own updates wait for this quorum's first commit, which waits for this re-shard.
+                    src = self.comm.peer_pointers("z1_param")[seed_src]
+                    device_copy([(src + 2 * lo, self.param.data_ptr() + 2 * lo, 2 * (hi - lo)) for lo, hi in same_w], s)
                 self._seed(plan.lost)  # nobody holds these: re-seed from the replicated bf16 weights
             if self.compact:
                 s.synchronize()
@@ -958,6 +1145,10 @@ class Zero1Optimizer:
             self.t = plan.tmax
             self._holdings = plan.hold
             self._refresh_pending = world > 1
+            self._updates_since_config = 0
+            self._audit_dropped = []
+            if self.audit_every and world > 1:
+                self._audit_setup(rank, world)
             self._configured, self._disk = True, None
 
     def _state_arrays(self, prefix: str = "") -> List[Tuple[str, torch.Tensor]]:
@@ -1172,6 +1363,105 @@ class Zero1Optimizer:
                                         **sched, **state)
             if events is not None:
                 events[i].record(stream)
+        if self.audit_every:
+            self._updates_since_config += 1
+            if self.comm.world > 1 and self._updates_since_config % self.audit_every == 0:
+                self._audit(stream)
+
+    # ------------------------------------------------------------------ replica audit
+    def _audit(self, stream: torch.cuda.Stream) -> None:
+        """Enqueue one audit on ``stream`` behind the last unit's update and weight handshake: zero the slots, copy the
+        update count, digest (one launch), handshake and compare (see DESIGN.md for why this is race-free)."""
+        rank, world = self.comm.rank, self.comm.world
+        nunits, stride, narrays = len(self.layout.units), self._audit_stride, len(self._state_arrays())
+        n = nunits * stride + 1
+        assert self._audit_table is not None and self._audit_table[0] == (rank, world), "set up at the quorum change"
+        _, table, nentries, chunks = self._audit_table
+        sp = int(stream.cuda_stream)
+        slots = self._audit_slots.data_ptr()
+        self._K.memset_async(slots, 0, 8 * n, sp)
+        self._K.memcpy_async(slots + 8 * (n - 1), self.gate.data_ptr() + 4, 4, sp)  # t = gate[1], little-endian
+        self._K.z1_digest(table.data_ptr(), nentries, chunks, slots, max(1, min(chunks, self._K.NUM_SMS * 3)), sp)
+        self._audit_seq += 1
+        self.comm.z1_audit_compare_("z1_audit", self._audit_report, self._audit_seq, nunits, stride,
+                                    self.layout.k(world), narrays, stream)
+        self._audit_event = stream.record_event()
+        self._audit_quorums = {s: q for s, q in self._audit_quorums.items() if s > self._audit_seen}
+        self._audit_quorums[self._audit_seq] = (rank, world)
+        self.audits += 1
+
+    def _audit_setup(self, rank: int, world: int) -> None:
+        """At a quorum change: the host-mapped report (once, for up to 8 ranks) and the digest kernel's rows
+        (``audit::DigestEntry``) for this rank at ``(rank, world)``: the weights of every unit, and with ``k > 1`` each
+        state array over each held slice. The copy is synchronous, so it is made here and never inside :meth:`update`,
+        whose launches must not wait for the device; the arrays and the page table stay where they are."""
+        if self._audit_report is None:
+            n = len(self.layout.units) * self._audit_stride + 1
+            self._audit_report = self._K.MappedWords(self._K.Z1_AUDIT_REPORT_HEADER + 8 * n)
+        if self._audit_table is not None and self._audit_table[0] == (rank, world):
+            return
+        cw = int(self._K.Z1_DIGEST_CHUNK_WORDS)
+        rows: List[Tuple[int, ...]] = []
+        chunk0 = 0
+        k, stride = self.layout.k(world), self._audit_stride
+        table = self._table.data_ptr() if self._table is not None else 0
+
+        def add(base: int, es: int, paged: bool, lo: int, hi: int, seed: int, slot: int) -> None:
+            nonlocal chunk0
+            if hi <= lo:
+                return  # an empty slice: its slot stays 0 on every holder
+            nwords = (hi - lo) * es // 8
+            pbs = self._page_shift + es.bit_length() - 1 if paged else 0
+            rows.append((base, table if paged else 0, pbs, lo * es // 8, nwords, seed, slot, chunk0))
+            chunk0 += (nwords + cw - 1) // cw
+
+        for u, (lo, hi) in enumerate(self.layout.units):
+            add(self.param.data_ptr(), 2, False, lo, hi, AUDIT_SEEDS["weights"], u * stride)
+            if k < 2:
+                continue
+            for j in range(k):
+                a, b = self.layout.slice_bounds(u, world, (rank - j) % world)
+                for x, (name, arr) in enumerate(self._state_arrays()):
+                    add(arr.data_ptr(), arr.element_size(), bool(table), a, b, AUDIT_SEEDS[name],
+                        u * stride + 1 + j * len(self._state_arrays()) + x)
+        self._audit_table = ((rank, world), torch.tensor(rows, dtype=torch.int64).to(self.device), len(rows), chunk0)
+
+    def audit_report(self) -> Optional[Dict[str, Any]]:
+        """The report of the last audit whose compare ran (:func:`decode_audit_report`), after waiting for the last
+        audit on the host; ``None`` before the first audit. Also kept as ``last_audit``."""
+        if self._audit_event is None:
+            return None
+        self._audit_event.synchronize()
+        seq = int.from_bytes(self._audit_report.read()[:8], "little")
+        rank_world = self._audit_quorums.get(seq)
+        if rank_world is None:
+            return self.last_audit  # no compare of a recorded audit has run
+        k = self.layout.k(rank_world[1])
+        self.last_audit = decode_audit_report(self._audit_report.read(), len(self.layout.units), self._audit_stride,
+                                              len(self._state_arrays()), k)
+        self.last_audit["rank"] = rank_world[0]
+        return self.last_audit
+
+    def _apply_audit(self) -> None:
+        """At a quorum change: act once on a report that shows a divergence. Log each finding and stop claiming the
+        ranges :func:`audit_findings` gives this rank, if this rank was at the audited quorum's update count and is
+        still there."""
+        rep = self.audit_report()
+        if rep is None or rep["seq"] <= self._audit_seen:
+            return
+        self._audit_seen = rep["seq"]
+        if not rep["mismatches"]:
+            return
+        self.divergences += 1
+        findings, drops = audit_findings(rep, self.layout, rep["world"])
+        for f in findings:
+            logger.warning("zero1: audit %d: %s of unit %d%s differs on quorum ranks %s at update %d", rep["seq"],
+                           f["array"], f["unit"], "" if f["slice"] is None else f" slice {f['slice']}", f["ranks"], f["t"])
+        me = rep["rank"]
+        if self.t == max(rep["t"]) == rep["t"][me] and drops[me]:
+            logger.warning("zero1: this rank stops claiming %s after the audit", drops[me])
+            self._holdings = subtract_ranges(self._holdings, drops[me])
+            self._audit_dropped = drops[me]
 
     def _update_state(self, lo: int) -> Dict[str, int]:
         """The state arguments of ``zero1_update_`` for the unit that starts at element ``lo``. Full-size state passes
