@@ -1,13 +1,14 @@
-"""Plain-PyTorch fp32 reference of the Llama forward/backward (test oracle only).
+"""Plain-PyTorch reference of the Llama forward/backward (test oracle only), in fp32 by default.
 
 Numerics tests compare every hand-written kernel path in ``models/llama.py``
 against this eager implementation, which shares nothing with it except the
-parameter tensors.
+parameter tensors. In fp64 it is the exact model; in bf16 it is an independent
+implementation at the fused model's precision.
 """
 
 from __future__ import annotations
 
-from typing import Dict, Tuple
+from typing import Callable, Dict, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -18,26 +19,42 @@ def _rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
 
 
 def _rope(x: torch.Tensor, theta: float) -> torch.Tensor:
+    """Interleaved-pair rotation by the fp32 angles of ``ops.fused.rope_table``; cos and sin in fp64 for an fp64 ``x``,
+    else in fp32, and the rotation rounded once to ``x``'s dtype (complex bf16 does not exist)."""
     B, S, H, D = x.shape
     inv = 1.0 / (theta ** (torch.arange(0, D, 2, device=x.device, dtype=torch.float32) / D))
     ang = torch.outer(torch.arange(S, device=x.device, dtype=torch.float32), inv)
-    f = torch.polar(torch.ones_like(ang), ang)
-    xc = torch.view_as_complex(x.reshape(B, S, H, D // 2, 2))
-    return torch.view_as_real(xc * f[None, :, None, :]).reshape(B, S, H, D)
+    if x.dtype in (torch.float32, torch.float64):
+        a = ang.to(x.dtype)
+        f = torch.polar(torch.ones_like(a), a)
+        xc = torch.view_as_complex(x.reshape(B, S, H, D // 2, 2))
+        return torch.view_as_real(xc * f[None, :, None, :]).reshape(B, S, H, D)
+    c, s = ang.cos()[None, :, None, :], ang.sin()[None, :, None, :]
+    x0, x1 = x.float().reshape(B, S, H, D // 2, 2).unbind(-1)
+    return torch.stack((x0 * c - x1 * s, x0 * s + x1 * c), -1).reshape(B, S, H, D).to(x.dtype)
 
 
-def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor) -> Tuple[float, Dict[str, torch.Tensor]]:
-    """Returns (loss, {param_name: fp32 grad}) computed with eager fp32 PyTorch."""
+def _matmul_t(x: torch.Tensor, W: torch.Tensor) -> torch.Tensor:
+    return x @ W.t()
+
+
+def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor, dtype: torch.dtype = torch.float32,
+                   linear: Optional[Callable[[torch.Tensor, torch.Tensor], torch.Tensor]] = None
+                   ) -> Tuple[float, Dict[str, torch.Tensor]]:
+    """Returns (loss, {param_name: grad in ``dtype``}) computed with eager PyTorch in ``dtype``. ``linear(x, W)``, by
+    default ``x @ W.T``, computes the four block linears (wqkv, wo, w13, w2), e.g. with quantised operands."""
 
     cfg = model.cfg
-    P = {n: p.detach().float().requires_grad_() for n, p in model.named_parameters()}
+    if linear is None:
+        linear = _matmul_t
+    P = {n: p.detach().to(dtype).requires_grad_() for n, p in model.named_parameters()}
     B, S = tokens.shape
     x = F.embedding(tokens, P["tok_embeddings"])
     Hq, Hkv, D = cfg.n_heads, cfg.n_kv_heads, cfg.head_dim
     for i in range(cfg.n_layers):
         pre = f"layers.{i}."
         n = _rmsnorm(x, P[pre + "attention_norm"], cfg.norm_eps)
-        qkv = (n @ P[pre + "wqkv"].t()).view(B, S, Hq + 2 * Hkv, D)
+        qkv = linear(n, P[pre + "wqkv"]).view(B, S, Hq + 2 * Hkv, D)
         q, k, v = qkv[:, :, :Hq], qkv[:, :, Hq : Hq + Hkv], qkv[:, :, Hq + Hkv :]
         q, k = _rope(q, cfg.rope_theta), _rope(k, cfg.rope_theta)
         rep = Hq // Hkv
@@ -45,11 +62,11 @@ def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor) -> Tuple[
         v = v.repeat_interleave(rep, dim=2)
         o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True)
         o = o.transpose(1, 2).reshape(B, S, cfg.dim)
-        h = x + o @ P[pre + "wo"].t()
+        h = x + linear(o, P[pre + "wo"])
         n2 = _rmsnorm(h, P[pre + "ffn_norm"], cfg.norm_eps)
-        gu = n2 @ P[pre + "w13"].t()
+        gu = linear(n2, P[pre + "w13"])
         a = F.silu(gu[..., : cfg.ffn_dim]) * gu[..., cfg.ffn_dim :]
-        x = h + a @ P[pre + "w2"].t()
+        x = h + linear(a, P[pre + "w2"])
     hfin = _rmsnorm(x, P["norm"], cfg.norm_eps)
     logits = hfin @ P["output"].t()
     loss = F.cross_entropy(logits.view(B * S, -1), targets.reshape(-1))
