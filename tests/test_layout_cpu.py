@@ -69,7 +69,7 @@ def test_param_stages_tile_the_flat_buffer_in_forward_order():
 @pytest.mark.parametrize("world", [2, 3, 4, 8])
 def test_allreduce_plan_is_well_formed(world):
     comm = SymmetricComm.__new__(SymmetricComm)  # planning needs no device state
-    comm._force_plan, comm._world, comm._oneshot_max, comm._max_blocks = None, world, 256 << 10, 64
+    comm._force_plan, comm._world, comm._max_blocks = None, world, 64
     prev_algo = 0
     for k in range(4, 31):
         nbytes = 1 << k

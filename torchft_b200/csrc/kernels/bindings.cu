@@ -214,6 +214,7 @@ PYBIND11_MODULE(_K, m) {
   m.attr("SIGNAL_PAD_BYTES") = sizeof(SignalPad);
   m.attr("Q8_GROUP") = 512;
   m.attr("ZERO1_MAX_NO_DECAY") = kMaxNoDecay;
+  m.attr("ZERO1_MAX_BLOCKS") = kZero1MaxBlocks;
   m.attr("ZERO1_BF16_MOMENTS") = true;  // zero1_update takes moment_dtype = bf16
   m.attr("ZERO1_EMA") = true;           // zero1_update takes an EMA of the weights and mode 2
 

@@ -584,7 +584,7 @@ __global__ void __launch_bounds__(512, 2) zero1_update_kernel(UpdArgs a) {
 }
 
 void check_grid(int blocks, int threads, const char* who) {
-  if (blocks < 1 || blocks > kNumSMs * 32) throw std::runtime_error(std::string(who) + ": bad grid");
+  if (blocks < 1 || blocks > kZero1MaxBlocks) throw std::runtime_error(std::string(who) + ": bad grid");
   if (threads < 32 || threads > 512 || (threads & 31)) throw std::runtime_error(std::string(who) + ": bad block size");
 }
 

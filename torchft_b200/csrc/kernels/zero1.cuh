@@ -7,6 +7,9 @@
 namespace tft {
 
 constexpr int kMaxNoDecay = 4;  // weight-decay exemption ranges per unit
+// Grid cap of the reduce and update kernels. The reduce kernel's gradient norm takes one fp64 partial per CTA, so the
+// host sizes that scratch from this cap (exported as ZERO1_MAX_BLOCKS).
+constexpr int kZero1MaxBlocks = kNumSMs * 32;
 
 namespace zero1 {
 

@@ -104,7 +104,7 @@ class ProcessGroupB200(ProcessGroup):
 
     Args:
         timeout: spin budget of every in-kernel wait and of store operations.
-        staging_bytes: size of the staging buffer used for tensors outside symmetric memory (default 64 MB).
+        staging_bytes: size of the staging buffer used for tensors outside symmetric memory (default 256 MiB).
         device: CUDA device of this rank (default: current device).
     """
 

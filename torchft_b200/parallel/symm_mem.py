@@ -42,6 +42,9 @@ _CH_HEAL = 2
 _CH_USER = 3
 
 _ALIGN = 2 << 20  # segment sizes rounded to 2 MiB (the VMM allocation granularity on H100)
+_STAGING_BYTES = 256 << 20  # staging buffer for tensors that do not live in a symmetric segment
+_ONESHOT_MAX = 256 << 10  # one-shot/two-shot cross-over at 5 ranks and more; x4 at 3-4 ranks, x8 at 2
+_ONESHOT, _TWOSHOT, _NVLS = 0, 1, 2  # all-reduce algorithms (_plan)
 
 
 class _CAI:
@@ -101,7 +104,7 @@ class SymmetricComm:
         self._configured = False
         self._timeout = timeout
         if staging_bytes is None:
-            staging_bytes = int(os.environ.get("TORCHFT_B200_STAGING_MB", "256")) << 20
+            staging_bytes = _STAGING_BYTES
         self._staging_bytes = (staging_bytes + _ALIGN - 1) // _ALIGN * _ALIGN
         # the tail of the staging buffer holds one send/recv mailbox per source rank; collectives use the head
         self._mailbox_bytes = min(4 << 20, (self._staging_bytes // 4 // 8) & ~15)
@@ -110,17 +113,13 @@ class SymmetricComm:
         self._send_seq: Dict[int, int] = {}
         self._recv_seq: Dict[int, int] = {}
         self._pad_bytes = (self._K.SIGNAL_PAD_BYTES + 65535) // 65536 * 65536
-        self._max_blocks = max(1, min(int(os.environ.get("TORCHFT_B200_AR_BLOCKS", "64")), self._K.MAX_BLOCKS))
+        self._max_blocks = min(64, self._K.MAX_BLOCKS)  # two-shot CTA cap: leave SMs to the backward pass it overlaps
         self._q8_max_blocks = self._K.NUM_SMS  # phases A/C of the fp8 kernel are local HBM passes: use the whole chip
-        self._threads = int(os.environ.get("TORCHFT_B200_AR_THREADS", "512"))
-        self._oneshot_max = int(os.environ.get("TORCHFT_B200_ONESHOT_KB", "256")) << 10
+        self._threads = 512
         # "vmm": cuMemCreate-backed segments (survive exporter death, NVLS-capable); "ipc": cudaMalloc + cudaIpc
         self._mode = os.environ.get("TORCHFT_B200_SYMM", "ipc")
         self._nvls_enabled = os.environ.get("TORCHFT_B200_NVLS", "1") != "0"
-        # NVLS threshold; None = pick by world size at configure() (see _default_nvls_min)
-        env_nvls = os.environ.get("TORCHFT_B200_NVLS_MIN_KB")
-        self._nvls_min_env: Optional[int] = (int(env_nvls) << 10) if env_nvls is not None else None
-        self._nvls_min = self._nvls_min_env if self._nvls_min_env is not None else (1 << 62)
+        self._nvls_min = self._default_nvls_min(self._world)  # smallest multicast message; set per quorum by _install
         self._fdserver: Any = None
         self._peer_vmm: Dict[Tuple[str, int, str], Tuple[int, int, int]] = {}  # (host, pid, seg) -> (va, handle, size)
         self._mc: Dict[str, Tuple[int, int, int]] = {}  # segment -> (mc handle, multicast va, size)
@@ -296,7 +295,7 @@ class SymmetricComm:
         self._flag = max(floor, int(epoch) << 32) + 16
         self._rank, self._world, self._epoch = rank, world, int(epoch)
         self._send_seq, self._recv_seq = {}, {}
-        self._nvls_min = self._nvls_min_env if self._nvls_min_env is not None else self._default_nvls_min(world)
+        self._nvls_min = self._default_nvls_min(world)
 
     @staticmethod
     def virtual_world(world: int, segments: Dict[str, int], device: Optional[torch.device] = None,
@@ -433,26 +432,27 @@ class SymmetricComm:
         self._mc_gen, self._mc_members = "", ""
 
     # ------------------------------------------------------------- collectives
-    def _plan(self, nbytes: int) -> Tuple[int, int]:
-        """(algo, blocks): identical on every rank for a given message size.
+    def _plan(self, nbytes: int, multicast: bool = False) -> Tuple[int, int]:
+        """(algo, blocks) of an all-reduce of ``nbytes``: identical on every rank for a given message size.
+        ``multicast``: the message lies in a segment :meth:`_mc_base` sends through the switch; ``_force_plan``
+        (algo 0 or 1) overrides everything.
 
         Thresholds from a ``bench/comm_tune.py`` sweep on an earlier NVLink generation; not re-measured on H100. One-shot (each
         rank reads the whole message from every peer; two flag exchanges, no write-back hop)
         wins while (world-1) x bytes still fits the latency budget; it likes MANY small CTAs
         (16 KB each, <= 64 KB because results stay in registers across the closing barrier).
-        Two-shot moves 2(N-1)/N of the bytes using both link directions; one CTA per 64 KB up
-        to ``max_blocks`` (a comm kernel that overlaps backward should not take every SM).
+        Two-shot moves 2(N-1)/N of the bytes using both link directions, NVLS (1 + 1/N); both take one CTA per 64 KB,
+        from 8 up to ``_max_blocks`` (a comm kernel that overlaps backward should not take every SM).
         """
         if self._force_plan is not None:
             return self._force_plan
         w = max(self._world, 2)
-        oneshot_max = self._oneshot_max * (8 if w == 2 else (4 if w <= 4 else 1))  # W=8: two-shot wins from 256 KB
-        if nbytes <= oneshot_max:
+        oneshot_max = _ONESHOT_MAX * (8 if w == 2 else (4 if w <= 4 else 1))  # W=8: two-shot wins from 256 KB
+        if not multicast and nbytes <= oneshot_max:
             blocks = max(1, min(128, (nbytes + (16 << 10) - 1) // (16 << 10)))
             if (nbytes + blocks - 1) // blocks <= (64 << 10):
-                return 0, blocks
-        blocks = max(8, min(self._max_blocks, nbytes // (64 << 10)))
-        return 1, blocks
+                return _ONESHOT, blocks
+        return _NVLS if multicast else _TWOSHOT, max(8, min(self._max_blocks, nbytes // (64 << 10)))
 
     @staticmethod
     def _default_nvls_min(world: int) -> int:
@@ -495,16 +495,14 @@ class SymmetricComm:
             if hit is not None and hit[0].name != "core" and hit[1] % 16 == 0:
                 seg, off = hit
                 n = t.numel()
-                mc = self._mc.get(seg.name)
                 # multimem stores write whole 16-byte vectors: a message that ends inside one goes to the P2P kernels
-                if (mc is not None and op == _native.OP_SUM and n * es >= self._nvls_min and self._world > 1
-                        and (n * es) % 16 == 0 and self._force_plan is None):
-                    blocks = max(8, min(self._max_blocks, (n * es) // (64 << 10)))
-                    K.allreduce_nvls(self._tables[seg.name], self._status, mc[1], off, n, dt, scale, self._next_flag(),
+                mc = self._mc_base(seg.name, n * es) if op == _native.OP_SUM and (n * es) % 16 == 0 else 0
+                algo, blocks = self._plan(n * es, multicast=mc != 0)
+                if algo == _NVLS:
+                    K.allreduce_nvls(self._tables[seg.name], self._status, mc, off, n, dt, scale, self._next_flag(),
                                      _CH_ALLREDUCE, contribute, blocks, self._threads, sp)
                     self.launches += 1
                     return
-                algo, blocks = self._plan(n * es)
                 K.allreduce(self._tables[seg.name], self._status, off, 0, 0, n, dt, op, scale, self._next_flag(),
                             _CH_ALLREDUCE, contribute, algo, blocks, self._threads, sp)
                 self.launches += 1
@@ -562,15 +560,17 @@ class SymmetricComm:
                 if name.endswith("_q8") and seg.nbytes >= need and name in self._tables:
                     table = self._tables[name]
                     ngroups = self._K.q8_ngroups(n, self._world)
-                    big = max(1, min(self._K.NUM_SMS * 16, ngroups // 16 + 1))
+                    # 16 groups per CTA: of this rank's slice for the reduce, of the whole message for the gather
+                    slice_blocks = max(1, min(self._K.NUM_SMS * 8, ngroups // self._world // 16 + 1))
+                    gather_blocks = max(1, min(self._K.NUM_SMS * 16, ngroups // 16 + 1))
                     if contribute:
                         K.q8_quantize(a.data_ptr(), b.data_ptr() if b is not None else 0, n, ngroups, dt, seg.ptr, sp)
                     else:
                         K.memset_async(seg.ptr, 0, q_bytes, sp)  # zero scales: this replica adds nothing
                     self._handshake(2, True, _CH_Q8, sp)
-                    K.q8_slice_reduce(table, self._z1_ok(2), 0, q_bytes, n, scale, max(1, min(self._K.NUM_SMS * 8, ngroups // self._world // 16 + 1)), sp)
+                    K.q8_slice_reduce(table, self._z1_ok(2), 0, q_bytes, n, scale, slice_blocks, sp)
                     self._handshake(2, True, _CH_Q8, sp)
-                    K.q8_gather_dequant(table, self._z1_ok(2), q_bytes, n, dt, out.data_ptr(), big, sp)
+                    K.q8_gather_dequant(table, self._z1_ok(2), q_bytes, n, dt, out.data_ptr(), gather_blocks, sp)
                     self.launches += 3
                     return
             # elements per launch such that the Q8G buffer fits in staging
@@ -579,10 +579,9 @@ class SymmetricComm:
             fb = b.view(-1) if b is not None else None
             for lo in range(0, fa.numel(), per):
                 n = min(per, fa.numel() - lo)
-                blocks = max(4, min(self._q8_max_blocks, (n // 512) // 32 + 1))
                 K.q8_allreduce(self._tables["core"], self._status, 0, fa.data_ptr() + lo * es,
                                (fb.data_ptr() + lo * es) if fb is not None else 0, fo.data_ptr() + lo * es, n, dt,
-                               scale, self._next_flag(), _CH_Q8, contribute, blocks, sp)
+                               scale, self._next_flag(), _CH_Q8, contribute, self._q8_blocks(n // 512), sp)
                 self.launches += 1
 
     def q8_reduce_scatter_(self, out: torch.Tensor, inp: torch.Tensor, slice_elems: int, scale: float = 1.0,
@@ -602,10 +601,14 @@ class SymmetricComm:
             if self._K.q8_rs_buffer_bytes(slice_elems, W) > self._staging_usable:
                 raise ValueError("q8_reduce_scatter_: message larger than the staging segment")
             groups = W * ((slice_elems + 511) // 512)
-            blocks = max(4, min(self._q8_max_blocks, groups // 32 + 1))
             self._K.q8_reduce_scatter(self._tables["core"], self._status, 0, inp.data_ptr(), out.data_ptr(), inp.numel(), slice_elems,
-                                      dt, scale, self._next_flag(), _CH_Q8, contribute, blocks, _native.stream_ptr(stream))
+                                      dt, scale, self._next_flag(), _CH_Q8, contribute, self._q8_blocks(groups),
+                                      _native.stream_ptr(stream))
             self.launches += 1
+
+    def _q8_blocks(self, groups: int) -> int:
+        """Grid of a one-launch fp8 collective over ``groups`` Q8G groups: one CTA per 32 groups, 4 to ``_q8_max_blocks``."""
+        return max(4, min(self._q8_max_blocks, groups // 32 + 1))
 
     # ------------------------------------------------------------------ the rest of the collective surface
     def _xblocks(self, nbytes: int) -> int:
@@ -801,6 +804,7 @@ class SymmetricComm:
         return list(self._ptrs[name])
 
     def _mc_base(self, name: str, nbytes: int) -> int:
+        """Multicast address of segment ``name`` if a message of ``nbytes`` in it goes through the switch (NVLS), else 0."""
         mc = self._mc.get(name)
         return mc[1] if (mc is not None and self._world > 1 and nbytes >= self._nvls_min) else 0
 
@@ -814,11 +818,16 @@ class SymmetricComm:
     def _z1_norm_scratch_ptrs(self) -> Tuple[int, int]:
         """Per-CTA fp64 partials and the last-CTA-done ticket of the reduce kernel's sum of squares (one launch at a
         time per rank: the launches of a rank are ordered on its comm stream)."""
-        n = self._K.NUM_SMS * 32  # the grid cap of the reduce kernel
+        n = self._K.ZERO1_MAX_BLOCKS
         if self._z1_norm_scratch is None:
             self._z1_norm_scratch = torch.zeros(n + 1, dtype=torch.float64, device=self.device)
         p = self._z1_norm_scratch.data_ptr()
         return p, p + 8 * n
+
+    def _z1_blocks(self, blocks: int, nelem: int) -> int:
+        """Grid of the FT-ZeRO-1 reduce or update of ``nelem`` elements: ``blocks`` CTAs, but no more than the kernels
+        take and than one per 512 16-byte vectors."""
+        return max(1, min(blocks, self._K.ZERO1_MAX_BLOCKS, (nelem // 8 + 511) // 512))
 
     def _handshake(self, slot: int, release: bool, channel: int, sp: int) -> None:
         self._K.zero1_handshake(self._tables["core"], self._status, self._z1_ok(slot), self._next_flag(), channel, release, sp)
@@ -848,7 +857,7 @@ class SymmetricComm:
             if not contribute:
                 # healing / spare replica: its gradients count as zeros (reference manager.py:441-442)
                 self._K.memset_async(self._segments[segment].ptr + off, 0, nelem * 2, sp)
-            blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
+            blocks = self._z1_blocks(blocks, nelem)
             scratch, ticket = self._z1_norm_scratch_ptrs() if gnorm else (0, 0)
             one = self._world == 1
             if not one:
@@ -921,7 +930,7 @@ class SymmetricComm:
                 raise RuntimeError("SymmetricComm is not configured")
             lr, b1, b2, eps, wd = hyper
             sp = _native.stream_ptr(stream)
-            blocks = max(1, min(blocks, self._K.NUM_SMS * 32, (nelem // 8 + 511) // 512))
+            blocks = self._z1_blocks(blocks, nelem)
             self._K.zero1_update(self._tables[segment], self._mc_base(segment, nelem * 2), gate.data_ptr(), poff, grad, master,
                                  m, v, nelem, lr, b1, b2, eps, wd, replication, mode, table, state_off, page_shift, coef,
                                  lr_table, lr_steps, [int(x) for lo, hi in no_decay for x in (lo, hi)],

@@ -111,7 +111,10 @@ class FaultTolerantTrainer:
             config's ``fp8_linears``, off by default)
         bucket_mb: gradient bucket size for the classic (all-reduce) pipeline
         should_quantize: fused fp8 gradient all-reduce (classic pipeline)
-        overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward
+        overlap_optimizer: classic pipeline: run AdamW stage by stage on a side stream under the next forward (default);
+            ``False``: one launch after ``should_commit``
+        optimizer_blocks: CTA cap of the AdamW launches (0: the kernel's default, 16 CTAs per SM); FT-ZeRO-1: of the
+            update launches
     """
 
     def __init__(self, model: str | LlamaConfig, lighthouse_addr: str, replica_id: str = "replica_0",
@@ -119,7 +122,7 @@ class FaultTolerantTrainer:
                  should_quantize: bool = False, lr: float = 3e-4, seed: int = 0,
                  timeout: timedelta = timedelta(seconds=60), device: Optional[torch.device] = None,
                  activation_checkpoint: Optional[str] = None, init_sync: bool = False,
-                 use_async_quorum: bool = True, overlap_optimizer: Optional[bool] = None,
+                 use_async_quorum: bool = True, overlap_optimizer: bool = True,
                  optimizer_blocks: int = 0, zero1: Optional[bool] = None, replication: int = 2,
                  compact_state: Optional[bool] = None, max_grad_norm: Optional[float] = None,
                  grad_accum_steps: int = 1, lr_lambda: Optional[Callable[[int], float]] = None,
@@ -243,9 +246,7 @@ class FaultTolerantTrainer:
             self.ddp = FlatDistributedDataParallel(self.manager, self.model, self.flat, bucket_mb=bucket_mb,
                                                    should_quantize=should_quantize)
             self.optim = OptimizerWrapper(self.manager, self.inner_optim)
-            if overlap_optimizer is None:
-                overlap_optimizer = os.environ.get("TORCHFT_B200_OVERLAP_OPT", "1") != "0"
-            self._opt_blocks = int(os.environ.get("TORCHFT_B200_OPT_BLOCKS", optimizer_blocks))
+            self._opt_blocks = int(optimizer_blocks)
             if overlap_optimizer:
                 self._setup_stage_gates()
         self._tok: Optional[torch.Tensor] = None

@@ -852,7 +852,7 @@ class Zero1Optimizer:
         self.comm = pg.comm
         self.device = pg.comm.device
         self.numel = numel
-        self._replication = int(os.environ.get("TORCHFT_B200_Z1_REPLICATION", replication))
+        self._replication = int(replication)
         self.layout: ShardLayout = ShardLayout(((0, numel),), self._replication)
         self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay
         self.param_groups = [{"lr": lr, "betas": betas, "eps": eps, "weight_decay": weight_decay}]
@@ -863,8 +863,8 @@ class Zero1Optimizer:
             torch.cuda.current_stream(self.device).synchronize()
         # the big kernels are sync-free, so their grids are free parameters: the reduce-scatter is NVLink-latency bound
         # and shares the SMs with backward; the update is HBM-bound and likes many short CTAs (cf. the AdamW cap sweep)
-        self._rs_blocks = int(os.environ.get("TORCHFT_B200_Z1_RS_BLOCKS", 128))
-        self._upd_blocks = int(os.environ.get("TORCHFT_B200_Z1_UPD_BLOCKS", blocks or self._K.NUM_SMS * 16))
+        self._rs_blocks = 128
+        self._upd_blocks = blocks or self._K.NUM_SMS * 16
         if compact is None:
             compact = os.environ.get("TORCHFT_B200_Z1_COMPACT", "0") == "1"
         self.compact = bool(compact)
