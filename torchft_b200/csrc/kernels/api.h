@@ -96,7 +96,8 @@ void rmsnorm_bwd_launch(const void* dy, const void* x, const void* w, const floa
 void swiglu_fwd_launch(const void* gu, void* y, size_t T, int F, cudaStream_t s);
 void swiglu_bwd_launch(const void* dy, const void* gu, void* dgu, size_t T, int F, cudaStream_t s);
 void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const int64_t* strides9, const void* cs,
-                     size_t T, int S, int D, int Hq, int Hkv, int dir, cudaStream_t s);
+                     size_t T, int S, int D, int Hq, int Hkv, int dir, cudaStream_t s,
+                     const int* positions = nullptr);
 void xent_launch(void* logits, const void* target, float* loss, size_t rows, int V,
                  size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s,
                  const float* scale = nullptr);

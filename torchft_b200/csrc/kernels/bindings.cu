@@ -523,11 +523,15 @@ PYBIND11_MODULE(_K, m) {
     swiglu_bwd_launch(P<void>(dy), P<void>(gu), P<void>(dgu), T, F, S(s));
   });
   m.def("rope_qkv", [](uintptr_t packed, size_t row, uintptr_t q, uintptr_t k, uintptr_t v, std::vector<int64_t> strides,
-                       uintptr_t cs, size_t T, int S_, int D, int Hq, int Hkv, int dir, uintptr_t s) {
+                       uintptr_t cs, size_t T, int S_, int D, int Hq, int Hkv, int dir, uintptr_t s, uintptr_t positions) {
     if (strides.size() != 9) throw std::runtime_error("rope_qkv: strides = (batch, position, head) x (q, k, v)");
     rope_qkv_launch(P<void>(packed), row, P<void>(q), P<void>(k), P<void>(v), strides.data(), P<void>(cs), T, S_, D, Hq,
-                    Hkv, dir, S(s));
-  }, "RoPE + q/k/v split of a packed projection (dir 0) or its backward (dir 1), one launch");
+                    Hkv, dir, S(s), P<const int>(positions));
+  }, "RoPE + q/k/v split of a packed projection (dir 0) or its backward (dir 1), one launch; positions (int32 [T], "
+     "optional) rotates token t by positions[t] instead of its offset in its row",
+     py::arg("packed"), py::arg("row"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("strides"), py::arg("cs"),
+     py::arg("T"), py::arg("S"), py::arg("D"), py::arg("Hq"), py::arg("Hkv"), py::arg("dir"), py::arg("stream"),
+     py::arg("positions") = 0);
   m.def("xent", [](uintptr_t logits, uintptr_t target, uintptr_t loss, size_t rows, int V,
                    size_t row_stride, float grad_scale, long long ignore_index, uintptr_t s, uintptr_t scale) {
     xent_launch(P<void>(logits), P<void>(target), P<float>(loss), rows, V, row_stride, grad_scale,

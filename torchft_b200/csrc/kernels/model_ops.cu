@@ -355,10 +355,17 @@ struct RopeQKVArgs {
   size_t sb[3], ss[3], sh[3];  // element strides of q / k / v: batch, position, head
   unsigned nh[3];
   const float2* cs;
+  const int* positions;  // kPositions: position of token t in the cs table (its offset in its document), [T]
   unsigned T, S, D;
   int dir;
 };
 
+// Packed documents (several documents per row of S tokens) rotate each token by its offset in its DOCUMENT, read from a
+// per-token table the host builds beside cu_seqlens and ships in the same copy. A search of cu_seqlens per (token, head)
+// slot would add log2(documents) dependent loads in front of every vector of a kernel that is already latency-bound; the
+// table costs one 4-byte load per slot, shared by the token's heads through L1. Without a table (kPositions = false) the
+// position is t - b*S and the instance is the kernel as it was before packing existed: same code, same bits, same time.
+template <bool kPositions>
 __global__ void __launch_bounds__(256) rope_qkv_kernel(const RopeQKVArgs a) {
   const unsigned vph = a.D / 8;
   const unsigned vh = threadIdx.x % vph, s0 = threadIdx.x / vph, per = blockDim.x / vph;
@@ -376,13 +383,18 @@ __global__ void __launch_bounds__(256) rope_qkv_kernel(const RopeQKVArgs a) {
       ok[j] = g < nslots;
       const unsigned t = g / heads, hh = g - t * heads;
       const unsigned b = t / a.S;
-      pos[j] = t - b * a.S;
+      const unsigned in_row = t - b * a.S;
       const int w = hh < a.nh[0] ? 0 : (hh < a.nh[0] + a.nh[1] ? 1 : 2);
       const unsigned h = hh - (w == 0 ? 0 : (w == 1 ? a.nh[0] : a.nh[0] + a.nh[1]));
       rot[j] = w < 2;
       bf16* pk = a.packed + (size_t)t * a.row + (size_t)hh * a.D + vh * 8;
-      bf16* sp = a.sep[w] + b * a.sb[w] + pos[j] * a.ss[w] + h * a.sh[w] + vh * 8;
+      bf16* sp = a.sep[w] + b * a.sb[w] + in_row * a.ss[w] + h * a.sh[w] + vh * 8;
       dst[j] = a.dir == 0 ? sp : pk;
+      if constexpr (kPositions) {
+        pos[j] = ok[j] && rot[j] ? (unsigned)__ldg(a.positions + t) : 0u;
+      } else {
+        pos[j] = in_row;
+      }
       if (ok[j]) v[j] = ld_stream(a.dir == 0 ? pk : sp);
     }
 #pragma unroll
@@ -726,7 +738,7 @@ void swiglu_bwd_launch(const void* dy, const void* gu, void* dgu, size_t T, int 
 }
 
 void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const int64_t* strides9, const void* cs,
-                     size_t T, int S, int D, int Hq, int Hkv, int dir, cudaStream_t s) {
+                     size_t T, int S, int D, int Hq, int Hkv, int dir, cudaStream_t s, const int* positions) {
   if (D % 8 || D > 2048) throw std::runtime_error("rope_qkv: head_dim must be a multiple of 8 and <= 2048");
   // v == nullptr: only q and k are produced (forward keeps v as a strided view of the packed projection)
   const size_t heads = (size_t)Hq + (size_t)Hkv * (v != nullptr ? 2 : 1);
@@ -749,6 +761,7 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
   a.nh[1] = Hkv;
   a.nh[2] = v != nullptr ? Hkv : 0;
   a.cs = (const float2*)cs;
+  a.positions = positions;
   a.T = (unsigned)T;
   a.S = (unsigned)S;
   a.D = (unsigned)D;
@@ -756,7 +769,10 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
   const unsigned vph = D / 8, per = 256 / vph, threads = per * vph;
   const unsigned nslots = (unsigned)(T * heads);
   const unsigned grid = std::min<unsigned>((nslots + 2 * per - 1) / (2 * per), kNumSMs * 8);
-  rope_qkv_kernel<<<grid, threads, 0, s>>>(a);
+  if (positions != nullptr)
+    rope_qkv_kernel<true><<<grid, threads, 0, s>>>(a);
+  else
+    rope_qkv_kernel<false><<<grid, threads, 0, s>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -13,19 +13,23 @@ laid out for one-GPU-per-replica training in the 80 GB of an H100:
   hand-written sm_90a kernels (``torchft_b200/csrc/kernels/model_ops.cu``);
 * normalised activations and the SwiGLU product are recomputed in backward
   instead of stored (see ``ops.fused.norm_linear_res`` / ``swiglu_linear``);
-* attention is the SDPA library kernel (flash / cuDNN), causal, GQA.
+* attention is the SDPA library kernel (flash / cuDNN), causal, GQA; with packed documents (``cu_seqlens``) it is the
+  library's variable-length flash kernel, causal within each document, and RoPE rotates each token by its offset in
+  its document.
 """
 
 from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.nn.attention.varlen import varlen_attn
 
+from torchft_b200.data import check_cu_seqlens, document_positions
 from torchft_b200.ops import fused
 
 
@@ -76,6 +80,29 @@ CONFIGS: Dict[str, LlamaConfig] = {
 }
 
 
+class Documents(NamedTuple):
+    """The device side of a packed batch (``data.check_cu_seqlens``), made once per forward and shared by every block:
+    ``cu_seqlens`` int32 ``[N+1]``, ``positions`` int32 ``[B*S]`` (each token's offset in its document) and the longest
+    document ``max_len``."""
+
+    cu_seqlens: torch.Tensor
+    positions: torch.Tensor
+    max_len: int
+
+
+def documents(cu_seqlens: torch.Tensor, B: int, S: int, device: torch.device) -> Documents:
+    """Validate a host ``cu_seqlens`` for a ``(B, S)`` batch (``ValueError`` before any launch) and stage it on
+    ``device``: ``cu_seqlens`` and the position table are built in one pinned buffer and cross in ONE asynchronous
+    copy, with no host sync."""
+    max_len = check_cu_seqlens(cu_seqlens, B, S)
+    n = cu_seqlens.numel()
+    host = torch.empty(n + B * S, dtype=torch.int32, pin_memory=True)
+    host[:n] = cu_seqlens
+    document_positions(cu_seqlens, out=host[n:])
+    dev = host.to(device, non_blocking=True)
+    return Documents(dev[:n], dev[n:], max_len)
+
+
 class Block(nn.Module):
     """Pre-norm transformer block on the fused kernels: norm+QKV GEMM, RoPE+split, SDPA, output GEMM with the residual in
     its epilogue, norm+gate/up GEMM, SwiGLU+down GEMM with the residual in its epilogue."""
@@ -92,19 +119,29 @@ class Block(nn.Module):
         self.w13 = nn.Parameter(torch.empty(2 * cfg.ffn_dim, d, **kw))
         self.w2 = nn.Parameter(torch.empty(d, cfg.ffn_dim, **kw))
 
-    def forward(self, x: torch.Tensor, cs: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, cs: torch.Tensor, docs: Optional[Documents] = None) -> torch.Tensor:
         cfg = self.cfg
         B, S, d = x.shape
         # residual stream is threaded through the norm nodes (norm_linear_res) and added in the
         # projection GEMMs' epilogues: no standalone elementwise add in forward or backward
         fp8 = cfg.fp8_linears
         x, qkv = fused.norm_linear_res(x, self.attention_norm, self.wqkv, cfg.norm_eps, fp8=fp8)
-        q, k, v = fused.rope_qkv(qkv.view(B * S, -1), cs, B, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
-        o = F.scaled_dot_product_attention(
-            q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True,
-            enable_gqa=cfg.n_kv_heads != cfg.n_heads,
-        )
-        o = o.transpose(1, 2).reshape(B, S, d)
+        if docs is None:
+            q, k, v = fused.rope_qkv(qkv.view(B * S, -1), cs, B, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
+            o = F.scaled_dot_product_attention(
+                q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True,
+                enable_gqa=cfg.n_kv_heads != cfg.n_heads,
+            )
+            o = o.transpose(1, 2).reshape(B, S, d)
+        else:
+            # packed documents: positions restart at every document, and attention is causal within each document
+            # (GQA natively; v stays the strided view of the projection, the flash kernel reads it in place)
+            q, k, v = fused.rope_qkv(qkv.view(B * S, -1), cs, B, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim,
+                                     positions=docs.positions)
+            T, D = B * S, cfg.head_dim
+            o = varlen_attn(q.view(T, cfg.n_heads, D), k.view(T, cfg.n_kv_heads, D), v.view(T, cfg.n_kv_heads, D),
+                            docs.cu_seqlens, docs.cu_seqlens, docs.max_len, docs.max_len, window_size=(-1, 0))
+            o = o.view(B, S, d)
         h = fused.linear(o, self.wo, res=x, fp8=fp8)
         h, gu = fused.norm_linear_res(h, self.ffn_norm, self.w13, cfg.norm_eps, fp8=fp8)
         return fused.swiglu_linear(gu, self.w2, res=h, fp8=fp8)
@@ -149,8 +186,11 @@ class Llama(nn.Module):
             self._cs = fused.rope_table(max(seq_len, 1), self.cfg.head_dim, self.cfg.rope_theta, device)
         return self._cs
 
-    def hidden(self, tokens: torch.Tensor) -> torch.Tensor:
+    def hidden(self, tokens: torch.Tensor, cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Final-layer activations ``[B, S, dim]`` (before the last norm). ``cu_seqlens``: packed documents, see
+        :meth:`forward`."""
         B, S = tokens.shape
+        docs = documents(cu_seqlens, B, S, tokens.device) if cu_seqlens is not None else None
         cs = self.rope_cache(S, tokens.device)
         hook = self.stage_hook
         if hook is not None:
@@ -162,14 +202,20 @@ class Llama(nn.Module):
             if self.cfg.activation_checkpoint == "full" and torch.is_grad_enabled():
                 from torch.utils.checkpoint import checkpoint
 
-                x = checkpoint(blk, x, cs, use_reentrant=False)
+                x = checkpoint(blk, x, cs, docs, use_reentrant=False)
             else:
-                x = blk(x, cs)
+                x = blk(x, cs, docs)
         return x
 
-    def forward(self, tokens: torch.Tensor, targets: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Returns the mean next-token loss over the targets that are not -100 when ``targets`` is given, else logits."""
-        x = self.hidden(tokens)
+    def forward(self, tokens: torch.Tensor, targets: Optional[torch.Tensor] = None,
+                cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Returns the mean next-token loss over the targets that are not -100 when ``targets`` is given, else logits.
+
+        ``cu_seqlens`` (CPU int32 ``[N+1]``, see ``data.check_cu_seqlens``) packs several documents into each row:
+        a token attends only to the earlier tokens of its own document, and its RoPE position is its offset in that
+        document. The targets are used as given: mark each document's last target ``-100`` (``data.pack_documents``
+        does) so that no token is trained to predict the next document."""
+        x = self.hidden(tokens, cu_seqlens)
         B, S, d = x.shape
         if self.stage_hook is not None:
             self.stage_hook(len(self.layers) + 1)

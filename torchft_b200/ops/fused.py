@@ -180,28 +180,34 @@ class _RoPEQKV(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, qkv: torch.Tensor, cs: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int):  # type: ignore[override]
+    def forward(ctx, qkv: torch.Tensor, cs: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int,  # type: ignore[override]
+                positions: Optional[torch.Tensor] = None):
         K = _native.load()
         assert qkv.is_contiguous() and qkv.dtype == torch.bfloat16
         # the kernel reads the table as fp32: a wrapper that down-casts module inputs (FSDP2's cast_forward_inputs) would
         # make it read garbage and past the end of the buffer
         assert cs.dtype == torch.float32 and cs.is_contiguous() and cs.shape[0] >= S, "rope table must be the fp32 table of rope_table()"
+        if positions is not None:
+            # every entry must index the table: data.document_positions of a valid cu_seqlens is < S
+            assert (positions.dtype == torch.int32 and positions.is_contiguous() and positions.device == qkv.device
+                    and positions.numel() == B * S), "positions must be a contiguous int32 [B*S] tensor on qkv's device"
         row = qkv.shape[-1]
         assert row == (Hq + 2 * Hkv) * D
         q = torch.empty((B, S, Hq, D), dtype=qkv.dtype, device=qkv.device)
         k = torch.empty((B, S, Hkv, D), dtype=qkv.dtype, device=qkv.device)
+        pp = positions.data_ptr() if positions is not None else 0
         # one launch rotates q and k out of the packed rows; v stays a strided view of the projection (no copy)
         K.rope_qkv(qkv.data_ptr(), row, q.data_ptr(), k.data_ptr(), 0, [*q.stride()[:3], *k.stride()[:3], 0, 0, 0],
-                   cs.data_ptr(), B * S, S, D, Hq, Hkv, 0, _native.stream_ptr())
+                   cs.data_ptr(), B * S, S, D, Hq, Hkv, 0, _native.stream_ptr(), pp)
         v = qkv.view(B * S, row)[:, (Hq + Hkv) * D :].reshape(B, S, Hkv, D)
-        ctx.save_for_backward(cs)
+        ctx.save_for_backward(cs, positions)
         ctx.meta = (B, S, Hq, Hkv, D, row)
         return q, k, v
 
     @staticmethod
     def backward(ctx, dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor):  # type: ignore[override]
         K = _native.load()
-        (cs,) = ctx.saved_tensors
+        cs, positions = ctx.saved_tensors
         B, S, Hq, Hkv, D, row = ctx.meta
 
         def usable(t: torch.Tensor) -> torch.Tensor:
@@ -214,13 +220,16 @@ class _RoPEQKV(torch.autograd.Function):
         dqkv = torch.empty((B * S, row), dtype=dq.dtype, device=dq.device)
         K.rope_qkv(dqkv.data_ptr(), row, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
                    [*dq.stride()[:3], *dk.stride()[:3], *dv.stride()[:3]], cs.data_ptr(), B * S, S, D, Hq, Hkv, 1,
-                   _native.stream_ptr())
-        return dqkv, None, None, None, None, None, None
+                   _native.stream_ptr(), positions.data_ptr() if positions is not None else 0)
+        return dqkv, None, None, None, None, None, None, None
 
 
-def rope_qkv(qkv: torch.Tensor, cs: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    """Split a packed ``[B*S, (Hq+2*Hkv)*D]`` projection into q, k, v with RoPE applied to q and k."""
-    return _RoPEQKV.apply(qkv, cs, B, S, Hq, Hkv, D)
+def rope_qkv(qkv: torch.Tensor, cs: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int,
+             positions: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Split a packed ``[B*S, (Hq+2*Hkv)*D]`` projection into q, k, v with RoPE applied to q and k. Token ``t`` is
+    rotated by ``cs[positions[t]]`` when ``positions`` (int32 ``[B*S]`` on the device, e.g. each token's offset in its
+    packed document) is given, else by ``cs[t mod S]``; the backward uses the same positions."""
+    return _RoPEQKV.apply(qkv, cs, B, S, Hq, Hkv, D, positions)
 
 
 class _LinearCrossEntropy(torch.autograd.Function):

@@ -34,6 +34,7 @@ import torch
 from torch import nn
 from torch.distributed import TCPStore
 
+from torchft_b200.data import check_cu_seqlens, slice_cu_seqlens
 from torchft_b200.ddp import FlatDistributedDataParallel
 from torchft_b200.manager import Manager
 from torchft_b200.models.llama import CONFIGS, FlatParams, Llama, LlamaConfig
@@ -334,17 +335,20 @@ class FaultTolerantTrainer:
         o.t = int(sd["t"])
 
     # -------------------------------------------------------------------- step
-    def step_device(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
+    def step_device(self, tokens: torch.Tensor, targets: torch.Tensor,
+                    cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One fault-tolerant optimisation step on device-resident inputs; returns the loss tensor (device). With
-        ``grad_accum_steps = M`` the inputs are ``(M * B, S)`` and the loss is the mean over the ``M`` micro-batches."""
+        ``grad_accum_steps = M`` the inputs are ``(M * B, S)`` and the loss is the mean over the ``M`` micro-batches.
+        ``cu_seqlens`` (host int32, ``data.check_cu_seqlens``) packs documents into the rows (``Llama.forward``); with
+        accumulation it describes the whole ``(M * B, S)`` batch and is cut per micro-batch on the host."""
         self._not_in_ema("step")
         self._steps_run += 1
         if self.zero1 and self.grad_accum_steps > 1:
-            return self._step_accumulate(tokens, targets)
+            return self._step_accumulate(tokens, targets, cu_seqlens)
         if self.zero1:
             self.manager.start_quorum()       # async; its thread first books the previous step's device verdict
             self.flat.reset_grads()           # wgrad GEMMs write the flat gradient buffer directly: no memset
-            loss = self.ddp(tokens, targets)  # forward; stage i waits for the event of unit i's update
+            loss = self.ddp(tokens, targets, cu_seqlens=cu_seqlens)  # forward; stage i waits for unit i's update
             loss.backward()                   # per-unit reduce-scatter kernels launch from the grad hooks
             self.ddp.finish(wait=False)       # issue what is left; the optimizer stream orders itself behind them
             self.manager.commit_on_device(self.zopt)  # verdict kernel (no host sync, no RPC in steady state)
@@ -353,21 +357,32 @@ class FaultTolerantTrainer:
             return loss
         self.optim.zero_grad(set_to_none=True)  # start_quorum (async); no memset:
         self.flat.reset_grads()                  # wgrad GEMMs write the flat gradient buffer directly
-        loss = self.ddp(tokens, targets)  # forward (fused kernels + cuBLAS + SDPA)
+        loss = self.ddp(tokens, targets, cu_seqlens=cu_seqlens)  # forward (fused kernels + cuBLAS + SDPA)
         loss.backward()                   # bucket all-reduces launch from grad hooks, overlapped
         self.ddp.finish()                 # current stream waits for the comm stream
         if self.manager.should_commit():  # OptimizerWrapper.step() semantics (optim.py), with the update
             self._optimizer_step()        # cut per layer so the next forward overlaps it
         return loss
 
-    def _step_accumulate(self, tokens: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
+    def _step_accumulate(self, tokens: torch.Tensor, targets: torch.Tensor,
+                         cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """FT-ZeRO-1 step over ``M`` micro-batches: one quorum, ``M`` forward/backward passes whose reduce-scatters
-        accumulate on the comm stream, one commit and one update."""
+        accumulate on the comm stream, one commit and one update.
+
+        The loss (and its gradient) is the mean of the ``M`` micro-batch means, each over its own targets that are not
+        -100, not the mean over all valid targets of the step. With packed documents the number of valid targets varies
+        more between micro-batches (one -100 per document), so a target in a micro-batch of many short documents weighs
+        a little more than one in a micro-batch of few long ones."""
         M = self.grad_accum_steps
         if tokens.shape[0] % M or tokens.shape[0] == 0 or targets.shape[0] != tokens.shape[0]:
             raise ValueError(f"grad_accum_steps={M} must divide the batch dimension of tokens and targets, got "
                              f"{tuple(tokens.shape)} and {tuple(targets.shape)}")
         B = tokens.shape[0] // M
+        micro_cu: List[Optional[torch.Tensor]] = [None] * M
+        if cu_seqlens is not None:
+            S = tokens.shape[1]
+            check_cu_seqlens(cu_seqlens, M * B, S)  # row-aligned, so every micro-batch boundary is a document start
+            micro_cu = [slice_cu_seqlens(cu_seqlens, m * B * S, (m + 1) * B * S) for m in range(M)]
         cur = torch.cuda.current_stream()
         read_done = torch.cuda.Event()
         losses = []
@@ -375,7 +390,8 @@ class FaultTolerantTrainer:
         for m in range(M):
             self._micro = m
             self.flat.reset_grads()
-            loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B])  # overlaps micro-batch m-1's tail
+            loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B],  # overlaps micro-batch m-1's tail
+                            cu_seqlens=micro_cu[m])
             if m > 0:
                 # backward overwrites the gradient buffer that the peers read in micro-batch m-1's reduce-scatters:
                 # wait until its last trailing handshake ("every peer is done reading mine") has passed
@@ -399,18 +415,21 @@ class FaultTolerantTrainer:
         self._tok.copy_(tokens_cpu, non_blocking=True)
         self._tgt.copy_(targets_cpu, non_blocking=True)
 
-    def step(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor) -> float:
-        """End-to-end step: pinned-host inputs -> H2D -> train step -> D2H loss (blocks until the loss is on the host)."""
+    def step(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor,
+             cu_seqlens: Optional[torch.Tensor] = None) -> float:
+        """End-to-end step: pinned-host inputs -> H2D -> train step -> D2H loss (blocks until the loss is on the host).
+        ``cu_seqlens``: packed documents, as in :meth:`step_device`."""
         self._not_in_ema("step")
         self._stage_inputs(tokens_cpu, targets_cpu)
-        loss = self.step_device(self._tok, self._tgt)
+        loss = self.step_device(self._tok, self._tgt, cu_seqlens)
         return float(loss.item())
 
-    def step_async(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor) -> Optional[float]:
+    def step_async(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor,
+                   cu_seqlens: Optional[torch.Tensor] = None) -> Optional[float]:
         """Like :meth:`step`, but the loss comes back one step late: this call enqueues the step and the D2H copy
         of ITS loss into pinned memory, and returns the PREVIOUS step's loss (``None`` on the first call). The host
         never waits for the step it just launched, so the GPU queue stays full; every step still performs its
-        H2D input copy and its D2H loss read."""
+        H2D input copy and its D2H loss read. ``cu_seqlens``: packed documents, as in :meth:`step_device`."""
         self._not_in_ema("step_async")
         prev: Optional[float] = None
         if self._loss_event is not None:
@@ -418,7 +437,7 @@ class FaultTolerantTrainer:
             assert self._loss_host is not None
             prev = float(self._loss_host[0])
         self._stage_inputs(tokens_cpu, targets_cpu)
-        loss = self.step_device(self._tok, self._tgt)
+        loss = self.step_device(self._tok, self._tgt, cu_seqlens)
         if self._loss_host is None:
             self._loss_host = torch.empty(1, dtype=torch.float32).pin_memory()
             self._loss_event = torch.cuda.Event()
