@@ -101,6 +101,12 @@ void rope_qkv_launch(void* packed, size_t row, void* q, void* k, void* v, const 
 void xent_launch(void* logits, const void* target, float* loss, size_t rows, int V,
                  size_t row_stride, float grad_scale, long long ignore_index, cudaStream_t s,
                  const float* scale = nullptr);
+// grad[v] += sum of dx[t] over the tokens t with id v, in place, bf16 [V, d], one rounding per touched row, deterministic.
+// sorted_ids / perm: a stable sort of the int64 token ids and the token index of each sorted position, [T]; dx: bf16
+// [T, d] with row stride ldx; partial: fp32 scratch [embedding_bwd_pieces(T), 2, d]. Two launches.
+int embedding_bwd_pieces(int T);
+void embedding_bwd_launch(const int64_t* sorted_ids, const int64_t* perm, const void* dx, size_t ldx, void* grad,
+                          float* partial, int T, int d, cudaStream_t s);
 void adamw_launch(void* p, float* master, float* m, float* v, const void* g, size_t n, float lr,
                   float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale,
                   const int* gate, int max_blocks, cudaStream_t s);

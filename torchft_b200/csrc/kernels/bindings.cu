@@ -538,6 +538,14 @@ PYBIND11_MODULE(_K, m) {
                 ignore_index, S(s), P<const float>(scale));
   }, py::arg("logits"), py::arg("target"), py::arg("loss"), py::arg("rows"), py::arg("V"), py::arg("row_stride"),
      py::arg("grad_scale"), py::arg("ignore_index"), py::arg("stream"), py::arg("scale") = 0);
+  m.def("embedding_bwd_pieces", &embedding_bwd_pieces, "rows of the embedding_bwd partial scratch [pieces, 2, d] for T tokens");
+  m.def("embedding_bwd", [](uintptr_t sorted_ids, uintptr_t perm, uintptr_t dx, size_t ldx, uintptr_t grad,
+                            uintptr_t partial, int T, int d, uintptr_t s) {
+    embedding_bwd_launch(P<const int64_t>(sorted_ids), P<const int64_t>(perm), P<void>(dx), ldx, P<void>(grad),
+                         P<float>(partial), T, d, S(s));
+  }, "grad[v] += sum of the dx rows of the tokens with id v, in place (stably sorted ids and their token indices)",
+     py::arg("sorted_ids"), py::arg("perm"), py::arg("dx"), py::arg("ldx"), py::arg("grad"), py::arg("partial"),
+     py::arg("T"), py::arg("d"), py::arg("stream"));
   m.def("adamw", [](uintptr_t p, uintptr_t master, uintptr_t mm, uintptr_t v, uintptr_t g, size_t n,
                     float lr, float b1, float b2, float eps, float wd, float bc1, float bc2,
                     float gscale, uintptr_t gate, uintptr_t s, int max_blocks) {

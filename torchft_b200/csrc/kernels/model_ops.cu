@@ -489,6 +489,148 @@ __global__ void __launch_bounds__(1024) xent_fwd_bwd_kernel(bf16* __restrict__ l
   }
 }
 
+// ------------------------------- Embedding backward -------------------------
+// grad[v] = bf16(float(grad[v]) + sum_{t : id[t] = v} float(dx[t])) in place, for every id v that occurs: one rounding
+// per touched row, untouched rows keep their bits. The caller sorts the ids stably (sid, with perm[i] the token at
+// sorted position i), so the tokens of one id form a run. The sorted order is cut into pieces of kEmbPiece positions
+// (boundaries depend on T only); a warp owns one piece and kEmbCols columns and walks its tokens in order, summing in
+// fp32. A run that starts and ends inside the piece is complete: the warp adds it into grad itself. The first and last
+// run of the piece may continue into its neighbours: they go to fp32 partials (slot 0: first run, slot 1: last run when
+// it is another), and a second launch adds up each such run's partials in piece order, the warp of the piece where the
+// run starts. So the order of every sum depends on the ids alone (bit-identical launches), and a hot id shared by all
+// T tokens is summed by T / kEmbPiece warps per column block instead of one.
+constexpr int kEmbPiece = 64;   // sorted positions per piece
+constexpr int kEmbCols = 256;   // columns per warp: 32 lanes x one 16-byte vector
+constexpr int kEmbWarps = 4;    // warps per CTA
+constexpr int kEmbUnroll = 8;   // dx rows in flight per lane
+
+struct EmbArgs {
+  const long long* sid;   // ids in sorted order [T]
+  const long long* perm;  // token of each sorted position [T]
+  const bf16* dx;         // [T, d], row stride ldx
+  size_t ldx;
+  bf16* grad;             // [V, d]
+  float* partial;         // [npieces, 2, d]
+  int T, d, npieces, nchunks;
+};
+
+__device__ __forceinline__ void emb_add_row(bf16* g, const float* a) {
+  float f[8];
+  P8::unpack(*reinterpret_cast<const Vec16*>(g), f);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) f[k] += a[k];
+  *reinterpret_cast<Vec16*>(g) = P8::pack(f);
+}
+
+__device__ __forceinline__ void emb_store_partial(float* o, const float* a) {
+  reinterpret_cast<float4*>(o)[0] = make_float4(a[0], a[1], a[2], a[3]);
+  reinterpret_cast<float4*>(o)[1] = make_float4(a[4], a[5], a[6], a[7]);
+}
+
+__device__ __forceinline__ void emb_add_partial(float* a, const float* o) {
+  const float4 x = reinterpret_cast<const float4*>(o)[0], y = reinterpret_cast<const float4*>(o)[1];
+  a[0] += x.x; a[1] += x.y; a[2] += x.z; a[3] += x.w;
+  a[4] += y.x; a[5] += y.y; a[6] += y.z; a[7] += y.w;
+}
+
+__global__ void __launch_bounds__(kEmbWarps * 32) embedding_bwd_pieces_kernel(const EmbArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int gw = blockIdx.x * kEmbWarps + (threadIdx.x >> 5);
+  if (gw >= a.npieces * a.nchunks) return;  // warp-uniform
+  const int p = gw / a.nchunks, col = (gw % a.nchunks) * kEmbCols + lane * 8;
+  const bool on = col < a.d;
+  const int lo = p * kEmbPiece, hi = min(lo + kEmbPiece, a.T);
+  float acc[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+  long long cur = a.sid[lo];
+  int seg = 0;  // runs of this piece already flushed
+  for (int base = lo; base < hi; base += 32) {
+    const int n = min(32, hi - base);
+    const long long my_id = lane < n ? a.sid[base + lane] : 0;
+    const long long my_tok = lane < n ? a.perm[base + lane] : 0;
+    for (int j0 = 0; j0 < n; j0 += kEmbUnroll) {
+      Vec16 v[kEmbUnroll];
+      long long id[kEmbUnroll];
+#pragma unroll
+      for (int u = 0; u < kEmbUnroll; ++u) {
+        const int j = (j0 + u) & 31;
+        id[u] = __shfl_sync(0xffffffffu, my_id, j);
+        const long long tok = __shfl_sync(0xffffffffu, my_tok, j);
+        if (on && j0 + u < n) v[u] = ld_stream(a.dx + (size_t)tok * a.ldx + col);
+      }
+#pragma unroll
+      for (int u = 0; u < kEmbUnroll; ++u) {
+        if (j0 + u >= n) break;
+        if (id[u] != cur) {  // the run of `cur` ends here
+          if (on) {
+            if (seg == 0) emb_store_partial(a.partial + (size_t)p * 2 * a.d + col, acc);
+            else emb_add_row(a.grad + (size_t)cur * a.d + col, acc);
+          }
+#pragma unroll
+          for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+          ++seg;
+          cur = id[u];
+        }
+        if (on) {
+          float f[8];
+          P8::unpack(v[u], f);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) acc[k] += f[k];
+        }
+      }
+    }
+  }
+  if (on) emb_store_partial(a.partial + ((size_t)p * 2 + (seg == 0 ? 0 : 1)) * a.d + col, acc);
+}
+
+// The run of id v whose first partial is slot s of piece p: add the first partials of the following pieces that start
+// inside the run (a prefix of them, found 32 pieces per ballot), in piece order, then grad[v] once.
+__device__ __forceinline__ void emb_combine(const EmbArgs& a, long long v, int p, int s, int col, bool on, int lane) {
+  int end = p + 1;
+  for (;;) {
+    const int x = end + lane;
+    const bool in = x < a.npieces && a.sid[(size_t)x * kEmbPiece] == v;
+    const int k = __popc(__ballot_sync(0xffffffffu, in));
+    end += k;
+    if (k < 32) break;
+  }
+  if (!on) return;
+  float acc[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+  emb_add_partial(acc, a.partial + ((size_t)p * 2 + s) * a.d + col);
+  int q = p + 1;
+  for (; q + kEmbUnroll <= end; q += kEmbUnroll) {
+    float4 r[kEmbUnroll][2];
+#pragma unroll
+    for (int u = 0; u < kEmbUnroll; ++u) {
+      const float4* o = reinterpret_cast<const float4*>(a.partial + (size_t)(q + u) * 2 * a.d + col);
+      r[u][0] = o[0];
+      r[u][1] = o[1];
+    }
+#pragma unroll
+    for (int u = 0; u < kEmbUnroll; ++u) {
+      acc[0] += r[u][0].x; acc[1] += r[u][0].y; acc[2] += r[u][0].z; acc[3] += r[u][0].w;
+      acc[4] += r[u][1].x; acc[5] += r[u][1].y; acc[6] += r[u][1].z; acc[7] += r[u][1].w;
+    }
+  }
+  for (; q < end; ++q) emb_add_partial(acc, a.partial + (size_t)q * 2 * a.d + col);
+  emb_add_row(a.grad + (size_t)v * a.d + col, acc);
+}
+
+__global__ void __launch_bounds__(kEmbWarps * 32) embedding_bwd_combine_kernel(const EmbArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int gw = blockIdx.x * kEmbWarps + (threadIdx.x >> 5);
+  if (gw >= a.npieces * a.nchunks) return;
+  const int p = gw / a.nchunks, col = (gw % a.nchunks) * kEmbCols + lane * 8;
+  const bool on = col < a.d;
+  const int lo = p * kEmbPiece, hi = min(lo + kEmbPiece, a.T);
+  const long long first = a.sid[lo], last = a.sid[hi - 1];
+  if (p == 0 || a.sid[lo - 1] != first) emb_combine(a, first, p, 0, col, on, lane);  // the first run starts here
+  if (last != first) emb_combine(a, last, p, 1, col, on, lane);                     // the last run, another one
+}
+
 // ------------------------------- AdamW --------------------------------------
 // Flat multi-tensor AdamW: bf16 params + fp32 master/m/v, bf16 grads.
 // `gate` (nullable) points at a device int: the update is skipped entirely
@@ -782,6 +924,34 @@ void xent_launch(void* logits, const void* target, float* loss, size_t rows, int
   if (rows == 0) return;
   xent_fwd_bwd_kernel<<<(unsigned)rows, 1024, 0, s>>>((bf16*)logits, (const long long*)target, loss,
                                                       V, row_stride, grad_scale, scale, ignore_index);
+  TFT_CUDA_CHECK(cudaGetLastError());
+}
+
+int embedding_bwd_pieces(int T) { return (T + kEmbPiece - 1) / kEmbPiece; }
+
+void embedding_bwd_launch(const int64_t* sorted_ids, const int64_t* perm, const void* dx, size_t ldx, void* grad,
+                          float* partial, int T, int d, cudaStream_t s) {
+  if (d <= 0 || d % 8) throw std::invalid_argument("embedding_bwd: the row width must be a positive multiple of 8");
+  if (ldx % 8 || (uintptr_t)dx % 16 || (uintptr_t)grad % 16 || (uintptr_t)partial % 16)
+    throw std::invalid_argument("embedding_bwd: dx rows, grad and the partials must be 16-byte aligned");
+  if (T < 0) throw std::invalid_argument("embedding_bwd: negative token count");
+  if (T == 0) return;
+  EmbArgs a{};
+  a.sid = (const long long*)sorted_ids;
+  a.perm = (const long long*)perm;
+  a.dx = (const bf16*)dx;
+  a.ldx = ldx;
+  a.grad = (bf16*)grad;
+  a.partial = partial;
+  a.T = T;
+  a.d = d;
+  a.npieces = embedding_bwd_pieces(T);
+  a.nchunks = (d + kEmbCols - 1) / kEmbCols;
+  const size_t warps = (size_t)a.npieces * a.nchunks;
+  if (warps >= (1ull << 31)) throw std::invalid_argument("embedding_bwd: too many tokens for this row width");
+  const unsigned grid = (unsigned)((warps + kEmbWarps - 1) / kEmbWarps);
+  embedding_bwd_pieces_kernel<<<grid, kEmbWarps * 32, 0, s>>>(a);
+  embedding_bwd_combine_kernel<<<grid, kEmbWarps * 32, 0, s>>>(a);
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

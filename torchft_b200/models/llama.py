@@ -15,7 +15,10 @@ laid out for one-GPU-per-replica training in the 80 GB of an H100:
   instead of stored (see ``ops.fused.norm_linear_res`` / ``swiglu_linear``);
 * attention is the SDPA library kernel (flash / cuDNN), causal, GQA; with packed documents (``cu_seqlens``) it is the
   library's variable-length flash kernel, causal within each document, and RoPE rotates each token by its offset in
-  its document.
+  its document;
+* with ``tie_embeddings`` (Llama-3.2 1B and 3B) the LM head reads the token embedding: there is no ``output``
+  parameter, and the embedding backward is a hand-written kernel that adds into the gradient the head already wrote
+  (``ops.fused.tied_embedding``).
 """
 
 from __future__ import annotations
@@ -31,6 +34,18 @@ from torch.nn.attention.varlen import varlen_attn
 
 from torchft_b200.data import check_cu_seqlens, document_positions
 from torchft_b200.ops import fused
+
+
+class RopeScaling(NamedTuple):
+    """Llama-3.1 RoPE frequency scaling (``ops.fused.rope_scaled_frequencies``)."""
+
+    factor: float
+    low_freq_factor: float
+    high_freq_factor: float
+    original_max_position: int
+
+
+LLAMA3_1_ROPE_SCALING = RopeScaling(32.0, 1.0, 4.0, 8192)
 
 
 @dataclass
@@ -52,6 +67,10 @@ class LlamaConfig:
     # the forward and input-gradient GEMMs of the four block linears (wqkv, wo, w13, w2) on fp8 tensor cores with
     # row-scaled e4m3 operands; weight gradients, the LM head, the embedding and attention stay bf16
     fp8_linears: bool = False
+    # the LM head is the token embedding (no separate output matrix), as in the released Llama-3.2 1B and 3B
+    tie_embeddings: bool = False
+    # Llama-3.1 RoPE frequency scaling; None: plain RoPE
+    rope_scaling: Optional[RopeScaling] = None
 
     @property
     def head_dim(self) -> int:
@@ -61,10 +80,11 @@ class LlamaConfig:
         d, f, v = self.dim, self.ffn_dim, self.vocab_size
         qkv = (self.n_heads + 2 * self.n_kv_heads) * self.head_dim * d
         per_layer = qkv + d * d + 2 * f * d + f * d + 2 * d
-        return 2 * v * d + self.n_layers * per_layer + d
+        return (1 if self.tie_embeddings else 2) * v * d + self.n_layers * per_layer + d
 
     def flops_per_token(self, seq_len: int) -> float:
-        """Training FLOPs/token: 6 * matmul params + causal attention (fwd+bwd)."""
+        """Training FLOPs/token: 6 * matmul params + causal attention (fwd+bwd). A tied head still runs its GEMMs, so
+        tying does not change this count."""
         d, f, v = self.dim, self.ffn_dim, self.vocab_size
         qkv = (self.n_heads + 2 * self.n_kv_heads) * self.head_dim * d
         mm = self.n_layers * (qkv + d * d + 3 * f * d) + v * d
@@ -75,6 +95,11 @@ class LlamaConfig:
 CONFIGS: Dict[str, LlamaConfig] = {
     "llama3_8b": LlamaConfig(),
     "llama3_1b": LlamaConfig(dim=2048, n_layers=16, n_heads=32, n_kv_heads=8, ffn_dim=8192),
+    # the released Llama-3.2 architectures: tied embeddings and Llama-3.1 RoPE scaling
+    "llama3_2_1b": LlamaConfig(dim=2048, n_layers=16, n_heads=32, n_kv_heads=8, ffn_dim=8192, tie_embeddings=True,
+                               rope_scaling=LLAMA3_1_ROPE_SCALING),
+    "llama3_2_3b": LlamaConfig(dim=3072, n_layers=28, n_heads=24, n_kv_heads=8, ffn_dim=8192, tie_embeddings=True,
+                               rope_scaling=LLAMA3_1_ROPE_SCALING),
     "llama3_debug": LlamaConfig(dim=256, n_layers=2, n_heads=8, n_kv_heads=2, vocab_size=2048, ffn_dim=768, max_seq_len=512),
     "llama3_tiny": LlamaConfig(dim=64, n_layers=2, n_heads=4, n_kv_heads=2, vocab_size=512, ffn_dim=192, max_seq_len=128),
 }
@@ -158,15 +183,22 @@ class Llama(nn.Module):
         self.tok_embeddings = nn.Parameter(torch.empty(cfg.vocab_size, cfg.dim, **kw))
         self.layers = nn.ModuleList(Block(cfg, device=device, dtype=dtype) for _ in range(cfg.n_layers))
         self.norm = nn.Parameter(torch.empty(cfg.dim, **kw))
-        self.output = nn.Parameter(torch.empty(cfg.vocab_size, cfg.dim, **kw))
+        if not cfg.tie_embeddings:  # tied: the head reads tok_embeddings (no alias: one parameter, one state_dict key)
+            self.output = nn.Parameter(torch.empty(cfg.vocab_size, cfg.dim, **kw))
         self._cs: Optional[torch.Tensor] = None
         # called with the stage index right before that stage's parameters are first read in forward
         # (stage order = param_stages()); lets an optimizer that updates stage by stage gate the forward
         self.stage_hook: Optional[Callable[[int], None]] = None
 
     def param_stages(self) -> List[List[nn.Parameter]]:
-        """Parameters grouped by first use in forward: [embedding], one group per block, [final norm, output]."""
-        return [[self.tok_embeddings], *[list(b.parameters()) for b in self.layers], [self.norm, self.output]]
+        """Parameters grouped by first use in forward: [embedding], one group per block, [final norm, output]. Tied, the
+        last group is [final norm] alone: the head's weight is first read as the embedding."""
+        head = [] if self.cfg.tie_embeddings else [self.output]
+        return [[self.tok_embeddings], *[list(b.parameters()) for b in self.layers], [self.norm, *head]]
+
+    def head_weight(self) -> nn.Parameter:
+        """The LM head's ``[vocab, dim]`` weight: ``output``, or ``tok_embeddings`` when tied."""
+        return self.tok_embeddings if self.cfg.tie_embeddings else self.output
 
     @torch.no_grad()
     def init_weights(self, seed: int = 0) -> None:
@@ -183,7 +215,8 @@ class Llama(nn.Module):
 
     def rope_cache(self, seq_len: int, device: torch.device) -> torch.Tensor:
         if self._cs is None or self._cs.shape[0] < seq_len or self._cs.device != device:
-            self._cs = fused.rope_table(max(seq_len, 1), self.cfg.head_dim, self.cfg.rope_theta, device)
+            self._cs = fused.rope_table(max(seq_len, 1), self.cfg.head_dim, self.cfg.rope_theta, device,
+                                        scaling=self.cfg.rope_scaling)
         return self._cs
 
     def hidden(self, tokens: torch.Tensor, cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -195,7 +228,10 @@ class Llama(nn.Module):
         hook = self.stage_hook
         if hook is not None:
             hook(0)
-        x = F.embedding(tokens, self.tok_embeddings)
+        if self.cfg.tie_embeddings:
+            x = fused.tied_embedding(tokens, self.tok_embeddings)
+        else:
+            x = F.embedding(tokens, self.tok_embeddings)
         for i, blk in enumerate(self.layers):
             if hook is not None:
                 hook(i + 1)
@@ -220,9 +256,10 @@ class Llama(nn.Module):
         if self.stage_hook is not None:
             self.stage_hook(len(self.layers) + 1)
         if targets is None:
-            return fused.rmsnorm(x, self.norm, self.cfg.norm_eps) @ self.output.t()
+            return fused.rmsnorm(x, self.norm, self.cfg.norm_eps) @ self.head_weight().t()
         h = fused.rmsnorm(x, self.norm, self.cfg.norm_eps).view(B * S, d)
-        return fused.linear_cross_entropy(h, self.output, targets.reshape(-1), chunk=self.cfg.loss_chunk)
+        return fused.linear_cross_entropy(h, self.head_weight(), targets.reshape(-1), chunk=self.cfg.loss_chunk,
+                                          tied=self.cfg.tie_embeddings)
 
 
 class FlatParams:

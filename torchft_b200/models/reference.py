@@ -18,12 +18,31 @@ def _rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
     return x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps) * w
 
 
-def _rope(x: torch.Tensor, theta: float, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+def _scaled(inv: torch.Tensor, scaling, dtype: torch.dtype) -> torch.Tensor:
+    """Llama-3.1 frequency scaling of ``inv`` computed in ``dtype`` (at least fp32): a wavelength ``w = 2 pi / f`` below
+    ``orig / high`` keeps ``f``, one above ``orig / low`` gets ``f / factor``, and in between ``f`` moves smoothly
+    from one to the other with ``s = (orig / w - low) / (high - low)``."""
+    factor, low, high, orig = (float(v) for v in scaling)
+    f = inv.to(torch.float64 if dtype == torch.float64 else torch.float32)
+    w = 2 * torch.pi / f
+    out = f.clone()
+    long_waves = w > orig / low
+    out[long_waves] = f[long_waves] / factor
+    band = (w >= orig / high) & ~long_waves
+    s = (orig / w[band] - low) / (high - low)
+    out[band] = (1 - s) * f[band] / factor + s * f[band]
+    return out
+
+
+def _rope(x: torch.Tensor, theta: float, pos: Optional[torch.Tensor] = None, scaling=None) -> torch.Tensor:
     """Interleaved-pair rotation by the fp32 angles of ``ops.fused.rope_table``; cos and sin in fp64 for an fp64 ``x``,
     else in fp32, and the rotation rounded once to ``x``'s dtype (complex bf16 does not exist). ``pos`` ``[B, S]``: the
-    position of each token (default: its offset in its row)."""
+    position of each token (default: its offset in its row). ``scaling``: Llama-3.1 frequency scaling, computed in
+    ``x``'s dtype (at least fp32); the angles are then the fp32 products of the scaled frequencies, as in the table."""
     B, S, H, D = x.shape
     inv = 1.0 / (theta ** (torch.arange(0, D, 2, device=x.device, dtype=torch.float32) / D))
+    if scaling is not None:
+        inv = _scaled(inv, scaling, x.dtype).float()
     if pos is None:
         ang = torch.outer(torch.arange(S, device=x.device, dtype=torch.float32), inv)[None]
     else:
@@ -62,7 +81,8 @@ def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor, dtype: to
     """Returns (loss, {param_name: grad in ``dtype``}) computed with eager PyTorch in ``dtype``. ``linear(x, W)``, by
     default ``x @ W.T``, computes the four block linears (wqkv, wo, w13, w2), e.g. with quantised operands.
     ``cu_seqlens``: packed documents, attended through an explicit block-diagonal causal mask and rotated by their
-    positions in their documents."""
+    positions in their documents. A config with ``tie_embeddings`` reads ``tok_embeddings`` as the head (autograd adds
+    both gradients), and one with ``rope_scaling`` rotates by the scaled frequencies."""
 
     cfg = model.cfg
     if linear is None:
@@ -77,7 +97,7 @@ def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor, dtype: to
         n = _rmsnorm(x, P[pre + "attention_norm"], cfg.norm_eps)
         qkv = linear(n, P[pre + "wqkv"]).view(B, S, Hq + 2 * Hkv, D)
         q, k, v = qkv[:, :, :Hq], qkv[:, :, Hq : Hq + Hkv], qkv[:, :, Hq + Hkv :]
-        q, k = _rope(q, cfg.rope_theta, pos), _rope(k, cfg.rope_theta, pos)
+        q, k = _rope(q, cfg.rope_theta, pos, cfg.rope_scaling), _rope(k, cfg.rope_theta, pos, cfg.rope_scaling)
         rep = Hq // Hkv
         k = k.repeat_interleave(rep, dim=2)
         v = v.repeat_interleave(rep, dim=2)
@@ -92,7 +112,7 @@ def reference_loss(model, tokens: torch.Tensor, targets: torch.Tensor, dtype: to
         a = F.silu(gu[..., : cfg.ffn_dim]) * gu[..., cfg.ffn_dim :]
         x = h + linear(a, P[pre + "w2"])
     hfin = _rmsnorm(x, P["norm"], cfg.norm_eps)
-    logits = hfin @ P["output"].t()
+    logits = hfin @ P["tok_embeddings" if cfg.tie_embeddings else "output"].t()
     loss = F.cross_entropy(logits.view(B * S, -1), targets.reshape(-1))
     loss.backward()
     return float(loss.item()), {n: p.grad for n, p in P.items()}

@@ -24,7 +24,7 @@ _LAUNCHES_PER_CALL = {
     "adamw": 1, "diloco_outer": 1, "heal_copy": 1,
     "q8_reduce_scatter": 1, "q8_slice_reduce": 1, "q8_gather_dequant": 1, "push_exchange": 1, "reduce_scatter": 1, "p2p": 1,
     "zero1_handshake": 1, "zero1_reduce": 1, "zero1_commit": 1, "zero1_update": 1, "z1_digest": 1, "z1_audit_compare": 1,
-    "rmsnorm_fwd_fp8": 1, "fp8_rows": 1, "fp8_swiglu": 1, "fp8_cols_t": 2,
+    "rmsnorm_fwd_fp8": 1, "fp8_rows": 1, "fp8_swiglu": 1, "fp8_cols_t": 2, "embedding_bwd": 2,
 }
 
 

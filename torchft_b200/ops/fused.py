@@ -7,6 +7,7 @@ There is no PyTorch fallback: on a CUDA box these always run ``_K`` kernels.
 
 from __future__ import annotations
 
+import math
 from typing import Optional, Tuple
 
 import numpy as np
@@ -162,10 +163,27 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
     return _SwiGLU.apply(gate_up)
 
 
-def rope_table(seq_len: int, head_dim: int, theta: float, device: torch.device) -> torch.Tensor:
-    """(cos, sin) table ``[seq_len, head_dim/2, 2]`` fp32 for interleaved-pair RoPE."""
+def rope_scaled_frequencies(inv: torch.Tensor, scaling: Tuple[float, float, float, int]) -> torch.Tensor:
+    """Llama-3.1 frequency scaling of the fp32 inverse frequencies ``inv``, computed in fp64 and rounded once to fp32.
+    ``scaling = (factor, low_freq_factor, high_freq_factor, original_max_position)``. With ``w = 2 pi / f``: ``w <
+    orig / high`` keeps ``f``; ``w > orig / low`` gives ``f / factor``; in between, with ``s = (orig / w - low) / (high -
+    low)``, ``(1 - s) f / factor + s f``."""
+    factor, low, high, orig = (float(x) for x in scaling)
+    f = inv.double()
+    w = 2 * math.pi / f
+    s = (orig / w - low) / (high - low)
+    out = torch.where(w < orig / high, f, torch.where(w > orig / low, f / factor, (1 - s) * f / factor + s * f))
+    return out.float()
+
+
+def rope_table(seq_len: int, head_dim: int, theta: float, device: torch.device,
+               scaling: Optional[Tuple[float, float, float, int]] = None) -> torch.Tensor:
+    """(cos, sin) table ``[seq_len, head_dim/2, 2]`` fp32 for interleaved-pair RoPE. ``scaling``: Llama-3.1 frequency
+    scaling ``(factor, low_freq_factor, high_freq_factor, original_max_position)`` (:func:`rope_scaled_frequencies`)."""
 
     inv = 1.0 / (theta ** (torch.arange(0, head_dim, 2, dtype=torch.float32, device=device) / head_dim))
+    if scaling is not None:
+        inv = rope_scaled_frequencies(inv, scaling)
     ang = torch.outer(torch.arange(seq_len, dtype=torch.float32, device=device), inv)
     return torch.stack((ang.cos(), ang.sin()), dim=-1).contiguous()
 
@@ -241,10 +259,9 @@ class _LinearCrossEntropy(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, h: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, chunk: int, ignore_index: int, count_valid: bool):  # type: ignore[override]
-        K = _native.load()
-        T, H = h.shape
-        V = weight.shape[0]
+    def forward(ctx, h: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, chunk: int, ignore_index: int,  # type: ignore[override]
+                count_valid: bool, tied: bool = False):
+        T = h.shape[0]
         # count_valid: divide by the number of non-ignored targets, counted on the device (no host sync). The kernels
         # keep grad_scale = 1/T and scale it by the device factor T / n_valid, which is exactly 1.0 when no target is
         # ignored, so that case is bit-identical to count_valid=False (divide by T).
@@ -253,47 +270,185 @@ class _LinearCrossEntropy(torch.autograd.Function):
             n_valid = (target != ignore_index).sum().clamp_(min=1).float()
             scale = torch.full((), float(T), dtype=torch.float32, device=h.device).div_(n_valid)
         need_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
-        dh = torch.empty_like(h) if need_grad else None
         slot = getattr(weight, "_flat_grad", None)
+        losses = torch.empty(T, dtype=torch.float32, device=h.device)
+        ctx.tied = None
+        if tied:
+            link = getattr(weight, "_tied_link", None)
+            if link is None or link.mode is not None:
+                raise RuntimeError("a tied head needs the weight's tied_embedding node earlier in the same forward")
+            if need_grad and slot is not None and weight.grad is not None and weight.grad.data_ptr() == slot.data_ptr():
+                # the slot already holds a gradient (reset_grads(zero=True)): the head's dW must be added to it times
+                # the upstream scale, which only backward knows, so backward recomputes the chunks (no [V, d] buffer)
+                _xent_chunks(h, weight, target, chunk, ignore_index, scale, losses, None, None)
+                ctx.save_for_backward(h, weight, target, scale)
+                ctx.meta = (chunk, ignore_index)
+                link.mode, link.buf = "accumulate", slot.view(weight.shape)
+                ctx.tied = link
+                loss = losses.sum() / max(T, 1)
+                return loss * scale if scale is not None else loss
+        dh = torch.empty_like(h) if need_grad else None
         direct = need_grad and slot is not None and weight.grad is None
         dW = (slot.view(weight.shape).zero_() if direct else torch.zeros_like(weight)) if need_grad else None
         ctx.direct = direct
-        losses = torch.empty(T, dtype=torch.float32, device=h.device)
-        sp = _native.stream_ptr()
-        for lo in range(0, T, chunk):
-            hi = min(lo + chunk, T)
-            hc = h[lo:hi]
-            logits = hc @ weight.t()  # [c, V] bf16, cuBLAS
-            K.xent(
-                logits.data_ptr(), target[lo:hi].data_ptr(), losses[lo:hi].data_ptr(), hi - lo, V,
-                logits.stride(0), 1.0 / max(T, 1), ignore_index, sp, scale.data_ptr() if scale is not None else 0,
-            )
-            if need_grad:
-                torch.mm(logits, weight, out=dh[lo:hi])
-                dW.addmm_(logits.t(), hc)
-            del logits
-        ctx.save_for_backward(dh, dW)
+        _xent_chunks(h, weight, target, chunk, ignore_index, scale, losses, dh, dW)
+        if tied and need_grad:
+            # the embedding node adds its part into dW and hands autograd the sum: the weight's only gradient
+            link.mode, link.buf = ("direct" if direct else "own"), dW
+            ctx.tied = link
+            ctx.save_for_backward(dh)
+        else:
+            ctx.save_for_backward(dh, dW)
         ctx.need = need_grad
         loss = losses.sum() / max(T, 1)
         return loss * scale if scale is not None else loss
 
     @staticmethod
     def backward(ctx, g: torch.Tensor):  # type: ignore[override]
+        link = ctx.tied
+        if link is not None and link.mode == "accumulate":
+            h, weight, target, scale = ctx.saved_tensors
+            chunk, ignore_index = ctx.meta
+            # the upstream scalar rides in the cross-entropy kernel's device factor: dlogits come out scaled by it
+            gs = g.float() if scale is None else scale * g.float()
+            dh = torch.empty_like(h)
+            losses = torch.empty(h.shape[0], dtype=torch.float32, device=h.device)
+            _xent_chunks(h, weight, target, chunk, ignore_index, gs, losses, dh, link.buf)
+            return dh, None, None, None, None, None, None
+        if link is not None:
+            (dh,) = ctx.saved_tensors
+            link.buf.mul_(g.to(link.buf.dtype))
+            return dh * g.to(dh.dtype), None, None, None, None, None, None
         dh, dW = ctx.saved_tensors
         # g is the upstream scalar (1.0 for a plain loss.backward()); fold it in
         # without a host sync.
         # (dW already sits in the flat gradient buffer when ctx.direct; scale in place)
-        return dh * g.to(dh.dtype), (dW.mul_(g.to(dW.dtype)) if ctx.direct else dW * g.to(dW.dtype)), None, None, None, None
+        return (dh * g.to(dh.dtype), (dW.mul_(g.to(dW.dtype)) if ctx.direct else dW * g.to(dW.dtype)), None, None, None,
+                None, None)
+
+
+def _xent_chunks(h: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, chunk: int, ignore_index: int,
+                 scale: Optional[torch.Tensor], losses: torch.Tensor, dh: Optional[torch.Tensor],
+                 dW: Optional[torch.Tensor]) -> None:
+    """The chunk loop of :class:`_LinearCrossEntropy`: per chunk the bf16 logits (cuBLAS), the fused softmax/CE kernel
+    that overwrites them with dlogits (``1/T`` times the device factor ``scale``), then ``dh = dlogits @ W`` and ``dW +=
+    dlogits^T h`` when ``dh`` is given."""
+    K = _native.load()
+    T, V = h.shape[0], weight.shape[0]
+    sp = _native.stream_ptr()
+    for lo in range(0, T, chunk):
+        hi = min(lo + chunk, T)
+        hc = h[lo:hi]
+        logits = hc @ weight.t()  # [c, V] bf16, cuBLAS
+        K.xent(
+            logits.data_ptr(), target[lo:hi].data_ptr(), losses[lo:hi].data_ptr(), hi - lo, V,
+            logits.stride(0), 1.0 / max(T, 1), ignore_index, sp, scale.data_ptr() if scale is not None else 0,
+        )
+        if dh is not None:
+            torch.mm(logits, weight, out=dh[lo:hi])
+            dW.addmm_(logits.t(), hc)
+        del logits
 
 
 def linear_cross_entropy(h: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, chunk: int = 2048,
-                         ignore_index: int = -100, count_valid: bool = True) -> torch.Tensor:
+                         ignore_index: int = -100, count_valid: bool = True, tied: bool = False) -> torch.Tensor:
     """Mean cross entropy of ``h @ weight.T`` against ``target`` (int64).
 
     With ``count_valid`` (the default) the mean is over targets that are not ``ignore_index``, counted on the device
-    without a host sync; with ``count_valid=False`` the sum is divided by the number of rows."""
+    without a host sync; with ``count_valid=False`` the sum is divided by the number of rows.
+
+    ``tied``: ``weight`` is also the token embedding, read earlier in the same forward through :func:`tied_embedding`.
+    This node then returns no gradient for ``weight``: it leaves its part in the buffer that the embedding node adds into
+    and hands to autograd, so the weight gets ONE gradient (one post-accumulate-grad event) after both parts. In a
+    ``FlatParams`` buffer with the gradient dropped that buffer is the weight's flat slot, written here during the
+    forward as the untied head does; with a zeroed slot (``reset_grads(zero=True)``) backward recomputes the chunks and
+    adds into the slot; without a flat slot it is a new zeroed gradient."""
     assert h.dim() == 2 and target.dim() == 1 and h.shape[0] == target.shape[0]
-    return _LinearCrossEntropy.apply(h.contiguous(), weight, target.contiguous(), chunk, ignore_index, count_valid)
+    return _LinearCrossEntropy.apply(h.contiguous(), weight, target.contiguous(), chunk, ignore_index, count_valid, tied)
+
+
+class _TiedLink:
+    """What the tied head of one forward left for the embedding node's backward: ``mode`` ``None`` (no tied head ran),
+    ``"direct"`` (``buf`` is the flat slot, holding the head's part only), ``"own"`` (``buf`` is a new gradient holding
+    the head's part) or ``"accumulate"`` (``buf`` is the flat slot, which is ``p.grad`` and already holds everything
+    else)."""
+
+    __slots__ = ("mode", "buf")
+
+    def __init__(self) -> None:
+        self.mode: Optional[str] = None
+        self.buf: Optional[torch.Tensor] = None
+
+
+def embedding_bwd(ids: torch.Tensor, dx: torch.Tensor, grad: torch.Tensor) -> torch.Tensor:
+    """``grad[v] = bf16(grad[v] + sum of dx[t] over the tokens t with ids[t] = v)`` in place, for every id that occurs;
+    the sum is fp32 with one rounding per touched row, and its order depends on the ids alone (bit-identical launches).
+    ``ids`` int64 ``[T]`` (any shape, flattened; ids must be in ``[0, V)``, which ``F.embedding`` checked in forward),
+    ``dx`` bf16 ``[T, d]`` with unit column stride and 16-byte aligned rows, ``grad`` a contiguous bf16 ``[V, d]``.
+    The ids are sorted stably on the current stream (no host sync). Returns ``grad``."""
+    K = _native.load()
+    if dx.dim() != 2 or grad.dim() != 2 or dx.shape[1] != grad.shape[1]:
+        raise ValueError(f"embedding_bwd takes dx [T, d] and grad [V, d], got {tuple(dx.shape)} and {tuple(grad.shape)}")
+    T, d = dx.shape
+    if d % 8:
+        raise ValueError(f"embedding_bwd: the row width must be a multiple of 8, got {d}")
+    if ids.dtype != torch.int64 or ids.numel() != T or ids.device != dx.device:
+        raise ValueError(f"embedding_bwd: ids must be {T} int64 values on {dx.device}")
+    _chk(grad, "grad")
+    _chk(dx, "dx")
+    if not grad.is_contiguous() or dx.stride(1) != 1 or dx.stride(0) % 8:
+        raise ValueError("embedding_bwd: grad must be contiguous and dx rows 16-byte aligned with unit column stride")
+    if T == 0:
+        return grad
+    sid, perm = torch.sort(ids.reshape(-1), stable=True)
+    partial = torch.empty((K.embedding_bwd_pieces(T), 2, d), dtype=torch.float32, device=dx.device)
+    K.embedding_bwd(sid.data_ptr(), perm.data_ptr(), dx.data_ptr(), dx.stride(0), grad.data_ptr(), partial.data_ptr(),
+                    T, d, _native.stream_ptr())
+    return grad
+
+
+# adding -0.0 is the identity on every bf16 value, -0.0 included
+_NEG_ZERO = {}
+
+
+class _TiedEmbedding(torch.autograd.Function):
+    """``F.embedding(tokens, W)`` whose backward adds the token gradients into the tied weight's gradient buffer in place
+    with :func:`embedding_bwd` (see :func:`linear_cross_entropy` ``tied``)."""
+
+    @staticmethod
+    def forward(ctx, tokens: torch.Tensor, W: torch.Tensor) -> torch.Tensor:  # type: ignore[override]
+        link = _TiedLink()
+        W._tied_link = link  # the tied head of this forward finds it here
+        ctx.link = link
+        ctx.save_for_backward(tokens, W)
+        return torch.nn.functional.embedding(tokens, W)
+
+    @staticmethod
+    def backward(ctx, dx: torch.Tensor):  # type: ignore[override]
+        tokens, W = ctx.saved_tensors
+        link = ctx.link
+        d = W.shape[1]
+        dx2 = _rows_ok(dx.reshape(-1, d))
+        mode, buf = link.mode, link.buf
+        link.buf = None  # the buffer handed to autograd must have no other owner, or AccumulateGrad copies it
+        if mode is None:  # no tied head in this forward (e.g. the logits path): the embedding's own gradient
+            buf = torch.zeros_like(W)
+        embedding_bwd(tokens, dx2, buf)
+        if mode == "accumulate":
+            # p.grad IS the slot and now holds the whole sum; autograd still owes the weight its one event, so it gets
+            # a stride-0 -0.0 (no [V, d] allocation) whose in-place add leaves every bit as it is
+            key = (W.device, W.dtype)
+            if key not in _NEG_ZERO:
+                _NEG_ZERO[key] = torch.full((), -0.0, dtype=W.dtype, device=W.device)
+            return None, _NEG_ZERO[key].expand(W.shape)
+        # "direct": the slot view the head wrote (AccumulateGrad adopts it without a copy); else a gradient of our own
+        return None, buf
+
+
+def tied_embedding(tokens: torch.Tensor, W: torch.Tensor) -> torch.Tensor:
+    """Token embedding of a model whose LM head is ``W`` too (``linear_cross_entropy(..., tied=True)``): the forward is
+    ``F.embedding`` (its bounds check is the one check on the ids), the backward the in-place :func:`embedding_bwd`."""
+    return _TiedEmbedding.apply(tokens, W)
 
 
 def cross_entropy_inplace(logits: torch.Tensor, target: torch.Tensor, grad_scale: float = 1.0, ignore_index: int = -100) -> torch.Tensor:

@@ -136,6 +136,12 @@ class HSDPTrainer:
         from torchft_b200 import ManagedProcessGroup, Manager, Optimizer
         from torchft_b200.models.llama import CONFIGS, Llama
 
+        if CONFIGS[model].tie_embeddings:
+            # the tied head writes the embedding's gradient during the forward, which FSDP2's sharded gradients and
+            # reduce-scatter hooks do not provide for
+            raise ValueError(f"HSDPTrainer does not train models with tied embeddings ({model}); use "
+                             "FaultTolerantTrainer")
+
         assert dist.is_initialized(), "init the NCCL world first (torchrun)"
         rank, world = dist.get_rank(), dist.get_world_size()
         assert world % shards == 0

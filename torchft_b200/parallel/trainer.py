@@ -235,6 +235,8 @@ class FaultTolerantTrainer:
         )
         self._opt_stream: Optional[torch.cuda.Stream] = None
         self._opt_pending = False
+        # tied embeddings with gradient accumulation: the event the head's forward write into the tied slot waits for
+        self._head_after: Optional[torch.cuda.Event] = None
         if self.zero1:
             self.ddp = FlatDistributedDataParallel(self.manager, self.model, self.flat,
                                                    bucket_ranges=sorted(self._stage_ranges), reduce_fn=self._reduce_unit)
@@ -278,9 +280,13 @@ class FaultTolerantTrainer:
         self._opt_events = [torch.cuda.Event() for _ in self._stage_ranges]
         self._opt_stream = torch.cuda.Stream(device=self.device)
 
+        head_stage = len(self._stage_ranges) - 1
+
         def gate(stage: int) -> None:
             if self._opt_pending:
                 torch.cuda.current_stream().wait_event(self._opt_events[stage])
+            if stage == head_stage and self._head_after is not None:
+                torch.cuda.current_stream().wait_event(self._head_after)
 
         self.model.stage_hook = gate
 
@@ -385,13 +391,21 @@ class FaultTolerantTrainer:
             micro_cu = [slice_cu_seqlens(cu_seqlens, m * B * S, (m + 1) * B * S) for m in range(M)]
         cur = torch.cuda.current_stream()
         read_done = torch.cuda.Event()
+        tied = self.cfg.tie_embeddings
         losses = []
         self.manager.start_quorum()              # once: the quorum is fixed for all micro-batches of the step
         for m in range(M):
             self._micro = m
             self.flat.reset_grads()
-            loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B],  # overlaps micro-batch m-1's tail
-                            cu_seqlens=micro_cu[m])
+            # tied: the head writes its dW into the tied slot during the FORWARD, while the peers may still read that
+            # slot for micro-batch m-1's tied unit, the last reduce-scatter of its backward. The head's stage waits for
+            # the same event as the backward below; the blocks' forward still overlaps that reduce-scatter.
+            self._head_after = read_done if tied and m > 0 else None
+            try:
+                loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B],  # overlaps micro-batch m-1's tail
+                                cu_seqlens=micro_cu[m])
+            finally:
+                self._head_after = None
             if m > 0:
                 # backward overwrites the gradient buffer that the peers read in micro-batch m-1's reduce-scatters:
                 # wait until its last trailing handshake ("every peer is done reading mine") has passed
