@@ -603,6 +603,7 @@ def test_flat_adamw_step_ranges_matches_step():
 @pytest.mark.parametrize("n", [1, 7, 8, 9, 4099, 10_000_005])
 def test_diloco_outer(K, dtype, n):
     """Torch-SGD semantics (momentum mu, optional Nesterov) on the last global weights, then lerp towards the local ones."""
+    from _diloco_ref import outer_ref
     from torchft_b200.ops import _native
 
     gen = torch.Generator(device="cuda").manual_seed(n)
@@ -617,26 +618,14 @@ def test_diloco_outer(K, dtype, n):
                 o0, l0, b0 = orig.clone(), param.clone(), mom.clone()
                 K.diloco_outer(param.data_ptr(), orig.data_ptr(), grad.data_ptr(), mom.data_ptr(), n, _native.dtype_code(grad),
                                lr, mu, nesterov, alpha, 0, _sp())
-                lr_, mu_, al = _f32(lr), _f32(mu), _f32(alpha)
-                gd, bd = grad.double(), b0.double()
-                b = mu_ * bd + gd if mu else bd
-                step = (gd + mu_ * b if nesterov else b) if mu else gd
-                o = o0.double() - lr_ * step
-                lw = o + al * (l0.double() - o)
+                ref = outer_ref(o0, l0, b0, grad, lr, mu, nesterov, alpha)
                 tag = f"{dtype} n={n} mu={mu} nesterov={nesterov} alpha={alpha}"
-                if mu:
-                    # b = mu b + g: two roundings of its terms
-                    assert_close_elementwise(mom, b, ulps=0, abs_slack=2 * U * (mu_ * bd.abs() + gd.abs()) + FTZ, what=f"diloco mom {tag}")
+                if ref.mom_slack is not None:
+                    assert_close_elementwise(mom, ref.mom, ulps=0, abs_slack=ref.mom_slack, what=f"diloco mom {tag}")
                 else:
                     assert torch.equal(mom, b0)  # no momentum: the buffer is not touched
-                # step carries <= 2 U of |g| + mu |b| (+ mu |b| for Nesterov); lr * step and o - that: 2 U more of their
-                # terms, rounded to the dtype once (1 ulp)
-                s_abs = gd.abs() + mu_ * b.abs() * (2 if nesterov else 1)
-                o_sl = 4 * U * (lr_ * s_abs + o0.double().abs())
-                assert_close_elementwise(orig, o, ulps=1, abs_slack=o_sl + FTZ, what=f"diloco original {tag}")
-                # param = o + alpha (l - o) from the fp32 o: (1 - alpha) of o's error, 3 U of alpha |l - o|, 1 U of |result|
-                l_sl = abs(1 - al) * o_sl + 3 * U * al * (l0.double() - o).abs() + U * lw.abs()
-                assert_close_elementwise(param, lw, ulps=1, abs_slack=l_sl + FTZ, what=f"diloco param {tag}")
+                assert_close_elementwise(orig, ref.orig, ulps=1, abs_slack=ref.orig_slack, what=f"diloco original {tag}")
+                assert_close_elementwise(param, ref.param, ulps=1, abs_slack=ref.param_slack, what=f"diloco param {tag}")
     gate = torch.zeros(1, dtype=torch.int32, device="cuda")
     before = [t.clone() for t in (param, orig, mom)]
     K.diloco_outer(param.data_ptr(), orig.data_ptr(), grad.data_ptr(), mom.data_ptr(), n, _native.dtype_code(grad), lr, 0.9,

@@ -37,6 +37,7 @@ from torch.distributed import Work
 from torch.utils.hooks import RemovableHandle
 
 from torchft_b200.manager import Manager
+from torchft_b200.work import DummyWork
 
 try:
     from torch.distributed.tensor import DTensor
@@ -197,6 +198,9 @@ class _StreamingDiLoCoFragment:
         self._allreduce_work: List[Work] = []
         self._stream: Optional[torch.cuda.Stream] = torch.cuda.Stream() if torch.cuda.is_available() else None
         self._stop_event: Optional[torch.cuda.Event] = None
+        # recorded by prepare_sync behind the pseudo-gradient all-reduce, and with it every read of the live weights; the
+        # next inner optimizer step waits for it before it writes the weights
+        self._read_event: Optional[torch.cuda.Event] = None
 
         self._names: List[str] = []
         self._params: List[torch.Tensor] = []
@@ -275,6 +279,8 @@ class _StreamingDiLoCoFragment:
         span = ((end - lo) // es + 7) // 8 * 8
         if (lo - store.data_ptr()) + span * es > store.nbytes():
             span = (end - lo) // es
+        if not self._span_is_own(lo, lo + span * es):
+            return False
         alloc = getattr(self._manager, "alloc_symmetric", None)
         if alloc is None or not self._manager.supports_fused_delta():
             return False
@@ -297,6 +303,19 @@ class _StreamingDiLoCoFragment:
         for name, p in zip(self._names, self._params):
             off = (p.data.data_ptr() - lo) // es
             self.original_parameters[name] = self._flat_orig[off: off + p.numel()].view(p.shape)
+        return True
+
+    def _span_is_own(self, lo: int, hi: int) -> bool:
+        """True when the bytes ``[lo, hi)`` hold no weight of the inner optimizer outside this fragment. The flat path
+        applies the outer step to its whole span, gaps and rounded tail included, so a weight of another fragment (or
+        of none) lying there would be moved by this fragment's sync."""
+        mine = {id(p) for p in self._params}
+        for group in self._local_optimizer.param_groups:
+            for q in group["params"]:
+                t = _local_view(q.data)
+                start = t.data_ptr()
+                if id(q) not in mine and t.numel() and start < hi and lo < start + t.numel() * t.element_size():
+                    return False
         return True
 
     def _group_sizes(self) -> Dict[Tuple[torch.dtype, torch.device], List[int]]:
@@ -472,6 +491,21 @@ class _StreamingDiLoCoFragment:
             self._stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(self._stream) if self._stream is not None else nullcontext():
             self._launch_pseudograd_allreduce()
+            if self._stream is not None:
+                # a fused collective reads the weights on the process group's own stream: wait for it on this one
+                for w in self._allreduce_work:
+                    if not isinstance(w, DummyWork):  # a latched error: nothing was launched
+                        w.block_current_stream()
+                self._read_event = self._stream.record_event()
+
+    def fence_weight_writes(self) -> None:
+        """Make the current stream wait until the launched pseudo-gradient no longer reads the live weights. Called
+        before every inner optimizer step: with ``fragment_sync_delay >= 1`` that step would otherwise write weights
+        the quantisation or the subtraction has not read yet, so the pseudo-gradient would hold part of an extra inner
+        step, different on every replica and every run. Forward and backward still run beside the all-reduce."""
+        if self._read_event is not None:
+            torch.cuda.current_stream().wait_event(self._read_event)
+            self._read_event = None
 
     @torch.profiler.record_function("torchft::local_sgd::perform_sync")
     def perform_sync(self) -> bool:
@@ -596,6 +630,8 @@ class DiLoCo:
 
     def _step_pre_hook(self, _optim: optim.Optimizer, _args: Tuple[Any, ...], _kwargs: Dict[str, Any]) -> None:
         self._manager.disallow_state_dict_read()
+        for f in self._fragments:
+            f.fence_weight_writes()
 
     def _wait(self) -> None:
         for f in self._fragments:
