@@ -58,6 +58,8 @@ class Status {
   }
   // Global gradient norm the clipping commit kernel posted for `seq` (valid once verdict(seq) is not -1).
   float grad_norm(uint32_t seq) const { return host_->gnorm[seq & (kVerdictRing - 1)]; }
+  // Why the token-mean commit kernel vetoed `seq` (zero1::kVetoRows bits; valid once verdict(seq) is not -1).
+  uint32_t reason(uint32_t seq) const { return host_->reason[seq & (kVerdictRing - 1)]; }
   void set_timeout_ms(double ms) { host_->timeout_ns = (uint64_t)(ms * 1e6); }
   double timeout_ms() const { return (double)host_->timeout_ns / 1e6; }
   StatusBlock* dev() const { return dev_; }
@@ -215,6 +217,8 @@ PYBIND11_MODULE(_K, m) {
   m.attr("Q8_GROUP") = 512;
   m.attr("ZERO1_MAX_NO_DECAY") = kMaxNoDecay;
   m.attr("ZERO1_MAX_BLOCKS") = kZero1MaxBlocks;
+  m.attr("ZERO1_TOKSLOT_BYTES") = (int)sizeof(zero1::TokSlot);
+  m.attr("ZERO1_VETO_ROWS") = zero1::kVetoRows;
   m.attr("ZERO1_BF16_MOMENTS") = true;  // zero1_update takes moment_dtype = bf16
   m.attr("ZERO1_EMA") = true;           // zero1_update takes an EMA of the weights and mode 2
 
@@ -227,6 +231,7 @@ PYBIND11_MODULE(_K, m) {
       .def("clear", &Status::clear)
       .def("verdict", &Status::verdict)
       .def("grad_norm", &Status::grad_norm)
+      .def("reason", &Status::reason)
       .def("set_timeout_ms", &Status::set_timeout_ms)
       .def("timeout_ms", &Status::timeout_ms);
 
@@ -321,9 +326,13 @@ PYBIND11_MODULE(_K, m) {
   m.def(
       "zero1_commit",
       [](const PeerTableH& pt, const Status& st, uintptr_t gate, uint64_t flag, uint32_t seq, int channel, bool host_ok,
-         bool exchange, const std::vector<uintptr_t>& gnorm, int nunits, float max_norm, uintptr_t norm, uintptr_t stream) {
+         bool exchange, const std::vector<uintptr_t>& gnorm, int nunits, float max_norm, uintptr_t norm,
+         const std::vector<uintptr_t>& tm, uintptr_t n_src, uintptr_t loss_src, long long rows, long long pmc,
+         bool contribute, uintptr_t tm_out, uintptr_t tm_count, uintptr_t stream) {
         if (!gnorm.empty() && (int)gnorm.size() != pt.pt.world)
           throw std::runtime_error("zero1_commit: need one z1_gnorm pointer per rank");
+        if (!tm.empty() && (int)tm.size() != pt.pt.world)
+          throw std::runtime_error("zero1_commit: need one z1_tokmean slot per rank");
         zero1::CommitArgs a{};
         a.pt = pt.pt;
         a.st = st.dev();
@@ -337,11 +346,20 @@ PYBIND11_MODULE(_K, m) {
         a.nunits = nunits;
         a.max_norm = max_norm;
         a.norm = P<float>(norm);
+        for (size_t r = 0; r < tm.size(); ++r) a.tm[r] = P<zero1::TokSlot>(tm[r]);
+        a.n_src = P<const long long>(n_src);
+        a.loss_src = P<const double>(loss_src);
+        a.rows = rows;
+        a.pmc = pmc;
+        a.contribute = contribute;
+        a.tm_out = P<float>(tm_out);
+        a.tm_count = P<long long>(tm_count);
         zero1_commit_launch(a, S(stream));
       },
       py::arg("pt"), py::arg("status"), py::arg("gate"), py::arg("flag"), py::arg("seq"), py::arg("channel"),
       py::arg("host_ok"), py::arg("exchange"), py::arg("gnorm"), py::arg("nunits"), py::arg("max_norm"), py::arg("norm"),
-      py::arg("stream"));
+      py::arg("tm"), py::arg("n_src"), py::arg("loss_src"), py::arg("rows"), py::arg("pmc"), py::arg("contribute"),
+      py::arg("tm_out"), py::arg("tm_count"), py::arg("stream"));
   m.def(
       "zero1_update",
       [](const PeerTableH& pt, uintptr_t mc_base, uintptr_t gate, size_t poff, uintptr_t grad, uintptr_t master, uintptr_t mm,

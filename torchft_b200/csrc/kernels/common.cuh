@@ -79,6 +79,9 @@ struct StatusBlock {
   // device -> host: global gradient norm of commit seq (slot seq % ring), written before the verdict of the same slot
   // when the commit kernel clips (zero1.cu); read once that verdict is there
   volatile float gnorm[64];
+  // device -> host: why the commit kernel vetoed commit seq (zero1::kVetoRows, 0 = no reason of its own), written before
+  // the verdict of the same slot when it averages over tokens (zero1.cu)
+  volatile uint32_t reason[64];
 };
 constexpr uint32_t kVerdictRing = 64;
 

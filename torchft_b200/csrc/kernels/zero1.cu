@@ -34,6 +34,11 @@
 // slice in fp32 into a per-rank accumulator of the primary slices only (no bf16 rounding, no gradient write, no push);
 // the last one adds the accumulator and finishes exactly like a single step (scale, bf16, buddy push, CLIP squares).
 //
+// Global token mean (opt-in, TM template flag of the commit kernel / non-null slots): every rank publishes its count of
+// valid targets, its row count and its loss sum beside the verdict; the commit kernel sums them over the quorum and
+// folds P * M * c / N into the coefficient the update kernel already multiplies the gradient by, so the step applies the
+// gradient of the mean over every valid target of the quorum. Ranks with different row counts veto the step.
+//
 // Learning-rate schedule and weight-decay exemptions (opt-in, non-null table / non-zero count, no template flag): the
 // update kernel reads the rate of the committed update count gate[1] from a device table, and vectors inside up to
 // kMaxNoDecay unit-relative ranges take no decay.
@@ -67,6 +72,8 @@ namespace tft {
 using zero1::CommitArgs;
 using zero1::HsArgs;
 using zero1::RSArgs;
+using zero1::TokSlot;
+using zero1::kVetoRows;
 using zero1::UpdArgs;
 
 namespace {
@@ -303,6 +310,20 @@ __device__ __forceinline__ double rank_sumsq(const double* p, int n) {
 // that kernel sits behind the reduce-scatter handshake every rank must reach. This rank reaches its next handshake only
 // after this commit kernel (Zero1Optimizer orders the comm stream behind its last commit), so the partials read here
 // cannot change under the loads. At W = 1 or without the exchange the same ordering protects this rank's own partials.
+//
+// Why the token counts need two slots, and why these two are enough (TM). A rank publishes (n, rows, loss) here, in the
+// kernel, before any lane stores an arrival flag; a peer reads them after acquiring that flag, in its own commit kernel
+// for the same step. The reduce-scatter handshake does not protect them as it protects the partials: they are written
+// in the commit, not in the reduce, so without clipping nothing orders a fast rank's next commit behind a slow peer's
+// current one. The host therefore alternates the two slots by the parity of the commits since the quorum was
+// configured, which is the same on every rank of a quorum (each commit kernel pairs with one of every peer's by flag).
+// The slot written for commit c was last read by the peers' kernels for commit c - 2. Each peer's kernel c - 2 finished
+// before its kernel c - 1 (same stream) stored the arrival flag that this rank's kernel c - 1 acquired, and this
+// kernel follows that one on the commit stream: the reads are done before the write. A kernel c - 1 that did not
+// acquire some peer latched an error, and then this kernel writes nothing (and vetoes). At a quorum change every rank
+// drains its device before it publishes its mappings, so the old quorum's reads precede the new quorum's writes. The
+// inputs n_src and loss_src come from the current stream, which Zero1Optimizer.enqueue orders the commit stream behind.
+template <bool TM>
 __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
   const int t = threadIdx.x;
   const int W = a.pt.world, rank = a.pt.rank;
@@ -311,6 +332,34 @@ __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
   __shared__ double rank_sq[kMaxRanks];  // a peer whose arrival was not acquired contributes 0 (the verdict is 0 anyway)
   if (clip) {
     if (t < kMaxRanks) rank_sq[t] = (t == rank) ? rank_sumsq(a.gn[rank], a.nunits) : 0.0;
+    __syncwarp();
+  }
+  // TM: every rank's (n, rows, loss); a peer whose arrival was not acquired counts as (0, rows, 0)
+  __shared__ unsigned long long rank_n[kMaxRanks], rank_rows[kMaxRanks];
+  __shared__ double rank_loss[kMaxRanks];
+  // own_*: this rank's real count and loss, which a vetoed step reports; pub_*: what it publishes (0s when it does not
+  // contribute, as its gradient counts as 0s)
+  unsigned long long own_n = 0, pub_n = 0;
+  double own_loss = 0.0, pub_loss = 0.0;
+  if constexpr (TM) {
+    own_n = (unsigned long long)*a.n_src;
+    own_loss = *a.loss_src;
+    if (a.contribute) {
+      pub_n = own_n;
+      pub_loss = own_loss;
+    }
+    if (t < kMaxRanks) {
+      rank_n[t] = t == rank ? pub_n : 0ull;
+      rank_rows[t] = (unsigned long long)a.rows;
+      rank_loss[t] = t == rank ? pub_loss : 0.0;
+    }
+    if (t == 0 && a.st->error == kOk) {
+      TokSlot* s = a.tm[rank];
+      st_relaxed_sys(&s->n, pub_n);
+      st_relaxed_sys(&s->rows, (uint64_t)a.rows);
+      st_relaxed_sys(&s->loss, (uint64_t)__double_as_longlong(pub_loss));
+      __threadfence_system();  // the slot is complete before any lane's arrival flag below
+    }
     __syncwarp();
   }
   int ok = local_ok;
@@ -336,28 +385,64 @@ __global__ void __launch_bounds__(32, 1) zero1_commit_kernel(CommitArgs a) {
         ok = (v >= f * 2 && (v & 1ull)) ? local_ok : 0;  // stale (older) verdicts compare smaller
         // the peer's reduce kernels (and so its partials) precede its arrival flag: read them over NVLink now
         if (clip) rank_sq[t] = rank_sumsq(a.gn[t], a.nunits);
+        if constexpr (TM) {
+          // the peer's slot precedes its arrival flag (see above)
+          const TokSlot* s = a.tm[t];
+          rank_n[t] = ld_relaxed_sys(&s->n);
+          rank_rows[t] = ld_relaxed_sys(&s->rows);
+          rank_loss[t] = __longlong_as_double((long long)ld_relaxed_sys(&s->loss));
+        }
       } else {
         ok = 0;
       }
     }
     ok = __all_sync(0xffffffffu, ok);
   }
-  if (clip) __syncwarp();  // rank_sq[] written by the other lanes is visible to lane 0
+  if (clip || TM) __syncwarp();  // rank_sq[] (and the TM arrays) written by the other lanes are visible to lane 0
   if (t == 0) {
+    // TM: the quorum's token count and loss sum, in rank order (integers exact, fp64 in a fixed order: the same bits on
+    // every rank), and the factor that turns the reduced gradient, divided by pmc, into one divided by N. With no
+    // ignored target N = pmc and f is exactly 1.
+    unsigned long long N = 0;
+    double L = 0.0;
+    float f = 1.f;
+    uint32_t reason = 0;
+    if constexpr (TM) {
+      for (int r = 0; r < W; ++r) {
+        N += rank_n[r];
+        L += rank_loss[r];
+        if (rank_rows[r] != (unsigned long long)a.rows) reason = kVetoRows;  // one f cannot serve different shapes
+      }
+      f = (float)((double)a.pmc / (double)(N > 0 ? N : 1ull));
+      if (reason) ok = 0;
+    }
     if (clip) {
       // ranks in rank order 0..W-1 in fp64: every rank of the quorum adds the same numbers in the same order, so norm
       // and coefficient are bit-identical everywhere. coef = min(1, max_norm / (norm + 1e-6)) with torch's clip_grad_norm_
       // rounding: torch evaluates float / tensor as reciprocal(tensor) * float, each step IEEE fp32 (max_norm = inf
-      // gives exactly 1).
+      // gives exactly 1). TM: the norm of the gradient the update applies is norm * f.
       double sq = 0.0;
       for (int r = 0; r < W; ++r) sq += rank_sq[r];
-      const float norm = (float)sqrt(sq);
+      float norm = (float)sqrt(sq);
+      if constexpr (TM) norm = __fmul_rn(norm, f);
       const float coef = fminf(1.f, __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), a.max_norm));
       if ((__float_as_uint(norm) & 0x7f800000u) == 0x7f800000u) ok = 0;  // inf / nan: vetoed on every rank alike
       a.norm[0] = norm;
-      a.norm[1] = coef;
+      a.norm[1] = TM ? __fmul_rn(f, coef) : coef;
       a.st->gnorm[a.seq & (kVerdictRing - 1)] = norm;
       __threadfence_system();  // the norm slot is complete before the host can see this seq's verdict
+    } else if (TM) {
+      a.norm[1] = f;
+    }
+    if constexpr (TM) {
+      // a vetoed step reports this rank's own token mean (a non-contributing rank's too, though it published 0s): the
+      // quorum's sums may be missing a peer
+      const unsigned long long n = ok ? N : own_n;
+      a.tm_out[0] = (float)((ok ? L : own_loss) / (double)(n > 0 ? n : 1ull));
+      a.tm_out[1] = f;
+      a.tm_count[0] = (long long)N;
+      a.st->reason[a.seq & (kVerdictRing - 1)] = reason;
+      __threadfence_system();  // the reason slot is complete before the host can see this seq's verdict
     }
     a.gate[0] = ok;
     if (ok) a.gate[1] += 1;
@@ -634,7 +719,14 @@ void zero1_commit_launch(const CommitArgs& a, cudaStream_t stream) {
     if (!(a.max_norm > 0.f)) throw std::runtime_error("zero1_commit: max_norm must be > 0");
     if (std::count(a.gn, a.gn + a.pt.world, nullptr) != 0) throw std::runtime_error("zero1_commit: one z1_gnorm pointer per rank");
   }
-  zero1_commit_kernel<<<1, 32, 0, stream>>>(a);
+  const bool tm = std::any_of(a.tm, a.tm + a.pt.world, [](const TokSlot* p) { return p != nullptr; });
+  if (tm) {
+    if (std::count(a.tm, a.tm + a.pt.world, nullptr) != 0) throw std::runtime_error("zero1_commit: one z1_tokmean slot per rank");
+    if (a.n_src == nullptr || a.loss_src == nullptr || a.tm_out == nullptr || a.tm_count == nullptr || a.norm == nullptr)
+      throw std::runtime_error("zero1_commit: the token mean needs its two inputs and three outputs");
+    if (a.rows < 1 || a.pmc < 1) throw std::runtime_error("zero1_commit: the token mean needs rows >= 1 and P * M * c >= 1");
+  }
+  dispatch<false, true>(tm, [&](auto TM) { zero1_commit_kernel<TM><<<1, 32, 0, stream>>>(a); });
   TFT_CUDA_CHECK(cudaGetLastError());
 }
 

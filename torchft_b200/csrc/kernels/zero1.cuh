@@ -47,6 +47,18 @@ struct RSArgs {
   int acc_first;
 };
 
+// Global token mean: what one rank publishes for one commit in its z1_tokmean segment, which holds two of these (the
+// commit kernel's comment says why two). Words, so that peers read them with one relaxed 64-bit load each.
+struct TokSlot {
+  uint64_t n;      // valid targets of this rank's step (0 on a rank that does not contribute)
+  uint64_t rows;   // M * B * S of this rank's step
+  uint64_t loss;   // bits of the fp64 sum of its per-target losses
+  uint64_t pad;
+};
+
+// Why the commit kernel vetoed a step, posted beside the verdict (StatusBlock::reason).
+constexpr uint32_t kVetoRows = 1;  // the ranks published different row counts M * B * S
+
 // Commit verdict on the device: this rank's verdict, ANDed over the quorum through the signal pads.
 struct CommitArgs {
   PeerTable pt;        // pads only
@@ -64,6 +76,19 @@ struct CommitArgs {
   int nunits;
   float max_norm;
   float* norm;
+  // global token mean (a slot for every rank, or none; needs norm): tm[r] is rank r's TokSlot for this commit. The
+  // kernel publishes (n_src, rows, loss_src) in tm[rank] (n and loss 0 when !contribute), sums every rank's (n, loss)
+  // in rank order into N and L, vetoes the step when some rank's rows differ from this rank's, and writes
+  // f = fp32(pmc / max(N, 1)), tm_count[0] = N and tm_out = {L / max(N, 1) (vetoed: this rank's own mean), f}. The
+  // coefficient norm[1] becomes f (with clipping: f times the clip coefficient of the norm times f).
+  TokSlot* tm[kMaxRanks];
+  const long long* n_src;  // device int64: this rank's valid targets
+  const double* loss_src;  // device fp64: this rank's sum of per-target losses
+  long long rows;          // M * B * S of this rank's step
+  long long pmc;           // P * M * c: what the reduced gradient is already divided by
+  int contribute;
+  float* tm_out;
+  long long* tm_count;
 };
 
 // Gated AdamW on the held slices of one unit + all-gather of the primary slice's new bf16 weights.

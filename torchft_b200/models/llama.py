@@ -244,8 +244,10 @@ class Llama(nn.Module):
         return x
 
     def forward(self, tokens: torch.Tensor, targets: Optional[torch.Tensor] = None,
-                cu_seqlens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                cu_seqlens: Optional[torch.Tensor] = None, count_valid: bool = True) -> torch.Tensor:
         """Returns the mean next-token loss over the targets that are not -100 when ``targets`` is given, else logits.
+        With ``count_valid=False`` the loss sum is divided by the number of positions ``B * S`` instead (a divisor that
+        does not depend on the mask, for callers that average over several batches themselves).
 
         ``cu_seqlens`` (CPU int32 ``[N+1]``, see ``data.check_cu_seqlens``) packs several documents into each row:
         a token attends only to the earlier tokens of its own document, and its RoPE position is its offset in that
@@ -259,7 +261,7 @@ class Llama(nn.Module):
             return fused.rmsnorm(x, self.norm, self.cfg.norm_eps) @ self.head_weight().t()
         h = fused.rmsnorm(x, self.norm, self.cfg.norm_eps).view(B * S, d)
         return fused.linear_cross_entropy(h, self.head_weight(), targets.reshape(-1), chunk=self.cfg.loss_chunk,
-                                          tied=self.cfg.tie_embeddings)
+                                          count_valid=count_valid, tied=self.cfg.tie_embeddings)
 
 
 class FlatParams:

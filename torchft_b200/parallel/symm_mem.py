@@ -870,7 +870,10 @@ class SymmetricComm:
 
     def zero1_commit_(self, gate: torch.Tensor, host_ok: bool, exchange: bool,
                       stream: Optional[torch.cuda.Stream] = None, gnorm: Optional[str] = None, nunits: int = 0,
-                      max_norm: float = float("inf"), norm: Optional[torch.Tensor] = None) -> int:
+                      max_norm: float = float("inf"), norm: Optional[torch.Tensor] = None,
+                      tokens: Optional[str] = None, slot: int = 0, n_valid: Optional[torch.Tensor] = None,
+                      loss_sum: Optional[torch.Tensor] = None, rows: int = 0, divisor: int = 0, contribute: bool = True,
+                      token_out: Optional[torch.Tensor] = None, token_count: Optional[torch.Tensor] = None) -> int:
         """Device-side commit verdict (AND over the quorum when ``exchange``): writes ``gate[0]`` (verdict),
         increments ``gate[1]`` on success and posts the verdict to the host-mapped ring. Returns the sequence
         number to pass to :meth:`verdict`.
@@ -878,17 +881,37 @@ class SymmetricComm:
         ``gnorm`` (name of a segment of ``nunits`` fp64 partials per rank, written by :meth:`zero1_reduce_scatter_`)
         adds gradient clipping: the kernel sums every rank's partials in rank order (its own only at world 1 or without
         ``exchange``), writes ``norm[0]`` = the global L2 norm and ``norm[1]`` = ``min(1, max_norm / (norm + 1e-6))``
-        (fp32 tensor of two), posts the norm for :meth:`grad_norm` and vetoes the step when the norm is not finite."""
+        (fp32 tensor of two), posts the norm for :meth:`grad_norm` and vetoes the step when the norm is not finite.
+
+        ``tokens`` (name of a segment of two ``ZERO1_TOKSLOT_BYTES`` slots per rank; ``slot`` picks one, alternating
+        with every commit since the quorum was configured) adds the global token mean: the kernel publishes this rank's
+        valid-target count ``n_valid`` (device int64), its loss sum ``loss_sum`` (device fp64) and ``rows`` (both
+        published as 0 when not ``contribute``), sums the quorum's counts ``N`` and losses ``L`` in rank order, vetoes
+        the step when the ranks' ``rows`` differ (:meth:`commit_reason`), and writes ``f = fp32(divisor / max(N, 1))``,
+        ``token_count[0] = N``, ``token_out = [L / max(N, 1), f]`` (vetoed: this rank's own mean) and ``norm[1]`` =
+        ``f`` times the clip coefficient (1 without clipping), whose norm is then ``f`` times the reduced one."""
         with self._lock:
             if not self._configured:
                 raise RuntimeError("SymmetricComm is not configured")
             self._commit_seq = (self._commit_seq + 1) & 0x3fffffff
             seq = self._commit_seq
-            if gnorm is not None:
+            if gnorm is not None or tokens is not None:
                 assert norm is not None and norm.dtype == torch.float32 and norm.numel() >= 2
+            tm: List[int] = []
+            tm_args = (0, 0, 0, 0, True, 0, 0)
+            if tokens is not None:
+                assert slot in (0, 1)
+                assert n_valid is not None and n_valid.dtype == torch.int64 and n_valid.numel() == 1
+                assert loss_sum is not None and loss_sum.dtype == torch.float64 and loss_sum.numel() == 1
+                assert token_out is not None and token_out.dtype == torch.float32 and token_out.numel() >= 2
+                assert token_count is not None and token_count.dtype == torch.int64 and token_count.numel() >= 1
+                tm = [p + slot * self._K.ZERO1_TOKSLOT_BYTES for p in self._ptrs[tokens]]
+                tm_args = (n_valid.data_ptr(), loss_sum.data_ptr(), int(rows), int(divisor), bool(contribute),
+                           token_out.data_ptr(), token_count.data_ptr())
             self._K.zero1_commit(self._tables["core"], self._status, gate.data_ptr(), self._next_flag(), seq, _CH_USER,
                                  bool(host_ok), bool(exchange), self._ptrs[gnorm] if gnorm is not None else [], int(nunits),
-                                 float(max_norm), norm.data_ptr() if norm is not None else 0, _native.stream_ptr(stream))
+                                 float(max_norm), norm.data_ptr() if norm is not None else 0, tm, *tm_args,
+                                 _native.stream_ptr(stream))
             self.launches += 1
             return seq
 
@@ -902,6 +925,13 @@ class SymmetricComm:
         if self.verdict(seq) is None:
             return None
         return float(self._status.grad_norm(seq))
+
+    def commit_reason(self, seq: int) -> Optional[int]:
+        """Why the token-mean commit ``seq`` vetoed its step (``ZERO1_VETO_ROWS`` bits, 0 = no reason of its own) if
+        the kernel has run, else ``None`` (never blocks)."""
+        if self.verdict(seq) is None:
+            return None
+        return int(self._status.reason(seq))
 
     def zero1_update_(self, segment: str, poff: int, grad: int, master: int, m: int, v: int, nelem: int,
                       hyper: Tuple[float, float, float, float, float], gate: torch.Tensor, replication: int, mode: int,

@@ -105,6 +105,14 @@ class FaultTolerantTrainer:
             replica holds the same bf16 weights and the holders of each slice the same optimizer state; a disagreement
             fails the next step on every replica, and the next quorum repairs it (``Zero1Optimizer``). ``None``: env
             ``TORCHFT_B200_Z1_AUDIT_EVERY``, unset = 0, off. Not available on the classic all-reduce pipeline.
+        global_token_mean: FT-ZeRO-1: apply the gradient of the mean loss over every target that is not -100, in every
+            micro-batch, on every participating replica of the quorum (a healing replica contributes none), instead of
+            the mean of each replica's and each micro-batch's own mean. Each micro-batch's loss is then divided by its
+            ``B * S`` positions, and the commit kernel, which already exchanges the verdict, sums every replica's target
+            count and loss and scales the update by ``P * M * B * S / N`` (exactly 1 when no target is ignored). ``step``
+            and friends return ``sum of losses / N`` over the quorum, the same on every replica of a committed step; a
+            vetoed step returns this replica's own token mean. Replicas fed batches of different shapes veto the step.
+            Not available on the classic all-reduce pipeline.
         fp8_linears: run the forward and input-gradient GEMMs of the four block linears on fp8 tensor cores with
             row-scaled e4m3 operands (``LlamaConfig.fp8_linears``); weight gradients, the LM head and attention stay
             bf16, so the gradient buffer and the optimizer see bf16 exactly as without it. A model property: it applies
@@ -130,9 +138,8 @@ class FaultTolerantTrainer:
                  lr_steps: Optional[int] = None,
                  no_decay: Optional[Callable[[str, nn.Parameter], bool]] = None,
                  moment_dtype: Optional[torch.dtype] = None, ema_decay: Optional[float] = None,
-                 fp8_linears: Optional[bool] = None, audit_every: Optional[int] = None) -> None:
-        self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
-        torch.cuda.set_device(self.device)
+                 fp8_linears: Optional[bool] = None, audit_every: Optional[int] = None,
+                 global_token_mean: bool = False) -> None:
         cfg = CONFIGS[model] if isinstance(model, str) else model
         if activation_checkpoint is not None:
             cfg = dataclasses.replace(cfg, activation_checkpoint=activation_checkpoint)
@@ -162,11 +169,18 @@ class FaultTolerantTrainer:
             raise ValueError("ema_decay needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
         if audit_every is not None and audit_every and not self.zero1:
             raise ValueError("audit_every needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        if global_token_mean and not self.zero1:
+            raise ValueError("global_token_mean needs the FT-ZeRO-1 pipeline (backend='b200', zero1=True)")
+        self.global_token_mean = bool(global_token_mean)
         self._in_ema = False  # inside ema_weights(): the model holds the EMA weights
         if lr_lambda is not None and lr_steps is None:
             raise ValueError("lr_lambda needs lr_steps, the length of the schedule")
         self._micro = 0  # FT-ZeRO-1: index of the micro-batch whose backward is running
         self._steps_run = 0  # steps started by this trainer (a checkpoint restore must come first)
+
+        # the options are checked above, before anything touches the device
+        self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+        torch.cuda.set_device(self.device)
 
         # the replica group's own store (group world size 1 => this process hosts it)
         self._store = TCPStore("127.0.0.1", 0, is_master=True, wait_for_workers=False)
@@ -195,7 +209,7 @@ class FaultTolerantTrainer:
                                        compact=compact_state, min_world=min_replica_size, max_grad_norm=max_grad_norm,
                                        grad_accum_steps=self.grad_accum_steps, lr_lambda=lr_lambda,
                                        lr_steps=lr_steps or 0, moment_dtype=moment_dtype, ema_decay=ema_decay,
-                                       audit_every=audit_every)
+                                       audit_every=audit_every, global_token_mean=self.global_token_mean)
             self.flat = FlatParams(self.model, grad_alloc=lambda n: self.zopt.grad, device=self.device,
                                    param_alloc=lambda n: self.zopt.param)
         else:
@@ -354,13 +368,16 @@ class FaultTolerantTrainer:
         if self.zero1:
             self.manager.start_quorum()       # async; its thread first books the previous step's device verdict
             self.flat.reset_grads()           # wgrad GEMMs write the flat gradient buffer directly: no memset
-            loss = self.ddp(tokens, targets, cu_seqlens=cu_seqlens)  # forward; stage i waits for unit i's update
+            loss = self.ddp(tokens, targets, cu_seqlens=cu_seqlens,  # forward; stage i waits for unit i's update
+                            **self._loss_kw())
             loss.backward()                   # per-unit reduce-scatter kernels launch from the grad hooks
             self.ddp.finish(wait=False)       # issue what is left; the optimizer stream orders itself behind them
+            if self.global_token_mean:
+                self._publish_tokens(targets, [loss], tokens.numel())
             self.manager.commit_on_device(self.zopt)  # verdict kernel (no host sync, no RPC in steady state)
             self.zopt.update(self._opt_events)        # gated AdamW + weight all-gather, unit by unit
             self._opt_pending = True
-            return loss
+            return self.zopt.token_mean_loss() if self.global_token_mean else loss
         self.optim.zero_grad(set_to_none=True)  # start_quorum (async); no memset:
         self.flat.reset_grads()                  # wgrad GEMMs write the flat gradient buffer directly
         loss = self.ddp(tokens, targets, cu_seqlens=cu_seqlens)  # forward (fused kernels + cuBLAS + SDPA)
@@ -375,10 +392,14 @@ class FaultTolerantTrainer:
         """FT-ZeRO-1 step over ``M`` micro-batches: one quorum, ``M`` forward/backward passes whose reduce-scatters
         accumulate on the comm stream, one commit and one update.
 
-        The loss (and its gradient) is the mean of the ``M`` micro-batch means, each over its own targets that are not
-        -100, not the mean over all valid targets of the step. With packed documents the number of valid targets varies
-        more between micro-batches (one -100 per document), so a target in a micro-batch of many short documents weighs
-        a little more than one in a micro-batch of few long ones."""
+        By default the loss (and its gradient) is the mean of the ``M`` micro-batch means, each over its own targets that
+        are not -100, not the mean over all valid targets of the step, and the replicas are averaged alike. With packed
+        documents the number of valid targets varies more between micro-batches (one -100 per document, and a padded
+        tail), so a target in a micro-batch of many short documents weighs more than one in a micro-batch of few long
+        ones. With ``global_token_mean`` each micro-batch's loss is its sum over ``B * S`` instead, and the commit kernel
+        rescales the reduced gradient to the mean over every valid target of every micro-batch on every participating
+        replica: ``M`` micro-batches of ``B`` rows then take the step one batch of ``M * B`` rows takes, and so do
+        replicas with different masks. The loss returned is that global mean."""
         M = self.grad_accum_steps
         if tokens.shape[0] % M or tokens.shape[0] == 0 or targets.shape[0] != tokens.shape[0]:
             raise ValueError(f"grad_accum_steps={M} must divide the batch dimension of tokens and targets, got "
@@ -403,7 +424,7 @@ class FaultTolerantTrainer:
             self._head_after = read_done if tied and m > 0 else None
             try:
                 loss = self.ddp(tokens[m * B:(m + 1) * B], targets[m * B:(m + 1) * B],  # overlaps micro-batch m-1's tail
-                                cu_seqlens=micro_cu[m])
+                                cu_seqlens=micro_cu[m], **self._loss_kw())
             finally:
                 self._head_after = None
             if m > 0:
@@ -415,10 +436,31 @@ class FaultTolerantTrainer:
             if m < M - 1:
                 read_done.record(self.pg.comm_stream)
             losses.append(loss.detach().float())
+        if self.global_token_mean:
+            self._publish_tokens(targets, losses, B * tokens.shape[1])
         self.manager.commit_on_device(self.zopt)
         self.zopt.update(self._opt_events)
         self._opt_pending = True
+        if self.global_token_mean:
+            return self.zopt.token_mean_loss()
         return torch.stack(losses).mean()
+
+    def _loss_kw(self) -> Dict[str, Any]:
+        """Global token mean: each micro-batch's loss is its sum over its ``B * S`` positions, a divisor every replica
+        shares; the commit kernel turns the reduced gradient into the mean over the quorum's valid targets."""
+        return {"count_valid": False} if self.global_token_mean else {}
+
+    def _publish_tokens(self, targets: torch.Tensor, losses: List[torch.Tensor], c: int) -> None:
+        """Hand the commit this step's count of valid targets (over the whole ``(M * B, S)`` input) and its loss sum
+        ``sum_m loss_m * c`` in fp64, added in micro-batch order as the commit kernel adds the replicas in rank order."""
+        n = (targets != -100).sum()
+        total: Optional[torch.Tensor] = None
+        for loss in losses:
+            x = loss.detach().double() * c
+            total = x if total is None else total + x
+        assert total is not None
+        m = self.manager
+        self.zopt.publish_tokens(n, total, targets.numel(), max(m.num_participants(), 1), m.is_participating())
 
     def _stage_inputs(self, tokens_cpu: torch.Tensor, targets_cpu: torch.Tensor) -> None:
         B, S = tokens_cpu.shape

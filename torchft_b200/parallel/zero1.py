@@ -48,11 +48,12 @@ __all__ = ["ShardLayout", "Zero1Optimizer", "merge_ranges", "subtract_ranges", "
            "lr_schedule_table", "split_no_decay", "schedule_digest", "check_moment_agreement", "moment_type", "sr_bits", "bf16_sr",
            "sr_bits_ema", "bf16_sr_ema", "ema_decay_value", "ema_coefficient", "ema_step", "ema_record", "check_ema_agreement",
            "split_ema_reads", "z1_digest", "audit_every_value", "audit_stride", "decode_audit_report", "audit_findings",
-           "audit_seed_source"]
+           "audit_seed_source", "token_mean_factor", "token_mean_commit"]
 
 PAGE_SHIFT = 16  # compact state: 64 Ki-element pages (256 KiB per fp32 array)
 CONVERT_CHUNK = 1 << 24  # restore into the other moment type: elements converted per device temporary
 GNORM_UNITS = 4096  # gradient clipping: capacity of the z1_gnorm segment in units (one fp64 partial per unit)
+TOKEN_SLOTS = 2  # global token mean: published slots per rank, used alternately by consecutive commits
 MAX_NO_DECAY = 4  # weight-decay exemptions per unit and update launch (kMaxNoDecay of csrc/kernels/api.h)
 SR_SEED = 0x27D4EB2F  # bf16 moments: the fixed seed of the rounding bits (sr_bits of csrc/kernels/zero1.cu)
 SR_SEED_EMA = 0x165667B1  # bf16 EMA of the weights: the seed of its rounding bits (sr_bits_ema of zero1.cu)
@@ -71,6 +72,49 @@ def clip_threshold(max_grad_norm: Optional[float]) -> Optional[float]:
     if not max_grad_norm > 0:
         raise ValueError(f"max_grad_norm must be > 0 (inf: compute the norm without scaling), got {max_grad_norm}")
     return max_grad_norm
+
+
+# --------------------------------------------------------------------------- global token mean
+def token_mean_factor(divisor: int, n: int) -> float:
+    """The global token mean's factor ``f = fp32(divisor / max(N, 1))``, from integers as the commit kernel computes it:
+    ``divisor = P * M * c`` is what the reduced gradient is already divided by, ``N`` the quorum's valid targets. Exactly
+    1.0 when no target is ignored (``N = P * M * c``); ``divisor`` itself when there is none (every gradient is then 0)."""
+    import numpy as np
+
+    return float(np.float32(int(divisor) / max(int(n), 1)))  # int / int is the correctly rounded fp64 quotient
+
+
+def token_mean_commit(published: Sequence[Tuple[int, float, int]], rows: int, divisor: int,
+                      max_norm: Optional[float] = None, norm: Optional[float] = None, own: int = 0,
+                      own_mean: Optional[Tuple[int, float]] = None) -> Dict[str, Any]:
+    """What the commit kernel of the rank at position ``own`` computes from the quorum's published ``(n, loss, rows)``
+    in rank order (a rank that does not contribute publishes ``n = 0, loss = 0``), given its own ``rows`` and
+    ``divisor``: ``N`` (exact), ``f`` (:func:`token_mean_factor`), ``veto`` (some rank's rows differ from ``rows``), the
+    reported ``loss`` (fp32 of ``L / max(N, 1)`` with ``L`` the fp64 sum in rank order; vetoed: ``own_mean``, the rank's
+    own ``(n, loss)``, which a non-contributing rank knows though it published 0s; default: its published pair) and
+    ``coef``, the coefficient the update multiplies the reduced gradient by. With clipping (``max_norm``, and ``norm``
+    the fp32 norm of the reduced gradient) also ``norm``, which becomes ``fp32(norm * f)``, and ``coef = f * min(1,
+    max_norm / (norm + 1e-6))`` with torch's fp32 rounding. Bit for bit what the kernel writes, on every rank alike."""
+    import numpy as np
+
+    f32 = np.float32
+    n_total = sum(int(n) for n, _, _ in published)
+    total = 0.0
+    for _, loss, _ in published:
+        total += float(loss)  # fp64, rank order
+    veto = any(int(r) != int(rows) for _, _, r in published)
+    f = token_mean_factor(divisor, n_total)
+    out: Dict[str, Any] = {"N": n_total, "f": f, "veto": veto, "coef": f}
+    if norm is not None:
+        assert max_norm is not None
+        g = f32(f32(norm) * f32(f))
+        clip = min(f32(1.0), f32(f32(1.0) / f32(g + f32(1e-6))) * f32(max_norm))
+        out["norm"], out["coef"] = float(g), float(f32(f32(f) * clip))
+        veto = veto or not math.isfinite(float(g))
+        out["veto"] = veto
+    n_own, l_own = (int(published[own][0]), float(published[own][1])) if own_mean is None else own_mean
+    out["loss"] = float(f32(l_own / max(n_own, 1))) if veto else float(f32(total / max(n_total, 1)))
+    return out
 
 
 # --------------------------------------------------------------------------- learning-rate schedule, decay exemptions
@@ -748,6 +792,17 @@ class Zero1Optimizer:
     every replica (counted in ``nonfinite_steps``): no state changes and ``t`` does not advance. ``grad_norm`` is the
     device scalar of the last commit, ``last_grad_norm`` the host value of the last resolved step.
 
+    With ``global_token_mean`` the step applies the gradient of the mean loss over every valid target of the quorum
+    instead of the mean of the replicas' (and micro-batches') own means. Before each commit the caller hands
+    :meth:`publish_tokens` this rank's count of valid targets ``n``, its loss sum ``L`` (losses normalised by the row
+    count ``c = B * S`` of a micro-batch, so ``L = sum_m loss_m * c``) and its shape. The commit kernel publishes them in
+    the small ``z1_tokmean`` segment, sums the quorum's counts ``N`` and losses in rank order and folds
+    ``f = fp32(P * M * c / max(N, 1))`` into the coefficient the update multiplies the reduced gradient by (with clipping
+    the norm is ``f`` times the reduced gradient's and the coefficient ``f`` times the clip coefficient). With no ignored
+    target ``f`` is exactly 1 and the step is bit-identical to one without the mode. Ranks whose ``M * B * S`` differ
+    veto the step on every rank (counted in ``row_mismatch_steps``). :meth:`token_mean_loss` gives ``L / N`` of the last
+    commit, the same bits on every rank of a committed step.
+
     With ``grad_accum_steps = M > 1`` one step reduces ``M`` micro-batches: :meth:`reduce_scatter` takes the micro-batch
     index, micro-batches ``0 .. M-2`` add their fp32 reduced slice into an accumulator that covers only this rank's
     primary slices (an ordinary device tensor of about ``4 * numel / min_world`` bytes, :meth:`accum_bytes`), and the
@@ -805,6 +860,8 @@ class Zero1Optimizer:
             ``k = 1`` only the weights are compared; at world 1 nothing is audited. ``audits``, ``divergences`` and
             ``last_audit`` (the decoded report, :meth:`audit_report`) tell what it found. Every replica of a quorum must
             use the same period.
+        global_token_mean: average over every valid target of the quorum (see above); every replica of a quorum must
+            use it alike (the ``z1_tokmean`` segment is allocated only with it)
     """
 
     def __init__(self, pg: Any, numel: int, units: Optional[Sequence[Range]] = None, lr: float = 3e-4,
@@ -814,7 +871,8 @@ class Zero1Optimizer:
                  max_grad_norm: Optional[float] = None, grad_accum_steps: int = 1,
                  lr_lambda: Optional[Callable[[int], float]] = None, lr_steps: int = 0,
                  no_decay: Sequence[Range] = (), moment_dtype: Optional[torch.dtype] = None,
-                 ema_decay: Optional[float] = None, audit_every: Optional[int] = None) -> None:
+                 ema_decay: Optional[float] = None, audit_every: Optional[int] = None,
+                 global_token_mean: bool = False) -> None:
         from torchft_b200.ops import _native
 
         self.moment_dtype = moment_type(moment_dtype)
@@ -885,6 +943,18 @@ class Zero1Optimizer:
             self._clip = torch.zeros(2, dtype=torch.float32, device=self.device)  # [norm, coef] of the last commit
             self.grad_norm = self._clip[0]
             self._resolved_norm: Optional[float] = None
+        self.global_token_mean = bool(global_token_mean)
+        self.row_mismatch_steps = 0      # token mean: steps vetoed because the ranks' M * B * S differed
+        self._tok_pending: Optional[Tuple[torch.Tensor, torch.Tensor, int, int, bool]] = None  # publish_tokens()
+        self._tok_commits = 0            # commits since the last quorum change: their parity picks the slot
+        self._resolved_reason: Optional[int] = None
+        if self.global_token_mean:
+            # two slots per rank (zero1_commit_kernel explains why two are enough); [N] and [L / N, f] of the last commit
+            self._tok_slots = pg.alloc_symmetric("z1_tokmean", TOKEN_SLOTS * self._K.ZERO1_TOKSLOT_BYTES)
+            self._tok_count = torch.zeros(1, dtype=torch.int64, device=self.device)
+            self._tok_out = torch.zeros(2, dtype=torch.float32, device=self.device)
+            if self.max_grad_norm is None:
+                self._clip = torch.zeros(2, dtype=torch.float32, device=self.device)  # [unused, f]: the coefficient
         # element e of the flat vector lives at pool index (table[e >> shift] << shift) | (e & mask) of paged state; full-size
         # state has no table and keeps it at e (see _pieces)
         self._table: Optional[torch.Tensor] = None
@@ -1041,12 +1111,14 @@ class Zero1Optimizer:
                 # a snapshot copy may still read the state that pulls, seeds, page reuse and heal are about to rewrite
                 self._snap_done.synchronize()
             names = ("z1_param", "z1_grad", "z1_master", "z1_m", "z1_v") + (("z1_gnorm",) if self.max_grad_norm is not None else ()) \
-                + (("z1_ema",) if self.ema is not None else ()) + (("z1_audit",) if self.audit_every else ())
+                + (("z1_ema",) if self.ema is not None else ()) + (("z1_audit",) if self.audit_every else ()) \
+                + (("z1_tokmean",) if self.global_token_mean else ())
             missing = [n for n in names if not self.comm.is_symmetric(n)]
             if missing:
                 # the kernels dereference peer pointers: every replica must construct its Zero1Optimizer before its first
                 # quorum (segments allocated later only become symmetric at the NEXT quorum change)
                 raise RuntimeError(f"FT-ZeRO-1 segments {missing} are not mapped on every replica of this quorum")
+            self._tok_commits = 0  # every rank of the new quorum starts its slot parity here
             if self.grad_accum_steps > 1:
                 self._accum_for(rank, world)
             self._apply_audit()  # before publishing: the ranges a diverged audit condemned are not claimed
@@ -1301,6 +1373,26 @@ class Zero1Optimizer:
         """The stream the verdict and update kernels run on (the trainer's optimizer stream)."""
         self._commit_stream = stream
 
+    def publish_tokens(self, n_valid: torch.Tensor, loss_sum: torch.Tensor, rows: int, participants: int,
+                       contribute: bool) -> None:
+        """Global token mean: what the next :meth:`enqueue` publishes for this rank. ``n_valid`` (device int64 scalar)
+        counts the step's targets that are not ignored, ``loss_sum`` (device fp64 scalar) is the sum of their losses,
+        ``rows`` is the step's ``M * B * S`` and ``participants`` the ``P`` the reduce-scatters divided by. Both tensors
+        are written on the current stream, which the commit stream waits for. A rank that does not ``contribute``
+        publishes 0 targets and a loss of 0 (a vetoed step still reports its own mean from the real pair)."""
+        if not self.global_token_mean:
+            raise RuntimeError("publish_tokens needs Zero1Optimizer(global_token_mean=True)")
+        self._tok_pending = (n_valid.reshape(1), loss_sum.reshape(1), int(rows), max(int(participants), 1), bool(contribute))
+
+    def token_mean_loss(self) -> torch.Tensor:
+        """Global token mean: ``L / N`` of the last commit as a new device scalar, copied on the current stream behind
+        that commit. The same bits on every rank of a committed step; a vetoed step gives this rank's own ``L / n``."""
+        if not self.global_token_mean or self._commit_event is None:
+            raise RuntimeError("token_mean_loss needs a commit of Zero1Optimizer(global_token_mean=True)")
+        cur = torch.cuda.current_stream(self.device)
+        cur.wait_event(self._commit_event)
+        return self._tok_out[0].clone()
+
     def enqueue(self, host_ok: bool) -> int:
         """Enqueue the verdict kernel behind this step's reduce-scatters (comm stream) and backward (current stream).
 
@@ -1323,7 +1415,20 @@ class Zero1Optimizer:
         self._commit_layout = (self.comm.rank, self.comm.world)
         clip = {} if self.max_grad_norm is None else dict(gnorm="z1_gnorm", nunits=len(self.layout.units),
                                                            max_norm=self.max_grad_norm, norm=self._clip)
-        seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream, **clip)
+        tok: Dict[str, Any] = {}
+        if self.global_token_mean:
+            if self._tok_pending is None:
+                raise RuntimeError("global_token_mean: publish_tokens must come before every commit")
+            (n, loss, rows, participants, contribute), self._tok_pending = self._tok_pending, None
+            for x in (n, loss):
+                x.record_stream(stream)  # read by the commit kernel on the commit stream
+            tok = dict(tokens="z1_tokmean", slot=self._tok_commits % TOKEN_SLOTS, n_valid=n, loss_sum=loss, rows=rows,
+                       divisor=participants * rows, contribute=contribute, token_out=self._tok_out,
+                       token_count=self._tok_count)
+            if not clip:
+                tok["norm"] = self._clip  # its second word is the coefficient the update reads
+            self._tok_commits += 1
+        seq = self.comm.zero1_commit_(self.gate, host_ok, True, stream, **clip, **tok)
         self._commit_event = stream.record_event()
         return seq
 
@@ -1335,6 +1440,8 @@ class Zero1Optimizer:
             raise RuntimeError(f"commit {seq}: the verdict kernel finished without posting a verdict")
         if self.max_grad_norm is not None:
             self._resolved_norm = self.comm.grad_norm(seq)
+        if self.global_token_mean:
+            self._resolved_reason = self.comm.commit_reason(seq)
         return v
 
     def update(self, events: Optional[Sequence[torch.cuda.Event]] = None) -> None:
@@ -1345,7 +1452,8 @@ class Zero1Optimizer:
         k = self.layout.replication
         lr = self.param_groups[0]["lr"]
         hp = (lr, self.betas[0], self.betas[1], self.eps, self.weight_decay)
-        coef = self._clip.data_ptr() + 4 if self.max_grad_norm is not None else 0
+        # clipping and the token mean: the coefficient the commit kernel wrote
+        coef = self._clip.data_ptr() + 4 if self.max_grad_norm is not None or self.global_token_mean else 0
         # with a schedule the kernel reads the rate of the device's update count from the table; lr is unused
         sched = {} if self._lr_tab is None else {"lr_table": self._lr_tab.data_ptr(), "lr_steps": self._lr_tab.numel()}
         nd = self._nd_units if self.no_decay else None
@@ -1494,6 +1602,11 @@ class Zero1Optimizer:
                     self.nonfinite_steps += 1
                     logger.warning("zero1: gradient norm is %s: the step was skipped on every replica (%d so far)",
                                    norm, self.nonfinite_steps)
+            reason, self._resolved_reason = self._resolved_reason, None
+            if reason and reason & self._K.ZERO1_VETO_ROWS:
+                self.row_mismatch_steps += 1
+                logger.warning("zero1: the replicas published different row counts M * B * S, so no one token-mean "
+                               "factor fits: the step was skipped on every replica (%d so far)", self.row_mismatch_steps)
 
     # ------------------------------------------------------------------ durable checkpoints
     @torch.no_grad()
